@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <cstdlib>
 #include <memory>
+#include <vector>
 
 namespace b200 {
 
@@ -33,15 +34,18 @@ constexpr int kWarpsPerCta = 8;
 // x a persistent CTA keeps in shared memory).  Rows keep their neighbours sorted by source id, so a row's adjacency is
 // already partitioned by block; every (row, block) SEGMENT is cut into PIECES of <= 64 entries.  A piece is stored with
 // 16-bit local column ids in one of 11 KINDS: S / Q / H = 1 / 2 / <= 4 entries (2 / 4 / 8 bytes of ids), F1..F8 = 1..8 lane
-// slots of 8 entries (16 bytes each; short pieces are padded with a column that reads 0).  Pieces are ordered by
-// (block, kind).  The unit every kernel step works on is a STEP-ROW = 32 lanes x 16 bytes of ids (one 128-bit load per
-// lane, 512 contiguous bytes per warp): it holds 256 S pieces, 128 Q pieces, 64 H pieces, or one of the c slots of 32 Fc
+// slots of 8 entries (16 bytes each; short pieces are padded with a column that reads 0).  The covered rows are split into
+// BANDS of consecutive rows (a multiple of kBandRowAlign each, sized so that a band's fp64 accumulators stay in the L2) and
+// pieces are ordered by (band, block, kind): the sweep runs band after band.  The unit every kernel step works on is a
+// STEP-ROW = 32 lanes x 16 bytes of ids (one 128-bit load per lane, 512 contiguous bytes per warp): it holds 256 S pieces, 128 Q pieces, 64 H pieces, or one of the c slots of 32 Fc
 // pieces (a GROUP of kind Fc is c consecutive step-rows, lane = piece).  Row ids (int32, -1 = unused piece) are stored per
 // group so that a lane's rows are contiguous: 8 / 4 / 2 / 1 per lane.
 // ---------------------------------------------------------------------------------------------
 constexpr int kHotSliceBytes = 192 * 1024;  // x slice a CTA keeps in shared memory
 constexpr int kHotZeroPad    = 64;          // trailing elements of the slice that hold zeros (padding target)
 constexpr int kHotSlot       = 8;           // entries per lane slot
+
+constexpr int kBandRowAlign = 512;  // band bounds: a multiple of the finish kernel's rows per warp (k_sweep_finish)
 
 constexpr int kNumKinds = 11;  // S, Q, H, F1..F8
 constexpr int kKindS = 0, kKindQ = 1, kKindH = 2, kKindF1 = 3;
@@ -81,11 +85,15 @@ struct sweep_layout_t {
   dbuf rows;       // n_rowslots x int32
   dbuf chunks;     // n_chunks x sweep_chunk_t
   dbuf phases;     // n_phases x sweep_phase_t
-  dbuf cta_phase;  // (n_cta + 1) x int32: CTA c owns phases [cta_phase[c], cta_phase[c+1]) (cost-balanced, contiguous chunks)
+  dbuf cta_phase;  // (n_bands * n_cta + 1) x int32: in band b, CTA c owns phases [cta_phase[b * n_cta + c], the next entry)
+                   // (cost-balanced, contiguous chunks)
   dbuf cursor;     // n_phases x int: next chunk of the phase (relative); reset by the finish kernel
   int32_t n_chunks{0};
   int32_t n_phases{0};
   int n_cta{0};
+  int n_bands{1};
+  std::vector<int32_t> band_row;    // n_bands + 1: band b holds rows [band_row[b], band_row[b+1]); band_row[n_bands] = n_cov
+  std::vector<int32_t> band_phase;  // n_bands + 1: the phases of band b are [band_phase[b], band_phase[b+1])
 };
 
 // One orientation: compressed rows over `n_rows` physical rows.

@@ -982,9 +982,9 @@ namespace {
 //      block than its predecessor's (neighbours are sorted by source id)
 //   2. segments = compacted head positions; each is cut into pieces of <= 64 entries, a piece gets its kind
 //      (S / Q / H = 1 / 2 / <= 4 entries, F1..F8 = that many lane slots of 8 entries)
-//   3. pieces are ordered (stable radix sort) by (block, kind); a run of one (block, kind) is cut into groups of
-//      256 / 128 / 64 / 32 pieces and chunks of a few groups; chunks are dealt to the persistent CTAs as contiguous,
-//      cost-balanced ranges, the part of one block inside a range is a phase
+//   3. pieces are ordered (stable radix sort) by (band, block, kind); a run of one (band, block, kind) is cut into groups
+//      of 256 / 128 / 64 / 32 pieces and chunks of a few groups; band by band, chunks are dealt to the persistent CTAs as
+//      contiguous, cost-balanced ranges, the part of one block inside a range is a phase
 //   4. one warp per group writes its step-rows (32 lanes x 16 bytes of ids) and row slots
 
 template <typename O>
@@ -1032,9 +1032,10 @@ __host__ __device__ __forceinline__ int piece_kind(int len)
   return len == 1 ? kKindS : (len == 2 ? kKindQ : (len <= 4 ? kKindH : kKindF1 + (len + kHotSlot - 1) / kHotSlot - 1));
 }
 
-// per segment: write its pieces (start edge, entries, row) and their key = block * kNumKinds + kind
+// per segment: write its pieces (start edge, entries, row) and their key = (band * B + block) * kNumKinds + kind
 __global__ void k_hot_emit_pieces(int32_t const* __restrict__ head_pos, int32_t n_segs, long long nnz,
-                                  int32_t const* __restrict__ idx, int W, int32_t const* __restrict__ seg_row,
+                                  int32_t const* __restrict__ idx, int W, int B, int32_t band_rows,
+                                  int32_t const* __restrict__ seg_row,
                                   int32_t const* __restrict__ piece_off, uint32_t* __restrict__ piece_key,
                                   int32_t* __restrict__ piece_start, int32_t* __restrict__ piece_len,
                                   int32_t* __restrict__ piece_row)
@@ -1043,12 +1044,12 @@ __global__ void k_hot_emit_pieces(int32_t const* __restrict__ head_pos, int32_t 
   if (k >= n_segs) return;
   const long long start = head_pos[k];
   const long long end   = (k + 1 < n_segs) ? (long long)head_pos[k + 1] : nnz;
-  const int b           = idx[start] / W;
   const int row         = seg_row[k];
+  const int bb          = (row / band_rows) * B + idx[start] / W;  // (band, block)
   int p                 = piece_off[k];
   for (long long s = start; s < end; s += kHotPieceEntries, ++p) {
     const int len  = (int)((end - s < kHotPieceEntries) ? end - s : kHotPieceEntries);
-    piece_key[p]   = (uint32_t)(b * kNumKinds + piece_kind(len));
+    piece_key[p]   = (uint32_t)(bb * kNumKinds + piece_kind(len));
     piece_start[p] = (int32_t)s;
     piece_len[p]   = len;
     piece_row[p]   = row;
@@ -1068,23 +1069,25 @@ __global__ void k_hot_class_starts(uint32_t const* __restrict__ sorted_key, int3
   class_start[key] = lo;
 }
 
-struct sweep_fill_t {  // build-time companion of a chunk: its pieces start at piece_begin, its (block, kind) run ends at piece_end
+struct sweep_fill_t {  // build-time companion of a chunk: its pieces start at piece_begin, its (band, block, kind) run ends at piece_end
   int32_t piece_begin, piece_end, block, pad;
 };
 
-// Host-side plan of the sweep's work structure, from the piece counts per (block, kind) alone (class_start[key] = first
-// piece of key = block * kNumKinds + kind, pieces ordered by key):
+// Host-side plan of the sweep's work structure, from the piece counts per (band, block, kind) alone (class_start[key] =
+// first piece of key = (band * B + block) * kNumKinds + kind, pieces ordered by key):
 //   group = 256 / 128 / 64 / 32 pieces of one kind (S / Q / H / F), 1 or (F kinds) 1..8 step-rows
-//   chunk = consecutive groups of one kind in one block, at most kind_chunk_groups(kind)
-//   range = contiguous chunks per persistent CTA, balanced by an estimate of their load/store-unit time (the sweep is
-//           bound by it: one cycle per 128-byte line of ids, per conflict-free 32 gathers, per sector of atomics)
+//   chunk = consecutive groups of one kind in one block of one band, at most kind_chunk_groups(kind)
+//   range = contiguous chunks of one band per persistent CTA, balanced by an estimate of their load/store-unit time (the
+//           sweep is bound by it: one cycle per 128-byte line of ids, per conflict-free 32 gathers, per sector of atomics);
+//           every band is dealt to the same n_cta CTAs on its own (one sweep launch per band)
 //   phase = the chunks of one block inside one range (a CTA loads the block's slice once per phase)
-// Pure host code: exercised on CPU through cugraph_b200_debug_plan_sweep (tests/test_sweep_plan_cpu.py).
+// Pure host code: exercised on CPU through cugraph_b200_debug_plan_sweep[_bands] (tests/test_sweep_plan*_cpu.py).
 struct sweep_plan_t {
   std::vector<sweep_chunk_t> chunks;
   std::vector<sweep_fill_t> fills;
   std::vector<sweep_phase_t> phases;
-  std::vector<int32_t> cta_phase;
+  std::vector<int32_t> cta_phase;   // n_bands * n_cta + 1
+  std::vector<int32_t> band_phase;  // n_bands + 1
   int64_t n_steprows{0}, n_rowslots{0};
   int n_cta{1};
 };
@@ -1099,50 +1102,61 @@ inline double sweep_group_cost(int kind)
 }
 constexpr double kPhaseCost = 2500.0;  // barrier + 192 KiB slice fill, in the same unit
 
-bool plan_sweep(std::vector<int32_t> const& cstart, int B, int sm_count, sweep_plan_t& P)
+bool plan_sweep(std::vector<int32_t> const& cstart, int n_bands, int B, int sm_count, sweep_plan_t& P)
 {
-  std::vector<double> cost;  // per chunk, the phase overhead on the first chunk of every block
-  for (int b = 0; b < B; ++b) {
-    bool first = true;
-    for (int kind = 0; kind < kNumKinds; ++kind) {
-      const int key    = b * kNumKinds + kind;
-      int32_t p        = cstart[key];
-      const int32_t pe = cstart[key + 1];
-      const int ppg = kind_pieces(kind), steps = kind_steps(kind), gmax = kind_chunk_groups(kind);
-      while (p < pe) {
-        const int groups = (int)std::min<int64_t>(gmax, ((int64_t)(pe - p) + ppg - 1) / ppg);
-        if (P.n_steprows + (int64_t)groups * steps >= (1ll << 31) - 64 || P.n_rowslots + (int64_t)groups * ppg >= (1ll << 31) - 64)
-          return false;  // 32-bit step-row / row-slot numbers
-        P.chunks.push_back({(int32_t)P.n_steprows, (int32_t)P.n_rowslots, groups, kind});
-        P.fills.push_back({p, pe, b, 0});
-        cost.push_back(groups * sweep_group_cost(kind) + (first ? kPhaseCost : 0.0));
-        first = false;
-        P.n_steprows += (int64_t)groups * steps;
-        P.n_rowslots += (int64_t)groups * ppg;
-        p += groups * ppg;  // may pass pe inside the last group: the fill pads
+  std::vector<double> cost;          // per chunk, the phase overhead on the first chunk of every block
+  std::vector<size_t> band_chunk(1);  // chunks of band k: [band_chunk[k], band_chunk[k+1])
+  for (int band = 0; band < n_bands; ++band) {
+    for (int b = 0; b < B; ++b) {
+      bool first = true;
+      for (int kind = 0; kind < kNumKinds; ++kind) {
+        const int key    = (band * B + b) * kNumKinds + kind;
+        int32_t p        = cstart[key];
+        const int32_t pe = cstart[key + 1];
+        const int ppg = kind_pieces(kind), steps = kind_steps(kind), gmax = kind_chunk_groups(kind);
+        while (p < pe) {
+          const int groups = (int)std::min<int64_t>(gmax, ((int64_t)(pe - p) + ppg - 1) / ppg);
+          if (P.n_steprows + (int64_t)groups * steps >= (1ll << 31) - 64 || P.n_rowslots + (int64_t)groups * ppg >= (1ll << 31) - 64)
+            return false;  // 32-bit step-row / row-slot numbers
+          P.chunks.push_back({(int32_t)P.n_steprows, (int32_t)P.n_rowslots, groups, kind});
+          P.fills.push_back({p, pe, b, 0});
+          cost.push_back(groups * sweep_group_cost(kind) + (first ? kPhaseCost : 0.0));
+          first = false;
+          P.n_steprows += (int64_t)groups * steps;
+          P.n_rowslots += (int64_t)groups * ppg;
+          p += groups * ppg;  // may pass pe inside the last group: the fill pads
+        }
+      }
+    }
+    band_chunk.push_back(P.chunks.size());
+  }
+  size_t most = 0;
+  for (int band = 0; band < n_bands; ++band) most = std::max(most, band_chunk[band + 1] - band_chunk[band]);
+  P.n_cta = (int)std::max<size_t>(1, std::min<size_t>((size_t)sm_count, most));
+  P.cta_phase.assign((size_t)n_bands * P.n_cta + 1, 0);
+  P.band_phase.assign(n_bands + 1, 0);
+  for (int band = 0; band < n_bands; ++band) {
+    const size_t c_lo = band_chunk[band], n = band_chunk[band + 1] - c_lo;
+    std::vector<double> pre(n + 1, 0.0);
+    for (size_t c = 0; c < n; ++c) pre[c + 1] = pre[c] + cost[c_lo + c];
+    P.band_phase[band] = (int32_t)P.phases.size();
+    size_t c = 0;
+    for (int cta = 0; cta < P.n_cta; ++cta) {
+      const double target = pre[n] * (cta + 1) / P.n_cta;
+      const size_t c0     = c;
+      if (cta == P.n_cta - 1) c = n;
+      else while (c < n && pre[c + 1] <= target) ++c;
+      P.cta_phase[(size_t)band * P.n_cta + cta] = (int32_t)P.phases.size();
+      for (size_t k = c_lo + c0; k < c_lo + c;) {  // split the range by block
+        size_t e = k;
+        while (e < c_lo + c && P.fills[e].block == P.fills[k].block) ++e;
+        P.phases.push_back({P.fills[k].block, (int32_t)k, (int32_t)e, 0});
+        k = e;
       }
     }
   }
-  const size_t n = P.chunks.size();
-  P.n_cta        = (int)std::max<size_t>(1, std::min<size_t>((size_t)sm_count, n));
-  std::vector<double> pre(n + 1, 0.0);
-  for (size_t c = 0; c < n; ++c) pre[c + 1] = pre[c] + cost[c];
-  P.cta_phase.assign(P.n_cta + 1, 0);
-  size_t c = 0;
-  for (int cta = 0; cta < P.n_cta; ++cta) {
-    const double target = pre[n] * (cta + 1) / P.n_cta;
-    const size_t c0     = c;
-    if (cta == P.n_cta - 1) c = n;
-    else while (c < n && pre[c + 1] <= target) ++c;
-    P.cta_phase[cta] = (int32_t)P.phases.size();
-    for (size_t k = c0; k < c;) {  // split the range by block
-      size_t e = k;
-      while (e < c && P.fills[e].block == P.fills[k].block) ++e;
-      P.phases.push_back({P.fills[k].block, (int32_t)k, (int32_t)e, 0});
-      k = e;
-    }
-  }
-  P.cta_phase[P.n_cta] = (int32_t)P.phases.size();
+  P.band_phase[n_bands]                  = (int32_t)P.phases.size();
+  P.cta_phase[(size_t)n_bands * P.n_cta] = (int32_t)P.phases.size();
   return true;
 }
 
@@ -1302,6 +1316,21 @@ k_sweep_fill(sweep_chunk_t const* __restrict__ chunks, sweep_fill_t const* __res
   }
 }
 
+// Row bands: the sweep's fp64 REDs into acc[row] hit the L2 only while the rows they scatter over fit in it (measured on an
+// H100 80GB HBM3 at 700 W, 50 MB of L2: a scattered RED.64 costs the same up to 24 MB of accumulators, 1.3x at 48 MB and
+// 3.7x at 64 MB), so the covered rows are split into bands whose accumulators take at most kBandL2Share of the L2.  Half
+// gave the fastest RMAT-24 sweep (3 bands, DESIGN.md §3.2); more bands add launch tails and slice loads.
+// CUGRAPH_B200_SWEEP_BANDS forces a count (tests, A/B runs).
+constexpr double kBandL2Share = 0.5;
+
+int sweep_bands(handle_impl const& h, int32_t n_cov)
+{
+  const int most = std::max(1, (int)(((int64_t)n_cov + kBandRowAlign - 1) / kBandRowAlign));
+  int P          = h.tune.sweep_bands;
+  if (P <= 0) P = h.l2_bytes ? (int)std::ceil(8.0 * n_cov / (kBandL2Share * (double)h.l2_bytes)) : 1;
+  return std::min(std::max(P, 1), most);
+}
+
 template <typename O>
 std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t const& c, int32_t nv, size_t es)
 {
@@ -1313,6 +1342,12 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   auto L              = std::make_unique<sweep_layout_t>();
   L->W = W; L->B = B; L->n_cov = n_cov; L->nnz = nnz;
   int32_t const* idx = c.indices.as<int32_t>();
+  // equal bands of whole kBandRowAlign spans; rounding may leave fewer than asked for
+  const int asked         = sweep_bands(h, n_cov);
+  const int32_t band_rows = (int32_t)((((int64_t)n_cov + asked - 1) / asked + kBandRowAlign - 1) / kBandRowAlign * kBandRowAlign);
+  const int n_bands       = (int)(((int64_t)n_cov + band_rows - 1) / band_rows);
+  L->n_bands              = n_bands;
+  for (int b = 0; b <= n_bands; ++b) L->band_row.push_back((int32_t)std::min<int64_t>((int64_t)b * band_rows, n_cov));
 
   // 1. segment heads
   dbuf flag = make_dbuf<uint8_t>(nnz, h.stream);
@@ -1351,16 +1386,16 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   dbuf piece_key = make_dbuf<uint32_t>(n_pieces, h.stream), piece_key2 = make_dbuf<uint32_t>(n_pieces, h.stream);
   dbuf piece_start = make_dbuf<int32_t>(n_pieces, h.stream), piece_len = make_dbuf<int32_t>(n_pieces, h.stream);
   dbuf piece_row = make_dbuf<int32_t>(n_pieces, h.stream);
-  B200_LAUNCH(h, k_hot_emit_pieces, grid_for(n_segs), kBlock, 0, head_pos.as<int32_t>(), n_segs, (long long)nnz, idx, W,
-              seg_row.as<int32_t>(), piece_off.as<int32_t>(), piece_key.as<uint32_t>(), piece_start.as<int32_t>(),
+  B200_LAUNCH(h, k_hot_emit_pieces, grid_for(n_segs), kBlock, 0, head_pos.as<int32_t>(), n_segs, (long long)nnz, idx, W, B,
+              band_rows, seg_row.as<int32_t>(), piece_off.as<int32_t>(), piece_key.as<uint32_t>(), piece_start.as<int32_t>(),
               piece_len.as<int32_t>(), piece_row.as<int32_t>());
   head_pos.release();
   seg_row.release();
   piece_off.release();
   tr.mark("sweep layout: pieces");
 
-  // 3. order pieces by (block, kind)
-  const int n_keys = B * kNumKinds;
+  // 3. order pieces by (band, block, kind)
+  const int n_keys = n_bands * B * kNumKinds;
   dbuf perm = make_dbuf<uint32_t>(n_pieces, h.stream), perm2 = make_dbuf<uint32_t>(n_pieces, h.stream);
   B200_LAUNCH(h, k_iota64, grid_for(n_pieces, 4), kBlock, 0, (int64_t)n_pieces, perm.as<uint32_t>());
   sort_pairs<uint32_t, uint32_t>(h, piece_key.as<uint32_t>(), piece_key2.as<uint32_t>(), perm.as<uint32_t>(),
@@ -1377,14 +1412,16 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   tr.mark("sweep layout: kind sort");
   if (tr.on) {  // layout statistics: pieces by kind, per range of blocks
     int edges[] = {0, 1, 4, 16, 64, 160, B};
-    std::fprintf(stderr, "[sweep] B=%d W=%d rows=%d nnz=%lld segments=%d pieces=%d\n", B, W, n_cov, (long long)nnz, n_segs, n_pieces);
+    std::fprintf(stderr, "[sweep] B=%d W=%d rows=%d nnz=%lld segments=%d pieces=%d bands=%d of %d rows\n", B, W, n_cov,
+                 (long long)nnz, n_segs, n_pieces, n_bands, band_rows);
     for (int k = 0; k + 1 < 7; ++k) {
       const int b0 = std::min(edges[k], B), b1 = std::min(edges[k + 1], B);
       if (b1 <= b0) continue;
       std::fprintf(stderr, "[sweep] blocks [%d,%d) pieces by kind S Q H F1..F8:", b0, b1);
       for (int kind = 0; kind < kNumKinds; ++kind) {
         long long np = 0;
-        for (int b = b0; b < b1; ++b) np += cstart[b * kNumKinds + kind + 1] - cstart[b * kNumKinds + kind];
+        for (int band = 0; band < n_bands; ++band)
+          for (int b = b0; b < b1; ++b) np += cstart[(band * B + b) * kNumKinds + kind + 1] - cstart[(band * B + b) * kNumKinds + kind];
         std::fprintf(stderr, " %lld", np);
       }
       std::fprintf(stderr, "\n");
@@ -1393,7 +1430,8 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
 
   // 4. chunks, CTA ranges, phases
   sweep_plan_t plan;
-  if (!plan_sweep(cstart, B, h.sm_count, plan)) return nullptr;  // step-row numbers overflow 31 bits
+  if (!plan_sweep(cstart, n_bands, B, h.sm_count, plan)) return nullptr;  // step-row numbers overflow 31 bits
+  L->band_phase = plan.band_phase;
   L->n_steprows = plan.n_steprows;
   L->n_rowslots = plan.n_rowslots;
   L->n_chunks   = (int32_t)plan.chunks.size();
@@ -1437,26 +1475,36 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   check_last("sweep layout");
   sync(h);
   tr.mark("sweep layout: fill");
-  if (tr.on)
+  if (tr.on) {
     std::fprintf(stderr, "[sweep] %lld step-rows = %.1f MB of ids, %lld row slots = %.1f MB, %d chunks, %d phases, %d CTAs\n",
                  (long long)L->n_steprows, (double)L->n_steprows * 512 / 1e6, (long long)L->n_rowslots,
                  (double)L->n_rowslots * 4 / 1e6, L->n_chunks, L->n_phases, L->n_cta);
+    for (int band = 0; band < n_bands; ++band) {  // slice loads: a CTA loads a block's slice once per phase
+      const int p0 = plan.band_phase[band], p1 = plan.band_phase[band + 1];
+      const int c0 = p1 > p0 ? plan.phases[p0].chunk_begin : 0, c1 = p1 > p0 ? plan.phases[p1 - 1].chunk_end : 0;
+      std::fprintf(stderr, "[sweep] band %d rows [%d,%d): %d pieces, %d chunks, %d phases = slice loads\n", band,
+                   L->band_row[band], L->band_row[band + 1], cstart[(band + 1) * B * kNumKinds] - cstart[band * B * kNumKinds],
+                   c1 - c0, p1 - p0);
+    }
+  }
   return L;
 }
 
 }  // namespace
 
-// flat copy of plan_sweep's result for the debug C entry (CPU tests)
-bool debug_plan_sweep(std::vector<int32_t> const& cstart, int B, int sm_count, int64_t totals[3], std::vector<int32_t>& chunks4,
-                      std::vector<int32_t>& fills4, std::vector<int32_t>& phases4, std::vector<int32_t>& cta_phase)
+// flat copy of plan_sweep's result for the debug C entries (CPU tests)
+bool debug_plan_sweep(std::vector<int32_t> const& cstart, int n_bands, int B, int sm_count, int64_t totals[3],
+                      std::vector<int32_t>& chunks4, std::vector<int32_t>& fills4, std::vector<int32_t>& phases4,
+                      std::vector<int32_t>& cta_phase, std::vector<int32_t>& band_phase)
 {
   sweep_plan_t P;
-  if (!plan_sweep(cstart, B, sm_count, P)) return false;
+  if (!plan_sweep(cstart, n_bands, B, sm_count, P)) return false;
   totals[0] = P.n_steprows; totals[1] = P.n_rowslots; totals[2] = P.n_cta;
   for (auto const& x : P.chunks) chunks4.insert(chunks4.end(), {x.sr_begin, x.row_begin, x.n_groups, x.kind});
   for (auto const& x : P.fills) fills4.insert(fills4.end(), {x.piece_begin, x.piece_end, x.block, x.pad});
   for (auto const& x : P.phases) phases4.insert(phases4.end(), {x.block, x.chunk_begin, x.chunk_end, x.pad});
-  cta_phase = P.cta_phase;
+  cta_phase  = P.cta_phase;
+  band_phase = P.band_phase;
   return true;
 }
 
@@ -1570,21 +1618,22 @@ template dbuf collect_vertex_values<double>(handle_impl const&, graph_impl const
 
 }  // namespace b200
 
-extern "C" cugraph_error_code_t cugraph_b200_debug_plan_sweep(const int32_t* class_start, int n_blocks, int sm_count,
-                                                              int64_t* totals, int32_t* chunks, int32_t* fills,
-                                                              size_t chunks_capacity, size_t* n_chunks, int32_t* phases,
-                                                              size_t phases_capacity, size_t* n_phases, int32_t* cta_phase,
-                                                              size_t cta_capacity, cugraph_error_t** error)
+extern "C" cugraph_error_code_t cugraph_b200_debug_plan_sweep_bands(const int32_t* class_start, int n_bands, int n_blocks,
+                                                                    int sm_count, int64_t* totals, int32_t* chunks,
+                                                                    int32_t* fills, size_t chunks_capacity, size_t* n_chunks,
+                                                                    int32_t* phases, size_t phases_capacity, size_t* n_phases,
+                                                                    int32_t* cta_phase, size_t cta_capacity,
+                                                                    int32_t* band_phase, cugraph_error_t** error)
 {
   using namespace b200;
   return guarded(error, [&] {
-    B200_EXPECTS(class_start && totals && chunks && fills && phases && cta_phase && n_chunks && n_phases, CUGRAPH_INVALID_INPUT,
-                 "null argument");
-    B200_EXPECTS(n_blocks >= 0 && sm_count >= 1, CUGRAPH_INVALID_INPUT, "bad parameter");
-    std::vector<int32_t> cstart(class_start, class_start + (size_t)n_blocks * kNumKinds + 1);
-    std::vector<int32_t> c4, f4, p4, r;
+    B200_EXPECTS(class_start && totals && chunks && fills && phases && cta_phase && band_phase && n_chunks && n_phases,
+                 CUGRAPH_INVALID_INPUT, "null argument");
+    B200_EXPECTS(n_bands >= 1 && n_blocks >= 0 && sm_count >= 1, CUGRAPH_INVALID_INPUT, "bad parameter");
+    std::vector<int32_t> cstart(class_start, class_start + (size_t)n_bands * n_blocks * kNumKinds + 1);
+    std::vector<int32_t> c4, f4, p4, r, bp;
     int64_t t[3];
-    B200_EXPECTS(debug_plan_sweep(cstart, n_blocks, sm_count, t, c4, f4, p4, r), CUGRAPH_INVALID_INPUT,
+    B200_EXPECTS(debug_plan_sweep(cstart, n_bands, n_blocks, sm_count, t, c4, f4, p4, r, bp), CUGRAPH_INVALID_INPUT,
                  "step-row numbers overflow 31 bits");
     B200_EXPECTS(c4.size() / 4 <= chunks_capacity && p4.size() / 4 <= phases_capacity && r.size() <= cta_capacity,
                  CUGRAPH_INVALID_INPUT, "output capacity too small");
@@ -1593,7 +1642,19 @@ extern "C" cugraph_error_code_t cugraph_b200_debug_plan_sweep(const int32_t* cla
     std::copy(f4.begin(), f4.end(), fills);
     std::copy(p4.begin(), p4.end(), phases);
     std::copy(r.begin(), r.end(), cta_phase);
+    std::copy(bp.begin(), bp.end(), band_phase);
     *n_chunks = c4.size() / 4;
     *n_phases = p4.size() / 4;
   });
+}
+
+extern "C" cugraph_error_code_t cugraph_b200_debug_plan_sweep(const int32_t* class_start, int n_blocks, int sm_count,
+                                                              int64_t* totals, int32_t* chunks, int32_t* fills,
+                                                              size_t chunks_capacity, size_t* n_chunks, int32_t* phases,
+                                                              size_t phases_capacity, size_t* n_phases, int32_t* cta_phase,
+                                                              size_t cta_capacity, cugraph_error_t** error)
+{
+  int32_t band_phase[2];
+  return cugraph_b200_debug_plan_sweep_bands(class_start, 1, n_blocks, sm_count, totals, chunks, fills, chunks_capacity, n_chunks,
+                                             phases, phases_capacity, n_phases, cta_phase, cta_capacity, band_phase, error);
 }

@@ -258,6 +258,10 @@ cugraph_error_code_t cugraph_b200_block_pull_sweep(const cugraph_resource_handle
     B200_EXPECTS(xv->size >= padded_x_elems(b->n_span, f32 ? 4 : 8), CUGRAPH_INVALID_INPUT,
                  "x must hold cugraph_b200_padded_elems(span) elements");
     B200_EXPECTS(yv->size >= (size_t)b->n_span, CUGRAPH_INVALID_INPUT, "y must hold `span` elements");
+    const size_t es = f32 ? 4 : 8;
+    auto const* x0  = static_cast<const char*>(xv->data);
+    auto const* y0  = static_cast<const char*>(yv->data);
+    B200_EXPECTS(y0 + yv->size * es <= x0 || x0 + xv->size * es <= y0, CUGRAPH_INVALID_INPUT, "x and y must not overlap");
     csx_t const& c = *b->csx;
     auto* st       = b->state.as<pr_state_t>();
     const bool covered_only = b->y_complete == yv->data;  // the empty rows of this y hold their zeros from an earlier sweep

@@ -20,6 +20,8 @@
 //     gather: 20 % of its instructions); slots, pieces and rows accumulate in fp64.
 //   * one fp64 RED per piece into acc[row] (L2); the pieces of a hub row that fill a whole warp are summed by shuffles
 //     first.  k_sweep_finish turns acc into y, clears it and resets the cursors.
+//   * the rows are split into bands whose accumulators fit in the L2 (graph.cuh); the sweep runs band by band, k_sweep over
+//     the band's phases, then k_sweep_finish over its rows while their accumulators are still in the L2.
 #pragma once
 #include "spmv.cuh"
 
@@ -405,7 +407,7 @@ struct sweep_args_t {
   int* __restrict__ cursor;
   T const* __restrict__ x;
   pr_state_t const* __restrict__ st;
-  int n_phases;
+  int ph_lo, ph_hi;  // the band's phases; a CTA only steals inside them (a later band's accumulators would enter the L2 early)
   int W;
 };
 
@@ -517,7 +519,7 @@ __global__ void __launch_bounds__(kSweepThreads, 1) k_sweep(sweep_args_t<T> a)
   const int me   = (int)blockIdx.x;
   if (threadIdx.x == 0) mbar_init(&bar, 1);
   if (threadIdx.x < kHotZeroPad) sx[a.W + threadIdx.x] = (T)0;  // the zero columns every slice ends with
-  const int own_lo = a.cta_phase[me], own_hi = a.cta_phase[me + 1];
+  const int own_lo = a.cta_phase[me], own_hi = a.cta_phase[me + 1];  // cta_phase: this band's entries
   int next_own    = own_lo;
   unsigned parity = 0;
   int cur_block   = -1;
@@ -530,7 +532,7 @@ __global__ void __launch_bounds__(kSweepThreads, 1) k_sweep(sweep_args_t<T> a)
       if (threadIdx.x == 0) s_best = 0;
       __syncthreads();
       int best = 0;
-      for (int q = (int)threadIdx.x; q < a.n_phases; q += kSweepThreads) {
+      for (int q = a.ph_lo + (int)threadIdx.x; q < a.ph_hi; q += kSweepThreads) {
         if (q >= own_lo && q < own_hi) continue;
         const sweep_phase_t ph = a.phases[q];
         const int left         = (ph.chunk_end - ph.chunk_begin) - ld_volatile(a.cursor + q);
@@ -541,16 +543,16 @@ __global__ void __launch_bounds__(kSweepThreads, 1) k_sweep(sweep_args_t<T> a)
       const int win = s_best;
       __syncthreads();
       if (win > 0) {
-        if (threadIdx.x == 0) s_best = a.n_phases;
+        if (threadIdx.x == 0) s_best = a.ph_hi;
         __syncthreads();
-        for (int q = (int)threadIdx.x; q < a.n_phases; q += kSweepThreads) {
+        for (int q = a.ph_lo + (int)threadIdx.x; q < a.ph_hi; q += kSweepThreads) {
           if (q >= own_lo && q < own_hi) continue;
           const sweep_phase_t ph = a.phases[q];
           const int left         = (ph.chunk_end - ph.chunk_begin) - ld_volatile(a.cursor + q);
           if (left >= kStealMin && left * 2 >= win) atomicMin(&s_best, q);
         }
         __syncthreads();
-        p = s_best < a.n_phases ? s_best : -1;
+        p = s_best < a.ph_hi ? s_best : -1;
       }
     }
     __syncthreads();  // every warp is done with the previous phase's slice (and has read s_best)
@@ -593,21 +595,22 @@ __global__ void __launch_bounds__(kSweepThreads, 1) k_sweep(sweep_args_t<T> a)
   }
 }
 
-// y[row] = acc * alpha + init for every covered row, init for the empty rows behind them; clears the accumulators and the
-// cursors.  A warp handles 256 consecutive rows in four steps of 64: every step is one 512-byte load + one 512-byte store of
+// y[row] = acc * alpha + init for the rows [row_lo, n_rows): acc for the covered ones (< n_cov), init for the empty rows behind
+// them; clears their accumulators and the n_phases cursors.  row_lo is a multiple of kBandRowAlign.  A warp handles 256 consecutive rows in four steps of 64: every step is one 512-byte load + one 512-byte store of
 // accumulators and one 256-byte store of y per warp (lane = two rows), all four loads issued before the first use.
 // (Eight CONSECUTIVE rows per thread looked the same on paper and ran at 2.3 TB/s: every warp-wide 128-bit access then
 // touched sixteen 128-byte lines for a quarter of their bytes.)
 template <typename T, int kFinishSteps>
 __global__ void __launch_bounds__(256)
-k_sweep_finish(double* __restrict__ acc, int n_cov, int n_rows, T* __restrict__ y, int32_t const* __restrict__ row_vertex,
+k_sweep_finish(double* __restrict__ acc, int row_lo, int n_cov, int n_rows, T* __restrict__ y, int32_t const* __restrict__ row_vertex,
                double alpha, int* __restrict__ cursor, int n_phases, pr_state_t const* __restrict__ st)
 {
+  static_assert(kBandRowAlign % (64 * kFinishSteps) == 0, "a warp's rows must not straddle a band bound");
   if (st->done) return;
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t < n_phases) cursor[t] = 0;
   const int lane = threadIdx.x & 31;
-  const int base = (t >> 5) * (64 * kFinishSteps) + 2 * lane;  // first of this lane's two rows in step 0
+  const int base = row_lo + (t >> 5) * (64 * kFinishSteps) + 2 * lane;  // first of this lane's two rows in step 0
   if (base - 2 * lane >= n_rows) return;
   const double init = st->init;
   double2 q[kFinishSteps];
@@ -649,24 +652,32 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
   a.p.acc     = acc;
   a.chunks    = L.chunks.as<sweep_chunk_t>();
   a.phases    = L.phases.as<sweep_phase_t>();
-  a.cta_phase = L.cta_phase.as<int32_t>();
   a.cursor    = L.cursor.as<int>();
   a.x         = x;
   a.st        = st;
-  a.n_phases  = L.n_phases;
   a.W         = L.W;
   a.p.pol     = 0;
   a.p.acc_pol = 0;
-  if (weighted) B200_LAUNCH(h, (k_sweep<T, true>), L.n_cta, kSweepThreads, kSweepDynSmem, a);
-  else B200_LAUNCH(h, (k_sweep<T, false>), L.n_cta, kSweepThreads, kSweepDynSmem, a);
   // 8 steps of 64 rows per warp: faster than 4 or 2 steps
   constexpr int kFinishSteps = 8;
   // covered_rows_only: y of the rows without edges already holds their (unvarying) value — multi-GPU blocks, where more than
   // half of the row slots are empty and the unvarying term is 0 (mg.cu)
   const int32_t finish_rows = covered_rows_only ? L.n_cov : c.n_rows;
-  const int n = std::max((finish_rows + 2 * kFinishSteps - 1) / (2 * kFinishSteps), L.n_phases);  // threads: 16 rows each
-  B200_LAUNCH(h, (k_sweep_finish<T, kFinishSteps>), (n + 255) / 256, 256, 0, acc, L.n_cov, finish_rows, y, c.row_vertex.as<int32_t>(), alpha,
-              L.cursor.as<int>(), L.n_phases, st);
+  // band by band: the band's rows are finished while its accumulators are in the L2, before the next band's REDs evict them.
+  // y must not overlap x: a band's finish writes y while later bands still read x.
+  for (int band = 0; band < L.n_bands; ++band) {
+    const int row_lo = L.band_row[band];
+    const int row_hi = band == L.n_bands - 1 ? finish_rows : L.band_row[band + 1];  // the last band also writes the empty rows
+    a.cta_phase      = L.cta_phase.as<int32_t>() + (size_t)band * L.n_cta;
+    a.ph_lo          = L.band_phase[band];
+    a.ph_hi          = L.band_phase[band + 1];
+    if (weighted) B200_LAUNCH(h, (k_sweep<T, true>), L.n_cta, kSweepThreads, kSweepDynSmem, a);
+    else B200_LAUNCH(h, (k_sweep<T, false>), L.n_cta, kSweepThreads, kSweepDynSmem, a);
+    const int n_ph = a.ph_hi - a.ph_lo;
+    const int n    = std::max((row_hi - row_lo + 2 * kFinishSteps - 1) / (2 * kFinishSteps), n_ph);  // threads: 16 rows each
+    B200_LAUNCH(h, (k_sweep_finish<T, kFinishSteps>), (std::max(n, 1) + 255) / 256, 256, 0, acc, row_lo, L.n_cov, row_hi, y,
+                c.row_vertex.as<int32_t>(), alpha, L.cursor.as<int>() + a.ph_lo, n_ph, st);
+  }
 }
 
 // dispatch: the piece stream when it exists for this graph, else the plain edge-balanced sweep

@@ -50,11 +50,26 @@ EMU_EXPORT int emu_sweep_layout(const cugraph_resource_handle_t* handle, cugraph
   }
   if (!L) return 1;
   ints[0] = L->W; ints[1] = L->B; ints[2] = L->n_cov; ints[3] = L->nnz; ints[4] = L->n_steprows; ints[5] = L->n_rowslots;
-  ints[6] = L->n_chunks; ints[7] = L->n_phases; ints[8] = L->n_cta; ints[9] = L->bank_order; ints[10] = (int64_t)es;
+  ints[6] = L->n_chunks; ints[7] = L->n_phases; ints[8] = (int64_t)L->n_bands * L->n_cta; ints[9] = L->bank_order; ints[10] = (int64_t)es;
   ints[11] = L->n_pieces;
   ptrs[0] = L->ids.data(); ptrs[1] = L->w.data(); ptrs[2] = L->rows.data(); ptrs[3] = L->chunks.data();
   ptrs[4] = L->phases.data(); ptrs[5] = L->cta_phase.data();
   return 0;
+}
+
+// row bands of that piece stream (call emu_sweep_layout first): returns n_bands and its CTAs per band (*n_cta);
+// band_row / band_phase receive n_bands + 1 entries each when they hold at least `capacity`
+EMU_EXPORT int emu_sweep_bands(cugraph_graph_t* graph, size_t es, int* n_cta, int32_t* band_row, int32_t* band_phase, size_t capacity)
+{
+  auto* g                 = reinterpret_cast<graph_impl*>(graph);
+  sweep_layout_t const* L = (es == 4 ? g->primary->hot4 : g->primary->hot8).get();
+  if (!L) return 0;
+  *n_cta = L->n_cta;
+  if ((size_t)L->n_bands + 1 <= capacity) {
+    std::copy(L->band_row.begin(), L->band_row.end(), band_row);
+    std::copy(L->band_phase.begin(), L->band_phase.end(), band_phase);
+  }
+  return L->n_bands;
 }
 
 EMU_EXPORT size_t emu_padded_x_elems(int32_t nv, size_t es) { return padded_x_elems(nv, es); }

@@ -52,7 +52,8 @@ CUGRAPH_EXPORT void cugraph_b200_block_free(cugraph_b200_block_t* block);
 CUGRAPH_EXPORT size_t cugraph_b200_block_span(const cugraph_b200_block_t* block);
 /* y[row] = alpha * sum over the block's edges (row, col) of x[col] * w; rows without edges get 0.  The FIRST sweep of a block
  * into a given y array writes every row slot; later sweeps into the same array only rewrite the rows that have edges (in a 2D
- * block most row slots are empty) — the caller must leave the other entries alone, or pass a zero-initialised array. */
+ * block most row slots are empty) — the caller must leave the other entries alone, or pass a zero-initialised array.
+ * x and y must not overlap: rows are written band by band while later bands still read x. */
 CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_pull_sweep(
   const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
   const cugraph_type_erased_device_array_view_t* x, cugraph_type_erased_device_array_view_t* y, double alpha,
@@ -106,6 +107,17 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_debug_plan_sweep(const int32_t*
                                                                  size_t chunks_capacity, size_t* n_chunks, int32_t* phases,
                                                                  size_t phases_capacity, size_t* n_phases, int32_t* cta_phase,
                                                                  size_t cta_capacity, cugraph_error_t** error);
+
+/* The same planner over n_bands row bands: class_start has n_bands * n_blocks * 11 + 1 entries, key (band * n_blocks +
+ * block) * 11 + kind.  Bands are planned one after the other over the same totals[2] CTAs: cta_phase has
+ * n_bands * totals[2] + 1 entries (entry band * totals[2] + c starts CTA c of that band) and band_phase n_bands + 1
+ * (the phases of band b are [band_phase[b], band_phase[b+1])).  n_bands = 1 is cugraph_b200_debug_plan_sweep. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_debug_plan_sweep_bands(const int32_t* class_start, int n_bands, int n_blocks,
+                                                                       int sm_count, int64_t* totals, int32_t* chunks,
+                                                                       int32_t* fills, size_t chunks_capacity, size_t* n_chunks,
+                                                                       int32_t* phases, size_t phases_capacity, size_t* n_phases,
+                                                                       int32_t* cta_phase, size_t cta_capacity,
+                                                                       int32_t* band_phase, cugraph_error_t** error);
 
 #ifdef __cplusplus
 }
