@@ -102,6 +102,8 @@ struct tuning_t {
   long long sweep_min_edges{1ll << 22};  // CUGRAPH_B200_SWEEP_MIN_EDGES: graphs below it use the plain sweep (tests: 0)
   bool sweep_bank_order{true};           // CUGRAPH_B200_SWEEP_BANK_ORDER
   int sweep_bands{0};                    // CUGRAPH_B200_SWEEP_BANDS: row bands of the piece stream (0: sized to the L2)
+  int sweep_tail_degree{0};              // CUGRAPH_B200_SWEEP_TAIL_DEGREE: rows below this in-degree leave the piece stream
+                                         // (0: the default rule, 1: no tail, 2/4/8/16/32: that bound on any graph)
   double bfs_alpha{40.0}, bfs_beta{24.0};  // CUGRAPH_B200_BFS_ALPHA / _BETA (Beamer switch points; alpha 14 -> 40: -7 % per source on RMAT-24, r02_notes)
   bool sssp_adaptive{true};                // CUGRAPH_B200_SSSP_ADAPTIVE
   double sssp_delta_scale{1.0};            // CUGRAPH_B200_SSSP_DELTA_SCALE
@@ -118,6 +120,7 @@ struct tuning_t {
     if (auto e = get("CUGRAPH_B200_SWEEP_MIN_EDGES")) t.sweep_min_edges = std::atoll(e);
     if (auto e = get("CUGRAPH_B200_SWEEP_BANK_ORDER")) t.sweep_bank_order = std::atoi(e) != 0;
     if (auto e = get("CUGRAPH_B200_SWEEP_BANDS")) t.sweep_bands = std::max(0, std::atoi(e));
+    if (auto e = get("CUGRAPH_B200_SWEEP_TAIL_DEGREE")) t.sweep_tail_degree = std::max(0, std::atoi(e));
     if (auto e = get("CUGRAPH_B200_BFS_ALPHA")) t.bfs_alpha = std::atof(e);
     if (auto e = get("CUGRAPH_B200_BFS_BETA")) t.bfs_beta = std::atof(e);
     if (auto e = get("CUGRAPH_B200_SSSP_ADAPTIVE")) t.sssp_adaptive = std::atoi(e) != 0;

@@ -29,12 +29,14 @@ constexpr int kWarpChunk  = 1024;
 constexpr int kWarpsPerCta = 8;
 
 // ---------------------------------------------------------------------------------------------
-// Column-blocked "piece stream" of ALL non-empty rows for the shared-memory pull sweep (sweep.cuh).
+// Column-blocked "piece stream" of the rows [0, n_str) for the shared-memory pull sweep (sweep.cuh).  n_str is a degree-bin
+// bound: on large graphs the rows of in-degree < kSweepTailDegree (the TAIL) leave the stream and are swept by the plain
+// row kernel instead (k_spmv_low); on smaller graphs the stream covers every non-empty row.
 // The source (column) space is cut into B blocks of W vertices (W * sizeof(T) = 192 KiB minus 64 zero columns: the slice of
 // x a persistent CTA keeps in shared memory).  Rows keep their neighbours sorted by source id, so a row's adjacency is
 // already partitioned by block; every (row, block) SEGMENT is cut into PIECES of <= 64 entries.  A piece is stored with
 // 16-bit local column ids in one of 11 KINDS: S / Q / H = 1 / 2 / <= 4 entries (2 / 4 / 8 bytes of ids), F1..F8 = 1..8 lane
-// slots of 8 entries (16 bytes each; short pieces are padded with a column that reads 0).  The covered rows are split into
+// slots of 8 entries (16 bytes each; short pieces are padded with a column that reads 0).  The stream rows are split into
 // BANDS of consecutive rows (a multiple of kBandRowAlign each, sized so that a band's fp64 accumulators stay in the L2) and
 // pieces are ordered by (band, block, kind): the sweep runs band after band.  The unit every kernel step works on is a
 // STEP-ROW = 32 lanes x 16 bytes of ids (one 128-bit load per lane, 512 contiguous bytes per warp): it holds 256 S pieces, 128 Q pieces, 64 H pieces, or one of the c slots of 32 Fc
@@ -46,6 +48,14 @@ constexpr int kHotZeroPad    = 64;          // trailing elements of the slice th
 constexpr int kHotSlot       = 8;           // entries per lane slot
 
 constexpr int kBandRowAlign = 512;  // band bounds: a multiple of the finish kernel's rows per warp (k_sweep_finish)
+
+// Tail of the piece stream: a row of small in-degree has its few edges in different column blocks, so the stream pays one
+// fp64 RED per edge for it, and such rows are most of the rows (their accumulators decide how many bands are needed).
+// Rows of in-degree < kSweepTailDegree are gathered by k_spmv_low instead, on graphs of at least kSweepTailMinEdges edges.
+// A kSegThreshold value.  Measured on an H100 80GB HBM3 at 700 W, RMAT-24 PageRank step: 86.3 ms without a tail, 78.8 / 73.4
+// / 72.7 / 74.5 ms with bounds 4 / 8 / 16 / 32 (DESIGN.md §3.2); from 8 on the stream needs one band.
+constexpr int kSweepTailDegree         = 16;
+constexpr long long kSweepTailMinEdges = 1ll << 24;
 
 constexpr int kNumKinds = 11;  // S, Q, H, F1..F8
 constexpr int kKindS = 0, kKindQ = 1, kKindH = 2, kKindF1 = 3;
@@ -75,7 +85,8 @@ struct sweep_layout_t {
   int W{0};               // source columns per block (= slice elements - kHotZeroPad)
   int B{0};               // blocks
   int32_t n_cov{0};       // rows [0, n_cov) are covered = every non-empty row (rows are degree-descending)
-  int64_t nnz{0};
+  int32_t n_str{0};       // rows [0, n_str) are in the piece stream (a degree-bin bound <= n_cov); [n_str, n_cov) is the tail
+  int64_t nnz{0};         // edges of the graph (the stream holds the first offsets[n_str] of them)
   bool bank_order{false};  // entries inside the F slots ordered by shared-memory bank (4-byte values)
   int64_t n_steprows{0};
   int64_t n_rowslots{0};
@@ -92,7 +103,7 @@ struct sweep_layout_t {
   int32_t n_phases{0};
   int n_cta{0};
   int n_bands{1};
-  std::vector<int32_t> band_row;    // n_bands + 1: band b holds rows [band_row[b], band_row[b+1]); band_row[n_bands] = n_cov
+  std::vector<int32_t> band_row;    // n_bands + 1: band b holds rows [band_row[b], band_row[b+1]); band_row[n_bands] = n_str
   std::vector<int32_t> band_phase;  // n_bands + 1: the phases of band b are [band_phase[b], band_phase[b+1])
 };
 

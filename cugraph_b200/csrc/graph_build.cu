@@ -1318,17 +1318,30 @@ k_sweep_fill(sweep_chunk_t const* __restrict__ chunks, sweep_fill_t const* __res
 
 // Row bands: the sweep's fp64 REDs into acc[row] hit the L2 only while the rows they scatter over fit in it (measured on an
 // H100 80GB HBM3 at 700 W, 50 MB of L2: a scattered RED.64 costs the same up to 24 MB of accumulators, 1.3x at 48 MB and
-// 3.7x at 64 MB), so the covered rows are split into bands whose accumulators take at most kBandL2Share of the L2.  Half
-// gave the fastest RMAT-24 sweep (3 bands, DESIGN.md §3.2); more bands add launch tails and slice loads.
+// 3.7x at 64 MB), so the stream rows are split into bands whose accumulators take at most kBandL2Share of the L2.  Half
+// gave the fastest RMAT-24 sweep without a tail (3 bands, DESIGN.md §3.2); more bands add launch tails and slice loads.
 // CUGRAPH_B200_SWEEP_BANDS forces a count (tests, A/B runs).
 constexpr double kBandL2Share = 0.5;
 
-int sweep_bands(handle_impl const& h, int32_t n_cov)
+int sweep_bands(handle_impl const& h, int32_t n_str)
 {
-  const int most = std::max(1, (int)(((int64_t)n_cov + kBandRowAlign - 1) / kBandRowAlign));
+  const int most = std::max(1, (int)(((int64_t)n_str + kBandRowAlign - 1) / kBandRowAlign));
   int P          = h.tune.sweep_bands;
-  if (P <= 0) P = h.l2_bytes ? (int)std::ceil(8.0 * n_cov / (kBandL2Share * (double)h.l2_bytes)) : 1;
+  if (P <= 0) P = h.l2_bytes ? (int)std::ceil(8.0 * n_str / (kBandL2Share * (double)h.l2_bytes)) : 1;
   return std::min(std::max(P, 1), most);
+}
+
+// The piece stream holds the rows [0, seg[k]) for the bin k this returns: rows of in-degree >= kSegThreshold[k].
+// By default the rows of in-degree < kSweepTailDegree leave it on graphs of at least kSweepTailMinEdges edges, and it holds
+// every non-empty row on smaller ones.  CUGRAPH_B200_SWEEP_TAIL_DEGREE forces a bound on any graph (tests, A/B runs):
+// 1 = no tail, other values are rounded down to a bin threshold.
+int sweep_stream_bin(handle_impl const& h, csx_t const& c)
+{
+  int bound = h.tune.sweep_tail_degree;
+  if (bound <= 0) bound = c.nnz >= kSweepTailMinEdges ? kSweepTailDegree : 1;
+  int k = 0;
+  while (kSegThreshold[k] > bound) ++k;  // kSegThreshold[kNumSeg - 2] = 1
+  return k;
 }
 
 template <typename O>
@@ -1337,22 +1350,30 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   phase_trace tr(h);
   const int W         = (int)(kHotSliceBytes / es) - kHotZeroPad;  // columns per block; the pad holds zeros
   const int32_t n_cov = c.seg[kNumSeg - 2];                         // rows of degree >= 1
+  const int32_t n_str = c.seg[sweep_stream_bin(h, c)];              // rows of the stream; the tail is swept by k_spmv_low
+  if (n_str <= 0) return nullptr;                                   // no row reaches the bound: the plain sweep fits better
   const int B         = (int)(((int64_t)nv + W - 1) / W);
-  const int64_t nnz   = c.nnz;
+  int64_t nnz = 0;  // edges of the stream rows: a prefix of indices (rows are degree-descending)
+  {
+    O off_str;
+    CUDA_TRY(cudaMemcpyAsync(&off_str, c.offsets.as<O>() + n_str, sizeof(O), cudaMemcpyDeviceToHost, h.stream));
+    sync(h);
+    nnz = (int64_t)off_str;
+  }
   auto L              = std::make_unique<sweep_layout_t>();
-  L->W = W; L->B = B; L->n_cov = n_cov; L->nnz = nnz;
+  L->W = W; L->B = B; L->n_cov = n_cov; L->n_str = n_str; L->nnz = c.nnz;
   int32_t const* idx = c.indices.as<int32_t>();
   // equal bands of whole kBandRowAlign spans; rounding may leave fewer than asked for
-  const int asked         = sweep_bands(h, n_cov);
-  const int32_t band_rows = (int32_t)((((int64_t)n_cov + asked - 1) / asked + kBandRowAlign - 1) / kBandRowAlign * kBandRowAlign);
-  const int n_bands       = (int)(((int64_t)n_cov + band_rows - 1) / band_rows);
+  const int asked         = sweep_bands(h, n_str);
+  const int32_t band_rows = (int32_t)((((int64_t)n_str + asked - 1) / asked + kBandRowAlign - 1) / kBandRowAlign * kBandRowAlign);
+  const int n_bands       = (int)(((int64_t)n_str + band_rows - 1) / band_rows);
   L->n_bands              = n_bands;
-  for (int b = 0; b <= n_bands; ++b) L->band_row.push_back((int32_t)std::min<int64_t>((int64_t)b * band_rows, n_cov));
+  for (int b = 0; b <= n_bands; ++b) L->band_row.push_back((int32_t)std::min<int64_t>((int64_t)b * band_rows, n_str));
 
   // 1. segment heads
   dbuf flag = make_dbuf<uint8_t>(nnz, h.stream);
   CUDA_TRY(cudaMemsetAsync(flag.data(), 0, nnz, h.stream));
-  B200_LAUNCH(h, (k_hot_row_starts<O>), grid_for(n_cov), kBlock, 0, c.offsets.as<O>(), n_cov, flag.as<uint8_t>());
+  B200_LAUNCH(h, (k_hot_row_starts<O>), grid_for(n_str), kBlock, 0, c.offsets.as<O>(), n_str, flag.as<uint8_t>());
   B200_LAUNCH(h, k_hot_heads, std::min(grid_for(nnz, 4), h.sm_count * 32), kBlock, 0, idx, (long long)nnz, W, flag.as<uint8_t>());
   dbuf head_pos = make_dbuf<int32_t>(nnz, h.stream);
   int64_t n_segs64;
@@ -1376,7 +1397,7 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   dbuf seg_row = make_dbuf<int32_t>(n_segs, h.stream), seg_pieces = make_dbuf<int32_t>((size_t)n_segs + 1, h.stream);
   dbuf piece_off = make_dbuf<int32_t>((size_t)n_segs + 1, h.stream);
   B200_LAUNCH(h, (k_hot_segment_info<O>), grid_for((int64_t)n_segs + 1), kBlock, 0, head_pos.as<int32_t>(), n_segs,
-              (long long)nnz, c.offsets.as<O>(), n_cov, seg_row.as<int32_t>(), seg_pieces.as<int32_t>());
+              (long long)nnz, c.offsets.as<O>(), n_str, seg_row.as<int32_t>(), seg_pieces.as<int32_t>());
   exclusive_scan_i32(h, seg_pieces.as<int32_t>(), piece_off.as<int32_t>(), (int64_t)n_segs + 1);
   int32_t n_pieces = 0;
   CUDA_TRY(cudaMemcpyAsync(&n_pieces, piece_off.as<int32_t>() + n_segs, sizeof(int32_t), cudaMemcpyDeviceToHost, h.stream));
@@ -1412,8 +1433,8 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   tr.mark("sweep layout: kind sort");
   if (tr.on) {  // layout statistics: pieces by kind, per range of blocks
     int edges[] = {0, 1, 4, 16, 64, 160, B};
-    std::fprintf(stderr, "[sweep] B=%d W=%d rows=%d nnz=%lld segments=%d pieces=%d bands=%d of %d rows\n", B, W, n_cov,
-                 (long long)nnz, n_segs, n_pieces, n_bands, band_rows);
+    std::fprintf(stderr, "[sweep] B=%d W=%d rows=%d (tail %d rows, %lld edges) nnz=%lld segments=%d pieces=%d bands=%d of %d rows\n",
+                 B, W, n_str, n_cov - n_str, (long long)(c.nnz - nnz), (long long)nnz, n_segs, n_pieces, n_bands, band_rows);
     for (int k = 0; k + 1 < 7; ++k) {
       const int b0 = std::min(edges[k], B), b1 = std::min(edges[k + 1], B);
       if (b1 <= b0) continue;

@@ -22,6 +22,8 @@
 //     first.  k_sweep_finish turns acc into y, clears it and resets the cursors.
 //   * the rows are split into bands whose accumulators fit in the L2 (graph.cuh); the sweep runs band by band, k_sweep over
 //     the band's phases, then k_sweep_finish over its rows while their accumulators are still in the L2.
+//   * on large graphs the rows of small in-degree (the tail, graph.cuh) are not in the stream: one k_spmv_low launch after
+//     the bands gathers their few edges from x directly (no RED, and fewer stream rows need fewer bands).
 #pragma once
 #include "spmv.cuh"
 
@@ -595,8 +597,8 @@ __global__ void __launch_bounds__(kSweepThreads, 1) k_sweep(sweep_args_t<T> a)
   }
 }
 
-// y[row] = acc * alpha + init for the rows [row_lo, n_rows): acc for the covered ones (< n_cov), init for the empty rows behind
-// them; clears their accumulators and the n_phases cursors.  row_lo is a multiple of kBandRowAlign.  A warp handles 256 consecutive rows in four steps of 64: every step is one 512-byte load + one 512-byte store of
+// y[row] = acc * alpha + init for the rows [row_lo, n_rows): acc for the stream rows (< n_cov, the caller passes n_str), init
+// for the empty rows behind them; clears their accumulators and the n_phases cursors.  row_lo is a multiple of kBandRowAlign.  A warp handles 256 consecutive rows in four steps of 64: every step is one 512-byte load + one 512-byte store of
 // accumulators and one 256-byte store of y per warp (lane = two rows), all four loads issued before the first use.
 // (Eight CONSECUTIVE rows per thread looked the same on paper and ran at 2.3 TB/s: every warp-wide 128-bit access then
 // touched sixteen 128-byte lines for a quarter of their bytes.)
@@ -663,11 +665,13 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
   // covered_rows_only: y of the rows without edges already holds their (unvarying) value — multi-GPU blocks, where more than
   // half of the row slots are empty and the unvarying term is 0 (mg.cu)
   const int32_t finish_rows = covered_rows_only ? L.n_cov : c.n_rows;
+  const bool tail           = L.n_str < L.n_cov;  // rows of small in-degree left the stream (graph.cuh)
   // band by band: the band's rows are finished while its accumulators are in the L2, before the next band's REDs evict them.
-  // y must not overlap x: a band's finish writes y while later bands still read x.
+  // y must not overlap x: a band's finish writes y while later bands (and the tail) still read x.
   for (int band = 0; band < L.n_bands; ++band) {
+    // the last band also writes the empty rows, unless the tail launch does
+    const int row_hi = band < L.n_bands - 1 ? L.band_row[band + 1] : (tail ? L.n_str : finish_rows);
     const int row_lo = L.band_row[band];
-    const int row_hi = band == L.n_bands - 1 ? finish_rows : L.band_row[band + 1];  // the last band also writes the empty rows
     a.cta_phase      = L.cta_phase.as<int32_t>() + (size_t)band * L.n_cta;
     a.ph_lo          = L.band_phase[band];
     a.ph_hi          = L.band_phase[band + 1];
@@ -675,8 +679,21 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
     else B200_LAUNCH(h, (k_sweep<T, false>), L.n_cta, kSweepThreads, kSweepDynSmem, a);
     const int n_ph = a.ph_hi - a.ph_lo;
     const int n    = std::max((row_hi - row_lo + 2 * kFinishSteps - 1) / (2 * kFinishSteps), n_ph);  // threads: 16 rows each
-    B200_LAUNCH(h, (k_sweep_finish<T, kFinishSteps>), (std::max(n, 1) + 255) / 256, 256, 0, acc, row_lo, L.n_cov, row_hi, y,
+    B200_LAUNCH(h, (k_sweep_finish<T, kFinishSteps>), (std::max(n, 1) + 255) / 256, 256, 0, acc, row_lo, L.n_str, row_hi, y,
                 c.row_vertex.as<int32_t>(), alpha, L.cursor.as<int>() + a.ph_lo, n_ph, st);
+  }
+  if (tail) {  // the rows [n_str, n_cov) and (unless covered_rows_only) the empty rows, by k_spmv_low
+    int first = 0;  // n_str is a bin bound: the tail starts at the first bin that begins there
+    while (c.seg[first] < L.n_str) ++first;
+    const low_bins_t bins = make_low_bins(c, first, !covered_rows_only);
+    const int blocks      = bins.block_begin[kNumSeg - 1];
+    T const* w            = weighted ? c.weights.as<T>() : nullptr;
+    if (weighted)
+      B200_LAUNCH(h, (k_spmv_low<int32_t, T, true>), blocks, 256, 0, c.offsets.as<int32_t>(), c.indices.as<int32_t>(), w, x, y,
+                  c.row_vertex.as<int32_t>(), bins, alpha, st);
+    else
+      B200_LAUNCH(h, (k_spmv_low<int32_t, T, false>), blocks, 256, 0, c.offsets.as<int32_t>(), c.indices.as<int32_t>(), w, x, y,
+                  c.row_vertex.as<int32_t>(), bins, alpha, st);
   }
 }
 

@@ -72,6 +72,14 @@ EMU_EXPORT int emu_sweep_bands(cugraph_graph_t* graph, size_t es, int* n_cta, in
   return L->n_bands;
 }
 
+// rows [0, n_str) of that piece stream are in it, the non-empty rows behind them are its tail; -1 without a layout
+EMU_EXPORT int32_t emu_sweep_stream_rows(cugraph_graph_t* graph, size_t es)
+{
+  auto* g                 = reinterpret_cast<graph_impl*>(graph);
+  sweep_layout_t const* L = (es == 4 ? g->primary->hot4 : g->primary->hot8).get();
+  return L ? L->n_str : -1;
+}
+
 EMU_EXPORT size_t emu_padded_x_elems(int32_t nv, size_t es) { return padded_x_elems(nv, es); }
 
 // forget the cached layouts of the primary orientation (so that another set of knobs can be staged)
