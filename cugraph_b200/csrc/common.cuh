@@ -112,6 +112,8 @@ struct tuning_t {
   int sssp_split_rounds{1};                // CUGRAPH_B200_SSSP_SPLIT_ROUNDS
   unsigned long long sssp_split_min_edges{1ull << 20};  // CUGRAPH_B200_SSSP_SPLIT_MIN_EDGES
   unsigned long long advance_split_edges{1ull << 31};  // CUGRAPH_B200_ADVANCE_SPLIT_EDGES: frontiers with this many edges are advanced in halves (tests lower it)
+  long long offs64_min_edges{1ll << 31};  // CUGRAPH_B200_OFFS64_MIN_EDGES: a csx with this many edges stores 64-bit offsets, in [0, 2^31]
+                                          // (tests: 0; lazily built views follow the handle passed to the algorithm)
   bool bfs_trace{false}, sssp_trace{false}, build_trace{false};  // CUGRAPH_B200_{BFS,SSSP,BUILD}_TRACE
   static tuning_t from_env()
   {
@@ -130,6 +132,7 @@ struct tuning_t {
     if (auto e = get("CUGRAPH_B200_SSSP_SPLIT_ROUNDS")) t.sssp_split_rounds = std::max(1, std::atoi(e));
     if (auto e = get("CUGRAPH_B200_SSSP_SPLIT_MIN_EDGES")) t.sssp_split_min_edges = std::strtoull(e, nullptr, 10);
     if (auto e = get("CUGRAPH_B200_ADVANCE_SPLIT_EDGES")) t.advance_split_edges = std::min<unsigned long long>(std::max<unsigned long long>(std::strtoull(e, nullptr, 10), 2ull), 1ull << 31);
+    if (auto e = get("CUGRAPH_B200_OFFS64_MIN_EDGES")) t.offs64_min_edges = std::min(std::max(std::atoll(e), 0ll), 1ll << 31);
     t.bfs_trace   = get("CUGRAPH_B200_BFS_TRACE") != nullptr;
     t.sssp_trace  = get("CUGRAPH_B200_SSSP_TRACE") != nullptr;
     t.build_trace = get("CUGRAPH_B200_BUILD_TRACE") != nullptr;

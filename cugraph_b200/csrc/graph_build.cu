@@ -467,7 +467,7 @@ void build_csx_typed(handle_impl const& h, csx_t& out, int32_t const* major, int
   }
   out.n_rows  = nv;
   out.nnz     = m;
-  out.offs64  = m >= (1ll << 31);
+  out.offs64  = m >= h.tune.offs64_min_edges;
   out.indices = make_dbuf<int32_t>(m, h.stream);
   B200_LAUNCH(h, k_indices, grid_for(m, 4), kBlock, 0, keys2.as<uint64_t>(), m, bits, out.indices.as<int32_t>());
   if (out.offs64) {

@@ -88,12 +88,11 @@ def primary(L, g):
     ptrs = (C.c_void_p * 5)()
     assert L.emu_graph_primary(g, ints, seg, ptrs) == 0
     n_rows, nnz, offs64, nnz_hi, nv, weighted, wsize = [int(x) for x in ints[:7]]
-    assert not offs64
-    off = as_np(ptrs[0], n_rows + 1, np.int32)
+    off = as_np(ptrs[0], n_rows + 1, np.int64 if offs64 else np.int32)
     idx = as_np(ptrs[1], nnz, np.int32)
-    w = as_np(ptrs[2], nnz, np.float32) if weighted else None
+    w = as_np(ptrs[2], nnz, np.float32 if wsize == 4 else np.float64) if weighted else None
     ext = as_np(ptrs[3], nv, np.int32)
-    return dict(n_rows=n_rows, nnz=nnz, nnz_hi=nnz_hi, nv=nv, off=off, idx=idx, w=w, ext=ext, seg=list(seg))
+    return dict(n_rows=n_rows, nnz=nnz, nnz_hi=nnz_hi, nv=nv, off=off, idx=idx, w=w, ext=ext, seg=list(seg), offs64=bool(offs64))
 
 
 def check_csr(P, src, dst, w):

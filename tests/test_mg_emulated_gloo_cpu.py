@@ -41,10 +41,12 @@ def _graph(V, E, seed):
     return ids, s_all, d_all
 
 
-def _worker(rank, world, port, V, E, min_edges, out_q):
+def _worker(rank, world, port, V, E, min_edges, offs64_min_edges, out_q):
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
     os.environ["CUGRAPH_B200_SWEEP_MIN_EDGES"] = min_edges
+    if offs64_min_edges is not None:
+        os.environ["CUGRAPH_B200_OFFS64_MIN_EDGES"] = offs64_min_edges
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from tests.emu_py import emulated_python_surface
     with emulated_python_surface():
@@ -67,14 +69,16 @@ def _worker(rank, world, port, V, E, min_edges, out_q):
     dist.destroy_process_group()
 
 
-@pytest.mark.parametrize("world,min_edges", [(2, "0"), (4, "1000000000"), (8, "0")])   # grids 2x1, 2x2, 4x2
-def test_mg_pagerank_and_bfs_emulated_gloo(world, min_edges):
+# grids 2x1, 2x2, 4x2; the last case gives every block 64-bit offsets (the int64_t block sweep and block BFS)
+@pytest.mark.parametrize("world,min_edges,offs64_min_edges", [(2, "0", None), (4, "1000000000", None), (8, "0", None), (2, "0", "0")],
+                         ids=["2-0", "4-1000000000", "8-0", "2-0-offs64"])
+def test_mg_pagerank_and_bfs_emulated_gloo(world, min_edges, offs64_min_edges):
     import oracle
     V, E = 1500, 12000
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, V, E, min_edges, q)) for r in range(world)]
+    procs = [ctx.Process(target=_worker, args=(r, world, port, V, E, min_edges, offs64_min_edges, q)) for r in range(world)]
     for p in procs:
         p.start()
     res, source = q.get(timeout=600)
