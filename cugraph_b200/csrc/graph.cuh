@@ -195,6 +195,8 @@ dbuf collect_vertex_values(handle_impl const& h, graph_impl const& g,
 
 std::unique_ptr<csx_t> build_binned_rows(handle_impl const& h, int32_t const* major, int32_t const* minor, void const* w,
                                          cugraph_data_type_id_t wtype, int64_t n, int32_t nv);
+// the vertex (row_vertex, or the physical row) of every edge of a csx, in edge order
+dbuf expand_majors(handle_impl const& h, csx_t const& c);
 
 // ---- multi-GPU hooks (mg.cu) ----
 struct mg_pr_args {

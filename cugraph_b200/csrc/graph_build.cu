@@ -550,6 +550,8 @@ void finish_binning(handle_impl const& h, csx_t& c)
   if (c.offs64) finish_binning_typed<int64_t>(h, c); else finish_binning_typed<int32_t>(h, c);
 }
 
+}  // namespace
+
 // expand a csx back into (vertex-of-row per edge)
 dbuf expand_majors(handle_impl const& h, csx_t const& c)
 {
@@ -563,6 +565,8 @@ dbuf expand_majors(handle_impl const& h, csx_t const& c)
                 c.row_vertex.as<int32_t>(), maj.as<int32_t>());
   return maj;
 }
+
+namespace {
 
 struct staged_ids {
   int32_t nv{0};

@@ -6,16 +6,33 @@
 // torch.distributed (NCCL on NVLink 5 / NVSwitch).  This file provides the device-side pieces behind
 // the C ABI: a resource handle bound to the caller's CUDA stream, rectangular edge blocks with the
 // same binned / column-blocked layout as the single-GPU graph, the block pull sweep and the fused
-// per-iteration vertex step.  All calls only ENQUEUE work on the handle's stream.
+// per-iteration vertex step, the BFS pull step and the SSSP push relaxation.  All calls only ENQUEUE work on the handle's
+// stream (the SSSP calls read back one queue size).
+#include "advance.cuh"
 #include "sweep.cuh"
 
 #include <algorithm>
+#include <climits>
+#include <cmath>
+#include <limits>
 
 namespace b200 {
 
+// the column-major copy of a block for multi-GPU SSSP (built by the first relaxation call on the block): physical rows are
+// the block's column slots in descending out-degree (row_vertex = column slot), neighbours are row slots
+struct block_push_t {
+  std::unique_ptr<csx_t> csx;
+  int32_t n_ne{0};     // physical rows with at least one edge (a prefix)
+  dbuf queue, q_deg;   // active physical rows and their degrees (q_deg has one element more: advance() reads n + 1)
+  dbuf counts;         // block_queue_counts_t
+  advance_scratch_t adv;
+};
+
 struct block_impl {
   std::unique_ptr<csx_t> csx;
+  std::unique_ptr<block_push_t> push;  // lazily built (multi-GPU SSSP only)
   int32_t n_rows{0}, n_cols{0}, n_span{0};
+  bool weighted{false};
   cugraph_data_type_id_t wtype{FLOAT32};
   dbuf acc_hi;
   dbuf state;  // pr_state_t with init = 0, done = 0
@@ -144,6 +161,151 @@ void block_bfs_pull(handle_impl const& h, csx_t const& c, uint8_t const* frontie
                 c.indices.as<int32_t>(), c.row_vertex.as<int32_t>(), n_hi, n_ne, frontier, visited, maxpart, grid_cols, grid_c, cand);
 }
 
+// ---- one relaxation round of multi-GPU SSSP on this GPU's edge block, push direction (the MG form of the SSSP rounds of
+// traverse.cu; reference: the multi_gpu branches of sssp_impl.cuh:301-375, whose frontier arrives through
+// update_edge_src_property).  The launcher gathers the distances of the frontier sources over the block's column slots
+// (+inf = not in the frontier); the block's column-major copy (block_push_t) turns the active columns into a queue of its
+// physical rows, and the same merge-path advance as on one GPU (advance.cuh) relaxes their edges into one INT64 key per row
+// slot, reduced to the owners by a MIN reduce-scatter.
+struct block_queue_counts_t {
+  int n;                     // active physical rows appended to the queue
+  int pad;
+  unsigned long long edges;  // their degree sum
+};
+
+// physical rows r < n_ne of the push copy whose column slot row_vertex[r] holds a finite distance, with their degrees
+template <typename O, typename T>
+__global__ void __launch_bounds__(kBlock)
+k_block_active_rows(O const* __restrict__ off, int32_t const* __restrict__ row_vertex, int32_t n_ne, T const* __restrict__ dist_cols,
+                    int32_t* __restrict__ q, int32_t* __restrict__ q_deg, block_queue_counts_t* __restrict__ cnt)
+{
+  unsigned long long edges = 0;
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < n_ne; r += gridDim.x * blockDim.x) {
+    if (dist_cols[row_vertex[r]] < (T)INFINITY) {
+      const int32_t d = (int32_t)((long long)off[r + 1] - (long long)off[r]);
+      const int pos   = warp_append(&cnt->n);
+      q[pos]          = r;
+      q_deg[pos]      = d;
+      edges += (unsigned long long)d;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) edges += __shfl_xor_sync(0xffffffffu, edges, o);
+  if ((threadIdx.x & 31) == 0 && edges) atomicAdd(&cnt->edges, edges);
+}
+
+// the global code of a column slot, as in the BFS pull kernels
+__device__ __forceinline__ long long column_code(int col, long long maxpart, int grid_cols, int grid_c)
+{
+  return ((long long)(col / maxpart) * grid_cols + grid_c) * maxpart + (col % maxpart);
+}
+
+// one key orders the proposals to a row: float (distance bits, code) — the smallest distance, among equal distances the
+// smallest code; double: the distance bits alone (non-negative doubles order like their int64 bit patterns)
+__device__ __forceinline__ long long sssp_key(float nd, long long code)
+{
+  return (long long)(((unsigned long long)__float_as_uint(nd) << 32) | (unsigned long long)code);
+}
+__device__ __forceinline__ long long sssp_key(double nd, long long) { return __double_as_longlong(nd); }
+
+template <typename T>
+struct block_relax_op {
+  int32_t const* col_of;  // column slot of a physical row of the push copy
+  T const* w;
+  T const* dist;          // over column slots, +inf = not in the frontier
+  T cutoff;
+  long long maxpart;
+  int grid_cols, grid_c;
+  long long* cand;        // over row slots
+  __device__ __forceinline__ void edge(int src, long long e, int nbr) const
+  {
+    const int col = col_of[src];
+    const T nd    = dist[col] + w[e];
+    if (!(nd < cutoff)) return;
+    const long long key = sssp_key(nd, column_code(col, maxpart, grid_cols, grid_c));
+    if (key < cand[nbr]) atomicMin(cand + nbr, key);  // a stale read is larger than the current value: never skips a win
+  }
+};
+
+// the smallest code among the frontier columns whose sum reproduces the distance a row accepted (double runs)
+template <typename T>
+struct block_pred_op {
+  int32_t const* col_of;
+  T const* w;
+  T const* dist;
+  T const* win;           // over row slots, +inf = not asked
+  long long maxpart;
+  int grid_cols, grid_c;
+  long long* code;        // over row slots
+  __device__ __forceinline__ void edge(int src, long long e, int nbr) const
+  {
+    const T want = win[nbr];
+    if (!(want < (T)INFINITY)) return;
+    const int col = col_of[src];
+    if (dist[col] + w[e] != want) return;
+    const long long k = column_code(col, maxpart, grid_cols, grid_c);
+    if (k < code[nbr]) atomicMin(code + nbr, k);
+  }
+};
+
+// the column-major copy of the block, built on first use (the mirror image of pull_view / out_sweep_view, graph_build.cu)
+block_push_t& push_copy(handle_impl const& h, block_impl& b)
+{
+  if (!b.push) {
+    auto p         = std::make_unique<block_push_t>();
+    csx_t const& c = *b.csx;
+    dbuf maj       = expand_majors(h, c);  // row slot of every edge
+    p->csx = build_binned_rows(h, c.indices.as<int32_t>(), maj.as<int32_t>(), b.weighted ? c.weights.data() : nullptr, b.wtype,
+                               c.nnz, b.n_span);
+    csx_t const& pc = *p->csx;
+    p->n_ne         = pc.degree_sorted ? pc.seg[kNumSeg - 2] : pc.n_rows;
+    p->queue        = make_dbuf<int32_t>((size_t)std::max(pc.n_rows, 1), h.stream);
+    p->q_deg        = make_dbuf<int32_t>((size_t)pc.n_rows + 1, h.stream);
+    p->counts       = make_dbuf<block_queue_counts_t>(1, h.stream);
+    p->adv.init(h, pc.n_rows, pc.nnz);
+    sync(h);
+    b.push = std::move(p);
+  }
+  return *b.push;
+}
+
+// active rows -> queue (one read-back of its size and edge count) -> advance with `op`
+template <typename O, typename T, typename Op>
+void block_push_round(handle_impl const& h, block_push_t& p, T const* dist_cols, Op op)
+{
+  csx_t const& pc = *p.csx;
+  auto* cnt       = p.counts.as<block_queue_counts_t>();
+  CUDA_TRY(cudaMemsetAsync(cnt, 0, sizeof(block_queue_counts_t), h.stream));
+  if (p.n_ne > 0)
+    B200_LAUNCH(h, (k_block_active_rows<O, T>), std::min((p.n_ne + kBlock - 1) / kBlock, h.sm_count * 8), kBlock, 0,
+                pc.offsets.as<O>(), pc.row_vertex.as<int32_t>(), p.n_ne, dist_cols, p.queue.as<int32_t>(), p.q_deg.as<int32_t>(),
+                cnt);
+  block_queue_counts_t hc{};
+  CUDA_TRY(cudaMemcpyAsync(&hc, cnt, sizeof(hc), cudaMemcpyDeviceToHost, h.stream));
+  sync(h);
+  advance<O>(h, p.adv, pc.offsets.as<O>(), pc.indices.as<int32_t>(), p.queue.as<int32_t>(), hc.n, hc.edges, op,
+             p.q_deg.as<int32_t>());
+}
+
+template <typename T>
+T rounded_cutoff(double cutoff)  // as cugraph_sssp rounds it (traverse.cu, sssp_windows)
+{
+  const T unreached = std::numeric_limits<T>::max();
+  return cutoff >= (double)unreached ? unreached : (T)cutoff;
+}
+
+// argument checks shared by the two SSSP block calls; `dv` over column slots, `out` (INT64) over row slots
+void check_sssp_block_args(block_impl const& b, device_array_view_impl const* dv, device_array_view_impl const* out, size_t maxpart,
+                           int grid_cols, int grid_c)
+{
+  B200_EXPECTS(b.weighted, CUGRAPH_INVALID_INPUT, "SSSP requires a weighted block");
+  B200_EXPECTS(dv->type == b.wtype, CUGRAPH_INVALID_INPUT, "dist_cols dtype must match the block's weights");
+  B200_EXPECTS(out->type == INT64, CUGRAPH_INVALID_INPUT, "cand_rows / code_rows must be INT64");
+  B200_EXPECTS(dv->size >= (size_t)b.n_cols && out->size >= (size_t)b.n_rows, CUGRAPH_INVALID_INPUT,
+               "distance / candidate arrays shorter than the block's slots");
+  B200_EXPECTS(maxpart > 0 && grid_cols > 0 && grid_c >= 0 && grid_c < grid_cols, CUGRAPH_INVALID_INPUT, "bad grid position");
+}
+
 }  // namespace
 
 void attach_comm(handle_impl*, void*)
@@ -218,6 +380,7 @@ cugraph_error_code_t cugraph_b200_block_create(const cugraph_resource_handle_t* 
     b->n_cols  = (int32_t)n_cols;
     b->n_span  = (int32_t)std::max(n_rows, n_cols);
     b->wtype   = w ? w->type : FLOAT32;
+    b->weighted = w != nullptr;
     b->csx     = build_binned_rows(h, (int32_t const*)r->data, (int32_t const*)c->data, w ? w->data : nullptr, b->wtype,
                                    (int64_t)r->size, b->n_span);
     b->acc_hi  = make_dbuf<double>(acc_rows(*b->csx), h.stream);
@@ -337,6 +500,79 @@ cugraph_error_code_t cugraph_b200_block_bfs_pull(const cugraph_resource_handle_t
       block_bfs_pull<int32_t>(h, c, (uint8_t const*)fv->data, (uint8_t const*)vv->data, (long long)maxpart, grid_cols, grid_c,
                               (long long*)cv->data, b->n_rows);
     check_last("block_bfs_pull");
+  });
+}
+
+// cand_rows[row slot] = min key over the proposals dist_cols[col] + w < cutoff of the active columns, else INT64_MAX
+cugraph_error_code_t cugraph_b200_block_sssp_relax(const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+                                                   const cugraph_type_erased_device_array_view_t* dist_cols, double cutoff,
+                                                   size_t maxpart, int grid_cols, int grid_c,
+                                                   cugraph_type_erased_device_array_view_t* cand_rows, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(block && dist_cols && cand_rows, CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto* b        = reinterpret_cast<block_impl*>(block);
+    auto const* dv = V(dist_cols);
+    auto const* cv = V(cand_rows);
+    check_sssp_block_args(*b, dv, cv, maxpart, grid_cols, grid_c);
+    if (b->wtype == FLOAT32) {  // the code takes the low 32 bits of the key
+      const unsigned long long parts = (((unsigned long long)b->n_cols + maxpart - 1) / maxpart) * (unsigned long long)grid_cols;
+      B200_EXPECTS(maxpart < (1ull << 32) && parts <= ((1ull << 32) - 1) / maxpart, CUGRAPH_INVALID_INPUT,
+                   "FLOAT32 SSSP keys need R * grid_cols * maxpart < 2^32");
+    }
+    block_push_t& p = push_copy(h, *b);
+    auto* cand      = (long long*)cv->data;
+    B200_LAUNCH(h, k_fill_i64, std::min((b->n_rows + 255) / 256 + 1, h.sm_count * 8), 256, 0, cand, (long long)b->n_rows, LLONG_MAX);
+    int32_t const* col_of = p.csx->row_vertex.as<int32_t>();
+    if (b->wtype == FLOAT32) {
+      block_relax_op<float> op{col_of, p.csx->weights.as<float>(), (float const*)dv->data, rounded_cutoff<float>(cutoff),
+                               (long long)maxpart, grid_cols, grid_c, cand};
+      if (p.csx->offs64) block_push_round<int64_t>(h, p, (float const*)dv->data, op);
+      else block_push_round<int32_t>(h, p, (float const*)dv->data, op);
+    } else {
+      block_relax_op<double> op{col_of, p.csx->weights.as<double>(), (double const*)dv->data, rounded_cutoff<double>(cutoff),
+                                (long long)maxpart, grid_cols, grid_c, cand};
+      if (p.csx->offs64) block_push_round<int64_t>(h, p, (double const*)dv->data, op);
+      else block_push_round<int32_t>(h, p, (double const*)dv->data, op);
+    }
+    check_last("block_sssp_relax");
+  });
+}
+
+// code_rows[row slot] = smallest code of an active column with dist_cols[col] + w == win_rows[row], else INT64_MAX
+cugraph_error_code_t cugraph_b200_block_sssp_pred(const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+                                                  const cugraph_type_erased_device_array_view_t* dist_cols,
+                                                  const cugraph_type_erased_device_array_view_t* win_rows, size_t maxpart,
+                                                  int grid_cols, int grid_c, cugraph_type_erased_device_array_view_t* code_rows,
+                                                  cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(block && dist_cols && win_rows && code_rows, CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto* b        = reinterpret_cast<block_impl*>(block);
+    auto const* dv = V(dist_cols);
+    auto const* wv = V(win_rows);
+    auto const* cv = V(code_rows);
+    check_sssp_block_args(*b, dv, cv, maxpart, grid_cols, grid_c);
+    B200_EXPECTS(wv->type == b->wtype, CUGRAPH_INVALID_INPUT, "win_rows dtype must match the block's weights");
+    B200_EXPECTS(wv->size >= (size_t)b->n_rows, CUGRAPH_INVALID_INPUT, "win_rows shorter than the block's row slots");
+    block_push_t& p = push_copy(h, *b);
+    auto* code      = (long long*)cv->data;
+    B200_LAUNCH(h, k_fill_i64, std::min((b->n_rows + 255) / 256 + 1, h.sm_count * 8), 256, 0, code, (long long)b->n_rows, LLONG_MAX);
+    int32_t const* col_of = p.csx->row_vertex.as<int32_t>();
+    if (b->wtype == FLOAT32) {
+      block_pred_op<float> op{col_of, p.csx->weights.as<float>(), (float const*)dv->data, (float const*)wv->data,
+                              (long long)maxpart, grid_cols, grid_c, code};
+      if (p.csx->offs64) block_push_round<int64_t>(h, p, (float const*)dv->data, op);
+      else block_push_round<int32_t>(h, p, (float const*)dv->data, op);
+    } else {
+      block_pred_op<double> op{col_of, p.csx->weights.as<double>(), (double const*)dv->data, (double const*)wv->data,
+                               (long long)maxpart, grid_cols, grid_c, code};
+      if (p.csx->offs64) block_push_round<int64_t>(h, p, (double const*)dv->data, op);
+      else block_push_round<int32_t>(h, p, (double const*)dv->data, op);
+    }
+    check_last("block_sssp_pred");
   });
 }
 

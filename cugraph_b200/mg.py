@@ -1,4 +1,4 @@
-"""Multi-GPU PageRank and BFS: 2D edge partition over one process per GPU (torch.distributed, NCCL on NVLink 5).
+"""Multi-GPU PageRank, BFS and SSSP: 2D edge partition over one process per GPU (torch.distributed, NCCL on NVLink 5).
 
 What the reference does (SURVEY.md §8e): P = R x C GPUs, vertex -> GPU by hash
 (cpp/include/cugraph/utilities/graph_partition_utils.cuh:30-43, 101-128), every GPU holds the edge
@@ -12,8 +12,12 @@ per iteration on equal-sized (padded) vertex partitions, the dangling / converge
 one 2-element all_reduce and never touch the host unless epsilon > 0, and the local sweep is the
 same column-blocked shared-memory kernel as on one GPU (C-ABI: cugraph_b200_block_*).
 
+BFS moves byte flags per level (one max-reduce-scatter of candidate predecessors); SSSP runs Δ-windows of rounds, each an
+all-gather of the frontier's distances, the block's push relaxation on the device and one min-reduce-scatter of INT64
+(distance, predecessor) keys (see MGGraph.sssp).
+
 `partition_edges` (pure torch, device agnostic: exercised on CPU with the gloo backend in
-tests/test_mg_partition_cpu.py) builds the blocks; `MGGraph` / `pagerank` need CUDA.
+tests/test_mg_partition_cpu.py) builds the blocks; `MGGraph` / `pagerank` / `bfs` / `sssp` need CUDA.
 """
 from __future__ import annotations
 
@@ -261,6 +265,10 @@ class MGGraph:
         reduce_scatter_into(ow, partial, g.col_group)
         self.out_w = ow.to(self.dtype)
         self.num_edges_local = int(p.rows.numel())
+        self.weighted = p.weights is not None
+        self._w_sum_local = float(ones.sum().item()) if self.weighted else 0.0   # SSSP's initial window width
+        self._sssp_avg = None                                                       # (average weight, average degree)
+        self.last_sssp_stats = None
         self.device = src.device
         p.rows = p.cols = p.weights = None  # the block owns its own copy
         torch.cuda.synchronize()
@@ -361,19 +369,11 @@ class MGGraph:
         visited = torch.zeros(mp, dtype=torch.uint8, device=dev)
         visited[p.n_local:] = 1                                  # padding slots never take part
         frontier = torch.zeros(mp, dtype=torch.uint8, device=dev)
-        owner = int(vertex_owner(torch.tensor([int(source)], dtype=torch.int64), g.world)[0])
-        found = torch.zeros(1, dtype=torch.int64, device=dev)
-        if owner == g.rank:
-            hit = (p.vertices == int(source)).nonzero()
-            if hit.numel():
-                lid = int(hit[0, 0])
-                dist_own[lid] = 0
-                visited[lid] = 1
-                frontier[lid] = 1
-                found += 1
-        dist.all_reduce(found)
-        if int(found.item()) == 0:
-            raise ValueError(f"bfs source {source} is not a vertex of the graph")
+        lid = self._source_lid(source, "bfs")
+        if lid >= 0:
+            dist_own[lid] = 0
+            visited[lid] = 1
+            frontier[lid] = 1
         f_cols = torch.zeros(self.n_cols, dtype=torch.uint8, device=dev)
         v_rows = torch.zeros(self.n_rows, dtype=torch.uint8, device=dev)
         cand = torch.full((self.n_rows,), -1, dtype=torch.int64, device=dev)
@@ -414,8 +414,30 @@ class MGGraph:
         d_out = dist_own[:p.n_local].clone()
         if not compute_predecessors:
             return verts, d_out, None
-        # predecessor codes (owner rank * maxpart + local id) -> external ids, answered by the owners
-        codes = pred_code[:p.n_local]
+        return verts, d_out, self._codes_to_external(pred_code[:p.n_local])
+
+    def _source_lid(self, source, what):
+        """local id of the external vertex `source` on this rank, -1 when another rank owns it; ValueError on every rank when
+        it is not a vertex (one all-reduce)"""
+        p, g = self.part, self.part.groups
+        owner = int(vertex_owner(torch.tensor([int(source)], dtype=torch.int64), g.world)[0])
+        found = torch.zeros(1, dtype=torch.int64, device=self.device)
+        lid = -1
+        if owner == g.rank:
+            hit = (p.vertices == int(source)).nonzero()
+            if hit.numel():
+                lid = int(hit[0, 0])
+                found += 1
+        dist.all_reduce(found)
+        if int(found.item()) == 0:
+            raise ValueError(f"{what} source {source} is not a vertex of the graph")
+        return lid
+
+    def _codes_to_external(self, codes):
+        """predecessor codes (owner rank * maxpart + local id, -1 = none) -> external ids, answered by the owners (one
+        all-to-all-v there and back)"""
+        p, g, dev, mp = self.part, self.part.groups, self.device, self.part.maxpart
+        verts = p.vertices
         has = codes >= 0
         ask = codes[has]
         (req,), order, sc, rc = exchange([ask % mp], torch.div(ask, mp, rounding_mode="floor"), g.world)
@@ -424,9 +446,156 @@ class MGGraph:
         dist.all_to_all_single(back, ans.contiguous(), output_split_sizes=sc, input_split_sizes=rc)
         got = torch.empty_like(back)
         got[order] = back
-        pred = torch.full((p.n_local,), -1, dtype=verts.dtype, device=dev)
+        pred = torch.full((codes.numel(),), -1, dtype=verts.dtype, device=dev)
         pred[has] = got
-        return verts, d_out, pred
+        return pred
+
+    # ------------------------------------------------------------------------------------------
+    # multi-GPU SSSP.  The reference's MG SSSP (sssp_impl.cuh:301-375) gathers the distances of the frontier's sources over
+    # the edge partitions (update_edge_src_property) and reduces the proposals per destination to the owners.  Here the
+    # owners keep dist / pred_code / pending (improved, not relaxed yet) for their vertices, and the rounds run inside
+    # Δ-windows [lo, hi) over the distance range.  One round: the pending vertices below hi are the frontier; their distances
+    # (+inf for everybody else) are all-gathered inside the column group over the block's source slots; the block relaxes
+    # their edges into one INT64 key per destination slot (cugraph_b200_block_sssp_relax: float = distance bits << 32 | code
+    # of the source, double = distance bits); ONE MIN reduce-scatter inside the row group brings the smallest key to the
+    # owner, who accepts strict improvements only.  Double runs with predecessors take a second exchange for the codes
+    # (cugraph_b200_block_sssp_pred).  Strict improvement with the "smallest distance, then smallest code" order keeps the
+    # predecessors a tree, also through zero-weight cycles.  Distances are the fixpoint of float add / min: bit-exact vs one GPU
+    # whatever Δ is.  Δ follows the single-GPU controller (DESIGN §3.4): the reference's 32 * avg weight / avg degree
+    # (sssp_impl.cuh:246-247) / 64 at the start, x2 after a window of <= 2 rounds, / 2 after one of >= 6;
+    # CUGRAPH_B200_MG_SSSP_DELTA_SCALE multiplies it (results never depend on it).
+    # ------------------------------------------------------------------------------------------
+    def _sssp_delta(self):
+        if self._sssp_avg is None:   # global averages, one all-reduce at the first call
+            t = torch.tensor([self._w_sum_local, float(self.num_edges_local)], dtype=torch.float64, device=self.device)
+            dist.all_reduce(t)
+            w_sum, n_edges = t.tolist()
+            avg_w = w_sum / n_edges if n_edges > 0 else 0.0
+            self._sssp_avg = (avg_w, n_edges / max(self.part.n_global, 1))
+        avg_w, avg_deg = self._sssp_avg
+        ref = 32.0 * avg_w / max(avg_deg, 1e-30) * float(os.environ.get("CUGRAPH_B200_MG_SSSP_DELTA_SCALE", "1"))
+        if not ref > 0.0 or math.isinf(ref):
+            ref = 1.0
+        return ref / 64.0, ref / 4096.0
+
+    def sssp(self, source, cutoff=math.inf, compute_predecessors=True):
+        """source: external vertex id (the same value on every rank).  Returns (vertices, distances, predecessors) of the
+        vertices this rank owns: distances in the weight dtype (FLT_MAX / DBL_MAX = unreachable, the reference's convention,
+        sssp_impl.cuh:215-229), predecessors as external ids (-1 = none), or None when not requested."""
+        if not self.weighted:
+            raise ValueError("SSSP requires a weighted graph")
+        assert self.block is not None, "sssp needs the unsplit block"
+        p, g, L, capi = self.part, self.part.groups, self.lib, self._capi
+        dev, dt, mp = self.device, self.dtype, p.maxpart
+        f32 = dt == torch.float32
+        lid = self._source_lid(source, "sssp")
+        inf = torch.tensor(math.inf, dtype=dt, device=dev)
+        dist_own = torch.full((mp,), torch.finfo(dt).max, dtype=dt, device=dev)
+        pred_code = torch.full((mp,), -1, dtype=torch.int64, device=dev)
+        pending = torch.zeros(mp, dtype=torch.bool, device=dev)
+        if lid >= 0:
+            dist_own[lid] = 0
+            pending[lid] = True
+        delta, delta_floor = self._sssp_delta()
+        want_codes = compute_predecessors and not f32
+        x_cols = torch.empty(self.n_cols, dtype=dt, device=dev)
+        cand = torch.empty(self.n_rows, dtype=torch.int64, device=dev)
+        cand_own = torch.empty(mp, dtype=torch.int64, device=dev)
+        bufs = dict(x=x_cols, c=cand)
+        if want_codes:
+            win_rows = torch.empty(self.n_rows, dtype=dt, device=dev)
+            code_rows = torch.empty(self.n_rows, dtype=torch.int64, device=dev)
+            code_own = torch.empty(mp, dtype=torch.int64, device=dev)
+            bufs.update(w=win_rows, k=code_rows)
+        views = {k: _view(v) for k, v in bufs.items()}
+        err = C.c_void_p()
+        count = torch.zeros(1, dtype=torch.int64, device=dev)
+        hi = window_bound(0.0, delta, dt, dev)
+        rounds = windows = window_rounds = 0
+        while True:
+            active = pending & (dist_own < hi)
+            count.copy_(active.sum().view(1))
+            dist.all_reduce(count)
+            if int(count.item()) == 0:   # the window is done: open the next one at the smallest pending distance
+                windows += 1
+                if window_rounds <= 2:
+                    delta = delta * 2.0 if delta < torch.finfo(dt).max / 4 else delta
+                elif window_rounds >= 6 and delta > delta_floor:
+                    delta = delta / 2.0
+                m = torch.where(pending, dist_own, inf).min().view(1)
+                dist.all_reduce(m, op=dist.ReduceOp.MIN)
+                lo = float(m.item())
+                if math.isinf(lo):
+                    break
+                hi = window_bound(lo, delta, dt, dev)
+                window_rounds = 0
+                continue
+            pending &= ~active
+            x = torch.where(active, dist_own, inf)
+            if g.R == 1:
+                x_cols.copy_(x)
+            else:
+                all_gather_into(x_cols, x, g.col_group)              # partition-major = the block's column order
+            code = L.cugraph_b200_block_sssp_relax(self.handle.ptr, self.block, views["x"].ptr, float(cutoff), mp, g.C, g.c,
+                                                   views["c"].ptr, C.byref(err))
+            capi.check(code, err, "cugraph_b200_block_sssp_relax")
+            if g.C == 1:
+                cand_own.copy_(cand)
+            else:
+                reduce_scatter_into(cand_own, cand, g.row_group, op=dist.ReduceOp.MIN)
+            improved = sssp_owner_step(dist_own, pred_code, pending, cand_own)
+            if want_codes:
+                win = torch.where(improved, dist_own, inf)
+                if g.C == 1:
+                    win_rows.copy_(win)
+                else:
+                    all_gather_into(win_rows, win, g.row_group)
+                code = L.cugraph_b200_block_sssp_pred(self.handle.ptr, self.block, views["x"].ptr, views["w"].ptr, mp, g.C, g.c,
+                                                      views["k"].ptr, C.byref(err))
+                capi.check(code, err, "cugraph_b200_block_sssp_pred")
+                if g.C == 1:
+                    code_own.copy_(code_rows)
+                else:
+                    reduce_scatter_into(code_own, code_rows, g.row_group, op=dist.ReduceOp.MIN)
+                pred_code.copy_(torch.where(improved, code_own, pred_code))
+            rounds += 1
+            window_rounds += 1
+        for v in views.values():
+            v.free()
+        self.last_sssp_stats = dict(rounds=rounds, windows=windows)
+        verts = p.vertices
+        d_out = dist_own[:p.n_local].clone()
+        if not compute_predecessors:
+            return verts, d_out, None
+        return verts, d_out, self._codes_to_external(pred_code[:p.n_local])
+
+
+INT64_MAX = torch.iinfo(torch.int64).max
+
+
+def window_bound(lo, delta, dtype, device):
+    """upper bound lo + delta of a Δ-window as a 0-d tensor of the distance dtype, strictly above lo after rounding"""
+    lo_t = torch.tensor(lo, dtype=dtype)
+    hi_t = torch.tensor(lo + delta, dtype=dtype)
+    if not bool(hi_t > lo_t):
+        hi_t = torch.nextafter(lo_t, torch.tensor(math.inf, dtype=dtype))
+    return hi_t.to(device)
+
+
+def sssp_owner_step(dist_own, pred_code, pending, cand_own):
+    """The owner's step of one multi-GPU SSSP round: decode the reduced keys (cugraph_b200_block_sssp_relax; INT64_MAX = no
+    proposal), accept strict improvements of dist_own, mark them pending and, for float keys, take the predecessor code from
+    the key's low 32 bits.  Updates the arrays in place and returns the mask of improved vertices."""
+    if dist_own.dtype == torch.float32:
+        d = (cand_own >> 32).to(torch.int32).view(torch.float32)
+    else:
+        d = cand_own.view(torch.float64)
+    improved = (cand_own != INT64_MAX) & (d < dist_own)
+    dist_own.copy_(torch.where(improved, d, dist_own))
+    pending |= improved
+    if dist_own.dtype == torch.float32:
+        pred_code.copy_(torch.where(improved, cand_own & 0xFFFFFFFF, pred_code))
+    return improved
 
 
 # EXPERIMENTAL: same iteration, but the block is split by destination partition: sweep j, then an asynchronous
@@ -489,6 +658,12 @@ MGGraph.pagerank_split = _pagerank_split
 def bfs(graph: MGGraph, source, depth_limit=-1, compute_predecessors=True):
     """(vertices, distances, predecessors) of the vertices owned by this rank (the MG contract of pylibcugraph.bfs)."""
     return graph.bfs(source, depth_limit, compute_predecessors)
+
+
+def sssp(graph: MGGraph, source, cutoff=math.inf, compute_predecessors=True):
+    """(vertices, distances, predecessors) of the vertices owned by this rank (the MG contract of pylibcugraph.sssp;
+    predecessors are None when not requested)."""
+    return graph.sssp(source, cutoff, compute_predecessors)
 
 
 def pagerank(graph: MGGraph, alpha=0.85, epsilon=1e-5, max_iterations=100):

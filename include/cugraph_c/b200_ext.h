@@ -4,9 +4,9 @@
  *  - multi-GPU: the reference receives NCCL communicators inside a raft::handle_t built by raft-dask / MPI
  *    (python/pylibcugraph/pylibcugraph/comms/comms_wrapper.pyx:10-32, cpp/tests/utilities/mg_utilities.cpp:37-55) and keeps
  *    the 2D-partitioned blocks inside graph_t.  raft is not part of this build: cugraph_graph_create_mg and the multi-GPU
- *    algorithm entry points return CUGRAPH_NOT_IMPLEMENTED; multi-GPU PageRank is driven by the launcher
- *    (cugraph_b200/mg.py, one process per GPU over torch.distributed / NCCL) on top of the cugraph_b200_block_* device
- *    pieces declared below.
+ *    algorithm entry points return CUGRAPH_NOT_IMPLEMENTED; multi-GPU PageRank, BFS and SSSP are driven by the
+ *    launcher (cugraph_b200/mg.py, one process per GPU over torch.distributed / NCCL) on top of the cugraph_b200_block_*
+ *    device pieces declared below.
  *  - profiling hooks used by bench.py to time the dominant kernel on the handle's stream.
  */
 #pragma once
@@ -88,6 +88,32 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_bfs_pull(
   const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
   const cugraph_type_erased_device_array_view_t* frontier_cols, const cugraph_type_erased_device_array_view_t* visited_rows,
   size_t maxpart, int grid_cols, int grid_c, cugraph_type_erased_device_array_view_t* cand, cugraph_error_t** error);
+
+/* One relaxation round of multi-GPU SSSP on this GPU's edge block (push direction; the role of the MG relaxation of
+ * cpp/src/traversal/sssp_impl.cuh:301-375 on one edge partition).  The block must have been created with weights.
+ * dist_cols (the block's weight type, one value per column slot, gathered by the launcher inside the column group) holds the
+ * tentative distance of every source in the frontier and +inf for all others.  For every edge (row, col) of an active column
+ * with nd = dist_cols[col] + w < cutoff, cand_rows[row] (INT64, one per row slot) is lowered with an atomic min to a key:
+ *   FLOAT32 blocks: (float bits of nd) << 32 | code(col)   -> the smallest distance, among equal ones the smallest code
+ *   FLOAT64 blocks: the bit pattern of nd                   (non-negative doubles order like their int64 bit patterns)
+ * code(col) = ((col / maxpart) * grid_cols + grid_c) * maxpart + col % maxpart, as in cugraph_b200_block_bfs_pull.  Row slots
+ * without a proposal hold INT64_MAX.  FLOAT32 keys need every code to fit in 32 bits (R * grid_cols * maxpart < 2^32 with
+ * R = ceil(n_cols / maxpart)), else CUGRAPH_INVALID_INPUT.  The cutoff is rounded to the weight type as cugraph_sssp does.
+ * The first call on a block builds its column-major (push) copy and keeps it; blocks that never run SSSP do not pay for it.
+ * Asynchronous, apart from one read-back of the number of active columns and their edge count. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_sssp_relax(
+  const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+  const cugraph_type_erased_device_array_view_t* dist_cols, double cutoff, size_t maxpart, int grid_cols, int grid_c,
+  cugraph_type_erased_device_array_view_t* cand_rows, cugraph_error_t** error);
+
+/* Predecessors of a FLOAT64 relaxation round.  win_rows (the block's weight type, one per row slot; +inf = not asked) holds
+ * the distance a row accepted in this round.  code_rows[row] (INT64) receives the smallest code(col) over the active columns
+ * of dist_cols with dist_cols[col] + w == win_rows[row] (the sum is recomputed exactly as the relaxation formed it), else
+ * INT64_MAX.  Arguments and asynchrony as in cugraph_b200_block_sssp_relax. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_sssp_pred(
+  const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+  const cugraph_type_erased_device_array_view_t* dist_cols, const cugraph_type_erased_device_array_view_t* win_rows,
+  size_t maxpart, int grid_cols, int grid_c, cugraph_type_erased_device_array_view_t* code_rows, cugraph_error_t** error);
 
 /* Debug hook: one sweep as PageRank would run it on this graph (the shared-memory piece stream when the graph has one)
  * against the plain sweep (an independent implementation) on the same pseudo-random x.  out[0..3] = degree >= 32 rows

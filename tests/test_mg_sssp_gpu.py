@@ -1,0 +1,141 @@
+"""Multi-GPU SSSP on the GPU.
+
+- All ranks of a 2D partition on ONE GPU (tests/mg_sssp_sim.py) through the real block kernels: grids 1x2, 2x1, 2x2 and 4x2
+  on symmetrised weighted RMAT-14 and RMAT-16, float32 and float64, with and without predecessors, a cutoff, 64-bit-offset
+  blocks, and the zero-weight graph.
+- A world-size-1 NCCL process group running cugraph_b200.mg.MGGraph.sssp (the 1x1 grid): the real orchestration and the
+  real stream ordering on the device.
+- 2 and 4 GPUs over NCCL (skipped when fewer GPUs are visible).
+Distances bit-exact vs the oracle in the same float type and vs single-GPU cugraph_sssp; predecessors by the oracle's
+predicate and by walking every chain back to the source."""
+import os
+import socket
+import sys
+
+import numpy as np
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+from tests import mg_sssp_sim as sim  # noqa: E402
+
+pytestmark = pytest.mark.gpu
+
+
+@pytest.mark.parametrize("R,Cc", [(1, 2), (2, 1), (2, 2), (4, 2)], ids=["1x2", "2x1", "2x2", "4x2"])
+@pytest.mark.parametrize("scale", [14, 16])
+def test_mg_sssp_simulated_on_one_gpu(R, Cc, scale):
+    for wdtype in (np.float32, np.float64):
+        s, d, w, V = sim.rmat_graph(scale, wdtype)
+        srcs = sim.sources(s, V)
+        for src in srcs:
+            single = sim.single_gpu_sssp(s, d, w, V, src)
+            dist, pred, _ = sim.simulate(s, d, w, V, R, Cc, src, device="cuda")
+            sim.check(s, d, w, V, src, dist, pred, single=single)
+        if wdtype == np.float32:
+            dist, _, _ = sim.simulate(s, d, w, V, R, Cc, srcs[0], predecessors=False, device="cuda")
+            sim.check(s, d, w, V, srcs[0], dist, None, single=sim.single_gpu_sssp(s, d, w, V, srcs[0]))
+            reach = single[single < np.finfo(wdtype).max]
+            co = float(np.quantile(reach, 0.3))
+            dist, pred, _ = sim.simulate(s, d, w, V, R, Cc, src, cutoff=co, device="cuda")
+            sim.check(s, d, w, V, src, dist, pred, cutoff=co, single=sim.single_gpu_sssp(s, d, w, V, src, cutoff=co))
+
+
+@pytest.mark.parametrize("wdtype", [np.float32, np.float64], ids=["f32", "f64"])
+def test_mg_sssp_simulated_offs64_on_one_gpu(monkeypatch, wdtype):
+    monkeypatch.setenv("CUGRAPH_B200_OFFS64_MIN_EDGES", "0")
+    s, d, w, V = sim.rmat_graph(14, wdtype)
+    src = sim.sources(s, V)[0]
+    dist, pred, _ = sim.simulate(s, d, w, V, 2, 2, src, device="cuda")
+    monkeypatch.delenv("CUGRAPH_B200_OFFS64_MIN_EDGES")
+    sim.check(s, d, w, V, src, dist, pred, single=sim.single_gpu_sssp(s, d, w, V, src))
+
+
+@pytest.mark.parametrize("wdtype", [np.float32, np.float64], ids=["f32", "f64"])
+def test_mg_sssp_zero_weights_on_one_gpu(wdtype):
+    s, d, w, V = sim.zero_weight_graph(wdtype)
+    for R, Cc in ((2, 2), (4, 2)):
+        for src in (0, 7):
+            dist, pred, _ = sim.simulate(s, d, w, V, R, Cc, src, device="cuda")
+            sim.check(s, d, w, V, src, dist, pred, single=sim.single_gpu_sssp(s, d, w, V, src))
+
+
+# ------------------------------------------------------------------------------------------------- NCCL process groups
+def _free_port():
+    s = socket.socket()
+    s.bind(("127.0.0.1", 0))
+    p = s.getsockname()[1]
+    s.close()
+    return p
+
+
+def _nccl_worker(rank, world, port, scale, q):
+    import torch
+    import torch.distributed as dist
+    os.environ["MASTER_ADDR"] = "127.0.0.1"
+    os.environ["MASTER_PORT"] = str(port)
+    torch.cuda.set_device(rank)
+    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
+    from cugraph_b200 import mg
+    out = {}
+    for wdtype in (np.float32, np.float64):
+        s, d, w, V = sim.rmat_graph(scale, wdtype)
+        E = s.size
+        lo, hi = rank * E // world, (rank + 1) * E // world
+        g = mg.MGGraph(torch.as_tensor(s[lo:hi]).cuda(), torch.as_tensor(d[lo:hi]).cuda(), torch.as_tensor(w[lo:hi]).cuda())
+        srcs = sim.sources(s, V)
+        runs = []
+        for src in srcs:
+            v, dd, pp = g.sssp(src)
+            runs.append((src, v.cpu().numpy(), dd.cpu().numpy(), pp.cpu().numpy()))
+        out[np.dtype(wdtype).name] = runs
+        del g
+    res = [None] * world
+    dist.all_gather_object(res, out)
+    if rank == 0:
+        q.put(res)
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+def _run_nccl(world, scale):
+    import torch
+    import torch.multiprocessing as mp
+    if torch.cuda.device_count() < world:
+        pytest.skip(f"needs {world} GPUs")
+    ctx = mp.get_context("spawn")
+    q = ctx.Queue()
+    port = _free_port()
+    procs = [ctx.Process(target=_nccl_worker, args=(r, world, port, scale, q)) for r in range(world)]
+    for p in procs:
+        p.start()
+    res = q.get(timeout=600)
+    for p in procs:
+        p.join(timeout=120)
+        assert p.exitcode == 0
+    for wdtype in (np.float32, np.float64):
+        s, d, w, V = sim.rmat_graph(scale, wdtype)
+        present = np.unique(np.concatenate([s, d]))
+        name = np.dtype(wdtype).name
+        for i, src in enumerate(sim.sources(s, V)):
+            unreached = np.finfo(wdtype).max
+            dist = np.full(V, unreached, dtype=wdtype)   # isolated ids are not vertices of the MG graph: unreached
+            pred = np.full(V, -1, dtype=np.int64)
+            n = 0
+            for r in res:
+                _, v, dd, pp = r[name][i]
+                dist[v] = dd
+                pred[v] = pp
+                n += v.size
+            assert n == present.size
+            sim.check(s, d, w, V, src, dist, pred, single=sim.single_gpu_sssp(s, d, w, V, src))
+
+
+def test_mg_sssp_nccl_world_size_1():
+    _run_nccl(1, 14)
+
+
+@pytest.mark.parametrize("world", [2, 4])
+def test_mg_sssp_multi_gpu(world):
+    _run_nccl(world, 14)
