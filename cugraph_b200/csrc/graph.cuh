@@ -30,8 +30,8 @@ constexpr int kWarpsPerCta = 8;
 
 // ---------------------------------------------------------------------------------------------
 // Column-blocked "piece stream" of the rows [0, n_str) for the shared-memory pull sweep (sweep.cuh).  n_str is a degree-bin
-// bound: on large graphs the rows of in-degree < kSweepTailDegree (the TAIL) leave the stream and are swept by the plain
-// row kernel instead (k_spmv_low); on smaller graphs the stream covers every non-empty row.
+// bound: on large graphs the rows of in-degree < kSweepTailDegree (the TAIL) leave the stream and are swept by a row
+// kernel instead (k_sweep_tail); on smaller graphs the stream covers every non-empty row.
 // The source (column) space is cut into B blocks of W vertices (W * sizeof(T) = 192 KiB minus 64 zero columns: the slice of
 // x a persistent CTA keeps in shared memory).  Rows keep their neighbours sorted by source id, so a row's adjacency is
 // already partitioned by block; every (row, block) SEGMENT is cut into PIECES of <= 64 entries.  A piece is stored with
@@ -51,7 +51,7 @@ constexpr int kBandRowAlign = 512;  // band bounds: a multiple of the finish ker
 
 // Tail of the piece stream: a row of small in-degree has its few edges in different column blocks, so the stream pays one
 // fp64 RED per edge for it, and such rows are most of the rows (their accumulators decide how many bands are needed).
-// Rows of in-degree < kSweepTailDegree are gathered by k_spmv_low instead, on graphs of at least kSweepTailMinEdges edges.
+// Rows of in-degree < kSweepTailDegree are gathered by k_sweep_tail instead, on graphs of at least kSweepTailMinEdges edges.
 // A kSegThreshold value.  Measured on an H100 80GB HBM3 at 700 W, RMAT-24 PageRank step: 86.3 ms without a tail, 78.8 / 73.4
 // / 72.7 / 74.5 ms with bounds 4 / 8 / 16 / 32 (DESIGN.md §3.2); from 8 on the stream needs one band.
 constexpr int kSweepTailDegree         = 16;

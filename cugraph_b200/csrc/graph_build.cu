@@ -1354,7 +1354,7 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   phase_trace tr(h);
   const int W         = (int)(kHotSliceBytes / es) - kHotZeroPad;  // columns per block; the pad holds zeros
   const int32_t n_cov = c.seg[kNumSeg - 2];                         // rows of degree >= 1
-  const int32_t n_str = c.seg[sweep_stream_bin(h, c)];              // rows of the stream; the tail is swept by k_spmv_low
+  const int32_t n_str = c.seg[sweep_stream_bin(h, c)];              // rows of the stream; the tail is swept by k_sweep_tail
   if (n_str <= 0) return nullptr;                                   // no row reaches the bound: the plain sweep fits better
   const int B         = (int)(((int64_t)nv + W - 1) / W);
   int64_t nnz = 0;  // edges of the stream rows: a prefix of indices (rows are degree-descending)

@@ -208,20 +208,19 @@ k_spmv_low(O const* __restrict__ offsets, int32_t const* __restrict__ indices, T
 // ------------------------------------------------------------------------------------------
 // host-side launcher of one full sweep
 // ------------------------------------------------------------------------------------------
-// the bins [first, kNumSeg - 1) of the rows below the degree-32 prefix; the bins before `first` get no blocks.
-// empty_rows == false: the last bin (the rows without edges) gets none either.
-inline low_bins_t make_low_bins(csx_t const& c, int first = 0, bool empty_rows = true)
+// the bins of the rows below the degree-32 prefix, the last one = the rows without edges
+inline low_bins_t make_low_bins(csx_t const& c)
 {
   low_bins_t b{};
   int blocks = 0;
   for (int k = 0; k < kNumSeg - 1; ++k) {
     b.row_begin[k]   = c.seg[k];
     b.block_begin[k] = blocks;
-    int rows         = k < first || (k == kNumSeg - 2 && !empty_rows) ? 0 : c.seg[k + 1] - c.seg[k];
+    int rows         = c.seg[k + 1] - c.seg[k];
     int per_block    = (k == kNumSeg - 2) ? 256 : 256 / low_bin_lanes(k);
     blocks += (rows + per_block - 1) / per_block;
   }
-  b.row_begin[kNumSeg - 1]   = empty_rows ? c.seg[kNumSeg] : c.seg[kNumSeg - 2];
+  b.row_begin[kNumSeg - 1]   = c.seg[kNumSeg];
   b.block_begin[kNumSeg - 1] = blocks;
   return b;
 }

@@ -22,8 +22,9 @@
 //     first.  k_sweep_finish turns acc into y, clears it and resets the cursors.
 //   * the rows are split into bands whose accumulators fit in the L2 (graph.cuh); the sweep runs band by band, k_sweep over
 //     the band's phases, then k_sweep_finish over its rows while their accumulators are still in the L2.
-//   * on large graphs the rows of small in-degree (the tail, graph.cuh) are not in the stream: one k_spmv_low launch after
-//     the bands gathers their few edges from x directly (no RED, and fewer stream rows need fewer bands).
+//   * on large graphs the rows of small in-degree (the tail, graph.cuh) are not in the stream: one k_sweep_tail launch after
+//     the bands gathers their few edges directly (no RED, and fewer stream rows need fewer bands), the hubs' x from a
+//     shared-memory copy of the first column block.
 #pragma once
 #include "spmv.cuh"
 
@@ -638,6 +639,76 @@ k_sweep_finish(double* __restrict__ acc, int row_lo, int n_cov, int n_rows, T* _
   }
 }
 
+// The tail rows [row_lo, row_hi) (graph.cuh), then y = init for the empty rows [row_hi, empty_hi).  A thread per row, the
+// row's entries gathered kTailBatch at a time with all loads of a batch issued back to back, the next row's offsets in
+// flight meanwhile; fp64 sum, rounded once, no RED.  The tail's sources are mostly hubs (RMAT-24: 47 % of them in the first
+// column block), and a plain row kernel pays a 32-byte L2 sector for each of those 4-byte gathers: here persistent CTAs
+// (one per SM) keep x[0, W) in shared memory, loaded once by TMA bulk copies as in k_sweep, and gather the rest through L1.
+constexpr int kTailThreads = 1024;
+constexpr int kTailBatch   = 8;
+
+template <typename T, bool WEIGHTED>
+__global__ void __launch_bounds__(kTailThreads, 1)
+k_sweep_tail(int32_t const* __restrict__ off, int32_t const* __restrict__ idx, T const* __restrict__ w, T const* __restrict__ x,
+             T* __restrict__ y, int32_t const* __restrict__ row_vertex, int row_lo, int row_hi, int empty_hi, int W,
+             double alpha, pr_state_t const* __restrict__ st)
+{
+  B200_DYN_SMEM(smem_raw);
+  T const* sx = reinterpret_cast<T const*>(smem_raw);
+  __shared__ uint64_t bar;
+  if (st->done) return;
+  if (threadIdx.x == 0) {
+    mbar_init(&bar, 1);
+    const unsigned bytes = (unsigned)(W * sizeof(T));
+    mbar_expect_tx(&bar, bytes);
+    const unsigned char* src = reinterpret_cast<const unsigned char*>(x);
+    for (unsigned o = 0; o < bytes; o += kTmaPiece)
+      tma_bulk_g2s(smem_raw + o, src + o, (bytes - o) < (unsigned)kTmaPiece ? (bytes - o) : (unsigned)kTmaPiece, &bar);
+  }
+  const double init = st->init;
+  const int stride  = gridDim.x * blockDim.x;
+  int r             = row_lo + (int)(blockIdx.x * blockDim.x + threadIdx.x);
+  int lo = 0, hi = 0;
+  if (r < row_hi) {
+    lo = __ldg(off + r);
+    hi = __ldg(off + r + 1);
+  }
+  __syncthreads();  // the barrier is initialised before anybody waits on it
+  mbar_wait(&bar, 0);
+  for (; r < row_hi; r += stride) {
+    const int rn = r + stride;
+    int nlo = 0, nhi = 0;
+    if (rn < row_hi) {
+      nlo = __ldg(off + rn);
+      nhi = __ldg(off + rn + 1);
+    }
+    double s = 0.0;
+    for (int e = lo; e < hi; e += kTailBatch) {
+      int c[kTailBatch];
+      T wv[kTailBatch];
+#pragma unroll
+      for (int k = 0; k < kTailBatch; ++k) {
+        c[k]  = 0;
+        wv[k] = (T)0;
+        if (e + k < hi) {
+          c[k]  = __ldg(idx + e + k);
+          wv[k] = WEIGHTED ? __ldg(w + e + k) : (T)1;
+        }
+      }
+      T v[kTailBatch];
+#pragma unroll
+      for (int k = 0; k < kTailBatch; ++k) v[k] = (c[k] < W ? sx[c[k]] : __ldg(x + c[k])) * wv[k];
+      s += (((double)v[0] + (double)v[1]) + ((double)v[2] + (double)v[3])) +
+           (((double)v[4] + (double)v[5]) + ((double)v[6] + (double)v[7]));
+    }
+    y[row_vertex ? row_vertex[r] : r] = (T)(s * alpha + init);
+    lo = nlo;
+    hi = nhi;
+  }
+  for (int q = row_hi + (int)(blockIdx.x * blockDim.x + threadIdx.x); q < empty_hi; q += stride)
+    y[row_vertex ? row_vertex[q] : q] = (T)init;
+}
+
 // x must hold padded_x_elems() elements, zero behind n_vertices (slices are copied whole)
 template <typename T>
 void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L, T const* x, T* y, double* acc, double alpha,
@@ -682,18 +753,19 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
     B200_LAUNCH(h, (k_sweep_finish<T, kFinishSteps>), (std::max(n, 1) + 255) / 256, 256, 0, acc, row_lo, L.n_str, row_hi, y,
                 c.row_vertex.as<int32_t>(), alpha, L.cursor.as<int>() + a.ph_lo, n_ph, st);
   }
-  if (tail) {  // the rows [n_str, n_cov) and (unless covered_rows_only) the empty rows, by k_spmv_low
-    int first = 0;  // n_str is a bin bound: the tail starts at the first bin that begins there
-    while (c.seg[first] < L.n_str) ++first;
-    const low_bins_t bins = make_low_bins(c, first, !covered_rows_only);
-    const int blocks      = bins.block_begin[kNumSeg - 1];
-    T const* w            = weighted ? c.weights.as<T>() : nullptr;
-    if (weighted)
-      B200_LAUNCH(h, (k_spmv_low<int32_t, T, true>), blocks, 256, 0, c.offsets.as<int32_t>(), c.indices.as<int32_t>(), w, x, y,
-                  c.row_vertex.as<int32_t>(), bins, alpha, st);
-    else
-      B200_LAUNCH(h, (k_spmv_low<int32_t, T, false>), blocks, 256, 0, c.offsets.as<int32_t>(), c.indices.as<int32_t>(), w, x, y,
-                  c.row_vertex.as<int32_t>(), bins, alpha, st);
+  if (tail) {  // the rows [n_str, n_cov) and (unless covered_rows_only) the empty rows, by k_sweep_tail
+    const int32_t rows = std::max(finish_rows, L.n_cov) - L.n_str;
+    const int blocks   = std::max(1, std::min(h.sm_count, (rows + kTailThreads - 1) / kTailThreads));
+    T const* w         = weighted ? c.weights.as<T>() : nullptr;
+    if (weighted) {
+      CUDA_TRY(cudaFuncSetAttribute(k_sweep_tail<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
+      B200_LAUNCH(h, (k_sweep_tail<T, true>), blocks, kTailThreads, kSweepDynSmem, c.offsets.as<int32_t>(),
+                  c.indices.as<int32_t>(), w, x, y, c.row_vertex.as<int32_t>(), L.n_str, L.n_cov, finish_rows, L.W, alpha, st);
+    } else {
+      CUDA_TRY(cudaFuncSetAttribute(k_sweep_tail<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
+      B200_LAUNCH(h, (k_sweep_tail<T, false>), blocks, kTailThreads, kSweepDynSmem, c.offsets.as<int32_t>(),
+                  c.indices.as<int32_t>(), w, x, y, c.row_vertex.as<int32_t>(), L.n_str, L.n_cov, finish_rows, L.W, alpha, st);
+    }
   }
 }
 
