@@ -1,9 +1,9 @@
 // Katz centrality and HITS on the pull sweep — the sibling algorithms that run on the same primitive as PageRank
 // (per_v_transform_reduce_incoming_e / _outgoing_e with reduce_op::plus; reference cpp/src/centrality/katz_centrality_impl.cuh:34-196,
 // cpp/src/link_analysis/hits_impl.cuh:29-206, C API cpp/src/c_api/katz.cpp, cpp/src/c_api/hits.cpp).  Both are host loops
-// over launch_pull_sweep_auto (the shared-memory piece stream when the graph has one) plus small vector passes; their
+// over pull_sweep (sweep.cu: the shared-memory piece stream when the graph has one) plus small vector passes; their
 // per-iteration convergence test reads one scalar back, as the reference does.
-#include "sweep.cuh"
+#include "graph.cuh"
 
 #include <cmath>
 #include <limits>
@@ -92,34 +92,6 @@ __global__ void k_count_negative(T const* __restrict__ v, int32_t n, int* __rest
     if (v[i] < (T)0) atomicAdd(out, 1);
 }
 
-struct sweep_scratch_t {
-  dbuf acc, state;
-  pr_state_t* st{nullptr};
-  void init(handle_impl const& h, size_t rows)
-  {
-    acc = make_dbuf<double>(std::max<size_t>(rows, 1), h.stream);
-    CUDA_TRY(cudaMemsetAsync(acc.data(), 0, sizeof(double) * std::max<size_t>(rows, 1), h.stream));
-    state = make_dbuf<pr_state_t>(1, h.stream);
-    CUDA_TRY(cudaMemsetAsync(state.data(), 0, sizeof(pr_state_t), h.stream));
-    st = state.as<pr_state_t>();
-  }
-  // the unvarying term the sweep adds to every row
-  void set_init(handle_impl const& h, double init)
-  {
-    pr_state_t hs{};
-    hs.init = init;
-    CUDA_TRY(cudaMemcpyAsync(state.data(), &hs, sizeof(pr_state_t), cudaMemcpyHostToDevice, h.stream));
-    sync(h);  // hs is a stack variable
-  }
-};
-
-template <typename T>
-void sweep(handle_impl const& h, csx_t const& c, int32_t nv, T const* x, T* y, sweep_scratch_t& sc, double alpha, bool use_weights)
-{
-  if (c.offs64) launch_pull_sweep<int64_t, T>(h, c, x, y, sc.acc.as<double>(), alpha, sc.st, use_weights);
-  else launch_pull_sweep_auto<int32_t, T>(h, c, nv, x, y, sc.acc.as<double>(), alpha, sc.st, use_weights);
-}
-
 double read_scalar(handle_impl const& h, double const* d)
 {
   double v = 0.0;
@@ -138,16 +110,14 @@ void katz_typed(handle_impl const& h, graph_impl& g, double alpha, double beta, 
 {
   const int32_t nv = g.n_vertices;
   csx_t const& c   = pull_view(h, g);
-  const size_t px  = padded_x_elems(nv, sizeof(T));
-  dbuf x = make_dbuf<T>(px, h.stream), y = make_dbuf<T>(std::max(nv, 1), h.stream);
-  CUDA_TRY(cudaMemsetAsync(x.data(), 0, px * sizeof(T), h.stream));  // no initial guess: zeros (katz_centrality_impl.cuh:88-93)
+  dbuf x = make_sweep_x<T>(h, nv), y = make_dbuf<T>(std::max(nv, 1), h.stream);  // x: zeros (katz_centrality_impl.cuh:88-93)
   sweep_scratch_t sc;
-  sc.init(h, acc_rows(c));
+  sc.init(h, c);
   sc.set_init(h, beta);
   dbuf d_diff = make_dbuf<double>(1, h.stream);
   size_t iter = 0;
   while (nv > 0) {
-    sweep<T>(h, c, nv, x.as<T>(), y.as<T>(), sc, alpha, true);
+    pull_sweep<T>(h, c, nv, x.as<T>(), y.as<T>(), sc, alpha);
     CUDA_TRY(cudaMemsetAsync(d_diff.data(), 0, sizeof(double), h.stream));
     B200_LAUNCH(h, (k_abs_diff<T>), cgrid(h, nv), kCBlock, 0, y.as<T>(), x.as<T>(), nv, 1, d_diff.as<double>());
     const double diff = read_scalar(h, d_diff.as<double>());
@@ -179,16 +149,14 @@ void eigenvector_typed(handle_impl const& h, graph_impl& g, double epsilon, size
 {
   const int32_t nv = g.n_vertices;
   csx_t const& c   = pull_view(h, g);
-  const size_t px  = padded_x_elems(nv, sizeof(T));
-  dbuf x = make_dbuf<T>(px, h.stream), y = make_dbuf<T>(std::max(nv, 1), h.stream);
-  CUDA_TRY(cudaMemsetAsync(x.data(), 0, px * sizeof(T), h.stream));
+  dbuf x = make_sweep_x<T>(h, nv), y = make_dbuf<T>(std::max(nv, 1), h.stream);
   if (nv > 0) B200_LAUNCH(h, (k_fill_vec<T>), cgrid(h, nv), kCBlock, 0, x.as<T>(), (int64_t)nv, (T)(1.0 / (double)nv));
   sweep_scratch_t sc;
-  sc.init(h, acc_rows(c));
+  sc.init(h, c);
   dbuf d2     = make_dbuf<double>(2, h.stream);
   size_t iter = 0;
   while (nv > 0) {
-    sweep<T>(h, c, nv, x.as<T>(), y.as<T>(), sc, 1.0, true);
+    pull_sweep<T>(h, c, nv, x.as<T>(), y.as<T>(), sc, 1.0);
     B200_LAUNCH(h, (k_add_vec<T>), cgrid(h, nv), kCBlock, 0, y.as<T>(), x.as<T>(), nv);
     CUDA_TRY(cudaMemsetAsync(d2.data(), 0, 2 * sizeof(double), h.stream));
     B200_LAUNCH(h, (k_norm<T>), cgrid(h, nv), kCBlock, 0, y.as<T>(), nv, 0, d2.as<double>());
@@ -238,9 +206,7 @@ void hits_typed(handle_impl const& h, graph_impl& g, double epsilon, size_t max_
   const int32_t nv   = g.n_vertices;
   csx_t const& c_in  = pull_view(h, g);       // rows = destinations: authorities <- hubs
   csx_t const& c_out = out_sweep_view(h, g);  // rows = sources: hubs <- authorities
-  const size_t px    = padded_x_elems(nv, sizeof(T));
-  dbuf hubs_a = make_dbuf<T>(px, h.stream), hubs_b = make_dbuf<T>(px, h.stream), auth = make_dbuf<T>(px, h.stream);
-  for (dbuf* b : {&hubs_a, &hubs_b, &auth}) CUDA_TRY(cudaMemsetAsync(b->data(), 0, px * sizeof(T), h.stream));
+  dbuf hubs_a = make_sweep_x<T>(h, nv), hubs_b = make_sweep_x<T>(h, nv), auth = make_sweep_x<T>(h, nv);
   dbuf d2 = make_dbuf<double>(2, h.stream);
   B200_EXPECTS(epsilon >= 0.0, CUGRAPH_INVALID_INPUT, "Invalid input argument: epsilon should be non-negative.");
   double diff = std::numeric_limits<T>::max();
@@ -264,14 +230,14 @@ void hits_typed(handle_impl const& h, graph_impl& g, double epsilon, size_t max_
       B200_LAUNCH(h, (k_fill_vec<T>), cgrid(h, nv), kCBlock, 0, hubs_a.as<T>(), (int64_t)nv, (T)(1.0 / (double)nv));
     }
     sweep_scratch_t sc_in, sc_out;
-    sc_in.init(h, acc_rows(c_in));
-    sc_out.init(h, acc_rows(c_out));
+    sc_in.init(h, c_in);
+    sc_out.init(h, c_out);
     T* prev = hubs_a.as<T>();
     T* curr = hubs_b.as<T>();
     iter    = 0;
     while (true) {
-      sweep<T>(h, c_in, nv, prev, auth.as<T>(), sc_in, 1.0, false);
-      sweep<T>(h, c_out, nv, auth.as<T>(), curr, sc_out, 1.0, false);
+      pull_sweep<T>(h, c_in, nv, prev, auth.as<T>(), sc_in, 1.0, false);
+      pull_sweep<T>(h, c_out, nv, auth.as<T>(), curr, sc_out, 1.0, false);
       normalize_by<T>(h, curr, nv, 2, d2);
       normalize_by<T>(h, auth.as<T>(), nv, 2, d2);
       CUDA_TRY(cudaMemsetAsync(d2.data(), 0, sizeof(double), h.stream));

@@ -319,6 +319,13 @@ __device__ __forceinline__ bool is_commit_lane() { return (threadIdx.x & 31) == 
 inline bool is_commit_lane() { return true; }
 #endif
 
+__device__ __forceinline__ double warp_sum(double v)
+{
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
 inline void check_last(const char* what)
 {
   cudaError_t e = cudaGetLastError();

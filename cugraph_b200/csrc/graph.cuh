@@ -133,9 +133,6 @@ struct csx_t {
   mutable dbuf out_w;  // n_vertices x T : per-source sum of edge weights (or out-degree), T = weight type
 };
 
-// rows that may need an fp64 accumulator in a sweep (callers size acc_hi with it): the piece stream covers every row
-inline int32_t acc_rows(csx_t const& c) { return std::max(c.n_rows, 1); }
-
 struct graph_impl {
   cugraph_data_type_id_t vertex_type{INT32};
   cugraph_data_type_id_t edge_type{INT32};
@@ -172,10 +169,40 @@ inline graph_impl* G(cugraph_graph_t* g)
 
 // Accessors that build the missing orientation on demand (graph_build.cu).
 csx_t const& pull_view(handle_impl const& h, graph_impl& g);  // rows = destinations, indices = sources
-// piece stream for elements of `elem_size` bytes, or nullptr when the graph is too small for it
+// piece stream for elements of `elem_size` bytes, or nullptr when the graph is too small for it or has 64-bit offsets
 sweep_layout_t const* sweep_layout(handle_impl const& h, csx_t const& c, int32_t n_vertices, size_t elem_size);
 csx_t const& push_view(handle_impl const& h, graph_impl& g);  // rows = sources, vertex-indexed offsets
 csx_t const& out_sweep_view(handle_impl const& h, graph_impl& g);  // rows = sources, binned for the sweep kernels (HITS)
+
+// ---- the pull sweep (sweep.cu): y[row] = init + alpha * sum_{(col -> row)} x[col] * w(col, row) for every row of a csx
+// device-resident loop state of one PageRank run (no per-iteration host round trip); a sweep is a no-op once `done` is set
+struct pr_state_t {
+  double diff;        // sum |pr_new - pr_old| of the iteration being computed
+  double dangling;    // sum of pr_new over vertices without out-edges
+  double init;        // unvarying part added to every row in the CURRENT sweep
+  double pers_scale;  // (dangling*alpha + 1-alpha) for the personalization scatter
+  double last_diff;
+  int iter;
+  int done;
+};
+// what sweeps over one csx need besides x and y: fp64 accumulators, zero between sweeps, and the device pr_state_t
+struct sweep_scratch_t {
+  dbuf acc, state;
+  void init(handle_impl const& h, csx_t const& c);   // zero accumulators for c's rows; a state of zeros (init 0, not done)
+  void set_init(handle_impl const& h, double init);  // the unvarying term the sweep adds to every row
+  pr_state_t* st() const { return state.as<pr_state_t>(); }
+};
+// elements an x buffer needs: whole slices are TMA-copied and everything behind n_vertices must read 0
+size_t padded_x_elems(int32_t n_vertices, size_t elem_size);
+// an x buffer of padded_x_elems() elements, zero-filled; only [0, n_vertices) is to be written afterwards
+template <typename T>
+dbuf make_sweep_x(handle_impl const& h, int32_t n_vertices);
+// The piece stream (sweep.cuh) when the graph has one, else the plain sweep (spmv.cuh).  x holds padded_x_elems() elements
+// and does not overlap y.  use_weights = false: plain neighbour sums on a weighted graph (HITS).  covered_rows_only: the
+// rows without edges may keep what y holds (multi-GPU blocks, whose unvarying term is 0).
+template <typename T>
+void pull_sweep(handle_impl const& h, csx_t const& c, int32_t n_vertices, T const* x, T* y, sweep_scratch_t& sc, double alpha,
+                bool use_weights = true, bool covered_rows_only = false);
 
 // external <-> internal id helpers (graph_build.cu)
 // out[i] = internal id of ext[i], or -1 if ext[i] is not a vertex.

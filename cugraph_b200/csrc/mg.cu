@@ -9,7 +9,6 @@
 // per-iteration vertex step, the BFS pull step and the SSSP push relaxation.  All calls only ENQUEUE work on the handle's
 // stream (the SSSP calls read back one queue size).
 #include "advance.cuh"
-#include "sweep.cuh"
 
 #include <algorithm>
 #include <climits>
@@ -34,8 +33,7 @@ struct block_impl {
   int32_t n_rows{0}, n_cols{0}, n_span{0};
   bool weighted{false};
   cugraph_data_type_id_t wtype{FLOAT32};
-  dbuf acc_hi;
-  dbuf state;  // pr_state_t with init = 0, done = 0
+  sweep_scratch_t scratch;  // init = 0
   // the y array whose rows WITHOUT edges this block has already written (0): later sweeps into the same array only finish the
   // rows that have edges — in a 2D block more than half of the row slots are empty (the caller must not write them either)
   void const* y_complete{nullptr};
@@ -383,12 +381,9 @@ cugraph_error_code_t cugraph_b200_block_create(const cugraph_resource_handle_t* 
     b->weighted = w != nullptr;
     b->csx     = build_binned_rows(h, (int32_t const*)r->data, (int32_t const*)c->data, w ? w->data : nullptr, b->wtype,
                                    (int64_t)r->size, b->n_span);
-    b->acc_hi  = make_dbuf<double>(acc_rows(*b->csx), h.stream);
-    CUDA_TRY(cudaMemsetAsync(b->acc_hi.data(), 0, sizeof(double) * acc_rows(*b->csx), h.stream));
-    b->state = make_dbuf<pr_state_t>(1, h.stream);
-    CUDA_TRY(cudaMemsetAsync(b->state.data(), 0, sizeof(pr_state_t), h.stream));
+    b->scratch.init(h, *b->csx);
     // build the column-blocked copy now (it is lazily created otherwise, inside the first timed sweep)
-    if (!b->csx->offs64) (void)sweep_layout(h, *b->csx, b->n_span, b->wtype == FLOAT64 ? 8 : 4);
+    (void)sweep_layout(h, *b->csx, b->n_span, b->wtype == FLOAT64 ? 8 : 4);
     sync(h);
     *block = reinterpret_cast<cugraph_b200_block_t*>(b.release());
   });
@@ -426,15 +421,9 @@ cugraph_error_code_t cugraph_b200_block_pull_sweep(const cugraph_resource_handle
     auto const* y0  = static_cast<const char*>(yv->data);
     B200_EXPECTS(y0 + yv->size * es <= x0 || x0 + xv->size * es <= y0, CUGRAPH_INVALID_INPUT, "x and y must not overlap");
     csx_t const& c = *b->csx;
-    auto* st       = b->state.as<pr_state_t>();
     const bool covered_only = b->y_complete == yv->data;  // the empty rows of this y hold their zeros from an earlier sweep
-    if (f32) {
-      if (c.offs64) launch_pull_sweep<int64_t, float>(h, c, (float const*)xv->data, (float*)yv->data, b->acc_hi.as<double>(), alpha, st);
-      else launch_pull_sweep_auto<int32_t, float>(h, c, b->n_span, (float const*)xv->data, (float*)yv->data, b->acc_hi.as<double>(), alpha, st, true, covered_only);
-    } else {
-      if (c.offs64) launch_pull_sweep<int64_t, double>(h, c, (double const*)xv->data, (double*)yv->data, b->acc_hi.as<double>(), alpha, st);
-      else launch_pull_sweep_auto<int32_t, double>(h, c, b->n_span, (double const*)xv->data, (double*)yv->data, b->acc_hi.as<double>(), alpha, st, true, covered_only);
-    }
+    if (f32) pull_sweep<float>(h, c, b->n_span, (float const*)xv->data, (float*)yv->data, b->scratch, alpha, true, covered_only);
+    else pull_sweep<double>(h, c, b->n_span, (double const*)xv->data, (double*)yv->data, b->scratch, alpha, true, covered_only);
     b->y_complete = yv->data;
     check_last("block_pull_sweep");
   });

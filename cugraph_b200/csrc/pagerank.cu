@@ -2,16 +2,15 @@
 // Replaces cpp/src/link_analysis/pagerank_impl.cuh:40-330 (driver) and cpp/src/c_api/pagerank.cpp.
 //
 // Per iteration the reference runs ~6 V-sized thrust passes and 2 blocking scalar read-backs
-// (pagerank_impl.cuh:225-318).  Here an iteration is: pull sweep (spmv.cuh) -> [personalization
+// (pagerank_impl.cuh:225-318).  Here an iteration is: pull sweep (sweep.cu) -> [personalization
 // scatter] -> ONE fused vertex pass (diff, dangling sum, next x = pr/out_w) -> 1-thread finalize that
 // advances the device-resident loop state.  The host enqueues iterations in batches and only reads the
 // `done` flag between batches; kernels of iterations past convergence are no-ops, so the iteration
 // count and result are exactly those of a check-every-iteration loop.
-#include "sweep.cuh"
+#include "graph.cuh"
 
 #include <algorithm>
 #include <cmath>
-#include <cstring>
 
 namespace b200 {
 namespace {
@@ -127,32 +126,6 @@ __global__ void k_count_negative(T const* a, int64_t n, int* out)
     if (a[i] < (T)0) atomicAdd(out, 1);
 }
 
-// ---- debug: compare the configured sweep with the plain reference sweep, row by row
-template <typename T>
-__global__ void k_fill_pattern(T* x, int32_t n)
-{
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) x[i] = (T)(0.5 + (double)((unsigned)(i * 2654435761u) >> 16) / 65536.0);
-}
-
-// packed (relative difference bits << 32 | row): atomicMax keeps the worst row of each class
-template <typename O, typename T>
-__global__ void k_compare_rows(O const* __restrict__ off, int32_t const* __restrict__ row_vertex, T const* __restrict__ a,
-                               T const* __restrict__ b, int32_t n_rows, int32_t n_hi, double tol,
-                               unsigned long long* __restrict__ worst /*[2]*/, unsigned long long* __restrict__ n_bad /*[2]*/)
-{
-  int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= n_rows) return;
-  const int v        = row_vertex ? row_vertex[r] : r;
-  const double va = (double)a[v], vb = (double)b[v];
-  const double den   = fmax(fabs(va), 1e-300);
-  const float rel    = (float)fmin(fabs(va - vb) / den, 1e30);
-  const int cls      = r < n_hi ? 0 : 1;
-  atomicMax(worst + cls, ((unsigned long long)__float_as_uint(rel) << 32) | (unsigned)r);
-  if (rel > tol) atomicAdd(n_bad + cls, 1ull);
-  (void)off;
-}
-
 struct pr_args {
   device_array_view_impl const* pre_v{nullptr};
   device_array_view_impl const* pre_w{nullptr};
@@ -254,13 +227,10 @@ void pagerank_typed(handle_impl const& h, graph_impl& g, pr_args const& a, centr
 
   // state
   dbuf pr_a = make_dbuf<T>(nv, h.stream), pr_b = make_dbuf<T>(nv, h.stream);
-  dbuf x    = make_dbuf<T>(padded_x_elems(nv, sizeof(T)), h.stream);  // whole smem slices are TMA-copied
-  CUDA_TRY(cudaMemsetAsync(x.data(), 0, padded_x_elems(nv, sizeof(T)) * sizeof(T), h.stream));  // zeros behind nv
-  dbuf acc_hi = make_dbuf<double>(acc_rows(c), h.stream);
-  CUDA_TRY(cudaMemsetAsync(acc_hi.data(), 0, sizeof(double) * acc_rows(c), h.stream));
-  dbuf state = make_dbuf<pr_state_t>(1, h.stream);
-  CUDA_TRY(cudaMemsetAsync(state.data(), 0, sizeof(pr_state_t), h.stream));
-  pr_state_t* st = state.as<pr_state_t>();
+  dbuf x    = make_sweep_x<T>(h, nv);
+  sweep_scratch_t sc;
+  sc.init(h, c);
+  pr_state_t* st = sc.st();
 
   if (a.init_val) {
     // the C API copies the guess as-is (cpp/src/c_api/pagerank.cpp:179-203, no normalisation)
@@ -290,8 +260,7 @@ void pagerank_typed(handle_impl const& h, graph_impl& g, pr_args const& a, centr
   while (true) {
     int todo = std::min(batch, std::max(max_it, 1) - enqueued);
     for (int k = 0; k < todo; ++k) {
-      if (c.offs64) launch_pull_sweep<int64_t, T>(h, c, x.as<T>(), nxt, acc_hi.as<double>(), a.alpha, st);
-      else launch_pull_sweep_auto<int32_t, T>(h, c, nv, x.as<T>(), nxt, acc_hi.as<double>(), a.alpha, st);
+      pull_sweep<T>(h, c, nv, x.as<T>(), nxt, sc, a.alpha);
       if (n_pers > 0)
         B200_LAUNCH(h, (k_personalize<T>), grid_for(n_pers), kBlock, 0, pers_idx.as<int32_t>(), (T const*)a.pers_val->data,
                     n_pers, pers_sum, nxt, st);
@@ -481,17 +450,11 @@ cugraph_error_code_t cugraph_b200_time_pull_spmv(const cugraph_resource_handle_t
     B200_EXPECTS(g->weight_type == FLOAT32, CUGRAPH_NOT_IMPLEMENTED, "time_pull_spmv: float32 graphs only");
     csx_t const& c = pull_view(h, *g);
     int32_t nv     = g->n_vertices;
-    dbuf x = make_dbuf<float>(padded_x_elems(nv, sizeof(float)), h.stream), y = make_dbuf<float>(nv, h.stream);
-    CUDA_TRY(cudaMemsetAsync(x.data(), 0, padded_x_elems(nv, sizeof(float)) * sizeof(float), h.stream));
+    dbuf x = make_sweep_x<float>(h, nv), y = make_dbuf<float>(nv, h.stream);
     B200_LAUNCH(h, (k_fill<float>), grid_for(nv), kBlock, 0, x.as<float>(), nv, 1.0f / (float)nv);
-    dbuf acc = make_dbuf<double>(acc_rows(c), h.stream);
-    CUDA_TRY(cudaMemsetAsync(acc.data(), 0, sizeof(double) * acc_rows(c), h.stream));
-    dbuf state = make_dbuf<pr_state_t>(1, h.stream);
-    CUDA_TRY(cudaMemsetAsync(state.data(), 0, sizeof(pr_state_t), h.stream));
-    auto sweep = [&] {
-      if (c.offs64) launch_pull_sweep<int64_t, float>(h, c, x.as<float>(), y.as<float>(), acc.as<double>(), 0.85, state.as<pr_state_t>());
-      else launch_pull_sweep_auto<int32_t, float>(h, c, nv, x.as<float>(), y.as<float>(), acc.as<double>(), 0.85, state.as<pr_state_t>());
-    };
+    sweep_scratch_t sc;
+    sc.init(h, c);
+    auto sweep = [&] { pull_sweep<float>(h, c, nv, x.as<float>(), y.as<float>(), sc, 0.85); };
     for (int k = 0; k < 3; ++k) sweep();
     cudaEvent_t e0, e1;
     CUDA_TRY(cudaEventCreate(&e0));
@@ -510,55 +473,6 @@ cugraph_error_code_t cugraph_b200_time_pull_spmv(const cugraph_resource_handle_t
     if (algorithmic_bytes_per_sweep)
       *algorithmic_bytes_per_sweep = (double)c.nnz * 4.0 * (g->weighted ? 2.0 : 1.0) +
                                      (double)(nv + 1) * (c.offs64 ? 8.0 : 4.0) + (double)nv * 8.0;
-  });
-}
-
-// Debug hook: y of the sweep PageRank would use on this graph (the shared-memory piece stream when the graph has one)
-// against the plain sweep (k_spmv_hi + k_spmv_low, an independent implementation) on the same pseudo-random x.  out[0..3] = degree >= 32 rows:
-// max relative difference, its row, that row's degree, rows above 1e-5; out[4..7] = the same for the degree < 32 rows.
-cugraph_error_code_t cugraph_b200_debug_compare_sweeps(const cugraph_resource_handle_t* handle, cugraph_graph_t* graph,
-                                                       double* out, cugraph_error_t** error)
-{
-  return guarded(error, [&] {
-    auto const& h = H(handle);
-    auto* g       = G(graph);
-    B200_EXPECTS(out != nullptr, CUGRAPH_INVALID_INPUT, "out is NULL");
-    B200_EXPECTS(g->mg == nullptr && g->weight_type == FLOAT32, CUGRAPH_NOT_IMPLEMENTED, "single-GPU float32 graphs only");
-    csx_t const& c = pull_view(h, *g);
-    B200_EXPECTS(!c.offs64, CUGRAPH_NOT_IMPLEMENTED, "32-bit offsets only");
-    const int32_t nv = g->n_vertices;
-    const size_t px  = padded_x_elems(nv, sizeof(float));
-    dbuf x = make_dbuf<float>(px, h.stream), y0 = make_dbuf<float>(nv, h.stream), y1 = make_dbuf<float>(nv, h.stream);
-    CUDA_TRY(cudaMemsetAsync(x.data(), 0, px * sizeof(float), h.stream));
-    B200_LAUNCH(h, (k_fill_pattern<float>), grid_for(nv), kBlock, 0, x.as<float>(), nv);
-    dbuf acc = make_dbuf<double>(acc_rows(c), h.stream);
-    CUDA_TRY(cudaMemsetAsync(acc.data(), 0, sizeof(double) * acc_rows(c), h.stream));
-    dbuf state = make_dbuf<pr_state_t>(1, h.stream);
-    CUDA_TRY(cudaMemsetAsync(state.data(), 0, sizeof(pr_state_t), h.stream));
-    launch_pull_sweep<int32_t, float>(h, c, x.as<float>(), y0.as<float>(), acc.as<double>(), 0.85, state.as<pr_state_t>());
-    launch_pull_sweep_auto<int32_t, float>(h, c, nv, x.as<float>(), y1.as<float>(), acc.as<double>(), 0.85, state.as<pr_state_t>());
-    dbuf res = make_dbuf<unsigned long long>(4, h.stream);
-    CUDA_TRY(cudaMemsetAsync(res.data(), 0, 4 * sizeof(unsigned long long), h.stream));
-    B200_LAUNCH(h, (k_compare_rows<int32_t, float>), grid_for(c.n_rows), kBlock, 0, c.offsets.as<int32_t>(),
-                c.row_vertex.as<int32_t>(), y0.as<float>(), y1.as<float>(), c.n_rows, c.seg[0], 1e-5,
-                res.as<unsigned long long>(), res.as<unsigned long long>() + 2);
-    unsigned long long hres[4];
-    CUDA_TRY(cudaMemcpyAsync(hres, res.data(), sizeof(hres), cudaMemcpyDeviceToHost, h.stream));
-    sync(h);
-    for (int k = 0; k < 2; ++k) {
-      const unsigned bits = (unsigned)(hres[k] >> 32);
-      float rel;
-      std::memcpy(&rel, &bits, sizeof(rel));
-      const int32_t row = (int32_t)(hres[k] & 0xffffffffu);
-      int32_t offs[2]   = {0, 0};
-      if (c.n_rows > 0)
-        CUDA_TRY(cudaMemcpy(offs, c.offsets.as<int32_t>() + row, sizeof(offs), cudaMemcpyDeviceToHost));
-      out[4 * k + 0] = rel;
-      out[4 * k + 1] = row;
-      out[4 * k + 2] = offs[1] - offs[0];
-      out[4 * k + 3] = (double)hres[2 + k];
-    }
-    check_last("debug_compare_sweeps");
   });
 }
 

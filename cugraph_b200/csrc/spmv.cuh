@@ -22,17 +22,6 @@
 
 namespace b200 {
 
-// device-resident loop state of one PageRank run (no per-iteration host round trip)
-struct pr_state_t {
-  double diff;        // sum |pr_new - pr_old| of the iteration being computed
-  double dangling;    // sum of pr_new over vertices without out-edges
-  double init;        // unvarying part added to every row in the CURRENT sweep
-  double pers_scale;  // (dangling*alpha + 1-alpha) for the personalization scatter
-  double last_diff;
-  int iter;
-  int done;
-};
-
 #ifndef B200_HOST_EMU
 __device__ __forceinline__ int ld_stream(const int* p)
 {
@@ -57,13 +46,6 @@ inline int ld_stream(const int* p) { return *p; }
 inline float ld_stream(const float* p) { return *p; }
 inline double ld_stream(const double* p) { return *p; }
 #endif
-
-__device__ __forceinline__ double warp_sum(double v)
-{
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 
 // ------------------------------------------------------------------------------------------
 // degree >= 32 prefix: one warp per 1024-edge chunk
@@ -234,26 +216,19 @@ void launch_pull_sweep(handle_impl const& h, csx_t const& c, T const* x, T* y, d
   T const* w          = use_weights ? c.weights.as<T>() : nullptr;  // HITS sums plain neighbour values on a weighted graph too
   int32_t const* rv   = c.row_vertex.as<int32_t>();
   const bool weighted = (w != nullptr);
+  auto* const hi_kernel  = weighted ? k_spmv_hi<O, T, true> : k_spmv_hi<O, T, false>;
+  auto* const low_kernel = weighted ? k_spmv_low<O, T, true> : k_spmv_low<O, T, false>;
   if (c.n_chunks > 0) {
     int grid = (c.n_chunks + kWarpsPerCta - 1) / kWarpsPerCta;
-    if (weighted)
-      B200_LAUNCH(h, (k_spmv_hi<O, T, true>), grid, 256, 0, off, idx, w, x, y, rv, c.chunk_first_row.as<int32_t>(),
-                  c.n_chunks, (long long)c.nnz_hi, acc_hi, alpha, st);
-    else
-      B200_LAUNCH(h, (k_spmv_hi<O, T, false>), grid, 256, 0, off, idx, w, x, y, rv, c.chunk_first_row.as<int32_t>(),
-                  c.n_chunks, (long long)c.nnz_hi, acc_hi, alpha, st);
+    B200_LAUNCH(h, hi_kernel, grid, 256, 0, off, idx, w, x, y, rv, c.chunk_first_row.as<int32_t>(), c.n_chunks,
+                (long long)c.nnz_hi, acc_hi, alpha, st);
     if (c.n_split > 0)
       B200_LAUNCH(h, (k_spmv_hi_finish<T>), (c.n_split + 255) / 256, 256, 0, c.split_rows.as<int32_t>(), c.n_split,
                   acc_hi, y, rv, alpha, st);
   }
   low_bins_t bins = make_low_bins(c);
   int lblocks     = bins.block_begin[kNumSeg - 1];
-  if (lblocks > 0) {
-    if (weighted)
-      B200_LAUNCH(h, (k_spmv_low<O, T, true>), lblocks, 256, 0, off, idx, w, x, y, rv, bins, alpha, st);
-    else
-      B200_LAUNCH(h, (k_spmv_low<O, T, false>), lblocks, 256, 0, off, idx, w, x, y, rv, bins, alpha, st);
-  }
+  B200_LAUNCH(h, low_kernel, lblocks, 256, 0, off, idx, w, x, y, rv, bins, alpha, st);
 }
 
 }  // namespace b200

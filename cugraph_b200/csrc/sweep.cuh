@@ -160,6 +160,18 @@ inline unsigned long long make_l2_policy_evict_last() { return 0ull; }
 #define B200_DYN_SMEM(name) extern unsigned char name[] /* one CTA at a time: emu/emu_debug.cpp defines b200::smem_raw */
 #endif
 
+// the slice of column block `block`, x[block * W, (block + 1) * W), into shared memory at `dst` by TMA bulk copies of
+// kTmaPiece bytes, completion signalled on `bar`; one thread issues it
+template <typename T>
+__device__ __forceinline__ void load_slice(unsigned char* dst, T const* x, int block, int W, uint64_t* bar)
+{
+  const unsigned bytes = (unsigned)(W * sizeof(T));
+  mbar_expect_tx(bar, bytes);
+  const unsigned char* src = reinterpret_cast<const unsigned char*>(x + (size_t)block * W);
+  for (unsigned o = 0; o < bytes; o += kTmaPiece)
+    tma_bulk_g2s(dst + o, src + o, (bytes - o) < (unsigned)kTmaPiece ? (bytes - o) : (unsigned)kTmaPiece, bar);
+}
+
 // ------------------------------------------------------------------------------------------
 // per-lane arithmetic
 // ------------------------------------------------------------------------------------------
@@ -564,13 +576,7 @@ __global__ void __launch_bounds__(kSweepThreads, 1) k_sweep(sweep_args_t<T> a)
     const int n            = ph.chunk_end - ph.chunk_begin;
     const bool fresh       = ph.block != cur_block;
     if (fresh) {
-      if (threadIdx.x == 0) {
-        const unsigned bytes = (unsigned)(a.W * sizeof(T));
-        mbar_expect_tx(&bar, bytes);
-        const unsigned char* src = reinterpret_cast<const unsigned char*>(a.x + (size_t)ph.block * a.W);
-        for (unsigned o = 0; o < bytes; o += kTmaPiece)
-          tma_bulk_g2s(smem_raw + o, src + o, (bytes - o) < (unsigned)kTmaPiece ? (bytes - o) : (unsigned)kTmaPiece, &bar);
-      }
+      if (threadIdx.x == 0) load_slice(smem_raw, a.x, ph.block, a.W, &bar);
       cur_block = ph.block;
     }
     // ---- the phase: chunk i is processed while the loads of i+1, the header of i+2 and the draw of i+3 are in flight
@@ -659,11 +665,7 @@ k_sweep_tail(int32_t const* __restrict__ off, int32_t const* __restrict__ idx, T
   if (st->done) return;
   if (threadIdx.x == 0) {
     mbar_init(&bar, 1);
-    const unsigned bytes = (unsigned)(W * sizeof(T));
-    mbar_expect_tx(&bar, bytes);
-    const unsigned char* src = reinterpret_cast<const unsigned char*>(x);
-    for (unsigned o = 0; o < bytes; o += kTmaPiece)
-      tma_bulk_g2s(smem_raw + o, src + o, (bytes - o) < (unsigned)kTmaPiece ? (bytes - o) : (unsigned)kTmaPiece, &bar);
+    load_slice(smem_raw, x, 0, W, &bar);
   }
   const double init = st->init;
   const int stride  = gridDim.x * blockDim.x;
@@ -712,12 +714,13 @@ k_sweep_tail(int32_t const* __restrict__ off, int32_t const* __restrict__ idx, T
 // x must hold padded_x_elems() elements, zero behind n_vertices (slices are copied whole)
 template <typename T>
 void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L, T const* x, T* y, double* acc, double alpha,
-                  pr_state_t const* st, bool use_weights = true, bool covered_rows_only = false)
+                  pr_state_t const* st, bool use_weights, bool covered_rows_only)
 {
-  // the attribute is per device and cheap to set: no process-wide "done" flag (a second device would miss it)
   const bool weighted = use_weights && L.w.data() != nullptr;
-  if (weighted) CUDA_TRY(cudaFuncSetAttribute(k_sweep<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
-  else CUDA_TRY(cudaFuncSetAttribute(k_sweep<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
+  auto* const sweep_kernel = weighted ? k_sweep<T, true> : k_sweep<T, false>;
+  auto* const tail_kernel  = weighted ? k_sweep_tail<T, true> : k_sweep_tail<T, false>;
+  // the attribute is per device and cheap to set: no process-wide "done" flag (a second device would miss it)
+  CUDA_TRY(cudaFuncSetAttribute(sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
   sweep_args_t<T> a;
   a.p.ids     = L.ids.as<uint4>();
   a.p.rows    = L.rows.as<int32_t>();
@@ -746,8 +749,7 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
     a.cta_phase      = L.cta_phase.as<int32_t>() + (size_t)band * L.n_cta;
     a.ph_lo          = L.band_phase[band];
     a.ph_hi          = L.band_phase[band + 1];
-    if (weighted) B200_LAUNCH(h, (k_sweep<T, true>), L.n_cta, kSweepThreads, kSweepDynSmem, a);
-    else B200_LAUNCH(h, (k_sweep<T, false>), L.n_cta, kSweepThreads, kSweepDynSmem, a);
+    B200_LAUNCH(h, sweep_kernel, L.n_cta, kSweepThreads, kSweepDynSmem, a);
     const int n_ph = a.ph_hi - a.ph_lo;
     const int n    = std::max((row_hi - row_lo + 2 * kFinishSteps - 1) / (2 * kFinishSteps), n_ph);  // threads: 16 rows each
     B200_LAUNCH(h, (k_sweep_finish<T, kFinishSteps>), (std::max(n, 1) + 255) / 256, 256, 0, acc, row_lo, L.n_str, row_hi, y,
@@ -757,35 +759,10 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
     const int32_t rows = std::max(finish_rows, L.n_cov) - L.n_str;
     const int blocks   = std::max(1, std::min(h.sm_count, (rows + kTailThreads - 1) / kTailThreads));
     T const* w         = weighted ? c.weights.as<T>() : nullptr;
-    if (weighted) {
-      CUDA_TRY(cudaFuncSetAttribute(k_sweep_tail<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
-      B200_LAUNCH(h, (k_sweep_tail<T, true>), blocks, kTailThreads, kSweepDynSmem, c.offsets.as<int32_t>(),
-                  c.indices.as<int32_t>(), w, x, y, c.row_vertex.as<int32_t>(), L.n_str, L.n_cov, finish_rows, L.W, alpha, st);
-    } else {
-      CUDA_TRY(cudaFuncSetAttribute(k_sweep_tail<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
-      B200_LAUNCH(h, (k_sweep_tail<T, false>), blocks, kTailThreads, kSweepDynSmem, c.offsets.as<int32_t>(),
-                  c.indices.as<int32_t>(), w, x, y, c.row_vertex.as<int32_t>(), L.n_str, L.n_cov, finish_rows, L.W, alpha, st);
-    }
+    CUDA_TRY(cudaFuncSetAttribute(tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
+    B200_LAUNCH(h, tail_kernel, blocks, kTailThreads, kSweepDynSmem, c.offsets.as<int32_t>(), c.indices.as<int32_t>(), w, x, y,
+                c.row_vertex.as<int32_t>(), L.n_str, L.n_cov, finish_rows, L.W, alpha, st);
   }
-}
-
-// dispatch: the piece stream when it exists for this graph, else the plain edge-balanced sweep
-template <typename O, typename T>
-void launch_pull_sweep_auto(handle_impl const& h, csx_t const& c, int32_t n_vertices, T const* x, T* y, double* acc,
-                            double alpha, pr_state_t const* st, bool use_weights = true, bool covered_rows_only = false)
-{
-  sweep_layout_t const* L = sweep_layout(h, c, n_vertices, sizeof(T));
-  if (!L) launch_pull_sweep<O, T>(h, c, x, y, acc, alpha, st, use_weights);  // the plain sweep writes every row
-  else launch_sweep<T>(h, c, *L, x, y, acc, alpha, st, use_weights, covered_rows_only);
-}
-
-// elements an x buffer needs: whole slices are TMA-copied and everything behind n_vertices must read 0.
-// The buffer must be zero-filled once at allocation; only [0, n_vertices) is ever written afterwards.
-inline size_t padded_x_elems(int32_t n_vertices, size_t elem_size)
-{
-  const size_t slice = kHotSliceBytes / elem_size;
-  const size_t W     = slice - kHotZeroPad;
-  return ((size_t)n_vertices / W + 2) * slice;
 }
 
 }  // namespace b200

@@ -1,6 +1,5 @@
 // Accessors for the CPU emulation build (libcugraph_c_emu.so): test infrastructure only, see emu/cuda_runtime.h.
 #include "graph.cuh"
-#include "sweep.cuh"
 
 #include <algorithm>
 #include <vector>
