@@ -52,8 +52,10 @@ constexpr int kBandRowAlign = 512;  // band bounds: a multiple of the finish ker
 // Tail of the piece stream: a row of small in-degree has its few edges in different column blocks, so the stream pays one
 // fp64 RED per edge for it, and such rows are most of the rows (their accumulators decide how many bands are needed).
 // Rows of in-degree < kSweepTailDegree are gathered by k_sweep_tail instead, on graphs of at least kSweepTailMinEdges edges.
-// A kSegThreshold value.  Measured on an H100 80GB HBM3 at 700 W, RMAT-24 PageRank step: 86.3 ms without a tail, 78.8 / 73.4
-// / 72.7 / 74.5 ms with bounds 4 / 8 / 16 / 32 (DESIGN.md §3.2); from 8 on the stream needs one band.
+// A kSegThreshold value.  Measured on an H100 80GB HBM3 at 700 W, RMAT-24 PageRank step, with the row-per-thread tail kernel
+// of before: 86.3 ms without a tail, 78.8 / 73.4 / 72.7 / 74.5 ms with bounds 4 / 8 / 16 / 32 (DESIGN.md §3.2); from 8 on the
+// stream needs one band.  With the tail layout below, at 400 W: 73.1 / 68.3-70.6 / 69.1 ms with bounds 8 / 16 / 32 (sweep
+// 0.660 / 0.635-0.642 / 0.612 ms): 32 is not yet separated from 16 by more than the run-to-run spread.
 constexpr int kSweepTailDegree         = 16;
 constexpr long long kSweepTailMinEdges = 1ll << 24;
 
@@ -81,6 +83,28 @@ struct sweep_phase_t {  // consecutive chunks of one block inside one CTA's rang
   int32_t pad;
 };
 
+// ---------------------------------------------------------------------------------------------
+// Tail layout of the rows [n_str, n_cov) for k_sweep_tail (sweep.cuh).  Rows are degree-descending, so the tail is made of
+// RUNS of rows of one in-degree d (< kSweepTailDegree <= 32).  A run is cut into TILES of 32 consecutive rows, lane l = row
+// first_row + 32 * t + l; entry k of lane l of tile t of a run sits at tail_ids[id_off + t * 32 * d + k * 32 + l] (int32 source
+// id, a row's entries in ascending source order: hubs first).  No offsets and no padding inside a run: every warp-wide load
+// of ids is one 128-byte line; only the last tile of a run has lanes without a row, whose entries read column n_vertices (x
+// is zero there).  A WORK UNIT is tail_unit_tiles(d) consecutive tiles of one run (the last one of a run may be shorter):
+// about kTailUnitEntries entries per lane whatever d, consecutive in tail_ids.
+// ---------------------------------------------------------------------------------------------
+constexpr int kTailTile        = 32;  // rows per tile (= lanes)
+constexpr int kTailUnitEntries = 24;  // entries per lane in a work unit, at least one tile (ids held in registers, twice)
+constexpr int kTailMaxDegree   = 31;  // kSegThreshold[0] - 1: the largest bound leaves rows of in-degree <= 31 in the tail
+__host__ __device__ constexpr int tail_unit_tiles(int d) { return d >= kTailUnitEntries ? 1 : kTailUnitEntries / d; }
+
+struct tail_run_t {   // 24 bytes; a run table ends with a sentinel that holds the totals (first_row = n_cov)
+  int32_t degree;
+  int32_t first_row;
+  int32_t first_tile;
+  int32_t first_unit;
+  int64_t id_off;     // first entry in tail_ids
+};
+
 struct sweep_layout_t {
   int W{0};               // source columns per block (= slice elements - kHotZeroPad)
   int B{0};               // blocks
@@ -98,13 +122,20 @@ struct sweep_layout_t {
   dbuf phases;     // n_phases x sweep_phase_t
   dbuf cta_phase;  // (n_bands * n_cta + 1) x int32: in band b, CTA c owns phases [cta_phase[b * n_cta + c], the next entry)
                    // (cost-balanced, contiguous chunks)
-  dbuf cursor;     // n_phases x int: next chunk of the phase (relative); reset by the finish kernel
+  dbuf cursor;     // n_phases + 1 x int: next chunk of the phase (relative), then the tail's next work unit; reset by the
+                   // finish kernel (the tail's by the last band's, which runs after the previous sweep's tail)
   int32_t n_chunks{0};
   int32_t n_phases{0};
   int n_cta{0};
   int n_bands{1};
   std::vector<int32_t> band_row;    // n_bands + 1: band b holds rows [band_row[b], band_row[b+1]); band_row[n_bands] = n_str
   std::vector<int32_t> band_phase;  // n_bands + 1: the phases of band b are [band_phase[b], band_phase[b+1])
+  // the tail (rows [n_str, n_cov)), when there is one
+  int n_tail_runs{0};
+  std::vector<tail_run_t> tail_runs;  // n_tail_runs + 1 (sentinel), on the host
+  dbuf tail_run;                      // the same on the device
+  dbuf tail_ids;                      // tail_runs[n_tail_runs].id_off x int32
+  dbuf tail_w;                        // the same x T, padding 0; or empty
 };
 
 // One orientation: compressed rows over `n_rows` physical rows.

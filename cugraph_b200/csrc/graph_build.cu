@@ -1320,6 +1320,86 @@ k_sweep_fill(sweep_chunk_t const* __restrict__ chunks, sweep_fill_t const* __res
   }
 }
 
+// ---- the tail layout (graph.cuh): runs of equal in-degree, tiles of 32 rows, lane-interleaved ids
+// below[d] = first row of [row_lo, row_hi) whose in-degree is < d (rows are degree-descending), d = 0 .. kTailMaxDegree + 1
+template <typename O>
+__global__ void k_tail_run_bounds(O const* __restrict__ off, int32_t row_lo, int32_t row_hi, int32_t* __restrict__ below)
+{
+  const int d = blockIdx.x * blockDim.x + threadIdx.x;
+  if (d > kTailMaxDegree + 1) return;
+  int lo = row_lo, hi = row_hi;
+  while (lo < hi) {
+    const int mid = lo + ((hi - lo) >> 1);
+    if ((long long)(off[mid + 1] - off[mid]) >= d) lo = mid + 1; else hi = mid;
+  }
+  below[d] = lo;
+}
+
+// one thread per lane of a tile
+template <typename O, typename T>
+__global__ void k_tail_fill(tail_run_t const* __restrict__ runs, int n_runs, O const* __restrict__ off,
+                            int32_t const* __restrict__ idx, T const* __restrict__ w, int32_t pad_col,
+                            int32_t* __restrict__ ids_out, T* __restrict__ w_out)
+{
+  const long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (t >= (long long)runs[n_runs].first_tile * kTailTile) return;
+  const int tile = (int)(t / kTailTile), lane = (int)(t % kTailTile);
+  int r = 0;
+  while (tile >= runs[r + 1].first_tile) ++r;
+  const tail_run_t R = runs[r];
+  const int d        = R.degree;
+  const int row      = R.first_row + (tile - R.first_tile) * kTailTile + lane;
+  const bool live    = row < runs[r + 1].first_row;
+  const long long e0 = live ? (long long)off[row] : 0;
+  const long long o  = R.id_off + (long long)(tile - R.first_tile) * kTailTile * d + lane;
+  for (int k = 0; k < d; ++k) {
+    ids_out[o + (long long)k * kTailTile] = live ? idx[e0 + k] : pad_col;
+    if (w_out) w_out[o + (long long)k * kTailTile] = live ? w[e0 + k] : (T)0;
+  }
+}
+
+template <typename O>
+void build_tail_layout(handle_impl const& h, csx_t const& c, int32_t nv, size_t es, sweep_layout_t& L)
+{
+  dbuf d_below = make_dbuf<int32_t>(kTailMaxDegree + 2, h.stream);
+  B200_LAUNCH(h, (k_tail_run_bounds<O>), 1, 64, 0, c.offsets.as<O>(), L.n_str, L.n_cov, d_below.as<int32_t>());
+  int32_t below[kTailMaxDegree + 2];
+  CUDA_TRY(cudaMemcpyAsync(below, d_below.data(), sizeof(below), cudaMemcpyDeviceToHost, h.stream));
+  sync(h);
+  tail_run_t at{0, L.n_str, 0, 0, 0};  // the next run starts here
+  for (int d = kTailMaxDegree; d >= 1; --d) {
+    const int32_t lo = below[d + 1], hi = below[d];  // the rows of in-degree d
+    if (hi <= lo) continue;
+    B200_EXPECTS(lo == at.first_row, CUGRAPH_UNKNOWN_ERROR, "tail rows are not degree-descending");
+    at.degree = d;
+    L.tail_runs.push_back(at);
+    const int32_t tiles = (hi - lo + kTailTile - 1) / kTailTile;
+    at.first_row = hi;
+    at.first_tile += tiles;
+    at.first_unit += (tiles + tail_unit_tiles(d) - 1) / tail_unit_tiles(d);
+    at.id_off += (int64_t)tiles * kTailTile * d;
+  }
+  B200_EXPECTS(at.first_row == L.n_cov, CUGRAPH_UNKNOWN_ERROR, "tail rows of in-degree >= the bound or 0");
+  at.degree     = 0;
+  L.n_tail_runs = (int)L.tail_runs.size();
+  L.tail_runs.push_back(at);
+  L.tail_run = make_dbuf<tail_run_t>(L.tail_runs.size(), h.stream);
+  CUDA_TRY(cudaMemcpyAsync(L.tail_run.data(), L.tail_runs.data(), sizeof(tail_run_t) * L.tail_runs.size(), cudaMemcpyHostToDevice,
+                           h.stream));
+  L.tail_ids = make_dbuf<int32_t>((size_t)std::max<int64_t>(at.id_off, 1), h.stream);
+  const bool weighted = c.weights.data() != nullptr;
+  if (weighted) L.tail_w = dbuf((size_t)std::max<int64_t>(at.id_off, 1) * es, h.stream);
+  const int64_t threads = (int64_t)at.first_tile * kTailTile;
+  if (es == 4)
+    B200_LAUNCH(h, (k_tail_fill<O, float>), grid_for(threads), kBlock, 0, L.tail_run.as<tail_run_t>(), L.n_tail_runs,
+                c.offsets.as<O>(), c.indices.as<int32_t>(), c.weights.as<float>(), nv, L.tail_ids.as<int32_t>(), L.tail_w.as<float>());
+  else
+    B200_LAUNCH(h, (k_tail_fill<O, double>), grid_for(threads), kBlock, 0, L.tail_run.as<tail_run_t>(), L.n_tail_runs,
+                c.offsets.as<O>(), c.indices.as<int32_t>(), c.weights.as<double>(), nv, L.tail_ids.as<int32_t>(), L.tail_w.as<double>());
+  check_last("sweep tail layout");
+  sync(h);  // the host run table is pageable
+}
+
 // Row bands: the sweep's fp64 REDs into acc[row] hit the L2 only while the rows they scatter over fit in it (measured on an
 // H100 80GB HBM3 at 700 W, 50 MB of L2: a scattered RED.64 costs the same up to 24 MB of accumulators, 1.3x at 48 MB and
 // 3.7x at 64 MB), so the stream rows are split into bands whose accumulators take at most kBandL2Share of the L2.  Half
@@ -1473,8 +1553,8 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   }
   CUDA_TRY(cudaMemcpyAsync(L->cta_phase.data(), plan.cta_phase.data(), sizeof(int32_t) * plan.cta_phase.size(), cudaMemcpyHostToDevice, h.stream));
   sync(h);  // the host vectors are pageable
-  L->cursor = make_dbuf<int>(std::max(L->n_phases, 1), h.stream);
-  CUDA_TRY(cudaMemsetAsync(L->cursor.data(), 0, sizeof(int) * std::max(L->n_phases, 1), h.stream));
+  L->cursor = make_dbuf<int>(L->n_phases + 1, h.stream);  // the last one: the tail's
+  CUDA_TRY(cudaMemsetAsync(L->cursor.data(), 0, sizeof(int) * (L->n_phases + 1), h.stream));
 
   // 5. step-rows and row slots
   L->ids  = make_dbuf<uint4>((size_t)std::max<int64_t>(L->n_steprows, 1) * 32, h.stream);
@@ -1500,6 +1580,14 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   check_last("sweep layout");
   sync(h);
   tr.mark("sweep layout: fill");
+  if (n_str < n_cov) {
+    build_tail_layout<O>(h, c, nv, es, *L);
+    tr.mark("sweep layout: tail");
+    if (tr.on) {
+      std::fprintf(stderr, "[sweep] tail: %d runs, %d tiles, %d units, %.1f MB of ids\n", L->n_tail_runs,
+                   L->tail_runs.back().first_tile, L->tail_runs.back().first_unit, (double)L->tail_runs.back().id_off * 4 / 1e6);
+    }
+  }
   if (tr.on) {
     std::fprintf(stderr, "[sweep] %lld step-rows = %.1f MB of ids, %lld row slots = %.1f MB, %d chunks, %d phases, %d CTAs\n",
                  (long long)L->n_steprows, (double)L->n_steprows * 512 / 1e6, (long long)L->n_rowslots,

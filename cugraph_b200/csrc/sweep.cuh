@@ -23,8 +23,8 @@
 //   * the rows are split into bands whose accumulators fit in the L2 (graph.cuh); the sweep runs band by band, k_sweep over
 //     the band's phases, then k_sweep_finish over its rows while their accumulators are still in the L2.
 //   * on large graphs the rows of small in-degree (the tail, graph.cuh) are not in the stream: one k_sweep_tail launch after
-//     the bands gathers their few edges directly (no RED, and fewer stream rows need fewer bands), the hubs' x from a
-//     shared-memory copy of the first column block.
+//     the bands gathers their few edges directly from a layout of their own (runs of equal in-degree, lane-interleaved: no
+//     RED, and fewer stream rows need fewer bands), the hubs' x from a shared-memory copy of the first column block.
 #pragma once
 #include "spmv.cuh"
 
@@ -645,70 +645,168 @@ k_sweep_finish(double* __restrict__ acc, int row_lo, int n_cov, int n_rows, T* _
   }
 }
 
-// The tail rows [row_lo, row_hi) (graph.cuh), then y = init for the empty rows [row_hi, empty_hi).  A thread per row, the
-// row's entries gathered kTailBatch at a time with all loads of a batch issued back to back, the next row's offsets in
-// flight meanwhile; fp64 sum, rounded once, no RED.  The tail's sources are mostly hubs (RMAT-24: 47 % of them in the first
-// column block), and a plain row kernel pays a 32-byte L2 sector for each of those 4-byte gathers: here persistent CTAs
-// (one per SM) keep x[0, W) in shared memory, loaded once by TMA bulk copies as in k_sweep, and gather the rest through L1.
-constexpr int kTailThreads = 1024;
+// The tail rows [n_str, n_cov) from the tail layout (graph.cuh), then y = init for the empty rows [n_cov, empty_hi).  Its
+// sources are mostly hubs (RMAT-24: 47 % of them in the first column block), and a plain row kernel pays a 32-byte L2 sector
+// for each of those 4-byte gathers: persistent CTAs (one per SM) keep x[0, W) in shared memory, loaded once by TMA bulk
+// copies as in k_sweep, and gather the other sources from global memory with an evict-LAST hint (x is reused across the
+// tail, the ids are read once and marked evict-first).  Warps draw WORK UNITS (a few tiles of one run, ~24 entries per lane)
+// from one cursor, so every SM works until the tail is done; a unit's ids are one contiguous lane-interleaved span, loaded by
+// one fully used 128-byte line per warp-wide load, and the next unit's ids are in flight while a unit is processed.  The
+// entries of a lane are its row's: the row sum is made in registers (products in T, batches of 8 summed in fp64 as a tree,
+// rounded once) and stored, no RED and no accumulator.  The processing is instantiated per in-degree d (registers are
+// indexed statically).
+constexpr int kTailThreads = 512;  // 16 warps, up to 128 registers: two units of ids and one unit of gathers per lane
 constexpr int kTailBatch   = 8;
 
+#ifndef B200_HOST_EMU
+__device__ __forceinline__ float ld_keep(float const* p, unsigned long long pol)
+{
+  float v;
+  asm("ld.global.nc.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(p), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ double ld_keep(double const* p, unsigned long long pol)
+{
+  double v;
+  asm("ld.global.nc.L2::cache_hint.f64 %0, [%1], %2;" : "=d"(v) : "l"(p), "l"(pol));
+  return v;
+}
+#else
+inline float ld_keep(float const* p, unsigned long long) { return *p; }
+inline double ld_keep(double const* p, unsigned long long) { return *p; }
+#endif
+
+template <typename T>
+struct tail_args_t {
+  tail_run_t const* __restrict__ runs;  // n_runs + 1
+  int32_t const* __restrict__ ids;
+  T const* __restrict__ w;  // or nullptr
+  T const* __restrict__ x;
+  T* __restrict__ y;
+  int32_t const* __restrict__ row_vertex;
+  int* __restrict__ cursor;
+  pr_state_t const* __restrict__ st;
+  int n_runs, empty_hi, W;
+  double alpha;
+};
+
+struct tail_unit_t {  // warp-uniform; d = 0: no unit
+  int d, n_tiles, row0, row_end;
+  long long base;  // first entry in tail_ids
+};
+
+__device__ __forceinline__ tail_unit_t tail_unit(tail_run_t const* runs, int n_runs, int u)
+{
+  tail_unit_t t{0, 0, 0, 0, 0};
+  if (u >= runs[n_runs].first_unit) return t;
+  int r = 0;
+  while (u >= runs[r + 1].first_unit) ++r;
+  const tail_run_t R = runs[r];
+  const int per      = tail_unit_tiles(R.degree);
+  const int tile     = (u - R.first_unit) * per;  // inside the run
+  t.d                = R.degree;
+  const int left     = runs[r + 1].first_tile - R.first_tile - tile;
+  t.n_tiles          = left < per ? left : per;
+  t.row0             = R.first_row + tile * kTailTile;
+  t.row_end          = runs[r + 1].first_row;
+  t.base             = R.id_off + (long long)tile * kTailTile * R.degree;
+  return t;
+}
+
+// the ids of a unit: entry j of this lane at base + 32 j (j < n_tiles * d <= kTailUnitEntries)
+__device__ __forceinline__ void tail_load(int (&q)[kTailUnitEntries], tail_unit_t const& u, int32_t const* __restrict__ ids,
+                                          unsigned long long pol, int lane)
+{
+  const int n         = u.n_tiles * u.d;  // the first kTailUnitEntries of them
+  int32_t const* base = ids + u.base + lane;
+#pragma unroll
+  for (int j = 0; j < kTailUnitEntries; ++j)
+    if (j < n) q[j] = ld_stream_i32(base + j * kTailTile, pol);
+}
+
+// the unit's rows, in-degree D: a row's entries in batches of 8, gathered, then summed as an fp64 tree (the order of
+// k_spmv_low), the batches added in order
+template <typename T, bool WEIGHTED, int D>
+__device__ __forceinline__ void tail_rows(int const (&q)[kTailUnitEntries], tail_unit_t const& u, tail_args_t<T> const& a,
+                                          T const* __restrict__ sx, double init, unsigned long long pol, unsigned long long keep,
+                                          int lane)
+{
+  constexpr int U = tail_unit_tiles(D);
+  T const* wp       = WEIGHTED ? a.w + u.base + lane : nullptr;  // entry j: wp[32 j]
+#pragma unroll
+  for (int t = 0; t < U; ++t) {
+    if (t < u.n_tiles) {
+      double s = 0.0;
+#pragma unroll
+      for (int k0 = 0; k0 < D; k0 += kTailBatch) {
+        double b[kTailBatch];
+#pragma unroll
+        for (int i = 0; i < kTailBatch; ++i) {
+          b[i] = 0.0;
+          if (k0 + i < D) {
+            const int j = t * D + k0 + i;  // a tile holds more entries than a unit's registers only at D > kTailUnitEntries
+            const int c = j < kTailUnitEntries ? q[j] : ld_stream_i32(a.ids + u.base + j * kTailTile + lane, pol);
+            T v         = c < a.W ? sx[c] : ld_keep(a.x + c, keep);
+            if (WEIGHTED) v *= ld_stream(wp + j * kTailTile);
+            b[i] = (double)v;
+          }
+        }
+        s += ((b[0] + b[1]) + (b[2] + b[3])) + ((b[4] + b[5]) + (b[6] + b[7]));
+      }
+      const int row = u.row0 + t * kTailTile + lane;
+      if (row < u.row_end) a.y[a.row_vertex ? a.row_vertex[row] : row] = (T)(s * a.alpha + init);
+    }
+  }
+}
+
+template <typename T, bool WEIGHTED, int D = 1>
+__device__ __forceinline__ void tail_process(int const (&q)[kTailUnitEntries], tail_unit_t const& u, tail_args_t<T> const& a,
+                                             T const* __restrict__ sx, double init, unsigned long long pol,
+                                             unsigned long long keep, int lane)
+{
+  if (u.d == D) tail_rows<T, WEIGHTED, D>(q, u, a, sx, init, pol, keep, lane);
+  else if constexpr (D < kTailMaxDegree) tail_process<T, WEIGHTED, D + 1>(q, u, a, sx, init, pol, keep, lane);
+}
+
 template <typename T, bool WEIGHTED>
-__global__ void __launch_bounds__(kTailThreads, 1)
-k_sweep_tail(int32_t const* __restrict__ off, int32_t const* __restrict__ idx, T const* __restrict__ w, T const* __restrict__ x,
-             T* __restrict__ y, int32_t const* __restrict__ row_vertex, int row_lo, int row_hi, int empty_hi, int W,
-             double alpha, pr_state_t const* __restrict__ st)
+__global__ void __launch_bounds__(kTailThreads, 1) k_sweep_tail(tail_args_t<T> a)
 {
   B200_DYN_SMEM(smem_raw);
   T const* sx = reinterpret_cast<T const*>(smem_raw);
   __shared__ uint64_t bar;
-  if (st->done) return;
+  __shared__ tail_run_t s_run[kTailMaxDegree + 1];
+  if (a.st->done) return;
+  const unsigned long long pol = make_l2_policy_evict_first(), keep = make_l2_policy_evict_last();
+  const int lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     mbar_init(&bar, 1);
-    load_slice(smem_raw, x, 0, W, &bar);
+    load_slice(smem_raw, a.x, 0, a.W, &bar);
   }
-  const double init = st->init;
-  const int stride  = gridDim.x * blockDim.x;
-  int r             = row_lo + (int)(blockIdx.x * blockDim.x + threadIdx.x);
-  int lo = 0, hi = 0;
-  if (r < row_hi) {
-    lo = __ldg(off + r);
-    hi = __ldg(off + r + 1);
-  }
-  __syncthreads();  // the barrier is initialised before anybody waits on it
+  if ((int)threadIdx.x <= a.n_runs) s_run[threadIdx.x] = a.runs[threadIdx.x];
+  const double init = a.st->init;
+  __syncthreads();  // the barrier is initialised before anybody waits on it, the run table is in place
+  // unit i is processed while the ids of unit i+1 and the draw of unit i+2 are in flight
+  const int ra = draw_issue(a.cursor, 1, lane, true), rb = draw_issue(a.cursor, 1, lane, true);
+  tail_unit_t A = tail_unit(s_run, a.n_runs, draw_get(ra));
+  int qa[kTailUnitEntries], qb[kTailUnitEntries];
+  tail_load(qa, A, a.ids, pol, lane);
+  tail_unit_t B = tail_unit(s_run, a.n_runs, draw_get(rb));
   mbar_wait(&bar, 0);
-  for (; r < row_hi; r += stride) {
-    const int rn = r + stride;
-    int nlo = 0, nhi = 0;
-    if (rn < row_hi) {
-      nlo = __ldg(off + rn);
-      nhi = __ldg(off + rn + 1);
-    }
-    double s = 0.0;
-    for (int e = lo; e < hi; e += kTailBatch) {
-      int c[kTailBatch];
-      T wv[kTailBatch];
-#pragma unroll
-      for (int k = 0; k < kTailBatch; ++k) {
-        c[k]  = 0;
-        wv[k] = (T)0;
-        if (e + k < hi) {
-          c[k]  = __ldg(idx + e + k);
-          wv[k] = WEIGHTED ? __ldg(w + e + k) : (T)1;
-        }
-      }
-      T v[kTailBatch];
-#pragma unroll
-      for (int k = 0; k < kTailBatch; ++k) v[k] = (c[k] < W ? sx[c[k]] : __ldg(x + c[k])) * wv[k];
-      s += (((double)v[0] + (double)v[1]) + ((double)v[2] + (double)v[3])) +
-           (((double)v[4] + (double)v[5]) + ((double)v[6] + (double)v[7]));
-    }
-    y[row_vertex ? row_vertex[r] : r] = (T)(s * alpha + init);
-    lo = nlo;
-    hi = nhi;
+  while (A.d > 0) {
+    tail_load(qb, B, a.ids, pol, lane);
+    const int rc = draw_issue(a.cursor, 1, lane, B.d > 0);
+    tail_process<T, WEIGHTED>(qa, A, a, sx, init, pol, keep, lane);
+    if (B.d == 0) break;
+    const tail_unit_t C = tail_unit(s_run, a.n_runs, draw_get(rc));
+    tail_load(qa, C, a.ids, pol, lane);
+    const int rd = draw_issue(a.cursor, 1, lane, C.d > 0);
+    tail_process<T, WEIGHTED>(qb, B, a, sx, init, pol, keep, lane);
+    A = C;
+    B = tail_unit(s_run, a.n_runs, draw_get(rd));
   }
-  for (int q = row_hi + (int)(blockIdx.x * blockDim.x + threadIdx.x); q < empty_hi; q += stride)
-    y[row_vertex ? row_vertex[q] : q] = (T)init;
+  const int stride = gridDim.x * blockDim.x;
+  for (int r = a.runs[a.n_runs].first_row + (int)(blockIdx.x * blockDim.x + threadIdx.x); r < a.empty_hi; r += stride)
+    a.y[a.row_vertex ? a.row_vertex[r] : r] = (T)init;
 }
 
 // x must hold padded_x_elems() elements, zero behind n_vertices (slices are copied whole)
@@ -750,18 +848,30 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
     a.ph_lo          = L.band_phase[band];
     a.ph_hi          = L.band_phase[band + 1];
     B200_LAUNCH(h, sweep_kernel, L.n_cta, kSweepThreads, kSweepDynSmem, a);
-    const int n_ph = a.ph_hi - a.ph_lo;
+    // the cursors to reset: the band's phases', and on the last band the tail's behind them (its previous sweep is done)
+    const int n_ph = a.ph_hi - a.ph_lo + (band == L.n_bands - 1 && tail ? 1 : 0);
     const int n    = std::max((row_hi - row_lo + 2 * kFinishSteps - 1) / (2 * kFinishSteps), n_ph);  // threads: 16 rows each
     B200_LAUNCH(h, (k_sweep_finish<T, kFinishSteps>), (std::max(n, 1) + 255) / 256, 256, 0, acc, row_lo, L.n_str, row_hi, y,
                 c.row_vertex.as<int32_t>(), alpha, L.cursor.as<int>() + a.ph_lo, n_ph, st);
   }
   if (tail) {  // the rows [n_str, n_cov) and (unless covered_rows_only) the empty rows, by k_sweep_tail
-    const int32_t rows = std::max(finish_rows, L.n_cov) - L.n_str;
-    const int blocks   = std::max(1, std::min(h.sm_count, (rows + kTailThreads - 1) / kTailThreads));
-    T const* w         = weighted ? c.weights.as<T>() : nullptr;
+    tail_args_t<T> t;
+    t.runs       = L.tail_run.as<tail_run_t>();
+    t.ids        = L.tail_ids.as<int32_t>();
+    t.w          = weighted ? L.tail_w.as<T>() : nullptr;
+    t.x          = x;
+    t.y          = y;
+    t.row_vertex = c.row_vertex.as<int32_t>();
+    t.cursor     = L.cursor.as<int>() + L.n_phases;
+    t.st         = st;
+    t.n_runs     = L.n_tail_runs;
+    t.empty_hi   = finish_rows;
+    t.W          = L.W;
+    t.alpha      = alpha;
+    const int units  = L.tail_runs.back().first_unit;
+    const int blocks = std::max(1, std::min(h.sm_count, (units + kTailThreads / 32 - 1) / (kTailThreads / 32)));
     CUDA_TRY(cudaFuncSetAttribute(tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
-    B200_LAUNCH(h, tail_kernel, blocks, kTailThreads, kSweepDynSmem, c.offsets.as<int32_t>(), c.indices.as<int32_t>(), w, x, y,
-                c.row_vertex.as<int32_t>(), L.n_str, L.n_cov, finish_rows, L.W, alpha, st);
+    B200_LAUNCH(h, tail_kernel, blocks, kTailThreads, kSweepDynSmem, t);
   }
 }
 

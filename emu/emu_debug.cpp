@@ -79,6 +79,24 @@ EMU_EXPORT int32_t emu_sweep_stream_rows(cugraph_graph_t* graph, size_t es)
   return L ? L->n_str : -1;
 }
 
+// tail layout of that piece stream: returns its runs (0 without a tail, -1 without a layout); runs receives n_runs + 1 x
+// {degree, first_row, first_tile, first_unit, id_off} when it holds `capacity` entries, ptrs[2] = tail_ids, tail_w
+EMU_EXPORT int emu_sweep_tail(cugraph_graph_t* graph, size_t es, int64_t* runs, size_t capacity, void** ptrs)
+{
+  auto* g                 = reinterpret_cast<graph_impl*>(graph);
+  sweep_layout_t const* L = (es == 4 ? g->primary->hot4 : g->primary->hot8).get();
+  if (!L) return -1;
+  if (L->tail_runs.size() <= capacity)
+    for (size_t k = 0; k < L->tail_runs.size(); ++k) {
+      tail_run_t const& r = L->tail_runs[k];
+      int64_t* o          = runs + 5 * k;
+      o[0] = r.degree; o[1] = r.first_row; o[2] = r.first_tile; o[3] = r.first_unit; o[4] = r.id_off;
+    }
+  ptrs[0] = L->tail_ids.data();
+  ptrs[1] = L->tail_w.data();
+  return L->n_tail_runs;
+}
+
 EMU_EXPORT size_t emu_padded_x_elems(int32_t nv, size_t es) { return padded_x_elems(nv, es); }
 
 // forget the cached layouts of the primary orientation (so that another set of knobs can be staged)
