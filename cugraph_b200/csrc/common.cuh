@@ -312,7 +312,7 @@ __device__ __forceinline__ bool is_commit_lane() { return (threadIdx.x & 31) == 
 #define B200_LAUNCH(h, kernel, grid, block, smem, ...)                           \
   do {                                                                           \
     if ((grid) > 0) {                                                            \
-      emu_launch((grid), (block), [&] { kernel(__VA_ARGS__); });                 \
+      emu_launch((grid), (block), (size_t)(smem), [&] { kernel(__VA_ARGS__); }); \
       (h).launches++;                                                            \
     }                                                                            \
   } while (0)

@@ -177,9 +177,10 @@ k_spmv_low(O const* __restrict__ offsets, int32_t const* __restrict__ indices, T
         wv[k] = WEIGHTED ? __ldg(weights + e) : (T)1;
       }
     }
+    // a lane's unused entries are 0, not x[0] * 0: x may hold anything (NaN, inf) in a column no edge reads
     T v[kR];
 #pragma unroll
-    for (int k = 0; k < kR; ++k) v[k] = x[c[k]] * wv[k];
+    for (int k = 0; k < kR; ++k) v[k] = lo + sub + (long long)k * g < hi ? x[c[k]] * wv[k] : (T)0;
     acc = (((double)v[0] + (double)v[1]) + ((double)v[2] + (double)v[3])) +
           (((double)v[4] + (double)v[5]) + ((double)v[6] + (double)v[7]));
   }

@@ -201,6 +201,26 @@ inline void emu_launch(long long grid, long long block, F&& body)
   }
 }
 
+// A launch with `smem` bytes of dynamic shared memory (b200::smem_raw, emu/emu_debug.cpp).  On the GPU a CTA finds whatever
+// the SM's shared memory held before; here every CTA finds NaN bytes (0xff: NaN as float and as double), so that a kernel
+// that reads shared memory it never wrote shows it in its results.
+namespace b200 {
+extern unsigned char smem_raw[];
+}
+template <typename F>
+inline void emu_launch(long long grid, long long block, size_t smem, F&& body)
+{
+  if (block > emu::kMaxThreads) { std::fprintf(stderr, "emu: block of %lld threads\n", block); std::abort(); }
+  gridDim        = dim3((unsigned)grid);
+  blockDim       = dim3((unsigned)block);
+  emu::cta().body = [&] { body(); };
+  for (long long b = 0; b < grid; ++b) {
+    blockIdx.x = (unsigned)b;
+    if (smem > 0) std::memset(b200::smem_raw, 0xff, smem);
+    emu::run_cta((int)block);
+  }
+}
+
 // ---- runtime API
 typedef int cudaError_t;
 enum { cudaSuccess = 0, cudaErrorMemoryAllocation = 2 };

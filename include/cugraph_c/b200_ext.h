@@ -51,9 +51,11 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_create(
 CUGRAPH_EXPORT void cugraph_b200_block_free(cugraph_b200_block_t* block);
 CUGRAPH_EXPORT size_t cugraph_b200_block_span(const cugraph_b200_block_t* block);
 /* y[row] = alpha * sum over the block's edges (row, col) of x[col] * w; rows without edges get 0.  The FIRST sweep of a block
- * into a given y array writes every row slot; later sweeps into the same array only rewrite the rows that have edges (in a 2D
- * block most row slots are empty) — the caller must leave the other entries alone, or pass a zero-initialised array.
- * x and y must not overlap: rows are written band by band while later bands still read x. */
+ * into a given y array writes every row slot; later sweeps into the same array may rewrite only the rows that have edges (in a
+ * 2D block most row slots are empty) — the caller must leave the other entries alone, or pass a zero-initialised array.
+ * x holds cugraph_b200_padded_elems(span) elements: x[col] for the columns, ZERO from index `span` on (whole slices of x are
+ * copied, and padding entries read a column at or behind the span); a column that no edge reads may hold anything, NaN
+ * included.  x and y must not overlap: rows are written band by band while later bands still read x. */
 CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_pull_sweep(
   const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
   const cugraph_type_erased_device_array_view_t* x, cugraph_type_erased_device_array_view_t* y, double alpha,

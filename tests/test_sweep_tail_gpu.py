@@ -1,6 +1,8 @@
-"""The piece-stream sweep with a tail on the GPU: the rows of in-degree < 8 are swept by the row kernel after the bands.  A
+"""The piece-stream sweep with a tail on the GPU: the rows of in-degree < 8 leave the stream and are swept by k_sweep_tail
+after the bands, from the tail layout (runs of equal in-degree, lane-interleaved ids, work units drawn from a cursor).  A
 forced bound on RMAT-16 (the default gives such a small graph no tail), with one band and with three, against the fp64 oracle
-(1e-6 relative at equal iteration count) and row by row against the plain sweep."""
+(1e-6 relative at equal iteration count) and row by row against the plain sweep.  Every bound, element type and layout path
+is checked row by row against an fp64 reference in tests/test_sweep_rows_gpu.py."""
 import ctypes as C
 
 import numpy as np
