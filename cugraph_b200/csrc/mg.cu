@@ -6,8 +6,8 @@
 // torch.distributed (NCCL on NVLink 5 / NVSwitch).  This file provides the device-side pieces behind
 // the C ABI: a resource handle bound to the caller's CUDA stream, rectangular edge blocks with the
 // same binned / column-blocked layout as the single-GPU graph, the block pull sweep and the fused
-// per-iteration vertex step, the BFS pull step and the SSSP push relaxation.  All calls only ENQUEUE work on the handle's
-// stream (the SSSP calls read back one queue size).
+// per-iteration vertex step, the BFS pull step, the SSSP push relaxation and the WCC min-label round.  All calls only
+// ENQUEUE work on the handle's stream (the SSSP and WCC calls read back one queue size).
 #include "advance.cuh"
 
 #include <algorithm>
@@ -171,7 +171,12 @@ struct block_queue_counts_t {
   unsigned long long edges;  // their degree sum
 };
 
-// physical rows r < n_ne of the push copy whose column slot row_vertex[r] holds a finite distance, with their degrees
+// whether a column takes part in a round: a finite SSSP distance, a WCC label other than INT64_MAX
+__device__ __forceinline__ bool column_active(float v) { return v < INFINITY; }
+__device__ __forceinline__ bool column_active(double v) { return v < INFINITY; }
+__device__ __forceinline__ bool column_active(long long v) { return v != LLONG_MAX; }
+
+// physical rows r < n_ne of the push copy whose column slot row_vertex[r] is active, with their degrees
 template <typename O, typename T>
 __global__ void __launch_bounds__(kBlock)
 k_block_active_rows(O const* __restrict__ off, int32_t const* __restrict__ row_vertex, int32_t n_ne, T const* __restrict__ dist_cols,
@@ -179,7 +184,7 @@ k_block_active_rows(O const* __restrict__ off, int32_t const* __restrict__ row_v
 {
   unsigned long long edges = 0;
   for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < n_ne; r += gridDim.x * blockDim.x) {
-    if (dist_cols[row_vertex[r]] < (T)INFINITY) {
+    if (column_active(dist_cols[row_vertex[r]])) {
       const int32_t d = (int32_t)((long long)off[r + 1] - (long long)off[r]);
       const int pos   = warp_append(&cnt->n);
       q[pos]          = r;
@@ -303,6 +308,22 @@ void check_sssp_block_args(block_impl const& b, device_array_view_impl const* dv
                "distance / candidate arrays shorter than the block's slots");
   B200_EXPECTS(maxpart > 0 && grid_cols > 0 && grid_c >= 0 && grid_c < grid_cols, CUGRAPH_INVALID_INPUT, "bad grid position");
 }
+
+// ---- one round of multi-GPU weakly connected components on this GPU's edge block (min-label propagation).  The launcher
+// gathers the labels of the vertices that changed in the last round (INT64_MAX for all others) over the block's column
+// slots; the push copy turns the active columns into a queue and the merge-path advance offers every active column's
+// label to its rows with atomicMin, reduced to the owners by a MIN reduce-scatter.  A dense pull over the block's rows
+// without atomics lost every round to this push on RMAT-24 and was removed (DESIGN §6).
+struct block_wcc_op {
+  int32_t const* col_of;  // column slot of a physical row of the push copy
+  long long const* label;  // over column slots, INT64_MAX = inactive
+  long long* cand;         // over row slots
+  __device__ __forceinline__ void edge(int src, long long, int nbr) const
+  {
+    const long long l = label[col_of[src]];
+    if (l < cand[nbr]) atomicMin(cand + nbr, l);  // a stale read is larger than the current value: never skips a win
+  }
+};
 
 }  // namespace
 
@@ -562,6 +583,31 @@ cugraph_error_code_t cugraph_b200_block_sssp_pred(const cugraph_resource_handle_
       else block_push_round<int32_t>(h, p, (double const*)dv->data, op);
     }
     check_last("block_sssp_pred");
+  });
+}
+
+// cand_rows[row slot] = smallest label_cols[col] over the row's sources, INT64_MAX when none is active
+cugraph_error_code_t cugraph_b200_block_wcc_min(const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+                                                const cugraph_type_erased_device_array_view_t* label_cols,
+                                                cugraph_type_erased_device_array_view_t* cand_rows, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(block && label_cols && cand_rows, CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto* b        = reinterpret_cast<block_impl*>(block);
+    auto const* lv = V(label_cols);
+    auto const* cv = V(cand_rows);
+    B200_EXPECTS(lv->type == INT64 && cv->type == INT64, CUGRAPH_INVALID_INPUT, "label_cols / cand_rows must be INT64");
+    B200_EXPECTS(lv->size >= (size_t)b->n_cols && cv->size >= (size_t)b->n_rows, CUGRAPH_INVALID_INPUT,
+                 "label / candidate arrays shorter than the block's slots");
+    block_push_t& p   = push_copy(h, *b);
+    auto const* label = (long long const*)lv->data;
+    auto* cand        = (long long*)cv->data;
+    B200_LAUNCH(h, k_fill_i64, std::min((b->n_rows + 255) / 256 + 1, h.sm_count * 8), 256, 0, cand, (long long)b->n_rows, LLONG_MAX);
+    block_wcc_op op{p.csx->row_vertex.as<int32_t>(), label, cand};
+    if (p.csx->offs64) block_push_round<int64_t>(h, p, label, op);
+    else block_push_round<int32_t>(h, p, label, op);
+    check_last("block_wcc_min");
   });
 }
 

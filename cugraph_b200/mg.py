@@ -1,4 +1,4 @@
-"""Multi-GPU PageRank, BFS and SSSP: 2D edge partition over one process per GPU (torch.distributed, NCCL on NVLink 5).
+"""Multi-GPU PageRank, BFS, SSSP and weakly connected components: 2D edge partition over one process per GPU (torch.distributed, NCCL on NVLink 5).
 
 What the reference does (SURVEY.md §8e): P = R x C GPUs, vertex -> GPU by hash
 (cpp/include/cugraph/utilities/graph_partition_utils.cuh:30-43, 101-128), every GPU holds the edge
@@ -14,10 +14,12 @@ same column-blocked shared-memory kernel as on one GPU (C-ABI: cugraph_b200_bloc
 
 BFS moves byte flags per level (one max-reduce-scatter of candidate predecessors); SSSP runs Δ-windows of rounds, each an
 all-gather of the frontier's distances, the block's push relaxation on the device and one min-reduce-scatter of INT64
-(distance, predecessor) keys (see MGGraph.sssp).
+(distance, predecessor) keys (see MGGraph.sssp); WCC propagates the smallest vertex code per round, with one
+min-reduce-scatter of INT64 labels (see MGGraph.weakly_connected_components).
 
 `partition_edges` (pure torch, device agnostic: exercised on CPU with the gloo backend in
-tests/test_mg_partition_cpu.py) builds the blocks; `MGGraph` / `pagerank` / `bfs` / `sssp` need CUDA.
+tests/test_mg_partition_cpu.py) builds the blocks; `MGGraph` / `pagerank` / `bfs` / `sssp` / `weakly_connected_components`
+need CUDA.
 """
 from __future__ import annotations
 
@@ -269,6 +271,7 @@ class MGGraph:
         self._w_sum_local = float(ones.sum().item()) if self.weighted else 0.0   # SSSP's initial window width
         self._sssp_avg = None                                                       # (average weight, average degree)
         self.last_sssp_stats = None
+        self.last_wcc_stats = None
         self.device = src.device
         p.rows = p.cols = p.weights = None  # the block owns its own copy
         torch.cuda.synchronize()
@@ -569,6 +572,56 @@ class MGGraph:
             return verts, d_out, None
         return verts, d_out, self._codes_to_external(pred_code[:p.n_local])
 
+    # ------------------------------------------------------------------------------------------
+    # multi-GPU weakly connected components: min-label propagation.  Every owned vertex starts with its own code (owner
+    # rank * maxpart + local id, as in bfs / sssp) and is marked changed.  One round: the labels of the changed vertices
+    # (INT64_MAX for the others) are all-gathered inside the column group over the block's source slots; the block gives
+    # every destination slot the smallest label among its sources (cugraph_b200_block_wcc_min: an atomicMin push over the
+    # active columns' edges); ONE MIN reduce-scatter inside the row group brings it to the owner, which keeps it when it is
+    # smaller (wcc_owner_step); one all-reduce of the number of changed vertices ends the loop at 0.  The fixpoint is the
+    # smallest code of each component: for a given grid it does not depend on timing.
+    # ------------------------------------------------------------------------------------------
+    def weakly_connected_components(self):
+        """Returns (vertices, labels) of the vertices this rank owns: a vertex's label is the external id of one member of
+        its component (the same member on every rank), in the vertices' dtype.  The graph must be symmetric: the caller
+        passes both directions of every edge (not checked).  Sets last_wcc_stats = dict(rounds)."""
+        assert self.block is not None, "weakly_connected_components needs the unsplit block"
+        p, g, L, capi = self.part, self.part.groups, self.lib, self._capi
+        dev, mp = self.device, p.maxpart
+        label_own = torch.full((mp,), INT64_MAX, dtype=torch.int64, device=dev)
+        label_own[:p.n_local] = g.rank * mp + torch.arange(p.n_local, dtype=torch.int64, device=dev)
+        changed = torch.zeros(mp, dtype=torch.bool, device=dev)
+        changed[:p.n_local] = True
+        label_cols = torch.empty(self.n_cols, dtype=torch.int64, device=dev)
+        cand = torch.empty(self.n_rows, dtype=torch.int64, device=dev)
+        cand_own = torch.empty(mp, dtype=torch.int64, device=dev)
+        views = {k: _view(v) for k, v in dict(x=label_cols, c=cand).items()}
+        err = C.c_void_p()
+        count = torch.zeros(1, dtype=torch.int64, device=dev)
+        rounds = 0
+        while True:
+            x = torch.where(changed, label_own, INT64_MAX)
+            if g.R == 1:
+                label_cols.copy_(x)
+            else:
+                all_gather_into(label_cols, x, g.col_group)           # partition-major = the block's column order
+            code = L.cugraph_b200_block_wcc_min(self.handle.ptr, self.block, views["x"].ptr, views["c"].ptr, C.byref(err))
+            capi.check(code, err, "cugraph_b200_block_wcc_min")
+            if g.C == 1:
+                cand_own.copy_(cand)
+            else:
+                reduce_scatter_into(cand_own, cand, g.row_group, op=dist.ReduceOp.MIN)
+            changed = wcc_owner_step(label_own, cand_own)
+            rounds += 1
+            count.copy_(changed.sum().view(1))
+            dist.all_reduce(count)
+            if int(count.item()) == 0:
+                break
+        for v in views.values():
+            v.free()
+        self.last_wcc_stats = dict(rounds=rounds)
+        return p.vertices, self._codes_to_external(label_own[:p.n_local])
+
 
 INT64_MAX = torch.iinfo(torch.int64).max
 
@@ -596,6 +649,15 @@ def sssp_owner_step(dist_own, pred_code, pending, cand_own):
     if dist_own.dtype == torch.float32:
         pred_code.copy_(torch.where(improved, cand_own & 0xFFFFFFFF, pred_code))
     return improved
+
+
+def wcc_owner_step(label_own, cand_own):
+    """The owner's step of one multi-GPU WCC round: keep the reduced candidate label (cugraph_b200_block_wcc_min; INT64_MAX =
+    no active neighbour) where it is smaller than label_own.  Updates label_own in place and returns the mask of changed
+    vertices."""
+    changed = cand_own < label_own
+    label_own.copy_(torch.where(changed, cand_own, label_own))
+    return changed
 
 
 # EXPERIMENTAL: same iteration, but the block is split by destination partition: sweep j, then an asynchronous
@@ -664,6 +726,12 @@ def sssp(graph: MGGraph, source, cutoff=math.inf, compute_predecessors=True):
     """(vertices, distances, predecessors) of the vertices owned by this rank (the MG contract of pylibcugraph.sssp;
     predecessors are None when not requested)."""
     return graph.sssp(source, cutoff, compute_predecessors)
+
+
+def weakly_connected_components(graph: MGGraph):
+    """(vertices, labels) of the vertices owned by this rank (the MG contract of pylibcugraph.weakly_connected_components;
+    the graph must be symmetric)."""
+    return graph.weakly_connected_components()
 
 
 def pagerank(graph: MGGraph, alpha=0.85, epsilon=1e-5, max_iterations=100):

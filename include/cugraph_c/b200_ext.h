@@ -4,7 +4,7 @@
  *  - multi-GPU: the reference receives NCCL communicators inside a raft::handle_t built by raft-dask / MPI
  *    (python/pylibcugraph/pylibcugraph/comms/comms_wrapper.pyx:10-32, cpp/tests/utilities/mg_utilities.cpp:37-55) and keeps
  *    the 2D-partitioned blocks inside graph_t.  raft is not part of this build: cugraph_graph_create_mg and the multi-GPU
- *    algorithm entry points return CUGRAPH_NOT_IMPLEMENTED; multi-GPU PageRank, BFS and SSSP are driven by the
+ *    algorithm entry points return CUGRAPH_NOT_IMPLEMENTED; multi-GPU PageRank, BFS, SSSP and WCC are driven by the
  *    launcher (cugraph_b200/mg.py, one process per GPU over torch.distributed / NCCL) on top of the cugraph_b200_block_*
  *    device pieces declared below.
  *  - profiling hooks used by bench.py to time the dominant kernel on the handle's stream.
@@ -116,6 +116,18 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_sssp_pred(
   const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
   const cugraph_type_erased_device_array_view_t* dist_cols, const cugraph_type_erased_device_array_view_t* win_rows,
   size_t maxpart, int grid_cols, int grid_c, cugraph_type_erased_device_array_view_t* code_rows, cugraph_error_t** error);
+
+/* One round of multi-GPU weakly connected components on this GPU's edge block (min-label propagation).  The block may be
+ * unweighted or weighted; weights are ignored.  label_cols (INT64, at least one per column slot, gathered by the launcher
+ * inside the column group) holds the label of every source that changed in the last round and INT64_MAX for all others.
+ * cand_rows (INT64, at least one per row slot) receives, for every row slot, the smallest label among the row's sources,
+ * INT64_MAX when none is active.  The active columns' edges are pushed with atomicMin through the block's column-major copy,
+ * built by the first SSSP or WCC call on the block and kept.  Asynchronous, apart from one read-back of the number of
+ * active columns and their edge count. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_wcc_min(
+  const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+  const cugraph_type_erased_device_array_view_t* label_cols,
+  cugraph_type_erased_device_array_view_t* cand_rows, cugraph_error_t** error);
 
 /* Debug hook: one sweep as PageRank would run it on this graph (the shared-memory piece stream when the graph has one)
  * against the plain sweep (an independent implementation) on the same pseudo-random x.  out[0..3] = degree >= 32 rows
