@@ -404,7 +404,7 @@ cugraph_error_code_t cugraph_b200_block_create(const cugraph_resource_handle_t* 
                                    (int64_t)r->size, b->n_span);
     b->scratch.init(h, *b->csx);
     // build the column-blocked copy now (it is lazily created otherwise, inside the first timed sweep)
-    (void)sweep_layout(h, *b->csx, b->n_span, b->wtype == FLOAT64 ? 8 : 4);
+    prepare_pull_sweep(h, *b->csx, b->n_span, b->wtype == FLOAT64 ? 8 : 4);
     sync(h);
     *block = reinterpret_cast<cugraph_b200_block_t*>(b.release());
   });

@@ -1,5 +1,6 @@
-// The pull sweep behind one entry point (pull_sweep, graph.cuh): which kernels run for a graph, and the scratch they need.  The
-// only translation unit that includes the sweep kernels (sweep.cuh, spmv.cuh), so each is compiled once.
+// The pull sweep behind one entry point (pull_sweep, graph.cuh): which kernels run for a graph, and the scratch they need; the
+// layout they read is built by sweep_layout.cu.  The only translation unit that includes the sweep kernels (sweep.cuh,
+// spmv.cuh), so each is compiled once.
 #include "sweep.cuh"
 
 namespace b200 {
@@ -83,6 +84,8 @@ void pull_sweep(handle_impl const& h, csx_t const& c, int32_t n_vertices, T cons
   else
     launch_pull_sweep<int32_t, T>(h, c, x, y, acc, alpha, sc.st(), use_weights);
 }
+
+void prepare_pull_sweep(handle_impl const& h, csx_t const& c, int32_t nv, size_t es) { sweep_layout(h, c, nv, es); }
 
 template dbuf make_sweep_x<float>(handle_impl const&, int32_t);
 template dbuf make_sweep_x<double>(handle_impl const&, int32_t);

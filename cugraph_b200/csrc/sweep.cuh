@@ -5,7 +5,7 @@
 // Why: the plain sweep (spmv.cuh) is bound by the L2 -> SM path: every gather of x[src] costs a 32-byte L2 sector for
 // 4 useful bytes.  Here the source space is cut into blocks of W
 // vertices whose x slice (192 KiB) a persistent CTA keeps in shared memory (TMA bulk copies + mbarrier), and the
-// adjacency is re-laid as a stream of PIECES with 16-bit local column ids (sweep_layout_t, graph.cuh).
+// adjacency is re-laid as a stream of PIECES with 16-bit local column ids (sweep_layout_t, sweep_layout.cuh).
 //
 // Execution structure (a kernel with one batch of id / row loads in flight per warp, nothing while it processed them,
 // spent most of its stall samples waiting on those loads, and some at CTA barriers):
@@ -20,17 +20,16 @@
 //     gather: 20 % of its instructions); slots, pieces and rows accumulate in fp64.
 //   * one fp64 RED per piece into acc[row] (L2); the pieces of a hub row that fill a whole warp are summed by shuffles
 //     first.  k_sweep_finish turns acc into y, clears it and resets the cursors.
-//   * the rows are split into bands whose accumulators fit in the L2 (graph.cuh); the sweep runs band by band, k_sweep over
+//   * the rows are split into bands whose accumulators fit in the L2 (sweep_layout.cuh); the sweep runs band by band, k_sweep over
 //     the band's phases, then k_sweep_finish over its rows while their accumulators are still in the L2.
-//   * on large graphs the rows of small in-degree (the tail, graph.cuh) are not in the stream: one k_sweep_tail launch after
+//   * on large graphs the rows of small in-degree (the tail, sweep_layout.cuh) are not in the stream: one k_sweep_tail launch after
 //     the bands gathers their few edges directly from a layout of their own (runs of equal in-degree, lane-interleaved: no
 //     RED, and fewer stream rows need fewer bands), the hubs' x from a shared-memory copy of the first column block.
 #pragma once
 #include "spmv.cuh"
+#include "sweep_layout.cuh"
 
 namespace b200 {
-
-
 
 constexpr int kSweepThreads = 512;  // 16 warps x 128 registers, two chunk buffers per warp (384 threads x 3 buffers: no faster)
 constexpr int kSweepWarps   = kSweepThreads / 32;
@@ -645,7 +644,7 @@ k_sweep_finish(double* __restrict__ acc, int row_lo, int n_cov, int n_rows, T* _
   }
 }
 
-// The tail rows [n_str, n_cov) from the tail layout (graph.cuh), then y = init for the empty rows [n_cov, empty_hi).  Its
+// The tail rows [n_str, n_cov) from the tail layout (sweep_layout.cuh), then y = init for the empty rows [n_cov, empty_hi).  Its
 // sources are mostly hubs (RMAT-24: 47 % of them in the first column block), and a plain row kernel pays a 32-byte L2 sector
 // for each of those 4-byte gathers: persistent CTAs (one per SM) keep x[0, W) in shared memory, loaded once by TMA bulk
 // copies as in k_sweep, and gather the other sources from global memory with an evict-LAST hint (x is reused across the
@@ -837,7 +836,7 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
   // covered_rows_only: y of the rows without edges already holds their (unvarying) value — multi-GPU blocks, where more than
   // half of the row slots are empty and the unvarying term is 0 (mg.cu)
   const int32_t finish_rows = covered_rows_only ? L.n_cov : c.n_rows;
-  const bool tail           = L.n_str < L.n_cov;  // rows of small in-degree left the stream (graph.cuh)
+  const bool tail           = L.n_str < L.n_cov;  // rows of small in-degree left the stream (sweep_layout.cuh)
   // band by band: the band's rows are finished while its accumulators are in the L2, before the next band's REDs evict them.
   // y must not overlap x: a band's finish writes y while later bands (and the tail) still read x.
   for (int band = 0; band < L.n_bands; ++band) {

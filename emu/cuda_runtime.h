@@ -1,5 +1,5 @@
 // HOST EMULATION of the sliver of CUDA that graph staging uses — test infrastructure only (tests/test_emu_staging_cpu.py).
-// The staging kernels (graph_build.cu) are simple data-parallel loops without intra-block communication, so they can
+// The staging kernels (graph_build.cu, sweep_layout.cu) are simple data-parallel loops without intra-block communication, so they can
 // run on the CPU unchanged: every "thread" of a launch is executed to completion, one after the other.  "Device"
 // memory is host memory.  Nothing here is part of the product; libcugraph_c.so is never built with it.
 #pragma once

@@ -1,5 +1,5 @@
 // Accessors for the CPU emulation build (libcugraph_c_emu.so): test infrastructure only, see emu/cuda_runtime.h.
-#include "graph.cuh"
+#include "sweep_layout.cuh"
 
 #include <algorithm>
 #include <vector>
@@ -56,12 +56,18 @@ EMU_EXPORT int emu_sweep_layout(const cugraph_resource_handle_t* handle, cugraph
   return 0;
 }
 
+// the layout emu_sweep_layout built for elements of `es` bytes, or nullptr: the accessors below read it, never build it
+static sweep_layout_t const* built_layout(cugraph_graph_t* graph, size_t es)
+{
+  csx_t const& c = *reinterpret_cast<graph_impl*>(graph)->primary;
+  return c.sweep ? c.sweep->of(es).layout.get() : nullptr;
+}
+
 // row bands of that piece stream (call emu_sweep_layout first): returns n_bands and its CTAs per band (*n_cta);
 // band_row / band_phase receive n_bands + 1 entries each when they hold at least `capacity`
 EMU_EXPORT int emu_sweep_bands(cugraph_graph_t* graph, size_t es, int* n_cta, int32_t* band_row, int32_t* band_phase, size_t capacity)
 {
-  auto* g                 = reinterpret_cast<graph_impl*>(graph);
-  sweep_layout_t const* L = (es == 4 ? g->primary->hot4 : g->primary->hot8).get();
+  sweep_layout_t const* L = built_layout(graph, es);
   if (!L) return 0;
   *n_cta = L->n_cta;
   if ((size_t)L->n_bands + 1 <= capacity) {
@@ -74,8 +80,7 @@ EMU_EXPORT int emu_sweep_bands(cugraph_graph_t* graph, size_t es, int* n_cta, in
 // rows [0, n_str) of that piece stream are in it, the non-empty rows behind them are its tail; -1 without a layout
 EMU_EXPORT int32_t emu_sweep_stream_rows(cugraph_graph_t* graph, size_t es)
 {
-  auto* g                 = reinterpret_cast<graph_impl*>(graph);
-  sweep_layout_t const* L = (es == 4 ? g->primary->hot4 : g->primary->hot8).get();
+  sweep_layout_t const* L = built_layout(graph, es);
   return L ? L->n_str : -1;
 }
 
@@ -83,8 +88,7 @@ EMU_EXPORT int32_t emu_sweep_stream_rows(cugraph_graph_t* graph, size_t es)
 // {degree, first_row, first_tile, first_unit, id_off} when it holds `capacity` entries, ptrs[2] = tail_ids, tail_w
 EMU_EXPORT int emu_sweep_tail(cugraph_graph_t* graph, size_t es, int64_t* runs, size_t capacity, void** ptrs)
 {
-  auto* g                 = reinterpret_cast<graph_impl*>(graph);
-  sweep_layout_t const* L = (es == 4 ? g->primary->hot4 : g->primary->hot8).get();
+  sweep_layout_t const* L = built_layout(graph, es);
   if (!L) return -1;
   if (L->tail_runs.size() <= capacity)
     for (size_t k = 0; k < L->tail_runs.size(); ++k) {
@@ -102,9 +106,5 @@ EMU_EXPORT size_t emu_padded_x_elems(int32_t nv, size_t es) { return padded_x_el
 // forget the cached layouts of the primary orientation (so that another set of knobs can be staged)
 EMU_EXPORT void emu_reset_layouts(cugraph_graph_t* graph)
 {
-  auto* g        = reinterpret_cast<graph_impl*>(graph);
-  csx_t const& c = *g->primary;
-  c.hot4.reset();
-  c.hot8.reset();
-  c.hot4_tried = c.hot8_tried = false;
+  reinterpret_cast<graph_impl*>(graph)->primary->sweep.reset();
 }

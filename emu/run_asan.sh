@@ -4,7 +4,7 @@
 #   bash emu/run_asan.sh [fuzz seconds]
 set -e
 ROOT=$(cd "$(dirname "$0")/.." && pwd); CSRC=$ROOT/cugraph_b200/csrc; OUT=/tmp/libcugraph_c_emu_asan.so
-SRCS=""; for f in capi_basic.cu capi_graph.cu graph_build.cu sweep.cu pagerank.cu traverse.cu mg.cu; do SRCS="$SRCS -x c++ $CSRC/$f"; done
+SRCS=""; for f in capi_basic.cu capi_graph.cu graph_build.cu sweep_layout.cu sweep.cu pagerank.cu traverse.cu mg.cu; do SRCS="$SRCS -x c++ $CSRC/$f"; done
 /usr/bin/g++ -std=c++17 -O1 -g -fPIC -shared -fvisibility=hidden -DB200_HOST_EMU -fsanitize=address -fno-omit-frame-pointer \
   -I $ROOT/emu -I $ROOT/include -I $CSRC -Wno-attributes $SRCS -x c++ $ROOT/emu/emu_debug.cpp -o $OUT
 # libstdc++ too: Python does not link it, and ASan resolves its __cxa_throw interceptor when it starts

@@ -1,4 +1,4 @@
-"""Graph staging on the CPU: the real staging code (capi_graph.cu, graph_build.cu — renumbering, the packed-key sort,
+"""Graph staging on the CPU: the real staging code (capi_graph.cu, graph_build.cu, sweep_layout.cu — renumbering, the packed-key sort,
 binning, the piece stream of the shared-memory sweep) compiled as plain C++ against
 the host emulation shim in emu/ and driven through the real C ABI with numpy arrays.  The staging kernels are
 data-parallel loops without intra-block communication, so executing every "thread" of a launch in turn is exact.

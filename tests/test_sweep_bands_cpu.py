@@ -1,4 +1,4 @@
-"""Row bands of the piece stream (graph_build.cu, sweep.cuh): the covered rows are split into bands whose fp64 accumulators
+"""Row bands of the piece stream (sweep_layout.cu, sweep.cuh): the covered rows are split into bands whose fp64 accumulators
 fit in the L2, pieces are ordered by (band, block, kind) and the sweep runs band after band.  Checked on the CPU: the
 banded layout holds every (row, source[, weight]) exactly once, a band's chunks hold only its rows, each band's CTA ranges
 partition its phases, the planner lays bands out one after the other, and PageRank through the emulated kernels matches the

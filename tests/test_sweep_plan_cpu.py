@@ -1,4 +1,4 @@
-"""Host-side planner of the shared-memory pull sweep (graph_build.cu: plan_sweep, reached through the C ABI debug hook
+"""Host-side planner of the shared-memory pull sweep (sweep_layout.cu: plan_sweep, reached through the C ABI debug hook
 cugraph_b200_debug_plan_sweep): groups -> chunks -> per-CTA ranges -> phases, from the piece counts per (block, kind)
 alone.  Pure host code, so the structure the GPU kernel relies on is checkable here."""
 import ctypes as C

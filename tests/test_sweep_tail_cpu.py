@@ -1,4 +1,4 @@
-"""The tail of the piece stream (graph_build.cu, sweep.cuh): rows of in-degree below a bound leave the stream and are swept
+"""The tail of the piece stream (sweep_layout.cu, sweep.cuh): rows of in-degree below a bound leave the stream and are swept
 by the plain row kernel after the bands.  Checked on the CPU with forced bounds (CUGRAPH_B200_SWEEP_TAIL_DEGREE): the stream
 holds exactly the edges of the rows [0, n_str), each once, and its bands partition [0, n_str); bound 1 is the layout without
 a tail; PageRank, Katz, HITS, the plain-vs-stream row comparison and the emulated 2D multi-GPU block sweep all match their

@@ -1,4 +1,4 @@
-"""The tail layout (graph.cuh, graph_build.cu): the rows of in-degree below the bound, in runs of equal in-degree cut into
+"""The tail layout (sweep_layout.cuh, sweep_layout.cu): the rows of in-degree below the bound, in runs of equal in-degree cut into
 tiles of 32 rows whose ids are lane-interleaved.  Checked on the CPU with forced bounds: the runs tile [n_str, n_cov) with one
 in-degree each, every (row, source[, weight]) of the tail sits exactly where the layout says, in the row's order, padding
 (column n_vertices, weight 0) only in the last tile of a run; and PageRank and the emulated 2D multi-GPU block sweep through
