@@ -3,6 +3,7 @@
 // cpp/src/link_analysis/hits_impl.cuh:29-206, C API cpp/src/c_api/katz.cpp, cpp/src/c_api/hits.cpp).  Both are host loops
 // over pull_sweep (sweep.cu: the shared-memory piece stream when the graph has one) plus small vector passes; their
 // per-iteration convergence test reads one scalar back, as the reference does.
+#include "centrality_ops.cuh"
 #include "graph.cuh"
 
 #include <cmath>
@@ -10,74 +11,6 @@
 
 namespace b200 {
 namespace {
-
-constexpr int kCBlock = 256;
-inline int cgrid(handle_impl const& h, int64_t n) { return (int)std::min<int64_t>(std::max<int64_t>((n + kCBlock - 1) / kCBlock, 1), (int64_t)h.sm_count * 8); }
-
-__device__ __forceinline__ double block_sum(double v, double* smem)
-{
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) smem[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double t = 0.0;
-  if (threadIdx.x < 32) {
-    t = (threadIdx.x < (blockDim.x >> 5)) ? smem[threadIdx.x] : 0.0;
-    t = warp_sum(t);
-  }
-  __syncthreads();
-  return t;
-}
-
-// out[0] += sum |a - b| ; optionally b <- a (the next sweep's input)
-template <typename T>
-__global__ void __launch_bounds__(kCBlock) k_abs_diff(T const* __restrict__ a, T* __restrict__ b, int32_t n, int copy, double* __restrict__ out)
-{
-  __shared__ double smem[kCBlock / 32];
-  double d = 0.0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    d += fabs((double)a[i] - (double)b[i]);
-    if (copy) b[i] = a[i];
-  }
-  d = block_sum(d, smem);
-  if (threadIdx.x == 0 && d != 0.0) atomicAdd(out, d);
-}
-
-template <typename T>
-__global__ void __launch_bounds__(kCBlock) k_add_vec(T* __restrict__ y, T const* __restrict__ add, int32_t n)
-{
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) y[i] += add[i];
-}
-
-// out[0] += sum v^2 (mode 0) | sum v (mode 1) ; out[1] = max v (mode 2, values are non-negative: integer compare of the bits)
-template <typename T>
-__global__ void __launch_bounds__(kCBlock) k_norm(T const* __restrict__ v, int32_t n, int mode, double* __restrict__ out)
-{
-  __shared__ double smem[kCBlock / 32];
-  double s = 0.0, m = 0.0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const double x = (double)v[i];
-    s += mode == 0 ? x * x : x;
-    m = x > m ? x : m;
-  }
-  if (mode == 2) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const double t = __shfl_xor_sync(0xffffffffu, m, o);
-      m              = t > m ? t : m;
-    }
-    if ((threadIdx.x & 31) == 0 && m > 0.0)
-      atomicMax(reinterpret_cast<unsigned long long*>(out + 1), (unsigned long long)__double_as_longlong(m));
-    return;
-  }
-  s = block_sum(s, smem);
-  if (threadIdx.x == 0 && s != 0.0) atomicAdd(out, s);
-}
-
-template <typename T>
-__global__ void __launch_bounds__(kCBlock) k_scale(T* __restrict__ v, int32_t n, double inv)
-{
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) v[i] = (T)((double)v[i] * inv);
-}
 
 template <typename T>
 __global__ void __launch_bounds__(kCBlock) k_fill_vec(T* __restrict__ v, int64_t n, T val)

@@ -6,18 +6,21 @@
 // torch.distributed (NCCL on NVLink 5 / NVSwitch).  This file provides the device-side pieces behind
 // the C ABI: a resource handle bound to the caller's CUDA stream, rectangular edge blocks with the
 // same binned / column-blocked layout as the single-GPU graph, the block pull sweep and the fused
-// per-iteration vertex step, the BFS pull step, the SSSP push relaxation and the WCC min-label round.  All calls only
-// ENQUEUE work on the handle's stream (the SSSP and WCC calls read back one queue size).
+// per-iteration vertex step, the transposed block sweep, the owner steps of Katz, eigenvector centrality and HITS, the BFS
+// pull step, the SSSP push relaxation and the WCC min-label round.  All calls only ENQUEUE work on the handle's stream (the
+// SSSP and WCC calls read back one queue size; the first transposed sweep of a block builds its column-major copy).
 #include "advance.cuh"
+#include "centrality_ops.cuh"
 
 #include <algorithm>
 #include <climits>
 #include <cmath>
+#include <initializer_list>
 #include <limits>
 
 namespace b200 {
 
-// the column-major copy of a block for multi-GPU SSSP (built by the first relaxation call on the block): physical rows are
+// the column-major copy of a block (built by the first SSSP, WCC or transposed sweep call on the block): physical rows are
 // the block's column slots in descending out-degree (row_vertex = column slot), neighbours are row slots
 struct block_push_t {
   std::unique_ptr<csx_t> csx;
@@ -25,18 +28,21 @@ struct block_push_t {
   dbuf queue, q_deg;   // active physical rows and their degrees (q_deg has one element more: advance() reads n + 1)
   dbuf counts;         // block_queue_counts_t
   advance_scratch_t adv;
+  sweep_scratch_t scratch;  // the transposed sweep's (a pull sweep over this copy), made by its first call
+  bool sweep_ready{false};
 };
 
 struct block_impl {
   std::unique_ptr<csx_t> csx;
-  std::unique_ptr<block_push_t> push;  // lazily built (multi-GPU SSSP only)
+  std::unique_ptr<block_push_t> push;  // lazily built (multi-GPU SSSP, WCC and transposed sweeps)
   int32_t n_rows{0}, n_cols{0}, n_span{0};
   bool weighted{false};
   cugraph_data_type_id_t wtype{FLOAT32};
   sweep_scratch_t scratch;  // init = 0
-  // the y array whose rows WITHOUT edges this block has already written (0): later sweeps into the same array only finish the
-  // rows that have edges — in a 2D block more than half of the row slots are empty (the caller must not write them either)
-  void const* y_complete{nullptr};
+  // per orientation (0 = pull, 1 = transposed): the y array whose slots WITHOUT edges this block has already written (0):
+  // later sweeps of that orientation into the same array only finish the slots that have edges — in a 2D block more than
+  // half of the slots are empty (the caller must not write them either)
+  void const* y_complete[2]{nullptr, nullptr};
 };
 
 namespace {
@@ -83,6 +89,97 @@ k_mg_vertex_step(T const* __restrict__ y, T* __restrict__ pr, T const* __restric
     atomicAdd(partial_out + 0, diff);
     atomicAdd(partial_out + 1, dang);
   }
+}
+
+// ---- owner steps of the multi-GPU Katz, eigenvector and HITS iterations over this rank's n_local slice.  Each adds its
+// partial scalars into a device double[] that the launcher all-reduces; the arithmetic is that of the single-GPU drivers
+// (centrality.cu) through the same helpers (centrality_ops.cuh), with their passes fused.
+
+// Katz: x_new = y + beta (y carries alpha from the sweep) ; out[0] += sum |x_new - x| ; out[1] += sum x_new^2 ; x = x_new
+template <typename T>
+__global__ void __launch_bounds__(kCBlock)
+k_katz_step(T const* __restrict__ y, T* __restrict__ x, int32_t n, double beta, double* __restrict__ out)
+{
+  __shared__ double smem[kCBlock / 32];
+  double d = 0.0, s = 0.0;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const T nv = (T)((double)y[i] + beta);
+    d += fabs((double)nv - (double)x[i]);
+    s += (double)nv * (double)nv;
+    x[i] = nv;
+  }
+  d = block_sum(d, smem);
+  s = block_sum(s, smem);
+  if (threadIdx.x == 0) {
+    if (d != 0.0) atomicAdd(out, d);
+    if (s != 0.0) atomicAdd(out + 1, s);
+  }
+}
+
+// eigenvector, first half: y += x ; out[0] += sum y^2   (k_add_vec + k_norm mode 0)
+template <typename T>
+__global__ void __launch_bounds__(kCBlock) k_eig_add(T* __restrict__ y, T const* __restrict__ x, int32_t n, double* __restrict__ out)
+{
+  __shared__ double smem[kCBlock / 32];
+  double s = 0.0;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const T v = y[i] + x[i];
+    y[i]      = v;
+    s += (double)v * (double)v;
+  }
+  s = block_sum(s, smem);
+  if (threadIdx.x == 0 && s != 0.0) atomicAdd(out, s);
+}
+
+// eigenvector, second half: y *= 1 / sqrt(sumsq[0]) ; out[0] += sum |y - x| ; x = y   (k_scale + k_abs_diff)
+template <typename T>
+__global__ void __launch_bounds__(kCBlock)
+k_eig_scale(T* __restrict__ y, T* __restrict__ x, int32_t n, double const* __restrict__ sumsq, double* __restrict__ out)
+{
+  __shared__ double smem[kCBlock / 32];
+  const double inv = 1.0 / sqrt(sumsq[0]);
+  double d         = 0.0;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const T v = scaled(y[i], inv);
+    d += fabs((double)v - (double)x[i]);
+    y[i] = v;
+    x[i] = v;
+  }
+  d = block_sum(d, smem);
+  if (threadIdx.x == 0 && d != 0.0) atomicAdd(out, d);
+}
+
+// HITS: out[0] = max(out[0], max hubs), out[1] = max(out[1], max auth)   (k_norm mode 2 of both arrays)
+template <typename T>
+__global__ void __launch_bounds__(kCBlock) k_hits_max(T const* __restrict__ hubs, T const* __restrict__ auth, int32_t n, double* __restrict__ out)
+{
+  double mh = 0.0, ma = 0.0;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const double h = (double)hubs[i], a = (double)auth[i];
+    mh = h > mh ? h : mh;
+    ma = a > ma ? a : ma;
+  }
+  warp_max_into(mh, out);
+  warp_max_into(ma, out + 1);
+}
+
+// HITS: hubs *= 1 / mx[0] ; auth *= 1 / mx[1] ; out[0] += sum |hubs - prev|   (two k_scale + k_abs_diff)
+template <typename T>
+__global__ void __launch_bounds__(kCBlock)
+k_hits_scale(T* __restrict__ hubs, T* __restrict__ auth, T const* __restrict__ prev, int32_t n, double const* __restrict__ mx,
+             double* __restrict__ out)
+{
+  __shared__ double smem[kCBlock / 32];
+  const double inv_h = 1.0 / mx[0], inv_a = 1.0 / mx[1];
+  double d = 0.0;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const T h = scaled(hubs[i], inv_h);
+    hubs[i]   = h;
+    auth[i]   = scaled(auth[i], inv_a);
+    d += fabs((double)h - (double)prev[i]);
+  }
+  d = block_sum(d, smem);
+  if (threadIdx.x == 0 && d != 0.0) atomicAdd(out, d);
 }
 
 
@@ -272,6 +369,53 @@ block_push_t& push_copy(handle_impl const& h, block_impl& b)
   return *b.push;
 }
 
+// a pull sweep of the block (transposed = false) or of its column-major copy (transposed = true: y over column slots,
+// x over row slots) — the copy is binned like the block, so the same sweep and the same layouts apply to it
+void block_sweep(handle_impl const& h, block_impl& b, bool transposed, bool use_weights, device_array_view_impl const* xv,
+                 device_array_view_impl const* yv, double alpha)
+{
+  const bool f32 = b.wtype == FLOAT32;
+  B200_EXPECTS(xv->type == b.wtype && yv->type == b.wtype, CUGRAPH_INVALID_INPUT, "x / y dtype must match the block");
+  B200_EXPECTS(xv->size >= padded_x_elems(b.n_span, f32 ? 4 : 8), CUGRAPH_INVALID_INPUT,
+               "x must hold cugraph_b200_padded_elems(span) elements");
+  B200_EXPECTS(yv->size >= (size_t)b.n_span, CUGRAPH_INVALID_INPUT, "y must hold `span` elements");
+  const size_t es = f32 ? 4 : 8;
+  auto const* x0  = static_cast<const char*>(xv->data);
+  auto const* y0  = static_cast<const char*>(yv->data);
+  B200_EXPECTS(y0 + yv->size * es <= x0 || x0 + xv->size * es <= y0, CUGRAPH_INVALID_INPUT, "x and y must not overlap");
+  csx_t const* c      = b.csx.get();
+  sweep_scratch_t* sc = &b.scratch;
+  if (transposed) {
+    block_push_t& p = push_copy(h, b);
+    if (!p.sweep_ready) {  // the layout is built here rather than inside the first sweep, as cugraph_b200_block_create does
+      p.scratch.init(h, *p.csx);
+      prepare_pull_sweep(h, *p.csx, b.n_span, es);
+      sync(h);
+      p.sweep_ready = true;
+    }
+    c  = p.csx.get();
+    sc = &p.scratch;
+  }
+  const int o             = transposed ? 1 : 0;
+  const bool covered_only = b.y_complete[o] == yv->data;  // the empty slots of this y hold their zeros from an earlier sweep
+  if (f32) pull_sweep<float>(h, *c, b.n_span, (float const*)xv->data, (float*)yv->data, *sc, alpha, use_weights, covered_only);
+  else pull_sweep<double>(h, *c, b.n_span, (double const*)xv->data, (double*)yv->data, *sc, alpha, use_weights, covered_only);
+  b.y_complete[o] = yv->data;
+  if (b.y_complete[1 - o] == yv->data) b.y_complete[1 - o] = nullptr;  // this sweep wrote the other orientation's empty slots
+}
+
+// arguments of the owner steps: arrays of one floating type, each at least n_local long
+void check_owner_args(std::initializer_list<device_array_view_impl const*> vs, size_t n_local, void const* partial)
+{
+  B200_EXPECTS(partial != nullptr, CUGRAPH_INVALID_INPUT, "NULL argument");
+  cugraph_data_type_id_t t = (*vs.begin()) ? (*vs.begin())->type : FLOAT32;
+  for (auto const* v : vs) {
+    B200_EXPECTS(v != nullptr, CUGRAPH_INVALID_INPUT, "NULL argument");
+    B200_EXPECTS(v->type == t && (t == FLOAT32 || t == FLOAT64), CUGRAPH_INVALID_INPUT, "arrays must share one FLOAT32 / FLOAT64 type");
+    B200_EXPECTS(v->size >= n_local, CUGRAPH_INVALID_INPUT, "arrays shorter than n_local");
+  }
+}
+
 // active rows -> queue (one read-back of its size and edge count) -> advance with `op`
 template <typename O, typename T, typename Op>
 void block_push_round(handle_impl const& h, block_push_t& p, T const* dist_cols, Op op)
@@ -426,27 +570,166 @@ cugraph_error_code_t cugraph_b200_block_pull_sweep(const cugraph_resource_handle
                                                    cugraph_type_erased_device_array_view_t* y, double alpha,
                                                    cugraph_error_t** error)
 {
+  return cugraph_b200_block_sweep(handle, block, FALSE, TRUE, x, y, alpha, error);
+}
+
+// transposed = FALSE: y[row] = alpha * sum_{edges (row, col)} x[col] * w ; TRUE: y[col] = alpha * sum_{edges (row, col)} x[row] * w
+// (w = 1 when use_weights is FALSE).  Asynchronous, apart from the first transposed sweep of a block.
+cugraph_error_code_t cugraph_b200_block_sweep(const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+                                              bool_t transposed, bool_t use_weights,
+                                              const cugraph_type_erased_device_array_view_t* x,
+                                              cugraph_type_erased_device_array_view_t* y, double alpha, cugraph_error_t** error)
+{
   return guarded(error, [&] {
     auto const& h = H(handle);
     B200_EXPECTS(block && x && y, CUGRAPH_INVALID_INPUT, "NULL argument");
-    auto* b        = reinterpret_cast<block_impl*>(block);
-    auto const* xv = V(x);
+    block_sweep(h, *reinterpret_cast<block_impl*>(block), transposed == TRUE, use_weights == TRUE, V(x), V(y), alpha);
+    check_last("block_sweep");
+  });
+}
+
+cugraph_error_code_t cugraph_b200_katz_step(const cugraph_resource_handle_t* handle,
+                                            const cugraph_type_erased_device_array_view_t* y,
+                                            cugraph_type_erased_device_array_view_t* x, size_t n_local, double beta,
+                                            double* partial_out_device, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
     auto const* yv = V(y);
-    const bool f32 = b->wtype == FLOAT32;
-    B200_EXPECTS(xv->type == b->wtype && yv->type == b->wtype, CUGRAPH_INVALID_INPUT, "x / y dtype must match the block");
-    B200_EXPECTS(xv->size >= padded_x_elems(b->n_span, f32 ? 4 : 8), CUGRAPH_INVALID_INPUT,
-                 "x must hold cugraph_b200_padded_elems(span) elements");
-    B200_EXPECTS(yv->size >= (size_t)b->n_span, CUGRAPH_INVALID_INPUT, "y must hold `span` elements");
-    const size_t es = f32 ? 4 : 8;
-    auto const* x0  = static_cast<const char*>(xv->data);
-    auto const* y0  = static_cast<const char*>(yv->data);
-    B200_EXPECTS(y0 + yv->size * es <= x0 || x0 + xv->size * es <= y0, CUGRAPH_INVALID_INPUT, "x and y must not overlap");
-    csx_t const& c = *b->csx;
-    const bool covered_only = b->y_complete == yv->data;  // the empty rows of this y hold their zeros from an earlier sweep
-    if (f32) pull_sweep<float>(h, c, b->n_span, (float const*)xv->data, (float*)yv->data, b->scratch, alpha, true, covered_only);
-    else pull_sweep<double>(h, c, b->n_span, (double const*)xv->data, (double*)yv->data, b->scratch, alpha, true, covered_only);
-    b->y_complete = yv->data;
-    check_last("block_pull_sweep");
+    auto const* xv = V(x);
+    check_owner_args({yv, xv}, n_local, partial_out_device);
+    if (n_local == 0) return;
+    const int32_t n = (int32_t)n_local;
+    if (yv->type == FLOAT32)
+      B200_LAUNCH(h, (k_katz_step<float>), cgrid(h, n), kCBlock, 0, (float const*)yv->data, (float*)xv->data, n, beta, partial_out_device);
+    else
+      B200_LAUNCH(h, (k_katz_step<double>), cgrid(h, n), kCBlock, 0, (double const*)yv->data, (double*)xv->data, n, beta,
+                  partial_out_device);
+    check_last("katz_step");
+  });
+}
+
+cugraph_error_code_t cugraph_b200_eigenvector_add_step(const cugraph_resource_handle_t* handle,
+                                                       cugraph_type_erased_device_array_view_t* y,
+                                                       const cugraph_type_erased_device_array_view_t* x, size_t n_local,
+                                                       double* partial_out_device, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    auto const* yv = V(y);
+    auto const* xv = V(x);
+    check_owner_args({yv, xv}, n_local, partial_out_device);
+    if (n_local == 0) return;
+    const int32_t n = (int32_t)n_local;
+    if (yv->type == FLOAT32)
+      B200_LAUNCH(h, (k_eig_add<float>), cgrid(h, n), kCBlock, 0, (float*)yv->data, (float const*)xv->data, n, partial_out_device);
+    else
+      B200_LAUNCH(h, (k_eig_add<double>), cgrid(h, n), kCBlock, 0, (double*)yv->data, (double const*)xv->data, n, partial_out_device);
+    check_last("eigenvector_add_step");
+  });
+}
+
+cugraph_error_code_t cugraph_b200_eigenvector_scale_step(const cugraph_resource_handle_t* handle,
+                                                         cugraph_type_erased_device_array_view_t* y,
+                                                         cugraph_type_erased_device_array_view_t* x, size_t n_local,
+                                                         const double* sumsq_device, double* partial_out_device,
+                                                         cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    auto const* yv = V(y);
+    auto const* xv = V(x);
+    check_owner_args({yv, xv}, n_local, partial_out_device);
+    B200_EXPECTS(sumsq_device != nullptr, CUGRAPH_INVALID_INPUT, "NULL argument");
+    if (n_local == 0) return;
+    const int32_t n = (int32_t)n_local;
+    if (yv->type == FLOAT32)
+      B200_LAUNCH(h, (k_eig_scale<float>), cgrid(h, n), kCBlock, 0, (float*)yv->data, (float*)xv->data, n, sumsq_device,
+                  partial_out_device);
+    else
+      B200_LAUNCH(h, (k_eig_scale<double>), cgrid(h, n), kCBlock, 0, (double*)yv->data, (double*)xv->data, n, sumsq_device,
+                  partial_out_device);
+    check_last("eigenvector_scale_step");
+  });
+}
+
+cugraph_error_code_t cugraph_b200_hits_max_step(const cugraph_resource_handle_t* handle,
+                                                const cugraph_type_erased_device_array_view_t* hubs,
+                                                const cugraph_type_erased_device_array_view_t* authorities, size_t n_local,
+                                                double* max_out_device, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    auto const* hv = V(hubs);
+    auto const* av = V(authorities);
+    check_owner_args({hv, av}, n_local, max_out_device);
+    if (n_local == 0) return;
+    const int32_t n = (int32_t)n_local;
+    if (hv->type == FLOAT32)
+      B200_LAUNCH(h, (k_hits_max<float>), cgrid(h, n), kCBlock, 0, (float const*)hv->data, (float const*)av->data, n, max_out_device);
+    else
+      B200_LAUNCH(h, (k_hits_max<double>), cgrid(h, n), kCBlock, 0, (double const*)hv->data, (double const*)av->data, n,
+                  max_out_device);
+    check_last("hits_max_step");
+  });
+}
+
+cugraph_error_code_t cugraph_b200_hits_scale_step(const cugraph_resource_handle_t* handle,
+                                                  cugraph_type_erased_device_array_view_t* hubs,
+                                                  cugraph_type_erased_device_array_view_t* authorities,
+                                                  const cugraph_type_erased_device_array_view_t* prev_hubs, size_t n_local,
+                                                  const double* max_device, double* partial_out_device, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    auto const* hv = V(hubs);
+    auto const* av = V(authorities);
+    auto const* pv = V(prev_hubs);
+    check_owner_args({hv, av, pv}, n_local, partial_out_device);
+    B200_EXPECTS(max_device != nullptr, CUGRAPH_INVALID_INPUT, "NULL argument");
+    if (n_local == 0) return;
+    const int32_t n = (int32_t)n_local;
+    if (hv->type == FLOAT32)
+      B200_LAUNCH(h, (k_hits_scale<float>), cgrid(h, n), kCBlock, 0, (float*)hv->data, (float*)av->data, (float const*)pv->data, n,
+                  max_device, partial_out_device);
+    else
+      B200_LAUNCH(h, (k_hits_scale<double>), cgrid(h, n), kCBlock, 0, (double*)hv->data, (double*)av->data,
+                  (double const*)pv->data, n, max_device, partial_out_device);
+    check_last("hits_scale_step");
+  });
+}
+
+cugraph_error_code_t cugraph_b200_vertex_sum(const cugraph_resource_handle_t* handle,
+                                             const cugraph_type_erased_device_array_view_t* v, size_t n_local, bool_t squares,
+                                             double* partial_out_device, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    auto const* vv = V(v);
+    check_owner_args({vv}, n_local, partial_out_device);
+    if (n_local == 0) return;
+    const int32_t n = (int32_t)n_local;
+    const int mode  = squares == TRUE ? 0 : 1;
+    if (vv->type == FLOAT32)
+      B200_LAUNCH(h, (k_norm<float>), cgrid(h, n), kCBlock, 0, (float const*)vv->data, n, mode, partial_out_device);
+    else
+      B200_LAUNCH(h, (k_norm<double>), cgrid(h, n), kCBlock, 0, (double const*)vv->data, n, mode, partial_out_device);
+    check_last("vertex_sum");
+  });
+}
+
+cugraph_error_code_t cugraph_b200_vertex_scale(const cugraph_resource_handle_t* handle, cugraph_type_erased_device_array_view_t* v,
+                                               size_t n_local, double inv, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    auto const* vv = V(v);
+    check_owner_args({vv}, n_local, &inv);
+    if (n_local == 0) return;
+    const int32_t n = (int32_t)n_local;
+    if (vv->type == FLOAT32) B200_LAUNCH(h, (k_scale<float>), cgrid(h, n), kCBlock, 0, (float*)vv->data, n, inv);
+    else B200_LAUNCH(h, (k_scale<double>), cgrid(h, n), kCBlock, 0, (double*)vv->data, n, inv);
+    check_last("vertex_scale");
   });
 }
 

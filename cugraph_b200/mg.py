@@ -1,4 +1,4 @@
-"""Multi-GPU PageRank, BFS, SSSP and weakly connected components: 2D edge partition over one process per GPU (torch.distributed, NCCL on NVLink 5).
+"""Multi-GPU PageRank, BFS, SSSP, weakly connected components, Katz, eigenvector centrality and HITS: 2D edge partition over one process per GPU (torch.distributed, NCCL on NVLink 5).
 
 What the reference does (SURVEY.md §8e): P = R x C GPUs, vertex -> GPU by hash
 (cpp/include/cugraph/utilities/graph_partition_utils.cuh:30-43, 101-128), every GPU holds the edge
@@ -15,11 +15,12 @@ same column-blocked shared-memory kernel as on one GPU (C-ABI: cugraph_b200_bloc
 BFS moves byte flags per level (one max-reduce-scatter of candidate predecessors); SSSP runs Δ-windows of rounds, each an
 all-gather of the frontier's distances, the block's push relaxation on the device and one min-reduce-scatter of INT64
 (distance, predecessor) keys (see MGGraph.sssp); WCC propagates the smallest vertex code per round, with one
-min-reduce-scatter of INT64 labels (see MGGraph.weakly_connected_components).
+min-reduce-scatter of INT64 labels (see MGGraph.weakly_connected_components); Katz, eigenvector centrality and HITS iterate
+the block sweep like PageRank, HITS also in the transposed orientation, with owner-step kernels between the collectives
+(see MGGraph.katz_centrality).
 
 `partition_edges` (pure torch, device agnostic: exercised on CPU with the gloo backend in
-tests/test_mg_partition_cpu.py) builds the blocks; `MGGraph` / `pagerank` / `bfs` / `sssp` / `weakly_connected_components`
-need CUDA.
+tests/test_mg_partition_cpu.py) builds the blocks; `MGGraph` and the module-level algorithm functions need CUDA.
 """
 from __future__ import annotations
 
@@ -28,6 +29,7 @@ import math
 import os
 from dataclasses import dataclass
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -272,6 +274,7 @@ class MGGraph:
         self._sssp_avg = None                                                       # (average weight, average degree)
         self.last_sssp_stats = None
         self.last_wcc_stats = None
+        self.last_katz_stats = self.last_eigenvector_stats = self.last_hits_stats = None
         self.device = src.device
         p.rows = p.cols = p.weights = None  # the block owns its own copy
         torch.cuda.synchronize()
@@ -622,6 +625,247 @@ class MGGraph:
         self.last_wcc_stats = dict(rounds=rounds)
         return p.vertices, self._codes_to_external(label_own[:p.n_local])
 
+    # ------------------------------------------------------------------------------------------
+    # multi-GPU Katz, eigenvector centrality and HITS: the single-GPU drivers of centrality.cu with the sweep spread over the
+    # grid.  A sweep y = A x over the owners' x is: x all-gathered inside the column group over the block's source slots,
+    # the block's pull sweep, ONE reduce-scatter of the partial y inside the row group.  HITS' hub sweep y = A^T x runs the
+    # other way round: x all-gathered inside the ROW group over the destination slots (row slot c(v) * maxpart + lid is that
+    # group's all-gather order), the block's transposed sweep (cugraph_b200_block_sweep over its column-major copy), ONE
+    # reduce-scatter inside the COLUMN group (column slot r(u) * maxpart + lid, the order __init__ already uses for out_w).
+    # The owner steps (cugraph_b200_katz_step, ...) pass once over the owned slice and leave fp64 partials on the device;
+    # one small all-reduce makes them global, and the one host read per iteration is the convergence test, taken on every
+    # rank from the same all-reduced scalars, so that every rank leaves the loop (or raises) in the same iteration.
+    # ------------------------------------------------------------------------------------------
+    def _centrality_setup(self, what):
+        assert self.block is not None, f"{what} needs the unsplit block"
+        return self.part, self.part.groups, self.device, self.dtype, self.part.maxpart
+
+    def _sweep(self, vx, vy, alpha, transposed, use_weights):
+        err = C.c_void_p()
+        code = self.lib.cugraph_b200_block_sweep(self.handle.ptr, self.block, 1 if transposed else 0, 1 if use_weights else 0,
+                                                 vx.ptr, vy.ptr, float(alpha), C.byref(err))
+        self._capi.check(code, err, "cugraph_b200_block_sweep")
+
+    def _spmv(self, x_own, y_own, bufs, alpha, transposed=False, use_weights=True):
+        """y_own = alpha * (A x) of the owned vertices (transposed: alpha * (A^T x)); bufs = (x_gathered, y_partial, views)"""
+        g, mp = self.part.groups, self.part.maxpart
+        xg, yp, vx, vy = bufs
+        n_in, in_group, n_in_parts = (self.n_rows, g.row_group, g.C) if transposed else (self.n_cols, g.col_group, g.R)
+        n_out, out_group, n_out_parts = (self.n_cols, g.col_group, g.R) if transposed else (self.n_rows, g.row_group, g.C)
+        if n_in_parts == 1:
+            xg[:mp].copy_(x_own)
+        else:
+            all_gather_into(xg[:n_in], x_own, in_group)
+        self._sweep(vx, vy, alpha, transposed, use_weights)
+        if n_out_parts == 1:
+            y_own.copy_(yp[:mp])
+        else:
+            reduce_scatter_into(y_own, yp[:n_out], out_group)
+
+    def _sweep_bufs(self, dt, dev):
+        xg = torch.zeros(self.x_elems, dtype=dt, device=dev)    # zero from the span on, as the block sweep requires
+        yp = torch.zeros(self.span, dtype=dt, device=dev)
+        return xg, yp, _view(xg), _view(yp)
+
+    def _owner_call(self, name, *args):
+        err = C.c_void_p()
+        code = getattr(self.lib, name)(self.handle.ptr, *args, C.byref(err))
+        self._capi.check(code, err, name)
+
+    @staticmethod
+    def _fail(where, message):
+        """the error the single-GPU entry point returns (CUGRAPH_UNKNOWN_ERROR -> RuntimeError), with its message"""
+        from cugraph_b200 import _capi as capi
+        return capi.CugraphRuntimeError(capi.UNKNOWN_ERROR, message, where)
+
+    def katz_centrality(self, alpha, beta=1.0, epsilon=1e-6, max_iterations=100):
+        """Katz centrality (cugraph_katz_centrality's semantics): x <- alpha * A^T x + beta from x = 0 until
+        sum |x_new - x| < epsilon (compared in the block's dtype), then x / ||x||_2.  Edge weights are used.
+        Returns (vertices, values) of the vertices this rank owns; sets last_katz_stats = dict(iterations)."""
+        from cugraph_b200 import _capi as capi
+        p, g, dev, dt, mp = self._centrality_setup("katz_centrality")
+        if not 0.0 <= alpha <= 1.0:
+            raise capi.CugraphValueError(capi.INVALID_INPUT, "Invalid input argument: alpha should be in [0.0, 1.0].",
+                                         "MGGraph.katz_centrality")
+        if not epsilon >= 0.0:
+            raise capi.CugraphValueError(capi.INVALID_INPUT, "Invalid input argument: epsilon should be non-negative.",
+                                         "MGGraph.katz_centrality")
+        T = _np_type(dt)
+        x = torch.zeros(mp, dtype=dt, device=dev)
+        y = torch.zeros(mp, dtype=dt, device=dev)
+        part = torch.zeros(2, dtype=torch.float64, device=dev)
+        bufs = self._sweep_bufs(dt, dev)
+        vxo, vyo = _view(x), _view(y)
+        it = 0
+        try:
+            while True:
+                self._spmv(x, y, bufs, alpha)
+                part.zero_()
+                self._owner_call("cugraph_b200_katz_step", vyo.ptr, vxo.ptr, p.n_local, float(beta), C.c_void_p(part.data_ptr()))
+                dist.all_reduce(part)
+                diff, sumsq = part.tolist()
+                it += 1
+                if T(diff) < T(epsilon):
+                    break
+                if it >= max_iterations:
+                    raise self._fail("MGGraph.katz_centrality", "Katz Centrality failed to converge.")
+            l2 = math.sqrt(sumsq)           # the last step's sum of x_new^2 = ||x||^2
+            if not l2 > 0.0:
+                raise self._fail("MGGraph.katz_centrality", "L2 norm of the computed Katz Centrality values should be positive.")
+            self._owner_call("cugraph_b200_vertex_scale", vxo.ptr, p.n_local, 1.0 / l2)
+        finally:
+            for v in (vxo, vyo) + bufs[2:]:
+                v.free()
+        self.last_katz_stats = dict(iterations=it)
+        return p.vertices, x[:p.n_local].clone()
+
+    def eigenvector_centrality(self, epsilon=1e-6, max_iterations=100):
+        """Eigenvector centrality (cugraph_eigenvector_centrality's semantics): x <- (A^T x + x) / ||A^T x + x||_2 from
+        x = 1 / V until sum |x_new - x| < V * epsilon (V = the global vertex count, compared in the block's dtype).  Edge
+        weights are used.  Returns (vertices, values) of the vertices this rank owns; sets last_eigenvector_stats."""
+        from cugraph_b200 import _capi as capi
+        p, g, dev, dt, mp = self._centrality_setup("eigenvector_centrality")
+        if not epsilon >= 0.0:
+            raise capi.CugraphValueError(capi.INVALID_INPUT, "Invalid input argument: epsilon should be non-negative.",
+                                         "MGGraph.eigenvector_centrality")
+        T = _np_type(dt)
+        V = p.n_global
+        x = torch.zeros(mp, dtype=dt, device=dev)
+        x[:p.n_local] = 1.0 / V
+        y = torch.zeros(mp, dtype=dt, device=dev)
+        sq = torch.zeros(1, dtype=torch.float64, device=dev)
+        part = torch.zeros(1, dtype=torch.float64, device=dev)
+        bufs = self._sweep_bufs(dt, dev)
+        vxo, vyo = _view(x), _view(y)
+        tolerance = T(V) * T(epsilon)
+        it = 0
+        try:
+            while True:
+                self._spmv(x, y, bufs, 1.0)
+                sq.zero_()
+                self._owner_call("cugraph_b200_eigenvector_add_step", vyo.ptr, vxo.ptr, p.n_local, C.c_void_p(sq.data_ptr()))
+                dist.all_reduce(sq)
+                part.zero_()
+                self._owner_call("cugraph_b200_eigenvector_scale_step", vyo.ptr, vxo.ptr, p.n_local, C.c_void_p(sq.data_ptr()),
+                                 C.c_void_p(part.data_ptr()))
+                dist.all_reduce(part)
+                diff = float(part.item())
+                it += 1
+                if T(diff) < tolerance:
+                    break
+                if it >= max_iterations:
+                    raise self._fail("MGGraph.eigenvector_centrality", "Eigenvector Centrality failed to converge.")
+        finally:
+            for v in (vxo, vyo) + bufs[2:]:
+                v.free()
+        self.last_eigenvector_stats = dict(iterations=it)
+        return p.vertices, x[:p.n_local].clone()
+
+    def _guess_to_owners(self, guess, out):
+        """(vertex ids, values) given by any rank -> `out` over the local ids of the vertices this rank owns (others 0)"""
+        from cugraph_b200 import _capi as capi
+        p, g, dev = self.part, self.part.groups, self.device
+        if guess is None:
+            gv = torch.zeros(0, dtype=torch.int64, device=dev)
+            gx = torch.zeros(0, dtype=out.dtype, device=dev)
+        else:
+            gv = torch.as_tensor(guess[0]).to(dev).to(torch.int64).reshape(-1)
+            gx = torch.as_tensor(guess[1]).to(dev).to(out.dtype).reshape(-1)
+            if gv.numel() != gx.numel():
+                raise capi.CugraphValueError(capi.INVALID_INPUT, "initial hubs guess needs vertices and values of equal size",
+                                             "MGGraph.hits")
+        neg = (gx < 0).any().to(torch.int64).reshape(1)
+        dist.all_reduce(neg, op=dist.ReduceOp.MAX)
+        if int(neg.item()):
+            raise capi.CugraphValueError(capi.INVALID_INPUT,
+                                         "Invalid input argument: initial guess values should be non-negative.", "MGGraph.hits")
+        (rv, rx), _, _, _ = exchange([gv, gx], vertex_owner(gv, g.world), g.world)
+        n = p.n_local
+        if n == 0 or rv.numel() == 0:
+            return
+        order = torch.argsort(p.vertices.to(torch.int64))
+        sv = p.vertices.to(torch.int64)[order]
+        pos = torch.searchsorted(sv, rv).clamp(max=n - 1)
+        hit = sv[pos] == rv                          # ids that are not vertices of the graph are dropped
+        out[order[pos[hit]]] = rx[hit]
+
+    def hits(self, epsilon=1e-5, max_iterations=100, initial_hubs_guess=None, normalize=True):
+        """HITS (cugraph_hits' semantics): authorities = A^T hubs, hubs = A authorities (the hubs sweep reads the authorities
+        before their normalisation), both divided by their maximum, until sum |hubs - previous hubs| < V * epsilon (V = the
+        global vertex count, compared in the block's dtype); then both divided by their sum when `normalize`.  Edge weights
+        are not used.  initial_hubs_guess = (vertex ids, values), from any rank for any vertices (others start at 0),
+        L1-normalised.  Returns (vertices, hubs, authorities) of the vertices this rank owns; sets
+        last_hits_stats = dict(iterations, hub_score_differences)."""
+        from cugraph_b200 import _capi as capi
+        p, g, dev, dt, mp = self._centrality_setup("hits")
+        if not epsilon >= 0.0:
+            raise capi.CugraphValueError(capi.INVALID_INPUT, "Invalid input argument: epsilon should be non-negative.",
+                                         "MGGraph.hits")
+        T = _np_type(dt)
+        V = p.n_global
+        prev = torch.zeros(mp, dtype=dt, device=dev)
+        curr = torch.zeros(mp, dtype=dt, device=dev)
+        auth = torch.zeros(mp, dtype=dt, device=dev)
+        mx = torch.zeros(2, dtype=torch.float64, device=dev)
+        part = torch.zeros(2, dtype=torch.float64, device=dev)
+        pull_bufs, push_bufs = self._sweep_bufs(dt, dev), self._sweep_bufs(dt, dev)
+        vp, vc, va = _view(prev), _view(curr), _view(auth)
+        where = "MGGraph.hits"
+
+        def l1_normalize(views):
+            part.zero_()
+            for k, v in enumerate(views):
+                self._owner_call("cugraph_b200_vertex_sum", v.ptr, p.n_local, 0, C.c_void_p(part.data_ptr() + 8 * k))
+            dist.all_reduce(part)
+            norms = part.tolist()
+            for k, v in enumerate(views):
+                if not T(norms[k]) > T(0):
+                    raise self._fail(where, "Norm is required to be a positive value.")
+                self._owner_call("cugraph_b200_vertex_scale", v.ptr, p.n_local, 1.0 / norms[k])
+
+        try:
+            has = torch.tensor([0 if initial_hubs_guess is None else 1], dtype=torch.int64, device=dev)
+            dist.all_reduce(has, op=dist.ReduceOp.MAX)   # a guess from any rank: every rank takes part in its exchange
+            if int(has.item()):
+                self._guess_to_owners(initial_hubs_guess, prev)
+                l1_normalize([vp])
+            else:
+                prev[:p.n_local] = 1.0 / V
+            tolerance = T(V) * T(epsilon)
+            it, diff = 0, float(np.finfo(T).max)
+            while True:
+                self._spmv(prev, auth, pull_bufs, 1.0, use_weights=False)
+                self._spmv(auth, curr, push_bufs, 1.0, transposed=True, use_weights=False)
+                mx.zero_()
+                self._owner_call("cugraph_b200_hits_max_step", vc.ptr, va.ptr, p.n_local, C.c_void_p(mx.data_ptr()))
+                dist.all_reduce(mx, op=dist.ReduceOp.MAX)
+                part.zero_()
+                self._owner_call("cugraph_b200_hits_scale_step", vc.ptr, va.ptr, vp.ptr, p.n_local, C.c_void_p(mx.data_ptr()),
+                                 C.c_void_p(part.data_ptr()))
+                dist.all_reduce(part)
+                d, h_max, a_max = torch.cat([part[:1], mx]).tolist()
+                if not (T(h_max) > T(0) and T(a_max) > T(0)):
+                    raise self._fail(where, "Norm is required to be a positive value.")
+                diff = float(T(d))
+                prev, curr, vp, vc = curr, prev, vc, vp
+                it += 1
+                if T(diff) < tolerance:
+                    break
+                if it >= max_iterations:
+                    raise self._fail(where, "HITS failed to converge.")
+            if normalize:
+                l1_normalize([vp, va])
+        finally:
+            for v in (vp, vc, va) + pull_bufs[2:] + push_bufs[2:]:
+                v.free()
+        self.last_hits_stats = dict(iterations=it, hub_score_differences=diff)
+        return p.vertices, prev[:p.n_local].clone(), auth[:p.n_local].clone()
+
+
+def _np_type(dtype):
+    """the numpy scalar type of a block dtype: convergence tests compare in it, as the single-GPU drivers compare in T"""
+    return np.float32 if dtype == torch.float32 else np.float64
+
 
 INT64_MAX = torch.iinfo(torch.int64).max
 
@@ -732,6 +976,21 @@ def weakly_connected_components(graph: MGGraph):
     """(vertices, labels) of the vertices owned by this rank (the MG contract of pylibcugraph.weakly_connected_components;
     the graph must be symmetric)."""
     return graph.weakly_connected_components()
+
+
+def katz_centrality(graph: MGGraph, alpha, beta=1.0, epsilon=1e-6, max_iterations=100):
+    """(vertices, values) of the vertices owned by this rank (the MG contract of pylibcugraph.katz_centrality)."""
+    return graph.katz_centrality(alpha, beta, epsilon, max_iterations)
+
+
+def eigenvector_centrality(graph: MGGraph, epsilon=1e-6, max_iterations=100):
+    """(vertices, values) of the vertices owned by this rank (the MG contract of pylibcugraph.eigenvector_centrality)."""
+    return graph.eigenvector_centrality(epsilon, max_iterations)
+
+
+def hits(graph: MGGraph, epsilon=1e-5, max_iterations=100, initial_hubs_guess=None, normalize=True):
+    """(vertices, hubs, authorities) of the vertices owned by this rank (the MG contract of pylibcugraph.hits)."""
+    return graph.hits(epsilon, max_iterations, initial_hubs_guess, normalize)
 
 
 def pagerank(graph: MGGraph, alpha=0.85, epsilon=1e-5, max_iterations=100):

@@ -4,9 +4,9 @@
  *  - multi-GPU: the reference receives NCCL communicators inside a raft::handle_t built by raft-dask / MPI
  *    (python/pylibcugraph/pylibcugraph/comms/comms_wrapper.pyx:10-32, cpp/tests/utilities/mg_utilities.cpp:37-55) and keeps
  *    the 2D-partitioned blocks inside graph_t.  raft is not part of this build: cugraph_graph_create_mg and the multi-GPU
- *    algorithm entry points return CUGRAPH_NOT_IMPLEMENTED; multi-GPU PageRank, BFS, SSSP and WCC are driven by the
- *    launcher (cugraph_b200/mg.py, one process per GPU over torch.distributed / NCCL) on top of the cugraph_b200_block_*
- *    device pieces declared below.
+ *    algorithm entry points return CUGRAPH_NOT_IMPLEMENTED; multi-GPU PageRank, BFS, SSSP, WCC, Katz, eigenvector centrality
+ *    and HITS are driven by the launcher (cugraph_b200/mg.py, one process per GPU over torch.distributed / NCCL) on top of
+ *    the cugraph_b200_block_* and owner-step device pieces declared below.
  *  - profiling hooks used by bench.py to time the dominant kernel on the handle's stream.
  */
 #pragma once
@@ -59,6 +59,58 @@ CUGRAPH_EXPORT size_t cugraph_b200_block_span(const cugraph_b200_block_t* block)
 CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_pull_sweep(
   const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
   const cugraph_type_erased_device_array_view_t* x, cugraph_type_erased_device_array_view_t* y, double alpha,
+  cugraph_error_t** error);
+/* The block sweep in either orientation.  transposed = FALSE, use_weights = TRUE is cugraph_b200_block_pull_sweep.
+ * transposed = TRUE: y[col] = alpha * sum over the block's edges (row, col) of x[row] * w for every column slot; x is indexed by
+ * row slot.  use_weights = FALSE sums plain neighbour values (w = 1) on a weighted block.  The rules of
+ * cugraph_b200_block_pull_sweep hold for both orientations: x holds cugraph_b200_padded_elems(span) elements, zero from
+ * `span` on, anything (NaN included) where no edge reads; y holds `span` elements; x and y do not overlap; the first sweep
+ * of an orientation into a given y writes every slot, later sweeps of that orientation into the same y only the slots that
+ * have edges (the two orientations keep this state apart; a sweep into an array the other orientation last swept writes it
+ * whole again).  The transposed sweep runs the same kernels over the block's column-major copy; the first transposed call
+ * on a block builds that copy (shared with cugraph_b200_block_sssp_relax / _wcc_min) when no earlier call did, together with
+ * its sweep layout and accumulators, and synchronises once.  Otherwise asynchronous. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_sweep(
+  const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block, bool_t transposed, bool_t use_weights,
+  const cugraph_type_erased_device_array_view_t* x, cugraph_type_erased_device_array_view_t* y, double alpha,
+  cugraph_error_t** error);
+/* Owner steps of multi-GPU Katz, eigenvector centrality and HITS (the launcher cugraph_b200/mg.py runs them between its
+ * collectives).  Each passes once over this rank's first n_local elements, which all arrays must hold, and ADDS its fp64
+ * partials into the caller's device doubles (max partials are merged with an atomic max), to be all-reduced by the launcher.
+ * All arrays share one FLOAT32 / FLOAT64 type.  The arithmetic is that of the single-GPU cugraph_katz_centrality /
+ * _eigenvector_centrality / cugraph_hits: scaling as (T)((double)v * inv), differences and norms in fp64.  Asynchronous.
+ *   katz_step:              x_new = (T)(y + beta); partial[0] += sum |x_new - x|, partial[1] += sum x_new^2; x = x_new.
+ *   eigenvector_add_step:   y += x; partial[0] += sum y^2.
+ *   eigenvector_scale_step: y = y / sqrt(sumsq[0]) (sumsq: the all-reduced sum of the add step, read on the device);
+ *                           partial[0] += sum |y - x|; x = y.
+ *   hits_max_step:          max_out[0] = max(max_out[0], max hubs), max_out[1] = max(max_out[1], max authorities); the values
+ *                           must be non-negative and max_out starts at 0.
+ *   hits_scale_step:        hubs /= max[0], authorities /= max[1] (the all-reduced maxima, read on the device);
+ *                           partial[0] += sum |hubs - prev_hubs|.
+ *   vertex_sum:             partial[0] += sum v^2 (squares = TRUE) or sum v.
+ *   vertex_scale:           v = (T)(v * inv). */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_katz_step(
+  const cugraph_resource_handle_t* handle, const cugraph_type_erased_device_array_view_t* y,
+  cugraph_type_erased_device_array_view_t* x, size_t n_local, double beta, double* partial_out_device, cugraph_error_t** error);
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_eigenvector_add_step(
+  const cugraph_resource_handle_t* handle, cugraph_type_erased_device_array_view_t* y,
+  const cugraph_type_erased_device_array_view_t* x, size_t n_local, double* partial_out_device, cugraph_error_t** error);
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_eigenvector_scale_step(
+  const cugraph_resource_handle_t* handle, cugraph_type_erased_device_array_view_t* y,
+  cugraph_type_erased_device_array_view_t* x, size_t n_local, const double* sumsq_device, double* partial_out_device,
+  cugraph_error_t** error);
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_hits_max_step(
+  const cugraph_resource_handle_t* handle, const cugraph_type_erased_device_array_view_t* hubs,
+  const cugraph_type_erased_device_array_view_t* authorities, size_t n_local, double* max_out_device, cugraph_error_t** error);
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_hits_scale_step(
+  const cugraph_resource_handle_t* handle, cugraph_type_erased_device_array_view_t* hubs,
+  cugraph_type_erased_device_array_view_t* authorities, const cugraph_type_erased_device_array_view_t* prev_hubs,
+  size_t n_local, const double* max_device, double* partial_out_device, cugraph_error_t** error);
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_vertex_sum(
+  const cugraph_resource_handle_t* handle, const cugraph_type_erased_device_array_view_t* v, size_t n_local, bool_t squares,
+  double* partial_out_device, cugraph_error_t** error);
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_vertex_scale(
+  const cugraph_resource_handle_t* handle, cugraph_type_erased_device_array_view_t* v, size_t n_local, double inv,
   cugraph_error_t** error);
 CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_pagerank_vertex_step(
   const cugraph_resource_handle_t* handle, const cugraph_type_erased_device_array_view_t* y,
