@@ -183,14 +183,21 @@ k_hits_scale(T* __restrict__ hubs, T* __restrict__ auth, T const* __restrict__ p
 }
 
 
+// the global code of a column slot: (owner rank) * maxpart + local id, owner rank = (col / maxpart) * grid_cols + grid_c
+__device__ __forceinline__ long long column_code(int col, long long maxpart, int grid_cols, int grid_c)
+{
+  return ((long long)(col / maxpart) * grid_cols + grid_c) * maxpart + (col % maxpart);
+}
+
 // ---- one level of multi-GPU BFS on this GPU's edge block, pull direction (the MG form of k_bfs_bottomup, traverse.cu;
 // reference: the bottom-up step of bfs_impl.cuh:593-869 on an edge partition, with the frontier arriving through
 // fill_edge_dst_property-style broadcasts, fill_edge_src_dst_property.cuh:1368).  The block stores its edges by destination
 // slot (rows) with the source slots as neighbours (columns, ascending).  frontier[col] / visited[row] are byte flags over
 // the block's column / row slots (the launcher all-gathers them inside the column / row group); every unvisited row scans
-// its sources until it meets one in the frontier and reports it as cand[row] = GLOBAL code of that source
-// ((owner rank) * maxpart + local id, owner rank = (col / maxpart) * grid_cols + grid_c), else -1.  Rows of degree >= 32
+// its sources until it meets one in the frontier and reports it as cand[row] = GLOBAL code of that source (column_code),
+// else -1.  Rows of degree >= 32
 // (the prefix of the degree-ordered physical rows) take a warp each with a ballot early exit, the others a thread each.
+
 template <typename O>
 __global__ void __launch_bounds__(256)
 k_block_bfs_pull_hi(O const* __restrict__ off, int32_t const* __restrict__ idx, int32_t const* __restrict__ row_vertex, int32_t n_hi,
@@ -212,7 +219,7 @@ k_block_bfs_pull_hi(O const* __restrict__ off, int32_t const* __restrict__ idx, 
         break;
       }
     }
-    if (lane == 0 && found >= 0) cand[slot] = ((long long)(found / maxpart) * grid_cols + grid_c) * maxpart + (found % maxpart);
+    if (lane == 0 && found >= 0) cand[slot] = column_code(found, maxpart, grid_cols, grid_c);
   }
 }
 
@@ -229,7 +236,7 @@ k_block_bfs_pull_low(O const* __restrict__ off, int32_t const* __restrict__ idx,
     for (long long e = (long long)off[r]; e < e1; ++e) {
       const int col = idx[e];
       if (frontier[col]) {
-        cand[slot] = ((long long)(col / maxpart) * grid_cols + grid_c) * maxpart + (col % maxpart);
+        cand[slot] = column_code(col, maxpart, grid_cols, grid_c);
         break;
       }
     }
@@ -292,12 +299,6 @@ k_block_active_rows(O const* __restrict__ off, int32_t const* __restrict__ row_v
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) edges += __shfl_xor_sync(0xffffffffu, edges, o);
   if ((threadIdx.x & 31) == 0 && edges) atomicAdd(&cnt->edges, edges);
-}
-
-// the global code of a column slot, as in the BFS pull kernels
-__device__ __forceinline__ long long column_code(int col, long long maxpart, int grid_cols, int grid_c)
-{
-  return ((long long)(col / maxpart) * grid_cols + grid_c) * maxpart + (col % maxpart);
 }
 
 // one key orders the proposals to a row: float (distance bits, code) — the smallest distance, among equal distances the
@@ -416,6 +417,14 @@ void check_owner_args(std::initializer_list<device_array_view_impl const*> vs, s
   }
 }
 
+// f(float{}) for FLOAT32, else f(double{}): the launchers' dispatch on the floating type of their (checked) arrays
+template <typename F>
+void by_float_type(cugraph_data_type_id_t t, F&& f)
+{
+  if (t == FLOAT32) f(float{});
+  else f(double{});
+}
+
 // active rows -> queue (one read-back of its size and edge count) -> advance with `op`
 template <typename O, typename T, typename Op>
 void block_push_round(handle_impl const& h, block_push_t& p, T const* dist_cols, Op op)
@@ -432,6 +441,15 @@ void block_push_round(handle_impl const& h, block_push_t& p, T const* dist_cols,
   sync(h);
   advance<O>(h, p.adv, pc.offsets.as<O>(), pc.indices.as<int32_t>(), p.queue.as<int32_t>(), hc.n, hc.edges, op,
              p.q_deg.as<int32_t>());
+}
+
+// out[row slot] = INT64_MAX (no proposal), then one push round of `op` over the columns active in `active_cols`
+template <typename T, typename Op>
+void block_push_min(handle_impl const& h, block_impl const& b, block_push_t& p, long long* out, T const* active_cols, Op op)
+{
+  B200_LAUNCH(h, k_fill_i64, std::min((b.n_rows + 255) / 256 + 1, h.sm_count * 8), 256, 0, out, (long long)b.n_rows, LLONG_MAX);
+  if (p.csx->offs64) block_push_round<int64_t>(h, p, active_cols, op);
+  else block_push_round<int32_t>(h, p, active_cols, op);
 }
 
 template <typename T>
@@ -600,11 +618,10 @@ cugraph_error_code_t cugraph_b200_katz_step(const cugraph_resource_handle_t* han
     check_owner_args({yv, xv}, n_local, partial_out_device);
     if (n_local == 0) return;
     const int32_t n = (int32_t)n_local;
-    if (yv->type == FLOAT32)
-      B200_LAUNCH(h, (k_katz_step<float>), cgrid(h, n), kCBlock, 0, (float const*)yv->data, (float*)xv->data, n, beta, partial_out_device);
-    else
-      B200_LAUNCH(h, (k_katz_step<double>), cgrid(h, n), kCBlock, 0, (double const*)yv->data, (double*)xv->data, n, beta,
-                  partial_out_device);
+    by_float_type(yv->type, [&](auto z) {
+      using T = decltype(z);
+      B200_LAUNCH(h, k_katz_step<T>, cgrid(h, n), kCBlock, 0, (T const*)yv->data, (T*)xv->data, n, beta, partial_out_device);
+    });
     check_last("katz_step");
   });
 }
@@ -621,10 +638,10 @@ cugraph_error_code_t cugraph_b200_eigenvector_add_step(const cugraph_resource_ha
     check_owner_args({yv, xv}, n_local, partial_out_device);
     if (n_local == 0) return;
     const int32_t n = (int32_t)n_local;
-    if (yv->type == FLOAT32)
-      B200_LAUNCH(h, (k_eig_add<float>), cgrid(h, n), kCBlock, 0, (float*)yv->data, (float const*)xv->data, n, partial_out_device);
-    else
-      B200_LAUNCH(h, (k_eig_add<double>), cgrid(h, n), kCBlock, 0, (double*)yv->data, (double const*)xv->data, n, partial_out_device);
+    by_float_type(yv->type, [&](auto z) {
+      using T = decltype(z);
+      B200_LAUNCH(h, k_eig_add<T>, cgrid(h, n), kCBlock, 0, (T*)yv->data, (T const*)xv->data, n, partial_out_device);
+    });
     check_last("eigenvector_add_step");
   });
 }
@@ -643,12 +660,10 @@ cugraph_error_code_t cugraph_b200_eigenvector_scale_step(const cugraph_resource_
     B200_EXPECTS(sumsq_device != nullptr, CUGRAPH_INVALID_INPUT, "NULL argument");
     if (n_local == 0) return;
     const int32_t n = (int32_t)n_local;
-    if (yv->type == FLOAT32)
-      B200_LAUNCH(h, (k_eig_scale<float>), cgrid(h, n), kCBlock, 0, (float*)yv->data, (float*)xv->data, n, sumsq_device,
-                  partial_out_device);
-    else
-      B200_LAUNCH(h, (k_eig_scale<double>), cgrid(h, n), kCBlock, 0, (double*)yv->data, (double*)xv->data, n, sumsq_device,
-                  partial_out_device);
+    by_float_type(yv->type, [&](auto z) {
+      using T = decltype(z);
+      B200_LAUNCH(h, k_eig_scale<T>, cgrid(h, n), kCBlock, 0, (T*)yv->data, (T*)xv->data, n, sumsq_device, partial_out_device);
+    });
     check_last("eigenvector_scale_step");
   });
 }
@@ -665,11 +680,10 @@ cugraph_error_code_t cugraph_b200_hits_max_step(const cugraph_resource_handle_t*
     check_owner_args({hv, av}, n_local, max_out_device);
     if (n_local == 0) return;
     const int32_t n = (int32_t)n_local;
-    if (hv->type == FLOAT32)
-      B200_LAUNCH(h, (k_hits_max<float>), cgrid(h, n), kCBlock, 0, (float const*)hv->data, (float const*)av->data, n, max_out_device);
-    else
-      B200_LAUNCH(h, (k_hits_max<double>), cgrid(h, n), kCBlock, 0, (double const*)hv->data, (double const*)av->data, n,
-                  max_out_device);
+    by_float_type(hv->type, [&](auto z) {
+      using T = decltype(z);
+      B200_LAUNCH(h, k_hits_max<T>, cgrid(h, n), kCBlock, 0, (T const*)hv->data, (T const*)av->data, n, max_out_device);
+    });
     check_last("hits_max_step");
   });
 }
@@ -689,12 +703,11 @@ cugraph_error_code_t cugraph_b200_hits_scale_step(const cugraph_resource_handle_
     B200_EXPECTS(max_device != nullptr, CUGRAPH_INVALID_INPUT, "NULL argument");
     if (n_local == 0) return;
     const int32_t n = (int32_t)n_local;
-    if (hv->type == FLOAT32)
-      B200_LAUNCH(h, (k_hits_scale<float>), cgrid(h, n), kCBlock, 0, (float*)hv->data, (float*)av->data, (float const*)pv->data, n,
-                  max_device, partial_out_device);
-    else
-      B200_LAUNCH(h, (k_hits_scale<double>), cgrid(h, n), kCBlock, 0, (double*)hv->data, (double*)av->data,
-                  (double const*)pv->data, n, max_device, partial_out_device);
+    by_float_type(hv->type, [&](auto z) {
+      using T = decltype(z);
+      B200_LAUNCH(h, k_hits_scale<T>, cgrid(h, n), kCBlock, 0, (T*)hv->data, (T*)av->data, (T const*)pv->data, n, max_device,
+                  partial_out_device);
+    });
     check_last("hits_scale_step");
   });
 }
@@ -710,10 +723,10 @@ cugraph_error_code_t cugraph_b200_vertex_sum(const cugraph_resource_handle_t* ha
     if (n_local == 0) return;
     const int32_t n = (int32_t)n_local;
     const int mode  = squares == TRUE ? 0 : 1;
-    if (vv->type == FLOAT32)
-      B200_LAUNCH(h, (k_norm<float>), cgrid(h, n), kCBlock, 0, (float const*)vv->data, n, mode, partial_out_device);
-    else
-      B200_LAUNCH(h, (k_norm<double>), cgrid(h, n), kCBlock, 0, (double const*)vv->data, n, mode, partial_out_device);
+    by_float_type(vv->type, [&](auto z) {
+      using T = decltype(z);
+      B200_LAUNCH(h, k_norm<T>, cgrid(h, n), kCBlock, 0, (T const*)vv->data, n, mode, partial_out_device);
+    });
     check_last("vertex_sum");
   });
 }
@@ -727,8 +740,10 @@ cugraph_error_code_t cugraph_b200_vertex_scale(const cugraph_resource_handle_t* 
     check_owner_args({vv}, n_local, &inv);
     if (n_local == 0) return;
     const int32_t n = (int32_t)n_local;
-    if (vv->type == FLOAT32) B200_LAUNCH(h, (k_scale<float>), cgrid(h, n), kCBlock, 0, (float*)vv->data, n, inv);
-    else B200_LAUNCH(h, (k_scale<double>), cgrid(h, n), kCBlock, 0, (double*)vv->data, n, inv);
+    by_float_type(vv->type, [&](auto z) {
+      using T = decltype(z);
+      B200_LAUNCH(h, k_scale<T>, cgrid(h, n), kCBlock, 0, (T*)vv->data, n, inv);
+    });
     check_last("vertex_scale");
   });
 }
@@ -754,14 +769,11 @@ cugraph_error_code_t cugraph_b200_pagerank_vertex_step(const cugraph_resource_ha
                  CUGRAPH_INVALID_INPUT, "arrays shorter than n_local");
     if (n_local == 0) return;
     const int grid = (int)std::min<size_t>((n_local + 255) / 256, (size_t)h.sm_count * 8);
-    if (yv->type == FLOAT32)
-      B200_LAUNCH(h, (k_mg_vertex_step<float>), grid, 256, 0, (float const*)yv->data, (float*)pv->data, (float const*)ov->data,
-                  (float*)xv->data, (int32_t)n_local, alpha, n_vertices_global, first == TRUE ? 1 : 0, totals_prev_device,
-                  partial_out_device);
-    else
-      B200_LAUNCH(h, (k_mg_vertex_step<double>), grid, 256, 0, (double const*)yv->data, (double*)pv->data,
-                  (double const*)ov->data, (double*)xv->data, (int32_t)n_local, alpha, n_vertices_global,
-                  first == TRUE ? 1 : 0, totals_prev_device, partial_out_device);
+    by_float_type(yv->type, [&](auto z) {
+      using T = decltype(z);
+      B200_LAUNCH(h, k_mg_vertex_step<T>, grid, 256, 0, (T const*)yv->data, (T*)pv->data, (T const*)ov->data, (T*)xv->data,
+                  (int32_t)n_local, alpha, n_vertices_global, first == TRUE ? 1 : 0, totals_prev_device, partial_out_device);
+    });
     check_last("pagerank_vertex_step");
   });
 }
@@ -816,19 +828,13 @@ cugraph_error_code_t cugraph_b200_block_sssp_relax(const cugraph_resource_handle
     }
     block_push_t& p = push_copy(h, *b);
     auto* cand      = (long long*)cv->data;
-    B200_LAUNCH(h, k_fill_i64, std::min((b->n_rows + 255) / 256 + 1, h.sm_count * 8), 256, 0, cand, (long long)b->n_rows, LLONG_MAX);
-    int32_t const* col_of = p.csx->row_vertex.as<int32_t>();
-    if (b->wtype == FLOAT32) {
-      block_relax_op<float> op{col_of, p.csx->weights.as<float>(), (float const*)dv->data, rounded_cutoff<float>(cutoff),
-                               (long long)maxpart, grid_cols, grid_c, cand};
-      if (p.csx->offs64) block_push_round<int64_t>(h, p, (float const*)dv->data, op);
-      else block_push_round<int32_t>(h, p, (float const*)dv->data, op);
-    } else {
-      block_relax_op<double> op{col_of, p.csx->weights.as<double>(), (double const*)dv->data, rounded_cutoff<double>(cutoff),
-                                (long long)maxpart, grid_cols, grid_c, cand};
-      if (p.csx->offs64) block_push_round<int64_t>(h, p, (double const*)dv->data, op);
-      else block_push_round<int32_t>(h, p, (double const*)dv->data, op);
-    }
+    by_float_type(b->wtype, [&](auto z) {
+      using T       = decltype(z);
+      auto const* d = (T const*)dv->data;
+      block_push_min(h, *b, p, cand, d,
+                     block_relax_op<T>{p.csx->row_vertex.as<int32_t>(), p.csx->weights.as<T>(), d, rounded_cutoff<T>(cutoff),
+                                       (long long)maxpart, grid_cols, grid_c, cand});
+    });
     check_last("block_sssp_relax");
   });
 }
@@ -852,19 +858,13 @@ cugraph_error_code_t cugraph_b200_block_sssp_pred(const cugraph_resource_handle_
     B200_EXPECTS(wv->size >= (size_t)b->n_rows, CUGRAPH_INVALID_INPUT, "win_rows shorter than the block's row slots");
     block_push_t& p = push_copy(h, *b);
     auto* code      = (long long*)cv->data;
-    B200_LAUNCH(h, k_fill_i64, std::min((b->n_rows + 255) / 256 + 1, h.sm_count * 8), 256, 0, code, (long long)b->n_rows, LLONG_MAX);
-    int32_t const* col_of = p.csx->row_vertex.as<int32_t>();
-    if (b->wtype == FLOAT32) {
-      block_pred_op<float> op{col_of, p.csx->weights.as<float>(), (float const*)dv->data, (float const*)wv->data,
-                              (long long)maxpart, grid_cols, grid_c, code};
-      if (p.csx->offs64) block_push_round<int64_t>(h, p, (float const*)dv->data, op);
-      else block_push_round<int32_t>(h, p, (float const*)dv->data, op);
-    } else {
-      block_pred_op<double> op{col_of, p.csx->weights.as<double>(), (double const*)dv->data, (double const*)wv->data,
-                               (long long)maxpart, grid_cols, grid_c, code};
-      if (p.csx->offs64) block_push_round<int64_t>(h, p, (double const*)dv->data, op);
-      else block_push_round<int32_t>(h, p, (double const*)dv->data, op);
-    }
+    by_float_type(b->wtype, [&](auto z) {
+      using T       = decltype(z);
+      auto const* d = (T const*)dv->data;
+      block_push_min(h, *b, p, code, d,
+                     block_pred_op<T>{p.csx->row_vertex.as<int32_t>(), p.csx->weights.as<T>(), d, (T const*)wv->data,
+                                      (long long)maxpart, grid_cols, grid_c, code});
+    });
     check_last("block_sssp_pred");
   });
 }
@@ -886,10 +886,7 @@ cugraph_error_code_t cugraph_b200_block_wcc_min(const cugraph_resource_handle_t*
     block_push_t& p   = push_copy(h, *b);
     auto const* label = (long long const*)lv->data;
     auto* cand        = (long long*)cv->data;
-    B200_LAUNCH(h, k_fill_i64, std::min((b->n_rows + 255) / 256 + 1, h.sm_count * 8), 256, 0, cand, (long long)b->n_rows, LLONG_MAX);
-    block_wcc_op op{p.csx->row_vertex.as<int32_t>(), label, cand};
-    if (p.csx->offs64) block_push_round<int64_t>(h, p, label, op);
-    else block_push_round<int32_t>(h, p, label, op);
+    block_push_min(h, *b, p, cand, label, block_wcc_op{p.csx->row_vertex.as<int32_t>(), label, cand});
     check_last("block_wcc_min");
   });
 }

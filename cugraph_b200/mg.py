@@ -24,6 +24,7 @@ tests/test_mg_partition_cpu.py) builds the blocks; `MGGraph` and the module-leve
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import math
 import os
@@ -115,7 +116,10 @@ def exchange(tensors, dest: torch.Tensor, world: int):
 
 
 def all_gather_into(out: torch.Tensor, inp: torch.Tensor, group):
-    if _is_nccl(group):
+    """out = every member's inp, in group-rank order.  A one-member group copies: no collective call."""
+    if dist.get_world_size(group) == 1:
+        out.copy_(inp)
+    elif _is_nccl(group):
         dist.all_gather_into_tensor(out, inp, group=group)
     else:
         n = dist.get_world_size(group)
@@ -125,8 +129,12 @@ def all_gather_into(out: torch.Tensor, inp: torch.Tensor, group):
 
 
 def reduce_scatter_into(out: torch.Tensor, inp: torch.Tensor, group, op=None):
+    """out = this member's slice of the members' inp reduced with op (default SUM).  A one-member group copies: no
+    collective call."""
     op = op or dist.ReduceOp.SUM
-    if _is_nccl(group):
+    if dist.get_world_size(group) == 1:
+        out.copy_(inp)
+    elif _is_nccl(group):
         dist.reduce_scatter_tensor(out, inp, op=op, group=group)
     else:
         tmp = inp.clone()
@@ -211,9 +219,25 @@ def partition_edges(src: torch.Tensor, dst: torch.Tensor, weights=None, groups: 
 # ----------------------------------------------------------------------------------------------
 # CUDA side
 # ----------------------------------------------------------------------------------------------
-def _view(t):
+@contextlib.contextmanager
+def _views(*tensors):
+    """C array views of the tensors (None gives a NULL view), freed when the block exits, also when it raises"""
     from cugraph_b200.pylibcugraph.utils import View
-    return View(t)
+    vs = []
+    try:
+        for t in tensors:
+            vs.append(View(t))
+        yield vs
+    finally:
+        for v in vs:
+            v.free()
+
+
+def _global_count(mask):
+    """the number of set entries of `mask` over all ranks, as a host int (one all-reduce)"""
+    n = mask.sum().to(torch.int64).reshape(1)
+    dist.all_reduce(n)
+    return int(n.item())
 
 
 class MGGraph:
@@ -232,34 +256,11 @@ class MGGraph:
         self.handle = ResourceHandle(stream=torch.cuda.current_stream().cuda_stream)
         self.n_rows, self.n_cols = g.C * p.maxpart, g.R * p.maxpart
         es = 4 if self.dtype == torch.float32 else 8
-        # EXPERIMENTAL (CUGRAPH_B200_MG_SPLIT=1): one block per destination partition of the row group, so that the
-        # reduction of partition j's partial sums runs under the sweep of partition j+1 (pagerank_split)
-        self.split = os.environ.get("CUGRAPH_B200_MG_SPLIT", "0") == "1" and g.C > 1
-        self.block, self.blocks = None, []
-
-        def make_block(rows, cols, w, n_rows):
-            rv, cv, wv = _view(rows), _view(cols), _view(w)
-            blk, err = C.c_void_p(), C.c_void_p()
-            code = self.lib.cugraph_b200_block_create(self.handle.ptr, n_rows, self.n_cols, rv.ptr, cv.ptr, wv.ptr,
-                                                      C.byref(blk), C.byref(err))
-            for v in (rv, cv, wv):
-                v.free()
-            _capi.check(code, err, "cugraph_b200_block_create")
-            return blk.value
-
-        if self.split:
-            part_of = torch.div(p.rows, p.maxpart, rounding_mode="floor")
-            for j in range(g.C):
-                m = part_of == j
-                rj = (p.rows[m] - j * p.maxpart).to(p.rows.dtype).contiguous()
-                cj = p.cols[m].contiguous()
-                wj = p.weights[m].contiguous() if p.weights is not None else None
-                self.blocks.append(make_block(rj, cj, wj, p.maxpart))
-            self.spans = [int(self.lib.cugraph_b200_block_span(b)) for b in self.blocks]
-            self.span = max(self.spans)
-        else:
-            self.block = make_block(p.rows, p.cols, p.weights, self.n_rows)
-            self.span = int(self.lib.cugraph_b200_block_span(self.block))
+        blk = C.c_void_p()
+        with _views(p.rows, p.cols, p.weights) as (rv, cv, wv):
+            self._call("cugraph_b200_block_create", self.n_rows, self.n_cols, rv.ptr, cv.ptr, wv.ptr, C.byref(blk))
+        self.block = blk.value
+        self.span = int(self.lib.cugraph_b200_block_span(self.block))
         self.x_elems = int(self.lib.cugraph_b200_padded_elems(self.span, es))
         # out-weight sums of the owned vertices: partial per column slot, reduce-scattered in the column group
         ones = p.weights.to(torch.float64) if p.weights is not None else torch.ones(p.cols.numel(), dtype=torch.float64, device=src.device)
@@ -284,17 +285,12 @@ class MGGraph:
             if getattr(self, "block", None):
                 self.lib.cugraph_b200_block_free(self.block)
                 self.block = None
-            for b in getattr(self, "blocks", []):
-                self.lib.cugraph_b200_block_free(b)
-            self.blocks = []
         except Exception:
             pass
 
     # one PageRank iteration = all-gather(x) -> block sweep -> reduce-scatter(y) -> vertex step -> all-reduce(2 scalars)
-    def pagerank(self, alpha=0.85, epsilon=1e-5, max_iterations=100, time_iterations=False):
-        if self.split:
-            return self.pagerank_split(alpha, epsilon, max_iterations)
-        p, g, L, capi = self.part, self.part.groups, self.lib, self._capi
+    def pagerank(self, alpha=0.85, epsilon=1e-5, max_iterations=100):
+        p, g = self.part, self.part.groups
         dev, dt, mp = self.out_w.device, self.dtype, p.maxpart
         pr = torch.zeros(mp, dtype=dt, device=dev)
         pr[:p.n_local] = 1.0 / p.n_global
@@ -304,54 +300,38 @@ class MGGraph:
         yred = torch.zeros(mp, dtype=dt, device=dev)
         tot = torch.zeros(2, dtype=torch.float64, device=dev)
         part = torch.zeros(2, dtype=torch.float64, device=dev)
-        views = {k: _view(v) for k, v in dict(pr=pr, x=x_local, xg=xg, yp=ypart, yr=yred, ow=self.out_w).items()}
-        err = C.c_void_p()
-
         pending = [None]
 
-        def vertex_step(first):
-            # the totals of the previous step are needed now: their all-reduce ran under the sweep in between
+        with _views(pr, x_local, xg, ypart, yred, self.out_w) as (vpr, vx, vxg, vyp, vyr, vow):
+            def vertex_step(first):
+                # the totals of the previous step are needed now: their all-reduce ran under the sweep in between
+                if pending[0] is not None:
+                    pending[0].wait()
+                    pending[0] = None
+                part.zero_()
+                self._call("cugraph_b200_pagerank_vertex_step", vyr.ptr, vpr.ptr, vow.ptr, vx.ptr, p.n_local, float(alpha),
+                           float(p.n_global), 1 if first else 0, C.c_void_p(tot.data_ptr()), C.c_void_p(part.data_ptr()))
+                pending[0] = dist.all_reduce(part, async_op=True)
+
+            vertex_step(True)
+            tot, part = part, tot
+            iters = 0
+            xcols = xg[:self.n_cols]
+            for _ in range(int(max_iterations)):
+                all_gather_into(xcols, x_local, g.col_group)            # partition-major = the block's column order
+                self._call("cugraph_b200_block_pull_sweep", self.block, vxg.ptr, vyp.ptr, float(alpha))
+                reduce_scatter_into(yred, ypart[:self.n_rows], g.row_group)
+                vertex_step(False)
+                tot, part = part, tot
+                iters += 1
+                if epsilon > 0.0:   # host sync only when a tolerance is requested
+                    pending[0].wait()
+                    pending[0] = None
+                    if float(tot[0].item()) < epsilon:
+                        break
             if pending[0] is not None:
                 pending[0].wait()
-                pending[0] = None
-            part.zero_()
-            code = L.cugraph_b200_pagerank_vertex_step(self.handle.ptr, views["yr"].ptr, views["pr"].ptr, views["ow"].ptr,
-                                                       views["x"].ptr, p.n_local, float(alpha), float(p.n_global),
-                                                       1 if first else 0, C.c_void_p(tot.data_ptr()),
-                                                       C.c_void_p(part.data_ptr()), C.byref(err))
-            capi.check(code, err, "cugraph_b200_pagerank_vertex_step")
-            pending[0] = dist.all_reduce(part, async_op=True)
-
-        vertex_step(True)
-        tot, part = part, tot
-        iters, converged = 0, False
-        xcols = xg[:self.n_cols]
-        for _ in range(int(max_iterations)):
-            if g.R == 1:
-                xcols[:mp].copy_(x_local)
-            else:
-                all_gather_into(xcols, x_local, g.col_group)            # partition-major = the block's column order
-            code = L.cugraph_b200_block_pull_sweep(self.handle.ptr, self.block, views["xg"].ptr, views["yp"].ptr,
-                                                   float(alpha), C.byref(err))
-            capi.check(code, err, "cugraph_b200_block_pull_sweep")
-            if g.C == 1:
-                yred.copy_(ypart[:mp])
-            else:
-                reduce_scatter_into(yred, ypart[:self.n_rows], g.row_group)
-            vertex_step(False)
-            tot, part = part, tot
-            iters += 1
-            if epsilon > 0.0:   # host sync only when a tolerance is requested
-                pending[0].wait()
-                pending[0] = None
-                if float(tot[0].item()) < epsilon:
-                    break
-        if pending[0] is not None:
-            pending[0].wait()
-        converged = iters < max_iterations
-        for v in views.values():
-            v.free()
-        return p.vertices, pr[:p.n_local].clone(), iters, converged
+        return p.vertices, pr[:p.n_local].clone(), iters, iters < max_iterations
 
     # ------------------------------------------------------------------------------------------
     # multi-GPU BFS.  The reference's MG BFS (bfs_impl.cuh:446-869) moves the frontier through the edge partitions with
@@ -366,8 +346,7 @@ class MGGraph:
     def bfs(self, source, depth_limit=-1, compute_predecessors=True):
         """source: external vertex id (the same value on every rank).  Returns (vertices, distances, predecessors) of the
         vertices this rank owns: int32 distances (INT32_MAX = unreachable), predecessors as external ids (-1 = none)."""
-        assert self.block is not None, "bfs needs the unsplit block"
-        p, g, L, capi = self.part, self.part.groups, self.lib, self._capi
+        p, g = self.part, self.part.groups
         dev, mp = self.device, p.maxpart
         imax = torch.iinfo(torch.int32).max
         dist_own = torch.full((mp,), imax, dtype=torch.int32, device=dev)
@@ -384,38 +363,21 @@ class MGGraph:
         v_rows = torch.zeros(self.n_rows, dtype=torch.uint8, device=dev)
         cand = torch.full((self.n_rows,), -1, dtype=torch.int64, device=dev)
         cand_own = torch.full((mp,), -1, dtype=torch.int64, device=dev)
-        views = {k: _view(v) for k, v in dict(f=f_cols, v=v_rows, c=cand).items()}
-        err = C.c_void_p()
         level = 0
-        count = torch.zeros(1, dtype=torch.int64, device=dev)
-        while depth_limit < 0 or level < depth_limit:
-            if g.R == 1:
-                f_cols.copy_(frontier)
-            else:
+        with _views(f_cols, v_rows, cand) as (vf, vv, vc):
+            while depth_limit < 0 or level < depth_limit:
                 all_gather_into(f_cols, frontier, g.col_group)
-            if g.C == 1:
-                v_rows.copy_(visited)
-            else:
                 all_gather_into(v_rows, visited, g.row_group)
-            code = L.cugraph_b200_block_bfs_pull(self.handle.ptr, self.block, views["f"].ptr, views["v"].ptr, mp, g.C, g.c,
-                                                 views["c"].ptr, C.byref(err))
-            capi.check(code, err, "cugraph_b200_block_bfs_pull")
-            if g.C == 1:
-                cand_own.copy_(cand)
-            else:
+                self._call("cugraph_b200_block_bfs_pull", self.block, vf.ptr, vv.ptr, mp, g.C, g.c, vc.ptr)
                 reduce_scatter_into(cand_own, cand, g.row_group, op=dist.ReduceOp.MAX)
-            new = (visited == 0) & (cand_own >= 0)
-            level += 1
-            dist_own[new] = level
-            pred_code[new] = cand_own[new]
-            visited |= new.to(torch.uint8)
-            frontier = new.to(torch.uint8)
-            count.fill_(int(new.sum().item()))
-            dist.all_reduce(count)
-            if int(count.item()) == 0:
-                break
-        for v in views.values():
-            v.free()
+                new = (visited == 0) & (cand_own >= 0)
+                level += 1
+                dist_own[new] = level
+                pred_code[new] = cand_own[new]
+                visited |= new.to(torch.uint8)
+                frontier = new.to(torch.uint8)
+                if _global_count(new) == 0:
+                    break
         verts = p.vertices
         d_out = dist_own[:p.n_local].clone()
         if not compute_predecessors:
@@ -490,8 +452,7 @@ class MGGraph:
         sssp_impl.cuh:215-229), predecessors as external ids (-1 = none), or None when not requested."""
         if not self.weighted:
             raise ValueError("SSSP requires a weighted graph")
-        assert self.block is not None, "sssp needs the unsplit block"
-        p, g, L, capi = self.part, self.part.groups, self.lib, self._capi
+        p, g = self.part, self.part.groups
         dev, dt, mp = self.device, self.dtype, p.maxpart
         f32 = dt == torch.float32
         lid = self._source_lid(source, "sssp")
@@ -507,67 +468,43 @@ class MGGraph:
         x_cols = torch.empty(self.n_cols, dtype=dt, device=dev)
         cand = torch.empty(self.n_rows, dtype=torch.int64, device=dev)
         cand_own = torch.empty(mp, dtype=torch.int64, device=dev)
-        bufs = dict(x=x_cols, c=cand)
+        win_rows = code_rows = None
         if want_codes:
             win_rows = torch.empty(self.n_rows, dtype=dt, device=dev)
             code_rows = torch.empty(self.n_rows, dtype=torch.int64, device=dev)
             code_own = torch.empty(mp, dtype=torch.int64, device=dev)
-            bufs.update(w=win_rows, k=code_rows)
-        views = {k: _view(v) for k, v in bufs.items()}
-        err = C.c_void_p()
-        count = torch.zeros(1, dtype=torch.int64, device=dev)
         hi = window_bound(0.0, delta, dt, dev)
         rounds = windows = window_rounds = 0
-        while True:
-            active = pending & (dist_own < hi)
-            count.copy_(active.sum().view(1))
-            dist.all_reduce(count)
-            if int(count.item()) == 0:   # the window is done: open the next one at the smallest pending distance
-                windows += 1
-                if window_rounds <= 2:
-                    delta = delta * 2.0 if delta < torch.finfo(dt).max / 4 else delta
-                elif window_rounds >= 6 and delta > delta_floor:
-                    delta = delta / 2.0
-                m = torch.where(pending, dist_own, inf).min().view(1)
-                dist.all_reduce(m, op=dist.ReduceOp.MIN)
-                lo = float(m.item())
-                if math.isinf(lo):
-                    break
-                hi = window_bound(lo, delta, dt, dev)
-                window_rounds = 0
-                continue
-            pending &= ~active
-            x = torch.where(active, dist_own, inf)
-            if g.R == 1:
-                x_cols.copy_(x)
-            else:
+        with _views(x_cols, cand, win_rows, code_rows) as (vx, vc, vw, vk):
+            while True:
+                active = pending & (dist_own < hi)
+                if _global_count(active) == 0:   # the window is done: open the next one at the smallest pending distance
+                    windows += 1
+                    if window_rounds <= 2:
+                        delta = delta * 2.0 if delta < torch.finfo(dt).max / 4 else delta
+                    elif window_rounds >= 6 and delta > delta_floor:
+                        delta = delta / 2.0
+                    m = torch.where(pending, dist_own, inf).min().view(1)
+                    dist.all_reduce(m, op=dist.ReduceOp.MIN)
+                    lo = float(m.item())
+                    if math.isinf(lo):
+                        break
+                    hi = window_bound(lo, delta, dt, dev)
+                    window_rounds = 0
+                    continue
+                pending &= ~active
+                x = torch.where(active, dist_own, inf)
                 all_gather_into(x_cols, x, g.col_group)              # partition-major = the block's column order
-            code = L.cugraph_b200_block_sssp_relax(self.handle.ptr, self.block, views["x"].ptr, float(cutoff), mp, g.C, g.c,
-                                                   views["c"].ptr, C.byref(err))
-            capi.check(code, err, "cugraph_b200_block_sssp_relax")
-            if g.C == 1:
-                cand_own.copy_(cand)
-            else:
+                self._call("cugraph_b200_block_sssp_relax", self.block, vx.ptr, float(cutoff), mp, g.C, g.c, vc.ptr)
                 reduce_scatter_into(cand_own, cand, g.row_group, op=dist.ReduceOp.MIN)
-            improved = sssp_owner_step(dist_own, pred_code, pending, cand_own)
-            if want_codes:
-                win = torch.where(improved, dist_own, inf)
-                if g.C == 1:
-                    win_rows.copy_(win)
-                else:
-                    all_gather_into(win_rows, win, g.row_group)
-                code = L.cugraph_b200_block_sssp_pred(self.handle.ptr, self.block, views["x"].ptr, views["w"].ptr, mp, g.C, g.c,
-                                                      views["k"].ptr, C.byref(err))
-                capi.check(code, err, "cugraph_b200_block_sssp_pred")
-                if g.C == 1:
-                    code_own.copy_(code_rows)
-                else:
+                improved = sssp_owner_step(dist_own, pred_code, pending, cand_own)
+                if want_codes:
+                    all_gather_into(win_rows, torch.where(improved, dist_own, inf), g.row_group)
+                    self._call("cugraph_b200_block_sssp_pred", self.block, vx.ptr, vw.ptr, mp, g.C, g.c, vk.ptr)
                     reduce_scatter_into(code_own, code_rows, g.row_group, op=dist.ReduceOp.MIN)
-                pred_code.copy_(torch.where(improved, code_own, pred_code))
-            rounds += 1
-            window_rounds += 1
-        for v in views.values():
-            v.free()
+                    pred_code.copy_(torch.where(improved, code_own, pred_code))
+                rounds += 1
+                window_rounds += 1
         self.last_sssp_stats = dict(rounds=rounds, windows=windows)
         verts = p.vertices
         d_out = dist_own[:p.n_local].clone()
@@ -588,8 +525,7 @@ class MGGraph:
         """Returns (vertices, labels) of the vertices this rank owns: a vertex's label is the external id of one member of
         its component (the same member on every rank), in the vertices' dtype.  The graph must be symmetric: the caller
         passes both directions of every edge (not checked).  Sets last_wcc_stats = dict(rounds)."""
-        assert self.block is not None, "weakly_connected_components needs the unsplit block"
-        p, g, L, capi = self.part, self.part.groups, self.lib, self._capi
+        p, g = self.part, self.part.groups
         dev, mp = self.device, p.maxpart
         label_own = torch.full((mp,), INT64_MAX, dtype=torch.int64, device=dev)
         label_own[:p.n_local] = g.rank * mp + torch.arange(p.n_local, dtype=torch.int64, device=dev)
@@ -598,30 +534,16 @@ class MGGraph:
         label_cols = torch.empty(self.n_cols, dtype=torch.int64, device=dev)
         cand = torch.empty(self.n_rows, dtype=torch.int64, device=dev)
         cand_own = torch.empty(mp, dtype=torch.int64, device=dev)
-        views = {k: _view(v) for k, v in dict(x=label_cols, c=cand).items()}
-        err = C.c_void_p()
-        count = torch.zeros(1, dtype=torch.int64, device=dev)
         rounds = 0
-        while True:
-            x = torch.where(changed, label_own, INT64_MAX)
-            if g.R == 1:
-                label_cols.copy_(x)
-            else:
-                all_gather_into(label_cols, x, g.col_group)           # partition-major = the block's column order
-            code = L.cugraph_b200_block_wcc_min(self.handle.ptr, self.block, views["x"].ptr, views["c"].ptr, C.byref(err))
-            capi.check(code, err, "cugraph_b200_block_wcc_min")
-            if g.C == 1:
-                cand_own.copy_(cand)
-            else:
+        with _views(label_cols, cand) as (vx, vc):
+            while True:
+                all_gather_into(label_cols, torch.where(changed, label_own, INT64_MAX), g.col_group)  # the block's column order
+                self._call("cugraph_b200_block_wcc_min", self.block, vx.ptr, vc.ptr)
                 reduce_scatter_into(cand_own, cand, g.row_group, op=dist.ReduceOp.MIN)
-            changed = wcc_owner_step(label_own, cand_own)
-            rounds += 1
-            count.copy_(changed.sum().view(1))
-            dist.all_reduce(count)
-            if int(count.item()) == 0:
-                break
-        for v in views.values():
-            v.free()
+                changed = wcc_owner_step(label_own, cand_own)
+                rounds += 1
+                if _global_count(changed) == 0:
+                    break
         self.last_wcc_stats = dict(rounds=rounds)
         return p.vertices, self._codes_to_external(label_own[:p.n_local])
 
@@ -636,38 +558,28 @@ class MGGraph:
     # one small all-reduce makes them global, and the one host read per iteration is the convergence test, taken on every
     # rank from the same all-reduced scalars, so that every rank leaves the loop (or raises) in the same iteration.
     # ------------------------------------------------------------------------------------------
-    def _centrality_setup(self, what):
-        assert self.block is not None, f"{what} needs the unsplit block"
-        return self.part, self.part.groups, self.device, self.dtype, self.part.maxpart
-
-    def _sweep(self, vx, vy, alpha, transposed, use_weights):
-        err = C.c_void_p()
-        code = self.lib.cugraph_b200_block_sweep(self.handle.ptr, self.block, 1 if transposed else 0, 1 if use_weights else 0,
-                                                 vx.ptr, vy.ptr, float(alpha), C.byref(err))
-        self._capi.check(code, err, "cugraph_b200_block_sweep")
-
     def _spmv(self, x_own, y_own, bufs, alpha, transposed=False, use_weights=True):
-        """y_own = alpha * (A x) of the owned vertices (transposed: alpha * (A^T x)); bufs = (x_gathered, y_partial, views)"""
-        g, mp = self.part.groups, self.part.maxpart
+        """y_own = alpha * (A x) of the owned vertices (transposed: alpha * (A^T x)); bufs = (x_gathered, y_partial) and
+        their views"""
+        g = self.part.groups
         xg, yp, vx, vy = bufs
-        n_in, in_group, n_in_parts = (self.n_rows, g.row_group, g.C) if transposed else (self.n_cols, g.col_group, g.R)
-        n_out, out_group, n_out_parts = (self.n_cols, g.col_group, g.R) if transposed else (self.n_rows, g.row_group, g.C)
-        if n_in_parts == 1:
-            xg[:mp].copy_(x_own)
-        else:
-            all_gather_into(xg[:n_in], x_own, in_group)
-        self._sweep(vx, vy, alpha, transposed, use_weights)
-        if n_out_parts == 1:
-            y_own.copy_(yp[:mp])
-        else:
-            reduce_scatter_into(y_own, yp[:n_out], out_group)
+        n_in, in_group = (self.n_rows, g.row_group) if transposed else (self.n_cols, g.col_group)
+        n_out, out_group = (self.n_cols, g.col_group) if transposed else (self.n_rows, g.row_group)
+        all_gather_into(xg[:n_in], x_own, in_group)
+        self._call("cugraph_b200_block_sweep", self.block, 1 if transposed else 0, 1 if use_weights else 0, vx.ptr, vy.ptr,
+                   float(alpha))
+        reduce_scatter_into(y_own, yp[:n_out], out_group)
 
-    def _sweep_bufs(self, dt, dev):
-        xg = torch.zeros(self.x_elems, dtype=dt, device=dev)    # zero from the span on, as the block sweep requires
-        yp = torch.zeros(self.span, dtype=dt, device=dev)
-        return xg, yp, _view(xg), _view(yp)
+    @contextlib.contextmanager
+    def _sweep_bufs(self):
+        """_spmv's bufs for one orientation, the views freed on exit"""
+        xg = torch.zeros(self.x_elems, dtype=self.dtype, device=self.device)    # zero from the span on, as the block sweep requires
+        yp = torch.zeros(self.span, dtype=self.dtype, device=self.device)
+        with _views(xg, yp) as (vx, vy):
+            yield xg, yp, vx, vy
 
-    def _owner_call(self, name, *args):
+    def _call(self, name, *args):
+        """self.lib.<name>(handle, *args, &error), looked up at call time, with its error code checked"""
         err = C.c_void_p()
         code = getattr(self.lib, name)(self.handle.ptr, *args, C.byref(err))
         self._capi.check(code, err, name)
@@ -683,7 +595,7 @@ class MGGraph:
         sum |x_new - x| < epsilon (compared in the block's dtype), then x / ||x||_2.  Edge weights are used.
         Returns (vertices, values) of the vertices this rank owns; sets last_katz_stats = dict(iterations)."""
         from cugraph_b200 import _capi as capi
-        p, g, dev, dt, mp = self._centrality_setup("katz_centrality")
+        p, dev, dt, mp = self.part, self.device, self.dtype, self.part.maxpart
         if not 0.0 <= alpha <= 1.0:
             raise capi.CugraphValueError(capi.INVALID_INPUT, "Invalid input argument: alpha should be in [0.0, 1.0].",
                                          "MGGraph.katz_centrality")
@@ -694,14 +606,12 @@ class MGGraph:
         x = torch.zeros(mp, dtype=dt, device=dev)
         y = torch.zeros(mp, dtype=dt, device=dev)
         part = torch.zeros(2, dtype=torch.float64, device=dev)
-        bufs = self._sweep_bufs(dt, dev)
-        vxo, vyo = _view(x), _view(y)
         it = 0
-        try:
+        with self._sweep_bufs() as bufs, _views(x, y) as (vxo, vyo):
             while True:
                 self._spmv(x, y, bufs, alpha)
                 part.zero_()
-                self._owner_call("cugraph_b200_katz_step", vyo.ptr, vxo.ptr, p.n_local, float(beta), C.c_void_p(part.data_ptr()))
+                self._call("cugraph_b200_katz_step", vyo.ptr, vxo.ptr, p.n_local, float(beta), C.c_void_p(part.data_ptr()))
                 dist.all_reduce(part)
                 diff, sumsq = part.tolist()
                 it += 1
@@ -712,10 +622,7 @@ class MGGraph:
             l2 = math.sqrt(sumsq)           # the last step's sum of x_new^2 = ||x||^2
             if not l2 > 0.0:
                 raise self._fail("MGGraph.katz_centrality", "L2 norm of the computed Katz Centrality values should be positive.")
-            self._owner_call("cugraph_b200_vertex_scale", vxo.ptr, p.n_local, 1.0 / l2)
-        finally:
-            for v in (vxo, vyo) + bufs[2:]:
-                v.free()
+            self._call("cugraph_b200_vertex_scale", vxo.ptr, p.n_local, 1.0 / l2)
         self.last_katz_stats = dict(iterations=it)
         return p.vertices, x[:p.n_local].clone()
 
@@ -724,7 +631,7 @@ class MGGraph:
         x = 1 / V until sum |x_new - x| < V * epsilon (V = the global vertex count, compared in the block's dtype).  Edge
         weights are used.  Returns (vertices, values) of the vertices this rank owns; sets last_eigenvector_stats."""
         from cugraph_b200 import _capi as capi
-        p, g, dev, dt, mp = self._centrality_setup("eigenvector_centrality")
+        p, dev, dt, mp = self.part, self.device, self.dtype, self.part.maxpart
         if not epsilon >= 0.0:
             raise capi.CugraphValueError(capi.INVALID_INPUT, "Invalid input argument: epsilon should be non-negative.",
                                          "MGGraph.eigenvector_centrality")
@@ -735,19 +642,17 @@ class MGGraph:
         y = torch.zeros(mp, dtype=dt, device=dev)
         sq = torch.zeros(1, dtype=torch.float64, device=dev)
         part = torch.zeros(1, dtype=torch.float64, device=dev)
-        bufs = self._sweep_bufs(dt, dev)
-        vxo, vyo = _view(x), _view(y)
         tolerance = T(V) * T(epsilon)
         it = 0
-        try:
+        with self._sweep_bufs() as bufs, _views(x, y) as (vxo, vyo):
             while True:
                 self._spmv(x, y, bufs, 1.0)
                 sq.zero_()
-                self._owner_call("cugraph_b200_eigenvector_add_step", vyo.ptr, vxo.ptr, p.n_local, C.c_void_p(sq.data_ptr()))
+                self._call("cugraph_b200_eigenvector_add_step", vyo.ptr, vxo.ptr, p.n_local, C.c_void_p(sq.data_ptr()))
                 dist.all_reduce(sq)
                 part.zero_()
-                self._owner_call("cugraph_b200_eigenvector_scale_step", vyo.ptr, vxo.ptr, p.n_local, C.c_void_p(sq.data_ptr()),
-                                 C.c_void_p(part.data_ptr()))
+                self._call("cugraph_b200_eigenvector_scale_step", vyo.ptr, vxo.ptr, p.n_local, C.c_void_p(sq.data_ptr()),
+                           C.c_void_p(part.data_ptr()))
                 dist.all_reduce(part)
                 diff = float(part.item())
                 it += 1
@@ -755,9 +660,6 @@ class MGGraph:
                     break
                 if it >= max_iterations:
                     raise self._fail("MGGraph.eigenvector_centrality", "Eigenvector Centrality failed to converge.")
-        finally:
-            for v in (vxo, vyo) + bufs[2:]:
-                v.free()
         self.last_eigenvector_stats = dict(iterations=it)
         return p.vertices, x[:p.n_local].clone()
 
@@ -797,7 +699,7 @@ class MGGraph:
         L1-normalised.  Returns (vertices, hubs, authorities) of the vertices this rank owns; sets
         last_hits_stats = dict(iterations, hub_score_differences)."""
         from cugraph_b200 import _capi as capi
-        p, g, dev, dt, mp = self._centrality_setup("hits")
+        p, dev, dt, mp = self.part, self.device, self.dtype, self.part.maxpart
         if not epsilon >= 0.0:
             raise capi.CugraphValueError(capi.INVALID_INPUT, "Invalid input argument: epsilon should be non-negative.",
                                          "MGGraph.hits")
@@ -808,22 +710,20 @@ class MGGraph:
         auth = torch.zeros(mp, dtype=dt, device=dev)
         mx = torch.zeros(2, dtype=torch.float64, device=dev)
         part = torch.zeros(2, dtype=torch.float64, device=dev)
-        pull_bufs, push_bufs = self._sweep_bufs(dt, dev), self._sweep_bufs(dt, dev)
-        vp, vc, va = _view(prev), _view(curr), _view(auth)
         where = "MGGraph.hits"
 
         def l1_normalize(views):
             part.zero_()
             for k, v in enumerate(views):
-                self._owner_call("cugraph_b200_vertex_sum", v.ptr, p.n_local, 0, C.c_void_p(part.data_ptr() + 8 * k))
+                self._call("cugraph_b200_vertex_sum", v.ptr, p.n_local, 0, C.c_void_p(part.data_ptr() + 8 * k))
             dist.all_reduce(part)
             norms = part.tolist()
             for k, v in enumerate(views):
                 if not T(norms[k]) > T(0):
                     raise self._fail(where, "Norm is required to be a positive value.")
-                self._owner_call("cugraph_b200_vertex_scale", v.ptr, p.n_local, 1.0 / norms[k])
+                self._call("cugraph_b200_vertex_scale", v.ptr, p.n_local, 1.0 / norms[k])
 
-        try:
+        with self._sweep_bufs() as pull_bufs, self._sweep_bufs() as push_bufs, _views(prev, curr, auth) as (vp, vc, va):
             has = torch.tensor([0 if initial_hubs_guess is None else 1], dtype=torch.int64, device=dev)
             dist.all_reduce(has, op=dist.ReduceOp.MAX)   # a guess from any rank: every rank takes part in its exchange
             if int(has.item()):
@@ -837,11 +737,11 @@ class MGGraph:
                 self._spmv(prev, auth, pull_bufs, 1.0, use_weights=False)
                 self._spmv(auth, curr, push_bufs, 1.0, transposed=True, use_weights=False)
                 mx.zero_()
-                self._owner_call("cugraph_b200_hits_max_step", vc.ptr, va.ptr, p.n_local, C.c_void_p(mx.data_ptr()))
+                self._call("cugraph_b200_hits_max_step", vc.ptr, va.ptr, p.n_local, C.c_void_p(mx.data_ptr()))
                 dist.all_reduce(mx, op=dist.ReduceOp.MAX)
                 part.zero_()
-                self._owner_call("cugraph_b200_hits_scale_step", vc.ptr, va.ptr, vp.ptr, p.n_local, C.c_void_p(mx.data_ptr()),
-                                 C.c_void_p(part.data_ptr()))
+                self._call("cugraph_b200_hits_scale_step", vc.ptr, va.ptr, vp.ptr, p.n_local, C.c_void_p(mx.data_ptr()),
+                           C.c_void_p(part.data_ptr()))
                 dist.all_reduce(part)
                 d, h_max, a_max = torch.cat([part[:1], mx]).tolist()
                 if not (T(h_max) > T(0) and T(a_max) > T(0)):
@@ -855,9 +755,6 @@ class MGGraph:
                     raise self._fail(where, "HITS failed to converge.")
             if normalize:
                 l1_normalize([vp, va])
-        finally:
-            for v in (vp, vc, va) + pull_bufs[2:] + push_bufs[2:]:
-                v.free()
         self.last_hits_stats = dict(iterations=it, hub_score_differences=diff)
         return p.vertices, prev[:p.n_local].clone(), auth[:p.n_local].clone()
 
@@ -902,63 +799,6 @@ def wcc_owner_step(label_own, cand_own):
     changed = cand_own < label_own
     label_own.copy_(torch.where(changed, cand_own, label_own))
     return changed
-
-
-# EXPERIMENTAL: same iteration, but the block is split by destination partition: sweep j, then an asynchronous
-# reduce of its partial sums to member j of the row group while sweep j+1 runs (the reference's per-block
-# ncclReduce, per_v_transform_reduce_e.cuh:3389-3407).  Only the last reduce and the all-gather stay exposed.
-def _pagerank_split(self, alpha=0.85, epsilon=1e-5, max_iterations=100):
-    p, g, L, capi = self.part, self.part.groups, self.lib, self._capi
-    dev, dt, mp = self.out_w.device, self.dtype, p.maxpart
-    pr = torch.zeros(mp, dtype=dt, device=dev)
-    pr[:p.n_local] = 1.0 / p.n_global
-    x_local = torch.zeros(mp, dtype=dt, device=dev)
-    xg = torch.zeros(self.x_elems, dtype=dt, device=dev)
-    ybufs = [torch.zeros(sp, dtype=dt, device=dev) for sp in self.spans]
-    ymine = ybufs[g.c][:mp]                      # the reduction for this rank's vertices lands here
-    tot = torch.zeros(2, dtype=torch.float64, device=dev)
-    part = torch.zeros(2, dtype=torch.float64, device=dev)
-    views = {k: _view(v) for k, v in dict(pr=pr, x=x_local, xg=xg, yr=ymine, ow=self.out_w).items()}
-    yviews = [_view(y) for y in ybufs]
-    err = C.c_void_p()
-
-    def vertex_step(first):
-        part.zero_()
-        code = L.cugraph_b200_pagerank_vertex_step(self.handle.ptr, views["yr"].ptr, views["pr"].ptr, views["ow"].ptr,
-                                                   views["x"].ptr, p.n_local, float(alpha), float(p.n_global),
-                                                   1 if first else 0, C.c_void_p(tot.data_ptr()),
-                                                   C.c_void_p(part.data_ptr()), C.byref(err))
-        capi.check(code, err, "cugraph_b200_pagerank_vertex_step")
-        dist.all_reduce(part)
-
-    vertex_step(True)
-    tot, part = part, tot
-    iters = 0
-    for _ in range(int(max_iterations)):
-        if g.R == 1:
-            xg[:mp].copy_(x_local)
-        else:
-            all_gather_into(xg[:self.n_cols], x_local, g.col_group)
-        works = []
-        for j in range(g.C):
-            code = L.cugraph_b200_block_pull_sweep(self.handle.ptr, self.blocks[j], views["xg"].ptr, yviews[j].ptr,
-                                                   float(alpha), C.byref(err))
-            capi.check(code, err, "cugraph_b200_block_pull_sweep")
-            works.append(dist.reduce(ybufs[j][:mp], dst=g.r * g.C + j, group=g.row_group, async_op=True))
-        for wk in works:
-            wk.wait()
-        vertex_step(False)
-        tot, part = part, tot
-        iters += 1
-        if epsilon > 0.0 and float(tot[0].item()) < epsilon:
-            break
-    converged = iters < max_iterations
-    for v in list(views.values()) + yviews:
-        v.free()
-    return p.vertices, pr[:p.n_local].clone(), iters, converged
-
-
-MGGraph.pagerank_split = _pagerank_split
 
 
 def bfs(graph: MGGraph, source, depth_limit=-1, compute_predecessors=True):

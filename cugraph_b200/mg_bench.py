@@ -211,7 +211,6 @@ def run_mg_pagerank(args, metric_name, alpha, iters, ClockSampler, peaks):
                           "mg_parity_ok": parity["ok"], "mg_parity_max_rel": parity["max_rel"],
                           "mg_parity_sample": f"RMAT-{parity['scale']} ef-16, {parity['iterations']} iterations, MG on {world} GPUs vs the single-GPU C-ABI on rank 0, {parity['vertices']} vertices",
                           "mg_bfs_parity": parity.get("bfs"), "mg_bfs": mg_bfs,
-                          "mg_split": os.environ.get("CUGRAPH_B200_MG_SPLIT", "0") == "1",
                           "l2": "inputs per sweep exceed the 50 MB L2; no explicit flush"},
                "clocks": clocks, "e2e": e2e, "gpu_launches": launches, "roofline": roofline, "cpu_baseline": None}
         print(json.dumps(out), flush=True)

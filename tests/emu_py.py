@@ -10,6 +10,8 @@ import os
 import sys
 import time
 
+import pytest
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -98,3 +100,16 @@ def emulated_python_surface():
         for obj, name, old in reversed(patched):
             setattr(obj, name, old)
         _capi.LIB_PATH, _capi._lib = saved["lib_path"], saved["lib"]
+
+
+@pytest.fixture(scope="module")
+def surface():
+    """emulated_python_surface() for the tests of one module; skips them when the emulation cannot be built"""
+    pytest.importorskip("torch")
+    try:
+        cm = emulated_python_surface()
+        L = cm.__enter__()
+    except Exception as e:  # no host compiler
+        pytest.skip(f"emulation build unavailable: {e}")
+    yield L
+    cm.__exit__(None, None, None)

@@ -1,133 +1,70 @@
-"""Multi-GPU SSSP with every rank in ONE process: all P = R x C ranks of a 2D edge partition run through the real block entry
-points (cugraph_b200_block_create / _block_sssp_relax / _block_sssp_pred) and the real owner step (mg.sssp_owner_step); the
-all-gathers and MIN reduce-scatters between them are tensor ops on one device.  Torch CPU tensors with the emulated library
-(tests/emu_py.py) or CUDA tensors with the real one.  The partition is built as in tests/test_emu_mg_cpu.py: edge (u -> v)
-lives on rank (r(v), c(u)), row slot c(v) * maxpart + lid(v), column slot r(u) * maxpart + lid(u).
+"""Multi-GPU SSSP with every rank in ONE process (tests/mg_grid.py): the real block entry points (cugraph_b200_block_sssp_relax /
+_block_sssp_pred) and the real owner step (mg.sssp_owner_step) in the rounds and windows of MGGraph.sssp.
 
 Shared by tests/test_mg_sssp_cpu.py and tests/test_mg_sssp_gpu.py, together with the checks below."""
-import ctypes as C
 import math
 
 import numpy as np
 
 import oracle
+from tests.mg_grid import Grid
 
 
 def simulate(s, d, w, V, R, Cc, source, cutoff=math.inf, predecessors=True, delta=None, device="cpu"):
     """Returns (distances [V] in w's dtype, predecessors [V] int64 (-1 = none) or None, stats) indexed by vertex id"""
     import torch
-    from cugraph_b200 import _capi, mg
-    from cugraph_b200.pylibcugraph.resource_handle import ResourceHandle
-    from cugraph_b200.pylibcugraph.utils import View
-    L = _capi.lib()
-    P = R * Cc
-    dt = torch.float32 if w.dtype == np.float32 else torch.float64
-    # vertex -> owner rank, local id inside the owner
-    owner = (np.arange(V, dtype=np.int64) * 2654435761 >> 7) % P
-    order = np.argsort(owner, kind="stable")
-    counts = np.bincount(owner, minlength=P)
-    mp = int(counts.max())
-    lid = np.empty(V, dtype=np.int64)
-    lid[order] = np.arange(V) - np.repeat(np.cumsum(counts) - counts, counts)
-    own = [np.where(owner == p)[0][np.argsort(lid[owner == p])] for p in range(P)]
-    r_of, c_of = owner // Cc, owner % Cc
-    n_rows, n_cols = Cc * mp, R * mp
-    handle = ResourceHandle(stream=torch.cuda.current_stream().cuda_stream)
-    err = C.c_void_p()
-
-    def t(a, dtype=None):
-        return torch.as_tensor(np.ascontiguousarray(a), dtype=dtype).to(device)
-
-    blocks, keep = {}, []
-    for r in range(R):
-        for c in range(Cc):
-            m = (r_of[d] == r) & (c_of[s] == c)
-            rows = t((c_of[d[m]] * mp + lid[d[m]]).astype(np.int32))
-            cols = t((r_of[s[m]] * mp + lid[s[m]]).astype(np.int32))
-            ww = t(w[m])
-            views = [View(rows), View(cols), View(ww)]
-            blk = C.c_void_p()
-            code = L.cugraph_b200_block_create(handle.ptr, n_rows, n_cols, views[0].ptr, views[1].ptr, views[2].ptr,
-                                               C.byref(blk), C.byref(err))
-            _capi.check(code, err, "cugraph_b200_block_create")
-            keep.append((rows, cols, ww, views))
-            blocks[(r, c)] = blk.value
-    if delta is None:
-        delta = 32.0 * float(np.mean(w.astype(np.float64))) / (s.size / V) / 64.0
-    inf = torch.tensor(math.inf, dtype=dt).to(device)
-    big = torch.finfo(dt).max
-    dist_own = [torch.full((mp,), big, dtype=dt).to(device) for _ in range(P)]
-    pred_code = [torch.full((mp,), -1, dtype=torch.int64).to(device) for _ in range(P)]
-    pending = [torch.zeros(mp, dtype=torch.bool).to(device) for _ in range(P)]
-    dist_own[owner[source]][lid[source]] = 0
-    pending[owner[source]][lid[source]] = True
-    want_codes = predecessors and dt == torch.float64
-    hi = mg.window_bound(0.0, delta, dt, device)
-    rounds = windows = 0
-    while True:
-        active = [pending[p] & (dist_own[p] < hi) for p in range(P)]
-        if sum(int(a.sum()) for a in active) == 0:
-            windows += 1
-            lo = min(float(torch.where(pending[p], dist_own[p], inf).min()) for p in range(P))
-            if math.isinf(lo):
-                break
-            hi = mg.window_bound(lo, delta, dt, device)
-            continue
-        x = []
-        for p in range(P):
-            pending[p] &= ~active[p]
-            x.append(torch.where(active[p], dist_own[p], inf))
-        cand = {}
-        x_cols = {}
-        for r in range(R):
-            for c in range(Cc):
-                xc = torch.cat([x[rr * Cc + c] for rr in range(R)])     # all-gather inside the column group
-                out = torch.empty(n_rows, dtype=torch.int64).to(device)
-                vx, vo = View(xc), View(out)
-                code = L.cugraph_b200_block_sssp_relax(handle.ptr, blocks[(r, c)], vx.ptr, float(cutoff), mp, Cc, c, vo.ptr,
-                                                       C.byref(err))
-                _capi.check(code, err, "cugraph_b200_block_sssp_relax")
-                vx.free()
-                vo.free()
-                cand[(r, c)], x_cols[(r, c)] = out, xc
-        improved = [None] * P
-        for r in range(R):                                            # MIN reduce-scatter inside the row group
-            total = torch.stack([cand[(r, c)] for c in range(Cc)]).min(0).values
-            for j in range(Cc):
-                p = r * Cc + j
-                improved[p] = mg.sssp_owner_step(dist_own[p], pred_code[p], pending[p], total[j * mp:(j + 1) * mp].clone())
-        if want_codes:
-            win = [torch.where(improved[p], dist_own[p], inf) for p in range(P)]
-            for r in range(R):
-                codes = []
-                for c in range(Cc):
-                    wr = torch.cat([win[r * Cc + j] for j in range(Cc)])   # all-gather inside the row group
-                    out = torch.empty(n_rows, dtype=torch.int64).to(device)
-                    vx, vw, vo = View(x_cols[(r, c)]), View(wr), View(out)
-                    code = L.cugraph_b200_block_sssp_pred(handle.ptr, blocks[(r, c)], vx.ptr, vw.ptr, mp, Cc, c, vo.ptr,
-                                                          C.byref(err))
-                    _capi.check(code, err, "cugraph_b200_block_sssp_pred")
-                    for v in (vx, vw, vo):
-                        v.free()
-                    codes.append(out)
-                total = torch.stack(codes).min(0).values
-                for j in range(Cc):
-                    p = r * Cc + j
-                    pred_code[p].copy_(torch.where(improved[p], total[j * mp:(j + 1) * mp], pred_code[p]))
-        rounds += 1
-    for blk in blocks.values():
-        L.cugraph_b200_block_free(blk)
-    for *_, views in keep:
-        for v in views:
-            v.free()
-    dist_g = np.empty(V, dtype=w.dtype)
-    pred_g = np.full(V, -1, dtype=np.int64)
-    for p in range(P):
-        dist_g[own[p]] = dist_own[p][:counts[p]].cpu().numpy()
-        codes = pred_code[p][:counts[p]].cpu().numpy()
-        has = codes >= 0
-        pred_g[own[p][has]] = [own[int(k) // mp][int(k) % mp] for k in codes[has]]
-    return dist_g, (pred_g if predecessors else None), dict(rounds=rounds, windows=windows)
+    from cugraph_b200 import mg
+    grid = Grid(s, d, V, R, Cc, w=w, device=device)
+    try:
+        P, mp, dt = grid.P, grid.mp, grid.tt
+        if delta is None:
+            delta = 32.0 * float(np.mean(w.astype(np.float64))) / (w.size / grid.V) / 64.0
+        inf = torch.tensor(math.inf, dtype=dt).to(device)
+        big = torch.finfo(dt).max
+        dist_own = [torch.full((mp,), big, dtype=dt).to(device) for _ in range(P)]
+        pred_code = [torch.full((mp,), -1, dtype=torch.int64).to(device) for _ in range(P)]
+        pending = [torch.zeros(mp, dtype=torch.bool).to(device) for _ in range(P)]
+        dist_own[grid.owner[source]][grid.lid[source]] = 0
+        pending[grid.owner[source]][grid.lid[source]] = True
+        want_codes = predecessors and dt == torch.float64
+        hi = mg.window_bound(0.0, delta, dt, device)
+        rounds = windows = 0
+        while True:
+            active = [pending[p] & (dist_own[p] < hi) for p in range(P)]
+            if sum(int(a.sum()) for a in active) == 0:
+                windows += 1
+                lo = min(float(torch.where(pending[p], dist_own[p], inf).min()) for p in range(P))
+                if math.isinf(lo):
+                    break
+                hi = mg.window_bound(lo, delta, dt, device)
+                continue
+            x = []
+            for p in range(P):
+                pending[p] &= ~active[p]
+                x.append(torch.where(active[p], dist_own[p], inf))
+            cand, x_cols = {}, {}
+            for (r, c), blk in grid.blocks.items():
+                x_cols[(r, c)] = grid.gather(x, r, c)
+                cand[(r, c)] = torch.empty(grid.n_rows, dtype=torch.int64).to(device)
+                grid.call("cugraph_b200_block_sssp_relax", blk, x_cols[(r, c)], float(cutoff), mp, Cc, c, cand[(r, c)])
+            cand_own = grid.reduce_scatter(cand, op="min")
+            improved = [mg.sssp_owner_step(dist_own[p], pred_code[p], pending[p], cand_own[p]) for p in range(P)]
+            if want_codes:
+                win = [torch.where(improved[p], dist_own[p], inf) for p in range(P)]
+                codes = {}
+                for (r, c), blk in grid.blocks.items():
+                    codes[(r, c)] = torch.empty(grid.n_rows, dtype=torch.int64).to(device)
+                    grid.call("cugraph_b200_block_sssp_pred", blk, x_cols[(r, c)], grid.gather(win, r, c, rows=True), mp, Cc, c,
+                              codes[(r, c)])
+                code_own = grid.reduce_scatter(codes, op="min")
+                for p in range(P):
+                    pred_code[p].copy_(torch.where(improved[p], code_own[p], pred_code[p]))
+            rounds += 1
+        dist_g = grid.by_vertex(dist_own, dtype=w.dtype)
+        pred_g = grid.vertex_of(grid.by_vertex(pred_code, dtype=np.int64))
+        return dist_g, (pred_g if predecessors else None), dict(rounds=rounds, windows=windows)
+    finally:
+        grid.free()
 
 
 def single_gpu_sssp(s, d, w, V, source, cutoff=math.inf):

@@ -1,95 +1,43 @@
-"""Multi-GPU weakly connected components with every rank in ONE process: all P = R x C ranks of a 2D edge partition run
-through the real block entry points (cugraph_b200_block_create / _block_wcc_min) and the real owner step
-(mg.wcc_owner_step); the all-gathers and MIN reduce-scatters between them are tensor ops on one device.  Torch CPU tensors
-with the emulated library (tests/emu_py.py) or CUDA tensors with the real one.  The partition is the one of
-tests/mg_sssp_sim.py: edge (u -> v) lives on rank (r(v), c(u)), row slot c(v) * maxpart + lid(v), column slot
-r(u) * maxpart + lid(u); every id 0..V-1 is a vertex.
+"""Multi-GPU weakly connected components with every rank in ONE process (tests/mg_grid.py): the real block entry point
+(cugraph_b200_block_wcc_min) and the real owner step (mg.wcc_owner_step) in the rounds of
+MGGraph.weakly_connected_components.
 
 Shared by tests/test_mg_wcc_cpu.py and tests/test_mg_wcc_gpu.py, together with the graphs and checks below."""
-import ctypes as C
-
 import numpy as np
 
 import oracle
+from tests.mg_grid import Grid
 
 
 def simulate(s, d, V, R, Cc, w=None, device="cpu"):
     """Returns (labels [V] int64: the vertex id each vertex's label code names, stats) indexed by vertex id"""
     import torch
-    from cugraph_b200 import _capi, mg
-    from cugraph_b200.pylibcugraph.resource_handle import ResourceHandle
-    from cugraph_b200.pylibcugraph.utils import View
-    L = _capi.lib()
-    P = R * Cc
-    owner = (np.arange(V, dtype=np.int64) * 2654435761 >> 7) % P
-    order = np.argsort(owner, kind="stable")
-    counts = np.bincount(owner, minlength=P)
-    mp = int(counts.max())
-    lid = np.empty(V, dtype=np.int64)
-    lid[order] = np.arange(V) - np.repeat(np.cumsum(counts) - counts, counts)
-    own = [np.where(owner == p)[0][np.argsort(lid[owner == p])] for p in range(P)]
-    r_of, c_of = owner // Cc, owner % Cc
-    n_rows, n_cols = Cc * mp, R * mp
-    handle = ResourceHandle(stream=torch.cuda.current_stream().cuda_stream)
-    err = C.c_void_p()
-
-    def t(a):
-        return torch.as_tensor(np.ascontiguousarray(a)).to(device)
-
-    blocks, keep, empty_blocks = {}, [], 0
-    for r in range(R):
-        for c in range(Cc):
-            m = (r_of[d] == r) & (c_of[s] == c)
-            empty_blocks += int(not m.any())
-            rows = t((c_of[d[m]] * mp + lid[d[m]]).astype(np.int32))
-            cols = t((r_of[s[m]] * mp + lid[s[m]]).astype(np.int32))
-            ww = t(w[m]) if w is not None else None
-            views = [View(rows), View(cols), View(ww)]
-            blk = C.c_void_p()
-            code = L.cugraph_b200_block_create(handle.ptr, n_rows, n_cols, views[0].ptr, views[1].ptr, views[2].ptr,
-                                               C.byref(blk), C.byref(err))
-            _capi.check(code, err, "cugraph_b200_block_create")
-            keep.append((rows, cols, ww, views))
-            blocks[(r, c)] = blk.value
-    imax = np.iinfo(np.int64).max
-    label_own, changed = [], []
-    for p in range(P):
-        lab = np.full(mp, imax, dtype=np.int64)
-        lab[:counts[p]] = p * mp + np.arange(counts[p])
-        label_own.append(t(lab))
-        changed.append(t(np.arange(mp) < counts[p]))
-    rounds = 0
-    while True:
-        x = [torch.where(changed[p], label_own[p], mg.INT64_MAX) for p in range(P)]
-        cand = {}
-        for r in range(R):
-            for c in range(Cc):
-                xc = torch.cat([x[rr * Cc + c] for rr in range(R)])     # all-gather inside the column group
-                out = torch.empty(n_rows, dtype=torch.int64).to(device)
-                vx, vo = View(xc), View(out)
-                code = L.cugraph_b200_block_wcc_min(handle.ptr, blocks[(r, c)], vx.ptr, vo.ptr, C.byref(err))
-                _capi.check(code, err, "cugraph_b200_block_wcc_min")
-                vx.free()
-                vo.free()
-                cand[(r, c)] = out
-        for r in range(R):                                            # MIN reduce-scatter inside the row group
-            total = torch.stack([cand[(r, c)] for c in range(Cc)]).min(0).values
-            for j in range(Cc):
-                p = r * Cc + j
-                changed[p] = mg.wcc_owner_step(label_own[p], total[j * mp:(j + 1) * mp].clone())
-        rounds += 1
-        if sum(int(ch.sum()) for ch in changed) == 0:
-            break
-    for blk in blocks.values():
-        L.cugraph_b200_block_free(blk)
-    for *_, views in keep:
-        for v in views:
-            v.free()
-    labels = np.empty(V, dtype=np.int64)
-    for p in range(P):
-        codes = label_own[p][:counts[p]].cpu().numpy()
-        labels[own[p]] = [own[int(k) // mp][int(k) % mp] for k in codes]
-    return labels, dict(rounds=rounds, empty_blocks=empty_blocks)
+    from cugraph_b200 import mg
+    grid = Grid(s, d, V, R, Cc, w=w, device=device)
+    try:
+        P, mp = grid.P, grid.mp
+        label_own, changed = [], []
+        for p in range(P):
+            lab = np.full(mp, mg.INT64_MAX, dtype=np.int64)
+            lab[:grid.counts[p]] = p * mp + np.arange(grid.counts[p])
+            label_own.append(grid.t(lab))
+            changed.append(grid.t(np.arange(mp) < grid.counts[p]))
+        rounds = 0
+        while True:
+            x = [torch.where(changed[p], label_own[p], mg.INT64_MAX) for p in range(P)]
+            cand = {}
+            for (r, c), blk in grid.blocks.items():
+                cand[(r, c)] = torch.empty(grid.n_rows, dtype=torch.int64).to(device)
+                grid.call("cugraph_b200_block_wcc_min", blk, grid.gather(x, r, c), cand[(r, c)])
+            cand_own = grid.reduce_scatter(cand, op="min")
+            changed = [mg.wcc_owner_step(label_own[p], cand_own[p]) for p in range(P)]
+            rounds += 1
+            if sum(int(ch.sum()) for ch in changed) == 0:
+                break
+        labels = grid.vertex_of(grid.by_vertex(label_own, dtype=np.int64))
+        return labels, dict(rounds=rounds, empty_blocks=grid.empty_blocks)
+    finally:
+        grid.free()
 
 
 def single_gpu_wcc(s, d, V):

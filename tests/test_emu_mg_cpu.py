@@ -1,142 +1,59 @@
-"""The C side of multi-GPU PageRank (mg.cu: cugraph_b200_block_create / _block_pull_sweep / _pagerank_vertex_step) on the CPU:
-all P = R x C ranks of a 2D edge partition are simulated in ONE process with the emulated library — every rank's rectangular
-block goes through the real block functions (binned rows with row_vertex, the piece layout, the sweep kernels, the fused
-vertex step), the all-gather / reduce-scatter / 2-scalar all-reduce between them are numpy.  Result vs the fp64 oracle.
-(The torch.distributed side — partition_edges, the collectives — is covered by tests/test_mg_partition_cpu.py with gloo.)"""
-import ctypes as C
-
+"""The C side of multi-GPU PageRank (mg.cu: cugraph_b200_block_create / _block_sweep / _pagerank_vertex_step) on the CPU: all
+P = R x C ranks of a 2D edge partition are simulated in ONE process (tests/mg_grid.py) with the emulated library — every
+rank's rectangular block goes through the real block functions (binned rows with row_vertex, the piece layout, the sweep
+kernels, the fused vertex step), the all-gather / reduce-scatter / 2-scalar all-reduce between them are tensor ops.  Result
+vs the fp64 oracle.  (The torch.distributed side — partition_edges, the collectives — is covered by
+tests/test_mg_partition_cpu.py with gloo.)"""
 import numpy as np
 import pytest
 
 import oracle
-from tests.test_emu_staging_cpu import FLOAT32, INT32, emu, make_edges  # noqa: F401
+from tests.emu_py import surface  # noqa: F401
+from tests.mg_grid import Grid
+from tests.test_emu_staging_cpu import make_edges
 
 
-def _api(L):
-    L.cugraph_b200_create_resource_handle_on_stream.restype = C.c_void_p
-    L.cugraph_b200_create_resource_handle_on_stream.argtypes = [C.c_void_p]
-    L.cugraph_b200_padded_elems.restype = C.c_size_t
-    L.cugraph_b200_padded_elems.argtypes = [C.c_size_t, C.c_size_t]
-    L.cugraph_b200_block_span.restype = C.c_size_t
-    L.cugraph_b200_block_span.argtypes = [C.c_void_p]
-    L.cugraph_b200_block_free.argtypes = [C.c_void_p]
-    L.cugraph_b200_block_create.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    L.cugraph_b200_block_pull_sweep.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p]
-    L.cugraph_b200_pagerank_vertex_step.argtypes = [C.c_void_p] * 5 + [C.c_size_t, C.c_double, C.c_double, C.c_int, C.c_void_p,
-                                                                    C.c_void_p, C.c_void_p]
-
-
-def view(L, a):
-    return C.c_void_p(L.cugraph_type_erased_device_array_view_create(a.ctypes.data, a.size, FLOAT32 if a.dtype == np.float32 else INT32))
-
-
-@pytest.mark.parametrize("R,Cc,weighted,min_edges,split", [(1, 2, False, "0", False), (2, 1, False, "0", False), (2, 2, False, "0", False), (2, 4, True, "0", False), (4, 2, True, "0", False),
-                                                            (2, 2, False, "1000000000", False), (2, 4, False, "0", True)])
-def test_2d_partitioned_pagerank_on_one_cpu(emu, monkeypatch, R, Cc, weighted, min_edges, split):  # noqa: F811
-    """split: one block per destination partition of the row group (the structure of mg.py's CUGRAPH_B200_MG_SPLIT path)"""
+@pytest.mark.parametrize("R,Cc,weighted,min_edges", [(1, 2, False, "0"), (2, 1, False, "0"), (2, 2, False, "0"), (2, 4, True, "0"),
+                                                     (4, 2, True, "0"), (2, 2, False, "1000000000")])
+def test_2d_partitioned_pagerank_on_one_cpu(surface, monkeypatch, R, Cc, weighted, min_edges):  # noqa: F811
     monkeypatch.setenv("CUGRAPH_B200_SWEEP_MIN_EDGES", min_edges)
-    L = emu
-    _api(L)
     P = R * Cc
     src, dst, w = make_edges(90_000, 400_000, seed=71 + P, weighted=weighted)
     ids, inv = np.unique(np.concatenate([src, dst]), return_inverse=True)
     s, d = inv[:src.size], inv[src.size:]
     V = ids.size
-    # vertex -> owner rank, local id inside the owner (any balanced assignment will do for this test)
-    owner = (ids.astype(np.int64) * 2654435761 >> 7) % P
-    order = np.argsort(owner, kind="stable")
-    counts = np.bincount(owner, minlength=P)
-    mp = int(counts.max())
-    lid = np.empty(V, dtype=np.int64)
-    lid[order] = np.arange(V) - np.repeat(np.cumsum(counts) - counts, counts)
-    r_of, c_of = owner // Cc, owner % Cc
-    handle = C.c_void_p(L.cugraph_b200_create_resource_handle_on_stream(None))
-    n_rows, n_cols = Cc * mp, R * mp
-    # rank (r, c): edges u -> v with r = r_of[v], c = c_of[u]; row = c_of[v] * mp + lid[v]; column = r_of[u] * mp + lid[u]
-    blocks, spans = {}, {}
-    keep = []
-
-    def make_block(rows, cols, ww, nr):
-        keep.extend([rows, cols, ww])
-        blk, err = C.c_void_p(), C.c_void_p()
-        vr, vc, vw = view(L, rows), view(L, cols), (view(L, ww) if ww is not None else None)
-        code = L.cugraph_b200_block_create(handle, nr, n_cols, vr, vc, vw, C.byref(blk), C.byref(err))
-        assert code == 0, L.cugraph_error_message(err)
-        return blk
-
-    for r in range(R):
-        for c in range(Cc):
-            m = (r_of[d] == r) & (c_of[s] == c)
-            rows = (c_of[d[m]] * mp + lid[d[m]]).astype(np.int32)
-            cols = (r_of[s[m]] * mp + lid[s[m]]).astype(np.int32)
-            ww = w[m].copy() if weighted else None
-            if not split:
-                blocks[(r, c)] = [make_block(rows, cols, ww, n_rows)]
-            else:  # rows of destination partition j only, renumbered from 0
-                part = rows // mp
-                blocks[(r, c)] = [make_block((rows[part == j] - j * mp).astype(np.int32), cols[part == j].copy(),
-                                             None if ww is None else ww[part == j].copy(), mp) for j in range(Cc)]
-            spans[(r, c)] = max(L.cugraph_b200_block_span(b) for b in blocks[(r, c)])
-    span = max(spans.values())
-    x_elems = L.cugraph_b200_padded_elems(span, 4)
-    # out-weight sums of the owned vertices
-    ow_global = np.bincount(s, weights=w.astype(np.float64) if weighted else None, minlength=V)
-    own = [np.where(owner == p)[0][np.argsort(lid[owner == p])] for p in range(P)]     # global ids by local id
-    out_w = [np.zeros(mp, np.float32) for _ in range(P)]
-    pr = [np.zeros(mp, np.float32) for _ in range(P)]
-    x_loc = [np.zeros(mp, np.float32) for _ in range(P)]
-    yred = [np.zeros(mp, np.float32) for _ in range(P)]
-    for p in range(P):
-        out_w[p][:counts[p]] = ow_global[own[p]]
-        pr[p][:counts[p]] = 1.0 / V
-    tot = np.zeros(2)
-    alpha, iters = 0.85, 8
-
-    def vertex_steps(first):
-        nonlocal tot
-        parts = np.zeros(2)
+    grid = Grid(s, d, V, R, Cc, w=w if weighted else None)
+    try:
+        # out-weight sums of the owned vertices
+        ow_global = np.bincount(s, weights=w.astype(np.float64) if weighted else None, minlength=V)
+        out_w, pr, x_loc, yred = [], [], [], [grid.zeros(grid.mp) for _ in range(P)]
         for p in range(P):
-            part = np.zeros(2)
-            err = C.c_void_p()
-            code = L.cugraph_b200_pagerank_vertex_step(handle, view(L, yred[p]), view(L, pr[p]), view(L, out_w[p]), view(L, x_loc[p]),
-                                                       int(counts[p]), alpha, float(V), int(first), tot.ctypes.data,
-                                                       part.ctypes.data, C.byref(err))
-            assert code == 0, L.cugraph_error_message(err)
-            parts += part
-        tot = parts                                                   # the 2-element all-reduce
+            n = grid.counts[p]
+            out_w.append(grid.zeros(grid.mp))
+            out_w[p][:n] = grid.t(ow_global[grid.own[p]].astype(np.float32))
+            pr.append(grid.zeros(grid.mp))
+            pr[p][:n] = 1.0 / V
+            x_loc.append(grid.zeros(grid.mp))
+        tot = grid.scalars(2)
+        alpha, iters = 0.85, 8
 
-    vertex_steps(True)
-    ybufs = {}
-    for _ in range(iters):
-        ypart = {}
-        for r in range(R):
-            for c in range(Cc):
-                xg = np.zeros(x_elems, np.float32)                     # all-gather inside the column group, partition-major
-                for rr in range(R):
-                    xg[rr * mp:(rr + 1) * mp] = x_loc[rr * Cc + c]
-                yp = np.zeros(max(span, n_rows), np.float32)
-                for j, blk in enumerate(blocks[(r, c)]):
-                    yj = ybufs.setdefault((r, c, j), np.zeros(span, np.float32))   # the same array every iteration: from the
-                    # second sweep on the block only rewrites the rows that have edges
-                    err = C.c_void_p()
-                    code = L.cugraph_b200_block_pull_sweep(handle, blk, view(L, xg), view(L, yj), alpha, C.byref(err))
-                    assert code == 0, L.cugraph_error_message(err)
-                    if split:
-                        yp[j * mp:(j + 1) * mp] = yj[:mp]
-                    else:
-                        yp[:span] = yj
-                ypart[(r, c)] = yp
-        for r in range(R):                                              # reduce-scatter inside the row group
-            total = np.sum([ypart[(r, c)][:n_rows].astype(np.float64) for c in range(Cc)], axis=0)
-            for j in range(Cc):
-                yred[r * Cc + j][:] = total[j * mp:(j + 1) * mp].astype(np.float32)
-        vertex_steps(False)
-    got = np.zeros(V)
-    for p in range(P):
-        got[own[p]] = pr[p][:counts[p]]
+        def vertex_steps(first):
+            parts = [grid.scalars(2) for _ in range(P)]
+            for p in range(P):
+                grid.call("cugraph_b200_pagerank_vertex_step", yred[p], pr[p], out_w[p], x_loc[p], int(grid.counts[p]), alpha,
+                          float(V), int(first), tot, parts[p])
+            grid.all_reduce(parts)                                     # the 2-element all-reduce
+            tot.copy_(parts[0])
+
+        vertex_steps(True)
+        for _ in range(iters):
+            # the block's y arrays are the same every iteration: from the second sweep on a block only rewrites the rows
+            # that have edges
+            yred = grid.spmv(x_loc, alpha)
+            vertex_steps(False)
+        got = grid.by_vertex(pr)
+    finally:
+        grid.free()
     ref, _, _ = oracle.pagerank(s.astype(np.int32), d.astype(np.int32), V, None if not weighted else w.astype(np.float64),
                                 alpha=alpha, epsilon=0.0, max_iterations=iters)
     np.testing.assert_allclose(got, ref, rtol=2e-5, atol=0)
-    for bl in blocks.values():
-        for blk in bl:
-            L.cugraph_b200_block_free(blk)

@@ -13,21 +13,9 @@ import pytest
 
 import oracle
 from oracle.rmat import rmat_edgelist as rmat_np
+from tests.emu_py import surface  # noqa: F401
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def surface():
-    torch = pytest.importorskip("torch")  # noqa: F841
-    from tests.emu_py import emulated_python_surface
-    try:
-        cm = emulated_python_surface()
-        L = cm.__enter__()
-    except Exception as e:  # no host compiler
-        pytest.skip(f"emulation build unavailable: {e}")
-    yield L
-    cm.__exit__(None, None, None)
 
 
 def _load(path, name):

@@ -7,11 +7,10 @@
   64-bit-offset blocks; HITS from an initial guess; non-convergence.
 - The owner-step entry points' error paths.
 - World sizes 2, 4 and 8 over gloo running cugraph_b200.mg.MGGraph.katz_centrality / .eigenvector_centrality / .hits (the
-  real orchestration), with an initial guess given by ranks that do not own those vertices, the non-convergence error on
-  every rank and the split-block error."""
+  real orchestration), with an initial guess given by ranks that do not own those vertices and the non-convergence error
+  on every rank."""
 import ctypes as C
 import os
-import socket
 import sys
 
 import numpy as np
@@ -22,25 +21,14 @@ sys.path.insert(0, ROOT)
 
 import oracle  # noqa: E402
 from tests import mg_centrality_sim as sim  # noqa: E402
+from tests import mg_procs  # noqa: E402
+from tests.emu_py import surface  # noqa: E402, F401
 
 GRIDS = [(1, 2), (2, 1), (2, 2), (4, 2)]
 GRID_IDS = ["1x2", "2x1", "2x2", "4x2"]
 KATZ_RTOL = 2e-5
 EIG_TOL = dict(rtol=2e-3, atol=1e-8)
 HITS_TOL = dict(rtol=2e-3, atol=1e-9)
-
-
-@pytest.fixture(scope="module")
-def surface():
-    pytest.importorskip("torch")
-    from tests.emu_py import emulated_python_surface
-    try:
-        cm = emulated_python_surface()
-        L = cm.__enter__()
-    except Exception as e:  # no host compiler
-        pytest.skip(f"emulation build unavailable: {e}")
-    yield L
-    cm.__exit__(None, None, None)
 
 
 def check_all(s, d, V, R, Cc, w=None, dtype=np.float32, device="cpu", single=True):
@@ -179,14 +167,6 @@ def test_owner_step_errors_emulated(surface):
 
 
 # ---------------------------------------------------------------------------------------------------------- gloo runs
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _gloo_graph():
     """the odd graph with scattered 64-bit external ids (isolated ids are not vertices of an MG graph)"""
     s, d, V = sim.odd_graph(seed=11)
@@ -200,81 +180,47 @@ def _guess(ids, s, d):
     return ids[present], vals
 
 
-def _gloo_worker(rank, world, port, out_q):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
+def _gloo_worker(rank, world):
     import torch
-    import torch.distributed as dist
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    from tests.emu_py import emulated_python_surface
-    with emulated_python_surface():
-        from cugraph_b200 import mg
-        ids, s, d, V = _gloo_graph()
-        n = s.size
-        lo, hi = rank * n // world, (rank + 1) * n // world
-        src, dst = torch.from_numpy(ids[s[lo:hi]]), torch.from_numpy(ids[d[lo:hi]])
-        g = mg.MGGraph(src, dst)
-        alpha = sim.katz_alpha(d, V)
-        out = {}
-        v, x = mg.katz_centrality(g, alpha, epsilon=1e-6, max_iterations=200)
-        out["katz"] = (v.numpy(), x.numpy(), g.last_katz_stats)
-        v, x = mg.eigenvector_centrality(g, epsilon=1e-6, max_iterations=500)
-        out["eig"] = (v.numpy(), x.numpy(), g.last_eigenvector_stats)
-        v, hb, au = mg.hits(g, epsilon=1e-6, max_iterations=500)
-        out["hits"] = (v.numpy(), hb.numpy(), au.numpy(), g.last_hits_stats)
-        gv, gx = _guess(ids, s, d)
-        mine = slice(None) if rank == world - 1 else slice(0, 0)     # the whole guess from the last rank only
-        v, hb, au = mg.hits(g, epsilon=1e-6, max_iterations=500,
-                            initial_hubs_guess=(torch.from_numpy(gv[mine]), torch.from_numpy(gx[mine])))
-        out["hits_guess"] = (v.numpy(), hb.numpy(), au.numpy(), g.last_hits_stats)
-        errs = []
-        for call in (lambda: g.katz_centrality(alpha, epsilon=1e-12, max_iterations=2),
-                     lambda: g.eigenvector_centrality(epsilon=1e-12, max_iterations=2),
-                     lambda: g.hits(epsilon=1e-12, max_iterations=2)):
-            try:
-                call()
-                errs.append(None)
-            except RuntimeError as e:
-                errs.append(str(e))
-        out["errors"] = errs
-        bad = torch.from_numpy(gx[:2] - 5.0) if rank == 0 else torch.zeros(0, dtype=torch.float64)
+    from cugraph_b200 import mg
+    ids, s, d, V = _gloo_graph()
+    n = s.size
+    lo, hi = rank * n // world, (rank + 1) * n // world
+    g = mg.MGGraph(torch.from_numpy(ids[s[lo:hi]]), torch.from_numpy(ids[d[lo:hi]]))
+    alpha = sim.katz_alpha(d, V)
+    out = {}
+    v, x = mg.katz_centrality(g, alpha, epsilon=1e-6, max_iterations=200)
+    out["katz"] = (v.numpy(), x.numpy(), g.last_katz_stats)
+    v, x = mg.eigenvector_centrality(g, epsilon=1e-6, max_iterations=500)
+    out["eig"] = (v.numpy(), x.numpy(), g.last_eigenvector_stats)
+    v, hb, au = mg.hits(g, epsilon=1e-6, max_iterations=500)
+    out["hits"] = (v.numpy(), hb.numpy(), au.numpy(), g.last_hits_stats)
+    gv, gx = _guess(ids, s, d)
+    mine = slice(None) if rank == world - 1 else slice(0, 0)     # the whole guess from the last rank only
+    v, hb, au = mg.hits(g, epsilon=1e-6, max_iterations=500,
+                        initial_hubs_guess=(torch.from_numpy(gv[mine]), torch.from_numpy(gx[mine])))
+    out["hits_guess"] = (v.numpy(), hb.numpy(), au.numpy(), g.last_hits_stats)
+    errs = []
+    for call in (lambda: g.katz_centrality(alpha, epsilon=1e-12, max_iterations=2),
+                 lambda: g.eigenvector_centrality(epsilon=1e-12, max_iterations=2),
+                 lambda: g.hits(epsilon=1e-12, max_iterations=2)):
         try:
-            g.hits(initial_hubs_guess=(torch.from_numpy(gv[:bad.numel()]), bad))
-        except ValueError as e:
-            out["negative_guess"] = str(e)
-        del g
-        if mg.grid_shape(world)[1] > 1:
-            os.environ["CUGRAPH_B200_MG_SPLIT"] = "1"
-            gs = mg.MGGraph(src, dst)
-            del os.environ["CUGRAPH_B200_MG_SPLIT"]
-            out["split_errors"] = []
-            for call in (lambda: gs.katz_centrality(alpha), gs.eigenvector_centrality, gs.hits):
-                try:
-                    call()
-                except AssertionError as e:
-                    out["split_errors"].append(str(e))
-            del gs
-        res = [None] * world
-        dist.all_gather_object(res, out)
-        if rank == 0:
-            out_q.put(res)
-        dist.barrier()
-    dist.destroy_process_group()
+            call()
+            errs.append(None)
+        except RuntimeError as e:
+            errs.append(str(e))
+    out["errors"] = errs
+    bad = torch.from_numpy(gx[:2] - 5.0) if rank == 0 else torch.zeros(0, dtype=torch.float64)
+    try:
+        g.hits(initial_hubs_guess=(torch.from_numpy(gv[:bad.numel()]), bad))
+    except ValueError as e:
+        out["negative_guess"] = str(e)
+    return out
 
 
 @pytest.mark.parametrize("world", [2, 4, 8])
 def test_mg_centrality_emulated_gloo(world):
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_gloo_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = q.get(timeout=900)
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    res = mg_procs.run(_gloo_worker, world, emulated=True)
     ids, s, d, V = _gloo_graph()
     present = np.unique(np.concatenate([s, d]))
     k_of = {int(ids[v]): int(v) for v in present}
@@ -315,7 +261,3 @@ def test_mg_centrality_emulated_gloo(world):
         assert "Eigenvector Centrality failed to converge." in r["errors"][1]
         assert "HITS failed to converge." in r["errors"][2]
         assert "initial guess values should be non-negative" in r["negative_guess"]
-    if world >= 4:
-        for r in res:
-            assert r["split_errors"] == ["katz_centrality needs the unsplit block",
-                                         "eigenvector_centrality needs the unsplit block", "hits needs the unsplit block"]

@@ -9,7 +9,6 @@
 - 2 and 4 GPUs over NCCL (skipped when fewer GPUs are visible)."""
 import ctypes as C
 import os
-import socket
 import sys
 
 import numpy as np
@@ -19,6 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import oracle  # noqa: E402
+from tests import mg_procs  # noqa: E402
 from tests import mg_centrality_sim as sim  # noqa: E402
 from tests.test_mg_centrality_cpu import EIG_TOL, HITS_TOL, KATZ_RTOL, check_all  # noqa: E402
 
@@ -76,21 +76,8 @@ def test_mg_centrality_offs64_on_one_gpu(monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------------- NCCL process groups
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _nccl_worker(rank, world, port, q):
+def _nccl_worker(rank, world):
     import torch
-    import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
     from cugraph_b200 import mg
     s, d, V = sim.rmat_graph(14)
     E = s.size
@@ -109,29 +96,11 @@ def _nccl_worker(rank, world, port, q):
     except RuntimeError as e:
         out["error"] = str(e)
     del g
-    res = [None] * world
-    dist.all_gather_object(res, out)
-    if rank == 0:
-        q.put(res)
-    dist.barrier()
-    dist.destroy_process_group()
+    return out
 
 
 def _run_nccl(world):
-    import torch
-    import torch.multiprocessing as mp
-    if torch.cuda.device_count() < world:
-        pytest.skip(f"needs {world} GPUs")
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_nccl_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = q.get(timeout=600)
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    res = mg_procs.run(_nccl_worker, world, backend="nccl", timeout=600)
     s, d, V = sim.rmat_graph(14)
     present = np.unique(np.concatenate([s, d]))
     remap = np.full(V, -1)

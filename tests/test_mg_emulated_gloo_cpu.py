@@ -6,25 +6,16 @@ emulation, torch's CUDA calls given CPU stand-ins).  Results vs the oracle: Page
 distances exact, BFS predecessors by the reference's validity predicate (cpp/tests/traversal/bfs_test.cpp:213-233).
 What this cannot show: NCCL, stream ordering — tests/test_mg_gpu.py does that on 2 / 4 GPUs."""
 import os
-import socket
 import sys
 
 import numpy as np
 import pytest
 import torch
-import torch.distributed as dist
-import torch.multiprocessing as mp
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
+from tests import mg_procs  # noqa: E402
 
 
 def _graph(V, E, seed):
@@ -41,32 +32,15 @@ def _graph(V, E, seed):
     return ids, s_all, d_all
 
 
-def _worker(rank, world, port, V, E, min_edges, offs64_min_edges, out_q):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    os.environ["CUGRAPH_B200_SWEEP_MIN_EDGES"] = min_edges
-    if offs64_min_edges is not None:
-        os.environ["CUGRAPH_B200_OFFS64_MIN_EDGES"] = offs64_min_edges
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    from tests.emu_py import emulated_python_surface
-    with emulated_python_surface():
-        from cugraph_b200 import mg
-        ids, s_all, d_all = _graph(V, E, 99)
-        n = s_all.size
-        lo, hi = rank * n // world, (rank + 1) * n // world
-        src = torch.from_numpy(ids[s_all[lo:hi]])
-        dst = torch.from_numpy(ids[d_all[lo:hi]])
-        g = mg.MGGraph(src, dst)
-        verts, pr, iters, _ = g.pagerank(alpha=0.85, epsilon=0.0, max_iterations=12)
-        source = int(ids[s_all[0]])
-        bv, bd, bp = g.bfs(source)
-        res = [None] * world
-        dist.all_gather_object(res, (verts.numpy(), pr.numpy(), bv.numpy(), bd.numpy(), bp.numpy()))
-        if rank == 0:
-            out_q.put((res, source))
-        dist.barrier()
-        del g
-    dist.destroy_process_group()
+def _worker(rank, world, V, E):
+    from cugraph_b200 import mg
+    ids, s_all, d_all = _graph(V, E, 99)
+    n = s_all.size
+    lo, hi = rank * n // world, (rank + 1) * n // world
+    g = mg.MGGraph(torch.from_numpy(ids[s_all[lo:hi]]), torch.from_numpy(ids[d_all[lo:hi]]))
+    verts, pr, iters, _ = g.pagerank(alpha=0.85, epsilon=0.0, max_iterations=12)
+    bv, bd, bp = g.bfs(int(ids[s_all[0]]))
+    return verts.numpy(), pr.numpy(), bv.numpy(), bd.numpy(), bp.numpy()
 
 
 # grids 2x1, 2x2, 4x2; the last case gives every block 64-bit offsets (the int64_t block sweep and block BFS)
@@ -75,22 +49,17 @@ def _worker(rank, world, port, V, E, min_edges, offs64_min_edges, out_q):
 def test_mg_pagerank_and_bfs_emulated_gloo(world, min_edges, offs64_min_edges):
     import oracle
     V, E = 1500, 12000
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, V, E, min_edges, offs64_min_edges, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res, source = q.get(timeout=600)
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    env = {"CUGRAPH_B200_SWEEP_MIN_EDGES": min_edges}
+    if offs64_min_edges is not None:
+        env["CUGRAPH_B200_OFFS64_MIN_EDGES"] = offs64_min_edges
+    res = mg_procs.run(_worker, world, V, E, emulated=True, env=env, timeout=600)
     ids, s_all, d_all = _graph(V, E, 99)
     present = np.unique(np.concatenate([s_all, d_all]))
     remap = -np.ones(V, dtype=np.int64)
     remap[present] = np.arange(present.size)
     s, d = remap[s_all], remap[d_all]
     ext = ids[present]
+    source = int(ids[s_all[0]])
     # ---- PageRank
     ref, _, _ = oracle.pagerank(s, d, present.size, None, alpha=0.85, epsilon=0.0, max_iterations=12)
     got = {}

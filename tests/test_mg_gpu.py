@@ -1,7 +1,6 @@
 """2- and 4-GPU NCCL run of the multi-GPU PageRank and BFS (skipped when fewer than 2 GPUs are visible): MG result ==
 oracle on the gathered graph, as the reference's mg_pagerank_test.cpp:158-248 compares MG with SG."""
 import os
-import socket
 import sys
 
 import numpy as np
@@ -11,22 +10,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 pytestmark = pytest.mark.gpu
 
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
+from tests import mg_procs  # noqa: E402
 
 
-def _worker(rank, world, port, scale, weighted, q):
+def _worker(rank, world, scale, weighted):
     import torch
-    import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
     from cugraph_b200 import mg
     from oracle.rmat import rmat_edgelist
     s, d = rmat_edgelist(scale, 16 << scale, seed=5)
@@ -36,39 +24,20 @@ def _worker(rank, world, port, scale, weighted, q):
     w = torch.as_tensor(w_all[lo:hi]).cuda() if weighted else None
     G = mg.MGGraph(torch.as_tensor(s[lo:hi]).cuda(), torch.as_tensor(d[lo:hi]).cuda(), w)
     verts, pr, iters, conv = G.pagerank(0.85, 0.0, 40)
-    res = [None] * world
-    dist.all_gather_object(res, (verts.cpu().numpy(), pr.cpu().numpy()))
     # converging run: iteration count must agree on all ranks and with the scalar exchange
     v2, p2, it2, c2 = G.pagerank(0.85, 1e-6, 500)
     bv, bd, bp = G.bfs(int(s[0]))
-    bres = [None] * world
-    dist.all_gather_object(bres, (bv.cpu().numpy(), bd.cpu().numpy(), bp.cpu().numpy()))
-    if rank == 0:
-        q.put((res, it2, c2, bres))
-    dist.barrier()
-    dist.destroy_process_group()
+    return (verts.cpu().numpy(), pr.cpu().numpy()), it2, c2, (bv.cpu().numpy(), bd.cpu().numpy(), bp.cpu().numpy())
 
 
 @pytest.mark.parametrize("world", [2, 4])
 @pytest.mark.parametrize("weighted", [False, True])
 def test_mg_pagerank_multi_gpu(weighted, world):
-    import torch
-    if torch.cuda.device_count() < world:
-        pytest.skip(f"needs {world} GPUs")
-    import torch.multiprocessing as mp
     import oracle
     from oracle.rmat import rmat_edgelist
     scale = 14
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, scale, weighted, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res, it2, c2, bres = q.get(timeout=300)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    out = mg_procs.run(_worker, world, scale, weighted, backend="nccl", timeout=300)
+    res, it2, c2, bres = [o[0] for o in out], out[0][1], out[0][2], [o[3] for o in out]
     s, d = rmat_edgelist(scale, 16 << scale, seed=5)
     w_all = np.random.default_rng(3).random(s.shape[0]).astype(np.float32) + 0.1
     present = np.unique(np.concatenate([s, d]))

@@ -4,37 +4,28 @@ kernels are covered by the -m gpu tests; this file checks that the blocks + coll
 global graph and the oracle's PageRank (the reference's MG tests compare MG vs SG the same way,
 cpp/tests/link_analysis/mg_pagerank_test.cpp:158-248)."""
 import os
-import socket
 import sys
 
 import numpy as np
 import pytest
 import torch
 import torch.distributed as dist
-import torch.multiprocessing as mp
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
+from tests import mg_procs  # noqa: E402
 
 
-def _worker(rank, world, port, V, E, weighted, out_q):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    from cugraph_b200 import mg
+def _graph(V, E):
     rng = np.random.default_rng(1234)
     ids = rng.choice(10**9, size=V, replace=False).astype(np.int64)      # arbitrary external ids
-    s_all = rng.integers(0, V, E)
-    d_all = rng.integers(0, V, E)
-    w_all = rng.random(E) + 0.25
+    return ids, rng.integers(0, V, E), rng.integers(0, V, E), rng.random(E) + 0.25
+
+
+def _worker(rank, world, V, E, weighted):
+    from cugraph_b200 import mg
+    ids, s_all, d_all, w_all = _graph(V, E)
     lo, hi = rank * E // world, (rank + 1) * E // world                  # this rank's share of the edge list
     src = torch.from_numpy(ids[s_all[lo:hi]])
     dst = torch.from_numpy(ids[d_all[lo:hi]])
@@ -52,8 +43,7 @@ def _worker(rank, world, port, V, E, weighted, out_q):
     dst_owner = g.r * g.C + c_v
     dec_src = np.array([verts[o][l] for o, l in zip(src_owner, (part.cols.long() % part.maxpart).numpy())], dtype=np.int64)
     dec_dst = np.array([verts[o][l] for o, l in zip(dst_owner, (part.rows.long() % mp_).numpy())], dtype=np.int64)
-    blocks = [None] * world
-    dist.all_gather_object(blocks, (dec_src, dec_dst, None if w is None else part.weights.numpy()))
+    block = (dec_src, dec_dst, None if w is None else part.weights.numpy())
     # ---- PageRank with the same iteration structure as MGGraph.pagerank, block sweep in torch
     alpha, iters = 0.85, 25
     ones = part.weights.double() if weighted else torch.ones(part.cols.numel(), dtype=torch.float64)
@@ -84,12 +74,7 @@ def _worker(rank, world, port, V, E, weighted, out_q):
         ypart = torch.zeros(g.C * mp_, dtype=torch.float64).index_add_(0, part.rows.long(), alpha * xg[part.cols.long()] * ones)
         mg.reduce_scatter_into(yred, ypart, g.row_group)
         x, dang = step(False, dang)
-    res = [None] * world
-    dist.all_gather_object(res, (part.vertices.numpy(), pr[:part.n_local].numpy()))
-    if rank == 0:
-        out_q.put((blocks, res, ids, s_all, d_all, w_all, part.n_global))
-    dist.barrier()
-    dist.destroy_process_group()
+    return block, part.vertices.numpy(), pr[:part.n_local].numpy(), part.n_global
 
 
 @pytest.mark.parametrize("world", [2, 4])
@@ -97,16 +82,11 @@ def _worker(rank, world, port, V, E, weighted, out_q):
 def test_partition_and_pagerank_gloo(world, weighted):
     import oracle
     V, E = 300, 4000
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, V, E, weighted, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    blocks, res, ids, s_all, d_all, w_all, n_global = q.get(timeout=180)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    out = mg_procs.run(_worker, world, V, E, weighted, timeout=180)
+    blocks = [o[0] for o in out]
+    res = [o[1:3] for o in out]
+    n_global = out[0][3]
+    ids, s_all, d_all, w_all = _graph(V, E)
     # the union of the blocks is exactly the input multigraph
     got = np.concatenate([np.stack([b[0], b[1]], 1) for b in blocks])
     exp = np.stack([ids[s_all], ids[d_all]], 1)

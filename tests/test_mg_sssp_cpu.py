@@ -10,7 +10,6 @@
 import ctypes as C
 import math
 import os
-import socket
 import sys
 
 import numpy as np
@@ -19,22 +18,11 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from tests import mg_procs  # noqa: E402
 from tests import mg_sssp_sim as sim  # noqa: E402
+from tests.emu_py import surface  # noqa: E402, F401
 
 SCALE = 8
-
-
-@pytest.fixture(scope="module")
-def surface():
-    pytest.importorskip("torch")
-    from tests.emu_py import emulated_python_surface
-    try:
-        cm = emulated_python_surface()
-        L = cm.__enter__()
-    except Exception as e:  # no host compiler
-        pytest.skip(f"emulation build unavailable: {e}")
-    yield L
-    cm.__exit__(None, None, None)
 
 
 @pytest.mark.parametrize("wdtype", [np.float32, np.float64], ids=["f32", "f64"])
@@ -149,14 +137,6 @@ def test_block_sssp_entry_errors_emulated(surface):
 
 
 # ---------------------------------------------------------------------------------------------------------- gloo runs
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _gloo_graph(V, E, seed, wdtype):
     """a hubby graph; a chain of weight-1 edges entered from the source only (its distances need many windows); a few
     vertices with out-edges only (present, unreachable)"""
@@ -173,67 +153,45 @@ def _gloo_graph(V, E, seed, wdtype):
     return ids, s_all, d_all, w_all
 
 
-def _gloo_worker(rank, world, port, V, E, delta_scale, out_q):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    os.environ["CUGRAPH_B200_MG_SSSP_DELTA_SCALE"] = delta_scale
+def _gloo_worker(rank, world, V, E):
     import torch
-    import torch.distributed as dist
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    from tests.emu_py import emulated_python_surface
-    with emulated_python_surface():
-        from cugraph_b200 import mg
-        out = {}
-        for wdtype in (np.float32, np.float64):
-            ids, s_all, d_all, w_all = _gloo_graph(V, E, 99, wdtype)
-            n = s_all.size
-            lo, hi = rank * n // world, (rank + 1) * n // world
-            src = torch.from_numpy(ids[s_all[lo:hi]])
-            dst = torch.from_numpy(ids[d_all[lo:hi]])
-            g = mg.MGGraph(src, dst, torch.from_numpy(w_all[lo:hi]))
-            source = int(ids[s_all[0]])
-            runs = [g.sssp(source), g.sssp(source, compute_predecessors=False), g.sssp(source, cutoff=3.0)]
-            stats = g.last_sssp_stats
-            out[np.dtype(wdtype).name] = ([tuple(None if a is None else a.numpy() for a in r) for r in runs], stats)
-            if wdtype == np.float32:
-                errors = []
-                try:
-                    g.sssp(-12345)
-                except ValueError as e:
-                    errors.append(str(e))
-                gu = mg.MGGraph(src, dst)
-                try:
-                    mg.sssp(gu, source)
-                except ValueError as e:
-                    errors.append(str(e))
-                out["errors"] = errors
-                del gu
-            del g
-        res = [None] * world
-        dist.all_gather_object(res, out)
-        if rank == 0:
-            out_q.put(res)
-        dist.barrier()
-    dist.destroy_process_group()
+    from cugraph_b200 import mg
+    out = {}
+    for wdtype in (np.float32, np.float64):
+        ids, s_all, d_all, w_all = _gloo_graph(V, E, 99, wdtype)
+        n = s_all.size
+        lo, hi = rank * n // world, (rank + 1) * n // world
+        src = torch.from_numpy(ids[s_all[lo:hi]])
+        dst = torch.from_numpy(ids[d_all[lo:hi]])
+        g = mg.MGGraph(src, dst, torch.from_numpy(w_all[lo:hi]))
+        source = int(ids[s_all[0]])
+        runs = [g.sssp(source), g.sssp(source, compute_predecessors=False), g.sssp(source, cutoff=3.0)]
+        stats = g.last_sssp_stats
+        out[np.dtype(wdtype).name] = ([tuple(None if a is None else a.numpy() for a in r) for r in runs], stats)
+        if wdtype == np.float32:
+            errors = []
+            try:
+                g.sssp(-12345)
+            except ValueError as e:
+                errors.append(str(e))
+            gu = mg.MGGraph(src, dst)
+            try:
+                mg.sssp(gu, source)
+            except ValueError as e:
+                errors.append(str(e))
+            out["errors"] = errors
+            del gu
+        del g
+    return out
 
 
 @pytest.mark.parametrize("world,delta_scale", [(2, "1"), (4, "1"), (8, "1"), (2, "1e9")],
                          ids=["2", "4", "8", "2-one-window"])
 def test_mg_sssp_emulated_gloo(world, delta_scale):
-    import torch.multiprocessing as mp
     import oracle
     from tests.test_paths_gpu import _assert_predecessor_tree
     V, E = 1500, 12000
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_gloo_worker, args=(r, world, port, V, E, delta_scale, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = q.get(timeout=900)
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    res = mg_procs.run(_gloo_worker, world, V, E, emulated=True, env={"CUGRAPH_B200_MG_SSSP_DELTA_SCALE": delta_scale})
     for errors in (r["errors"] for r in res):
         assert errors == ["sssp source -12345 is not a vertex of the graph", "SSSP requires a weighted graph"]
     for wdtype in (np.float32, np.float64):

@@ -9,7 +9,6 @@
 Distances bit-exact vs the oracle in the same float type and vs single-GPU cugraph_sssp; predecessors by the oracle's
 predicate and by walking every chain back to the source."""
 import os
-import socket
 import sys
 
 import numpy as np
@@ -18,6 +17,7 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from tests import mg_procs  # noqa: E402
 from tests import mg_sssp_sim as sim  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -62,21 +62,8 @@ def test_mg_sssp_zero_weights_on_one_gpu(wdtype):
 
 
 # ------------------------------------------------------------------------------------------------- NCCL process groups
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _nccl_worker(rank, world, port, scale, q):
+def _nccl_worker(rank, world, scale):
     import torch
-    import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
     from cugraph_b200 import mg
     out = {}
     for wdtype in (np.float32, np.float64):
@@ -91,29 +78,11 @@ def _nccl_worker(rank, world, port, scale, q):
             runs.append((src, v.cpu().numpy(), dd.cpu().numpy(), pp.cpu().numpy()))
         out[np.dtype(wdtype).name] = runs
         del g
-    res = [None] * world
-    dist.all_gather_object(res, out)
-    if rank == 0:
-        q.put(res)
-    dist.barrier()
-    dist.destroy_process_group()
+    return out
 
 
 def _run_nccl(world, scale):
-    import torch
-    import torch.multiprocessing as mp
-    if torch.cuda.device_count() < world:
-        pytest.skip(f"needs {world} GPUs")
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_nccl_worker, args=(r, world, port, scale, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = q.get(timeout=600)
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    res = mg_procs.run(_nccl_worker, world, scale, backend="nccl", timeout=600)
     for wdtype in (np.float32, np.float64):
         s, d, w, V = sim.rmat_graph(scale, wdtype)
         present = np.unique(np.concatenate([s, d]))

@@ -6,10 +6,9 @@
   label a vertex of its own component that carries its own label.
 - cugraph_b200_block_wcc_min called directly against a numpy min: every column active, a few, none.
 - World sizes 2, 4 and 8 over gloo running cugraph_b200.mg.MGGraph.weakly_connected_components (the real orchestration).
-- The error paths of the entry point and of a split block."""
+- The error paths of the entry point."""
 import ctypes as C
 import os
-import socket
 import sys
 
 import numpy as np
@@ -18,23 +17,12 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from tests import mg_procs  # noqa: E402
 from tests import mg_wcc_sim as sim  # noqa: E402
+from tests.emu_py import surface  # noqa: E402, F401
 
 GRIDS = [(1, 2), (2, 1), (2, 2), (4, 2)]
 GRID_IDS = ["1x2", "2x1", "2x2", "4x2"]
-
-
-@pytest.fixture(scope="module")
-def surface():
-    pytest.importorskip("torch")
-    from tests.emu_py import emulated_python_surface
-    try:
-        cm = emulated_python_surface()
-        L = cm.__enter__()
-    except Exception as e:  # no host compiler
-        pytest.skip(f"emulation build unavailable: {e}")
-    yield L
-    cm.__exit__(None, None, None)
 
 
 @pytest.mark.parametrize("R,Cc", GRIDS, ids=GRID_IDS)
@@ -177,14 +165,6 @@ def test_block_wcc_entry_errors_emulated(surface):
 
 
 # ---------------------------------------------------------------------------------------------------------- gloo runs
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _gloo_graph():
     """the components graph with scattered 64-bit external ids (isolated ids are not vertices of an MG graph)"""
     s, d, V, path_len = sim.components_graph(seed=9)
@@ -192,54 +172,21 @@ def _gloo_graph():
     return ids, s, d, V, path_len
 
 
-def _gloo_worker(rank, world, port, out_q):
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
+def _gloo_worker(rank, world):
     import torch
-    import torch.distributed as dist
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    from tests.emu_py import emulated_python_surface
-    with emulated_python_surface():
-        from cugraph_b200 import mg
-        ids, s, d, V, _ = _gloo_graph()
-        n = s.size
-        lo, hi = rank * n // world, (rank + 1) * n // world
-        src, dst = torch.from_numpy(ids[s[lo:hi]]), torch.from_numpy(ids[d[lo:hi]])
-        g = mg.MGGraph(src, dst)
-        verts, labels = mg.weakly_connected_components(g)
-        out = dict(verts=verts.numpy(), labels=labels.numpy(), stats=g.last_wcc_stats)
-        del g
-        if mg.grid_shape(world)[1] > 1:                            # a split block has no WCC
-            os.environ["CUGRAPH_B200_MG_SPLIT"] = "1"
-            gs = mg.MGGraph(src, dst)
-            del os.environ["CUGRAPH_B200_MG_SPLIT"]
-            try:
-                gs.weakly_connected_components()
-            except AssertionError as e:
-                out["split_error"] = str(e)
-            del gs
-        res = [None] * world
-        dist.all_gather_object(res, out)
-        if rank == 0:
-            out_q.put(res)
-        dist.barrier()
-    dist.destroy_process_group()
+    from cugraph_b200 import mg
+    ids, s, d, V, _ = _gloo_graph()
+    n = s.size
+    lo, hi = rank * n // world, (rank + 1) * n // world
+    g = mg.MGGraph(torch.from_numpy(ids[s[lo:hi]]), torch.from_numpy(ids[d[lo:hi]]))
+    verts, labels = mg.weakly_connected_components(g)
+    return dict(verts=verts.numpy(), labels=labels.numpy(), stats=g.last_wcc_stats)
 
 
 @pytest.mark.parametrize("world", [2, 4, 8])
 def test_mg_wcc_emulated_gloo(world):
-    import torch.multiprocessing as mp
     import oracle
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_gloo_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = q.get(timeout=900)
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    res = mg_procs.run(_gloo_worker, world, emulated=True)
     ids, s, d, V, path_len = _gloo_graph()
     present = np.unique(np.concatenate([s, d]))
     k_of = {int(ids[v]): int(v) for v in present}
@@ -257,5 +204,3 @@ def test_mg_wcc_emulated_gloo(world):
     stats = [r["stats"] for r in res]
     assert all(st == stats[0] for st in stats)                     # every rank ran the same rounds
     assert stats[0]["rounds"] >= path_len // 2, stats[0]
-    if world >= 4:
-        assert all(r["split_error"] == "weakly_connected_components needs the unsplit block" for r in res)

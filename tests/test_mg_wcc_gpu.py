@@ -9,7 +9,6 @@
 Partition = the oracle's and single-GPU cugraph_weakly_connected_components'; every label a vertex of its own component
 that carries its own label."""
 import os
-import socket
 import sys
 
 import numpy as np
@@ -18,6 +17,7 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from tests import mg_procs  # noqa: E402
 from tests import mg_wcc_sim as sim  # noqa: E402
 
 pytestmark = pytest.mark.gpu
@@ -53,27 +53,14 @@ def test_mg_wcc_weighted_blocks_on_one_gpu(wdtype):
 
 
 # ------------------------------------------------------------------------------------------------- NCCL process groups
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _graphs():
     s, d, V = sim.rmat_graph(14)
     cs, cd, cV, _ = sim.components_graph()
     return [(s, d, V), (cs, cd, cV)]
 
 
-def _nccl_worker(rank, world, port, q):
+def _nccl_worker(rank, world):
     import torch
-    import torch.distributed as dist
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
     from cugraph_b200 import mg
     out = []
     for s, d, V in _graphs():
@@ -83,29 +70,11 @@ def _nccl_worker(rank, world, port, q):
         v, lab = mg.weakly_connected_components(g)
         out.append((v.cpu().numpy(), lab.cpu().numpy(), g.last_wcc_stats))
         del g
-    res = [None] * world
-    dist.all_gather_object(res, out)
-    if rank == 0:
-        q.put(res)
-    dist.barrier()
-    dist.destroy_process_group()
+    return out
 
 
 def _run_nccl(world):
-    import torch
-    import torch.multiprocessing as mp
-    if torch.cuda.device_count() < world:
-        pytest.skip(f"needs {world} GPUs")
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_nccl_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = q.get(timeout=600)
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
+    res = mg_procs.run(_nccl_worker, world, backend="nccl", timeout=600)
     for i, (s, d, V) in enumerate(_graphs()):
         present = np.unique(np.concatenate([s, d]))
         labels = np.arange(V, dtype=np.int64)    # ids that are not vertices of the MG graph: components of their own

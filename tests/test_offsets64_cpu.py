@@ -11,20 +11,8 @@ import numpy as np
 import pytest
 
 from tests import test_paths_gpu as paths
+from tests.emu_py import surface  # noqa: F401
 from tests.test_emu_staging_cpu import create_graph, emu, make_edges, primary  # noqa: F401
-
-
-@pytest.fixture(scope="module")
-def surface():
-    pytest.importorskip("torch")
-    from tests.emu_py import emulated_python_surface
-    try:
-        cm = emulated_python_surface()
-        L = cm.__enter__()
-    except Exception as e:  # no host compiler
-        pytest.skip(f"emulation build unavailable: {e}")
-    yield L
-    cm.__exit__(None, None, None)
 
 
 @pytest.mark.parametrize("weighted", [False, True])

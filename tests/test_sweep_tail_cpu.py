@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 import oracle
+from tests.emu_py import surface  # noqa: F401
 from tests.test_emu_algorithms_cpu import dense_ids, run_pagerank
 from tests.test_emu_algorithms_cpu import test_sweep_against_plain_sweep_emulated as compare_sweeps_case
 from tests.test_emu_mg_cpu import test_2d_partitioned_pagerank_on_one_cpu as mg_case
@@ -125,8 +126,8 @@ def test_hits_with_tail(emu, monkeypatch, transposed, weighted, normalize, guess
     emu.emu_reload_tuning(C.c_void_p(emu.handle))
 
 
-@pytest.mark.parametrize("R,Cc,weighted,split", [(2, 2, False, False), (2, 4, True, True)])
-def test_mg_blocks_with_tail(emu, monkeypatch, R, Cc, weighted, split):  # noqa: F811
+@pytest.mark.parametrize("R,Cc,weighted", [(2, 2, False), (2, 4, True)])
+def test_mg_blocks_with_tail(surface, monkeypatch, R, Cc, weighted):  # noqa: F811
     """covered_rows_only + row_vertex: the block sweep leaves the empty rows of y alone, the tail writes its rows"""
     monkeypatch.setenv("CUGRAPH_B200_SWEEP_TAIL_DEGREE", "4")
-    mg_case(emu, monkeypatch, R, Cc, weighted, "0", split)
+    mg_case(surface, monkeypatch, R, Cc, weighted, "0")

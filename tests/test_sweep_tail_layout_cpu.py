@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 import oracle
+from tests.emu_py import surface  # noqa: F401
 from tests.test_emu_algorithms_cpu import dense_ids, run_pagerank
 from tests.test_emu_mg_cpu import test_2d_partitioned_pagerank_on_one_cpu as mg_case
 from tests.test_emu_staging_cpu import as_np, create_graph, emu, make_edges, primary  # noqa: F401
@@ -95,7 +96,7 @@ def test_pagerank_through_tail_kernel(emu, monkeypatch, bound, weighted):  # noq
     emu.cugraph_graph_free(g)
 
 
-@pytest.mark.parametrize("R,Cc,weighted,split", [(2, 2, True, False), (2, 4, False, True)])
-def test_mg_blocks_with_tail_bound_16(emu, monkeypatch, R, Cc, weighted, split):  # noqa: F811
+@pytest.mark.parametrize("R,Cc,weighted", [(2, 2, True), (2, 4, False)])
+def test_mg_blocks_with_tail_bound_16(surface, monkeypatch, R, Cc, weighted):  # noqa: F811
     monkeypatch.setenv("CUGRAPH_B200_SWEEP_TAIL_DEGREE", "16")
-    mg_case(emu, monkeypatch, R, Cc, weighted, "0", split)
+    mg_case(surface, monkeypatch, R, Cc, weighted, "0")
