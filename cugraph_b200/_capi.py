@@ -141,6 +141,7 @@ def lib():
     _sig(L.cugraph_b200_block_sssp_pred, i32, [vp, vp, vp, vp, sz, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_block_wcc_min, i32, [vp, vp, vp, vp, pvp])
     _sig(L.cugraph_b200_pagerank_vertex_step, i32, [vp, vp, vp, vp, vp, sz, dbl, dbl, i32, vp, vp, pvp])
+    _sig(L.cugraph_b200_pagerank_personalized_vertex_step, i32, [vp, vp, vp, vp, vp, vp, sz, dbl, dbl, i32, vp, vp, pvp])
     _sig(L.cugraph_b200_block_sweep, i32, [vp, vp, i32, i32, vp, vp, dbl, pvp])
     _sig(L.cugraph_b200_katz_step, i32, [vp, vp, vp, sz, dbl, vp, pvp])
     _sig(L.cugraph_b200_eigenvector_add_step, i32, [vp, vp, vp, sz, vp, pvp])

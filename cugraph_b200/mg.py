@@ -273,6 +273,7 @@ class MGGraph:
         self.weighted = p.weights is not None
         self._w_sum_local = float(ones.sum().item()) if self.weighted else 0.0   # SSSP's initial window width
         self._sssp_avg = None                                                       # (average weight, average degree)
+        self._id_order = None                                  # (local ids by external id, sorted external ids)
         self.last_sssp_stats = None
         self.last_wcc_stats = None
         self.last_katz_stats = self.last_eigenvector_stats = self.last_hits_stats = None
@@ -289,11 +290,32 @@ class MGGraph:
             pass
 
     # one PageRank iteration = all-gather(x) -> block sweep -> reduce-scatter(y) -> vertex step -> all-reduce(2 scalars)
-    def pagerank(self, alpha=0.85, epsilon=1e-5, max_iterations=100):
+    def pagerank(self, alpha=0.85, epsilon=1e-5, max_iterations=100, *, personalization=None, initial_guess=None,
+                 precomputed_out_weights=None, fail_on_nonconvergence=False):
+        """PageRank of the vertices this rank owns: returns (vertices, values, iterations, converged).
+
+        personalization, initial_guess and precomputed_out_weights are each a pair (external vertex ids, values), or None.
+        Any rank may pass pairs for any vertices; an argument counts as given when some rank passes it.  As on one GPU:
+        personalization teleports only to its vertices, in proportion to their values (cugraph_personalized_pagerank);
+        initial_guess is the starting vector as given, without normalisation, 0 for vertices it does not name;
+        precomputed_out_weights replace the out-weight sums, 0 (dangling) for vertices it does not name.  Every rank raises
+        the same error for an invalid argument (see _pagerank_inputs).  fail_on_nonconvergence: FailedToConvergeError on
+        every rank when max_iterations pass without convergence."""
         p, g = self.part, self.part.groups
         dev, dt, mp = self.out_w.device, self.dtype, p.maxpart
-        pr = torch.zeros(mp, dtype=dt, device=dev)
-        pr[:p.n_local] = 1.0 / p.n_global
+        given = torch.tensor([a is not None for a in (personalization, initial_guess, precomputed_out_weights)],
+                             dtype=torch.int64, device=dev)
+        dist.all_reduce(given, op=dist.ReduceOp.MAX)   # a pair from any rank: every rank takes part in its exchange
+        pers, pers_sum, guess, out_w = None, 0.0, None, self.out_w
+        flags = given.tolist()
+        if any(flags):
+            pers, pers_sum, guess, ow = self._pagerank_inputs((personalization, initial_guess, precomputed_out_weights), flags)
+            out_w = self.out_w if ow is None else ow
+        if guess is not None:
+            pr = guess
+        else:
+            pr = torch.zeros(mp, dtype=dt, device=dev)
+            pr[:p.n_local] = 1.0 / p.n_global
         x_local = torch.zeros(mp, dtype=dt, device=dev)
         xg = torch.zeros(self.x_elems, dtype=dt, device=dev)
         ypart = torch.zeros(self.span, dtype=dt, device=dev)
@@ -302,15 +324,21 @@ class MGGraph:
         part = torch.zeros(2, dtype=torch.float64, device=dev)
         pending = [None]
 
-        with _views(pr, x_local, xg, ypart, yred, self.out_w) as (vpr, vx, vxg, vyp, vyr, vow):
+        with _views(pr, x_local, xg, ypart, yred, out_w, pers) as (vpr, vx, vxg, vyp, vyr, vow, vpers):
             def vertex_step(first):
                 # the totals of the previous step are needed now: their all-reduce ran under the sweep in between
                 if pending[0] is not None:
                     pending[0].wait()
                     pending[0] = None
                 part.zero_()
-                self._call("cugraph_b200_pagerank_vertex_step", vyr.ptr, vpr.ptr, vow.ptr, vx.ptr, p.n_local, float(alpha),
-                           float(p.n_global), 1 if first else 0, C.c_void_p(tot.data_ptr()), C.c_void_p(part.data_ptr()))
+                if pers is None:
+                    self._call("cugraph_b200_pagerank_vertex_step", vyr.ptr, vpr.ptr, vow.ptr, vx.ptr, p.n_local,
+                               float(alpha), float(p.n_global), 1 if first else 0, C.c_void_p(tot.data_ptr()),
+                               C.c_void_p(part.data_ptr()))
+                else:
+                    self._call("cugraph_b200_pagerank_personalized_vertex_step", vyr.ptr, vpr.ptr, vow.ptr, vx.ptr,
+                               vpers.ptr, p.n_local, float(alpha), pers_sum, 1 if first else 0, C.c_void_p(tot.data_ptr()),
+                               C.c_void_p(part.data_ptr()))
                 pending[0] = dist.all_reduce(part, async_op=True)
 
             vertex_step(True)
@@ -331,7 +359,76 @@ class MGGraph:
                         break
             if pending[0] is not None:
                 pending[0].wait()
-        return p.vertices, pr[:p.n_local].clone(), iters, iters < max_iterations
+        converged = iters < max_iterations
+        if fail_on_nonconvergence and not converged:   # every rank ran the same iterations: every rank raises
+            from cugraph_b200.pylibcugraph.exceptions import FailedToConvergeError
+            raise FailedToConvergeError(f"MGGraph.pagerank: PageRank failed to converge in {iters} iterations.")
+        return p.vertices, pr[:p.n_local].clone(), iters, converged
+
+    def _pagerank_inputs(self, args, given):
+        """MGGraph.pagerank's (personalization, initial guess, precomputed out-weights) pairs -> (pers, pers_sum, guess,
+        out_w) over this rank's owned slice (None where the argument is not given).  `given` says which arguments some rank
+        passed.  Each given argument takes one all-to-all-v to the owners; one all-reduce then gathers every rank's error
+        counts and the personalization sum, and every rank raises the first failing check in this order:
+          personalization: ids and values differ in size on some rank; no pair on any rank; an id that is not a vertex; a
+            negative value; an id given twice; a sum that is not positive  (the single-GPU messages and exception types,
+            the reference's multi-GPU checks of pagerank_impl.cuh for the negative values and duplicates)
+          initial guess, then precomputed out-weights: sizes differ; an id that is not a vertex."""
+        from cugraph_b200 import _capi as capi
+        dev, dt, mp = self.device, self.dtype, self.part.maxpart
+        got, counts = [], []
+        for a, f in zip(args, given):
+            if f:
+                lid, val, cnt = self._pairs_to_owners(a, dt)
+            else:
+                lid, val, cnt = None, None, torch.zeros(5, dtype=torch.float64, device=dev)
+            got.append((lid, val))
+            counts.append(cnt)
+        pers_sum = got[0][1].to(torch.float64).sum().reshape(1) if given[0] else torch.zeros(1, dtype=torch.float64,
+                                                                                               device=dev)
+        tot = torch.cat(counts + [pers_sum])
+        dist.all_reduce(tot)
+        (pm, pn, pneg, pinv, pdup), (gm, _, _, ginv, _), (om, _, _, oinv, _) = [tot[5 * k:5 * k + 5].tolist() for k in range(3)]
+        total_sum = float(tot[15].item())
+        where = "MGGraph.pagerank"
+
+        def fail(cls, code, message):
+            raise cls(code, message, where)
+
+        if given[0]:
+            if pm:
+                fail(capi.CugraphRuntimeError, capi.UNKNOWN_ERROR, "Invalid input argument: if personalization.has_value() is "
+                     "true, the size of vertices and values should match")
+            if pn == 0:
+                fail(capi.CugraphRuntimeError, capi.UNKNOWN_ERROR, "Invalid input argument: if personalizations.has_value() "
+                     "is true, the input personalization vector size should not be 0.")
+            if pinv:
+                fail(capi.CugraphValueError, capi.INVALID_INPUT,
+                     "Invalid input argument: peresonalization vertices have invalid vertex IDs.")
+            if pneg:
+                fail(capi.CugraphValueError, capi.INVALID_INPUT,
+                     "Invalid input argument: peresonalization values should be non-negative.")
+            if pdup:
+                fail(capi.CugraphValueError, capi.INVALID_INPUT,
+                     "Invalid input argument: personalization vertices should not contain duplicate entries.")
+            if not total_sum > 0.0:
+                fail(capi.CugraphRuntimeError, capi.UNKNOWN_ERROR,
+                     "Invalid input argument: sum of personalization valuese should be positive.")
+        for k, name, mism, inv in ((1, "initial_guess", gm, ginv), (2, "precomputed_out_weights", om, oinv)):
+            if given[k] and mism:
+                fail(capi.CugraphValueError, capi.INVALID_INPUT, f"{name}: vertex and value arrays differ in size")
+            if given[k] and inv:
+                fail(capi.CugraphValueError, capi.INVALID_INPUT,
+                     f"{name}: vertex list contains ids that are not vertices of the graph")
+        dense = []
+        for k, (lid, val) in enumerate(got):
+            if not given[k]:
+                dense.append(None)
+                continue
+            out = torch.zeros(mp, dtype=dt, device=dev)
+            out[lid] = val
+            dense.append(out)
+        return dense[0], total_sum, dense[1], dense[2]
 
     # ------------------------------------------------------------------------------------------
     # multi-GPU BFS.  The reference's MG BFS (bfs_impl.cuh:446-869) moves the frontier through the edge partitions with
@@ -663,33 +760,43 @@ class MGGraph:
         self.last_eigenvector_stats = dict(iterations=it)
         return p.vertices, x[:p.n_local].clone()
 
-    def _guess_to_owners(self, guess, out):
-        """(vertex ids, values) given by any rank -> `out` over the local ids of the vertices this rank owns (others 0)"""
-        from cugraph_b200 import _capi as capi
+    def _pairs_to_owners(self, pairs, dtype):
+        """(vertex ids, values) given by this rank (None: nothing) for any vertices -> the pairs of the vertices this rank
+        owns, from every rank, with one all-to-all-v (every rank must call it).  Returns (local ids, values in `dtype`,
+        counts): the received pairs whose id is a vertex of the graph, and this rank's float64 counts [ids and values differ
+        in size (then nothing is sent), pairs sent, negative values sent, ids received that are not vertices, ids received
+        more than once] for the caller's one all-reduce."""
         p, g, dev = self.part, self.part.groups, self.device
-        if guess is None:
-            gv = torch.zeros(0, dtype=torch.int64, device=dev)
-            gx = torch.zeros(0, dtype=out.dtype, device=dev)
-        else:
-            gv = torch.as_tensor(guess[0]).to(dev).to(torch.int64).reshape(-1)
-            gx = torch.as_tensor(guess[1]).to(dev).to(out.dtype).reshape(-1)
-            if gv.numel() != gx.numel():
-                raise capi.CugraphValueError(capi.INVALID_INPUT, "initial hubs guess needs vertices and values of equal size",
-                                             "MGGraph.hits")
-        neg = (gx < 0).any().to(torch.int64).reshape(1)
-        dist.all_reduce(neg, op=dist.ReduceOp.MAX)
-        if int(neg.item()):
-            raise capi.CugraphValueError(capi.INVALID_INPUT,
-                                         "Invalid input argument: initial guess values should be non-negative.", "MGGraph.hits")
+        gv = torch.zeros(0, dtype=torch.int64, device=dev)
+        gx = torch.zeros(0, dtype=dtype, device=dev)
+        mismatch = 0
+        if pairs is not None:
+            v = torch.as_tensor(pairs[0]).to(dev).to(torch.int64).reshape(-1)
+            x = torch.as_tensor(pairs[1]).to(dev).to(dtype).reshape(-1)
+            if v.numel() == x.numel():
+                gv, gx = v, x
+            else:
+                mismatch = 1
         (rv, rx), _, _, _ = exchange([gv, gx], vertex_owner(gv, g.world), g.world)
         n = p.n_local
-        if n == 0 or rv.numel() == 0:
-            return
-        order = torch.argsort(p.vertices.to(torch.int64))
-        sv = p.vertices.to(torch.int64)[order]
-        pos = torch.searchsorted(sv, rv).clamp(max=n - 1)
-        hit = sv[pos] == rv                          # ids that are not vertices of the graph are dropped
-        out[order[pos[hit]]] = rx[hit]
+        if n > 0 and rv.numel() > 0:
+            if self._id_order is None:   # sorted once per graph: a sort of the owned ids costs milliseconds at scale
+                vid = p.vertices.to(torch.int64)
+                order = torch.argsort(vid)
+                self._id_order = (order, vid[order])
+            order, sv = self._id_order
+            pos = torch.searchsorted(sv, rv).clamp(max=n - 1)
+            hit = sv[pos] == rv
+            lid, val = order[pos[hit]], rx[hit]
+        else:
+            hit = torch.zeros(rv.numel(), dtype=torch.bool, device=dev)
+            lid, val = torch.zeros(0, dtype=torch.int64, device=dev), rx[:0]
+        srt = torch.sort(lid).values
+        counts = torch.stack([torch.tensor(mismatch, dtype=torch.float64, device=dev),
+                              torch.tensor(gv.numel(), dtype=torch.float64, device=dev),
+                              (gx < 0).sum().to(torch.float64), (~hit).sum().to(torch.float64),
+                              (srt[1:] == srt[:-1]).sum().to(torch.float64)])
+        return lid, val, counts
 
     def hits(self, epsilon=1e-5, max_iterations=100, initial_hubs_guess=None, normalize=True):
         """HITS (cugraph_hits' semantics): authorities = A^T hubs, hubs = A authorities (the hubs sweep reads the authorities
@@ -727,7 +834,16 @@ class MGGraph:
             has = torch.tensor([0 if initial_hubs_guess is None else 1], dtype=torch.int64, device=dev)
             dist.all_reduce(has, op=dist.ReduceOp.MAX)   # a guess from any rank: every rank takes part in its exchange
             if int(has.item()):
-                self._guess_to_owners(initial_hubs_guess, prev)
+                lid, val, counts = self._pairs_to_owners(initial_hubs_guess, dt)
+                dist.all_reduce(counts)
+                mismatch, _, neg, _, _ = counts.tolist()
+                if mismatch:
+                    raise capi.CugraphValueError(capi.INVALID_INPUT,
+                                                 "initial hubs guess needs vertices and values of equal size", where)
+                if neg:
+                    raise capi.CugraphValueError(capi.INVALID_INPUT,
+                                                 "Invalid input argument: initial guess values should be non-negative.", where)
+                prev[lid] = val                              # ids that are not vertices of the graph are dropped
                 l1_normalize([vp])
             else:
                 prev[:p.n_local] = 1.0 / V
@@ -833,8 +949,22 @@ def hits(graph: MGGraph, epsilon=1e-5, max_iterations=100, initial_hubs_guess=No
     return graph.hits(epsilon, max_iterations, initial_hubs_guess, normalize)
 
 
-def pagerank(graph: MGGraph, alpha=0.85, epsilon=1e-5, max_iterations=100):
+def pagerank(graph: MGGraph, alpha=0.85, epsilon=1e-5, max_iterations=100, *, initial_guess=None,
+             precomputed_out_weights=None, fail_on_nonconvergence=False):
     """Returns (vertices, pageranks, converged) for the vertices owned by this rank
-    (the MG contract of pylibcugraph.pagerank: every rank gets its local part)."""
-    v, p, it, conv = graph.pagerank(alpha, epsilon, max_iterations)
+    (the MG contract of pylibcugraph.pagerank: every rank gets its local part).  The keywords are MGGraph.pagerank's."""
+    v, p, it, conv = graph.pagerank(alpha, epsilon, max_iterations, initial_guess=initial_guess,
+                                    precomputed_out_weights=precomputed_out_weights,
+                                    fail_on_nonconvergence=fail_on_nonconvergence)
+    return v, p, conv
+
+
+def personalized_pagerank(graph: MGGraph, personalization, alpha=0.85, epsilon=1e-5, max_iterations=100, *,
+                          initial_guess=None, precomputed_out_weights=None, fail_on_nonconvergence=False):
+    """Returns (vertices, pageranks, converged) for the vertices owned by this rank (the MG contract of
+    pylibcugraph.personalized_pagerank).  personalization = (external vertex ids, values) from this rank, or None when
+    another rank gives them; the keywords are MGGraph.pagerank's."""
+    v, p, it, conv = graph.pagerank(alpha, epsilon, max_iterations, personalization=personalization,
+                                    initial_guess=initial_guess, precomputed_out_weights=precomputed_out_weights,
+                                    fail_on_nonconvergence=fail_on_nonconvergence)
     return v, p, conv

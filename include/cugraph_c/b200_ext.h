@@ -112,11 +112,28 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_vertex_sum(
 CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_vertex_scale(
   const cugraph_resource_handle_t* handle, cugraph_type_erased_device_array_view_t* v, size_t n_local, double inv,
   cugraph_error_t** error);
+/* Owner step of one multi-GPU PageRank iteration over this rank's first n_local vertices (y: the reduce-scattered sweep
+ * output, alpha applied; pr: the ranks, updated in place; out_w: out-weight sums, 0 = dangling; x: pr / out_w for the next
+ * sweep, pr where out_w is 0).  All arrays share one FLOAT32 / FLOAT64 type and hold at least n_local elements.  With
+ * base = totals_prev[1] * alpha + 1 - alpha (totals_prev: the all-reduced partials of the previous step, read on the device):
+ *   pagerank_vertex_step:              pr = (T)(y + base / n_vertices_global)
+ *   pagerank_personalized_vertex_step: pr = (T)(y + base * ((double)pers / pers_sum)), pers dense over the owned slice
+ *                                      (0 for the vertices not personalized), pers_sum > 0 the global sum of its values —
+ *                                      the single-GPU personalized rule (cugraph_personalized_pagerank), divided in fp64.
+ * first = TRUE keeps pr as it is and reads no totals_prev (the prologue that derives x and the dangling sum of the start
+ * vector).  Both then ADD partial_out[0] += sum |pr_new - pr_old| and partial_out[1] += sum of pr_new over the dangling
+ * vertices, to be all-reduced by the launcher.  n_local = 0 is a no-op.  Asynchronous. */
 CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_pagerank_vertex_step(
   const cugraph_resource_handle_t* handle, const cugraph_type_erased_device_array_view_t* y,
   cugraph_type_erased_device_array_view_t* pr, const cugraph_type_erased_device_array_view_t* out_w,
   cugraph_type_erased_device_array_view_t* x, size_t n_local, double alpha, double n_vertices_global, bool_t first,
   const double* totals_prev_device, double* partial_out_device, cugraph_error_t** error);
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_pagerank_personalized_vertex_step(
+  const cugraph_resource_handle_t* handle, const cugraph_type_erased_device_array_view_t* y,
+  cugraph_type_erased_device_array_view_t* pr, const cugraph_type_erased_device_array_view_t* out_w,
+  cugraph_type_erased_device_array_view_t* x, const cugraph_type_erased_device_array_view_t* pers, size_t n_local,
+  double alpha, double pers_sum, bool_t first, const double* totals_prev_device, double* partial_out_device,
+  cugraph_error_t** error);
 
 /* RMAT edge list written into caller-allocated INT32 arrays (the role of cugraph_generate_rmat_edgelist,
  * cpp/include/cugraph_c/graph_generators.h, without its rng_state / coo objects): the reference's sampling rule, clip-and-flip
