@@ -41,10 +41,6 @@ def lib():
         raise ImportError(
             f"{LIB_PATH} not found: build it with `python -m cugraph_b200.build` "
             "(nvcc, sm_90a). cugraph_b200 has no CPU fallback.")
-    try:
-        import torch  # noqa: F401  (loads libnccl.so.2 / libcudart first so sonames resolve)
-    except Exception:
-        pass
     L = C.CDLL(LIB_PATH, mode=C.RTLD_GLOBAL)
     vp, sz, i32, dbl = C.c_void_p, C.c_size_t, C.c_int, C.c_double
     pvp = C.POINTER(C.c_void_p)

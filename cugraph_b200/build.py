@@ -65,8 +65,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
                 if rc != 0:
                     raise RuntimeError(f"nvcc failed on {src}")
     if jobs or not os.path.exists(LIB) or any(_newer(o, LIB) for o in objs):
-        nccl = _find_nccl()
-        cmd = [NVCC] + ARCH + ["-shared", "-o", LIB] + objs + ["-ccbin", "/usr/bin/g++", "-Xcompiler", "-fPIC"] + nccl
+        cmd = [NVCC] + ARCH + ["-shared", "-o", LIB] + objs + ["-ccbin", "/usr/bin/g++", "-Xcompiler", "-fPIC"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             sys.stderr.write(r.stdout + r.stderr)
@@ -86,22 +85,6 @@ def _build_cbench(force):
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:  # a development tool: report, do not fail the library build
         sys.stderr.write("cbench not built:\n" + r.stdout + r.stderr)
-
-
-def _find_nccl():
-    """Link against libnccl.so.2 by soname; at run time the copy torch already loaded is reused."""
-    cands = ["/usr/lib/x86_64-linux-gnu/libnccl.so.2"]
-    try:
-        import importlib.util
-        spec = importlib.util.find_spec("nvidia.nccl")
-        if spec and spec.submodule_search_locations:
-            cands.insert(0, os.path.join(list(spec.submodule_search_locations)[0], "lib", "libnccl.so.2"))
-    except Exception:
-        pass
-    for c in cands:
-        if os.path.exists(c):
-            return ["-Xlinker", c, "-Xlinker", "-rpath", "-Xlinker", os.path.dirname(c)]
-    return []
 
 
 if __name__ == "__main__":

@@ -12,8 +12,6 @@
 namespace b200 {
 namespace {
 
-constexpr int kBlock       = 256;
-
 // ------------------------------------------------------------------------------------------
 // warp-aggregated append: the active lanes of a diverged warp claim consecutive queue slots
 // ------------------------------------------------------------------------------------------
@@ -185,11 +183,9 @@ void advance(handle_impl const& h, advance_scratch_t& sc, O const* off, int32_t 
     const int n1 = n / 2;
     dbuf d_sum   = make_dbuf<unsigned long long>(1, h.stream);
     CUDA_TRY(cudaMemsetAsync(d_sum.data(), 0, sizeof(unsigned long long), h.stream));
-    B200_LAUNCH(h, (k_queue_degree_sum<O>), std::min((n1 + kBlock - 1) / kBlock, h.sm_count * 8), kBlock, 0, off, queue, ready_deg, n1,
+    B200_LAUNCH(h, (k_queue_degree_sum<O>), grid_for(n1, 1, h.sm_count * 8), kBlock, 0, off, queue, ready_deg, n1,
                 d_sum.as<unsigned long long>());
-    unsigned long long e1 = 0;
-    CUDA_TRY(cudaMemcpyAsync(&e1, d_sum.data(), sizeof(e1), cudaMemcpyDeviceToHost, h.stream));
-    sync(h);
+    const unsigned long long e1 = read_back(h, d_sum.as<unsigned long long>());
     advance<O, Op>(h, sc, off, idx, queue, n1, e1, op, ready_deg);
     advance<O, Op>(h, sc, off, idx, queue + n1, n - n1, total_edges - e1, op, ready_deg ? ready_deg + n1 : nullptr);
     return;

@@ -56,12 +56,12 @@ void expensive_check(handle_impl const& h, graph_impl const& g, bool check_sym, 
   if ((!check_sym && !check_dup) || c.nnz == 0) return;
   dbuf flags = make_dbuf<int>(2, h.stream);
   CUDA_TRY(cudaMemsetAsync(flags.data(), 0, 2 * sizeof(int), h.stream));
-  const int grid = (int)std::min<int64_t>(std::max<int64_t>(((int64_t)c.n_rows * 32 + 255) / 256, 1), (int64_t)h.sm_count * 32);
+  const int grid = grid_for((int64_t)c.n_rows * 32, 1, h.sm_count * 32);
   if (c.offs64)
-    B200_LAUNCH(h, (k_expensive_check<int64_t>), grid, 256, 0, c.offsets.as<int64_t>(), c.indices.as<int32_t>(), c.n_rows,
+    B200_LAUNCH(h, (k_expensive_check<int64_t>), grid, kBlock, 0, c.offsets.as<int64_t>(), c.indices.as<int32_t>(), c.n_rows,
                 check_sym ? 1 : 0, check_dup ? 1 : 0, flags.as<int>());
   else
-    B200_LAUNCH(h, (k_expensive_check<int32_t>), grid, 256, 0, c.offsets.as<int32_t>(), c.indices.as<int32_t>(), c.n_rows,
+    B200_LAUNCH(h, (k_expensive_check<int32_t>), grid, kBlock, 0, c.offsets.as<int32_t>(), c.indices.as<int32_t>(), c.n_rows,
                 check_sym ? 1 : 0, check_dup ? 1 : 0, flags.as<int>());
   int hf[2] = {0, 0};
   CUDA_TRY(cudaMemcpyAsync(hf, flags.data(), sizeof(hf), cudaMemcpyDeviceToHost, h.stream));
@@ -238,9 +238,7 @@ cugraph_error_code_t cugraph_graph_create_sg_from_csr(
 void cugraph_graph_free(cugraph_graph_t* graph)
 {
   if (!graph) return;
-  auto* g = reinterpret_cast<graph_impl*>(graph);
-  if (g->mg) free_mg_graph(g);
-  delete g;
+  delete reinterpret_cast<graph_impl*>(graph);
 }
 
 }  // extern "C"

@@ -12,27 +12,6 @@
 namespace b200 {
 namespace {
 
-template <typename T>
-__global__ void __launch_bounds__(kCBlock) k_fill_vec(T* __restrict__ v, int64_t n, T val)
-{
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) v[i] = val;
-}
-
-template <typename T>
-__global__ void k_count_negative(T const* __restrict__ v, int32_t n, int* __restrict__ out)
-{
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
-    if (v[i] < (T)0) atomicAdd(out, 1);
-}
-
-double read_scalar(handle_impl const& h, double const* d)
-{
-  double v = 0.0;
-  CUDA_TRY(cudaMemcpyAsync(&v, d, sizeof(double), cudaMemcpyDeviceToHost, h.stream));
-  sync(h);
-  return v;
-}
-
 // ------------------------------------------------------------------------------------------
 // Katz: x <- alpha * A^T x + beta until sum |x_new - x_old| < epsilon; then x / ||x||_2 (the C API always normalises,
 // c_api/katz.cpp:116-129, and — faithfully — passes betas = nullptr whatever the caller gave, katz.cpp:151-152)
@@ -52,18 +31,18 @@ void katz_typed(handle_impl const& h, graph_impl& g, double alpha, double beta, 
   while (nv > 0) {
     pull_sweep<T>(h, c, nv, x.as<T>(), y.as<T>(), sc, alpha);
     CUDA_TRY(cudaMemsetAsync(d_diff.data(), 0, sizeof(double), h.stream));
-    B200_LAUNCH(h, (k_abs_diff<T>), cgrid(h, nv), kCBlock, 0, y.as<T>(), x.as<T>(), nv, 1, d_diff.as<double>());
-    const double diff = read_scalar(h, d_diff.as<double>());
+    B200_LAUNCH(h, (k_abs_diff<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, y.as<T>(), x.as<T>(), nv, 1, d_diff.as<double>());
+    const double diff = read_back(h, d_diff.as<double>());
     ++iter;
     if ((T)diff < (T)epsilon) break;
     B200_EXPECTS(iter < max_iterations, CUGRAPH_UNKNOWN_ERROR, "Katz Centrality failed to converge.");
   }
   if (nv > 0) {  // x holds the final values (copied by k_abs_diff)
     CUDA_TRY(cudaMemsetAsync(d_diff.data(), 0, sizeof(double), h.stream));
-    B200_LAUNCH(h, (k_norm<T>), cgrid(h, nv), kCBlock, 0, x.as<T>(), nv, 0, d_diff.as<double>());
-    const double l2 = std::sqrt(read_scalar(h, d_diff.as<double>()));
+    B200_LAUNCH(h, (k_norm<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, x.as<T>(), nv, 0, d_diff.as<double>());
+    const double l2 = std::sqrt(read_back(h, d_diff.as<double>()));
     B200_EXPECTS(l2 > 0.0, CUGRAPH_UNKNOWN_ERROR, "L2 norm of the computed Katz Centrality values should be positive.");
-    B200_LAUNCH(h, (k_scale<T>), cgrid(h, nv), kCBlock, 0, x.as<T>(), nv, 1.0 / l2);
+    B200_LAUNCH(h, (k_scale<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, x.as<T>(), nv, 1.0 / l2);
   }
   res.vertices   = new device_array_impl{reported_vertices(h, g), (size_t)nv, g.vertex_type};
   res.values     = new device_array_impl{to_reported_order(h, g, x.data(), sizeof(T)), (size_t)nv, g.weight_type};
@@ -83,21 +62,21 @@ void eigenvector_typed(handle_impl const& h, graph_impl& g, double epsilon, size
   const int32_t nv = g.n_vertices;
   csx_t const& c   = pull_view(h, g);
   dbuf x = make_sweep_x<T>(h, nv), y = make_dbuf<T>(std::max(nv, 1), h.stream);
-  if (nv > 0) B200_LAUNCH(h, (k_fill_vec<T>), cgrid(h, nv), kCBlock, 0, x.as<T>(), (int64_t)nv, (T)(1.0 / (double)nv));
+  if (nv > 0) B200_LAUNCH(h, (k_fill<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, x.as<T>(), (int64_t)nv, (T)(1.0 / (double)nv));
   sweep_scratch_t sc;
   sc.init(h, c);
   dbuf d2     = make_dbuf<double>(2, h.stream);
   size_t iter = 0;
   while (nv > 0) {
     pull_sweep<T>(h, c, nv, x.as<T>(), y.as<T>(), sc, 1.0);
-    B200_LAUNCH(h, (k_add_vec<T>), cgrid(h, nv), kCBlock, 0, y.as<T>(), x.as<T>(), nv);
+    B200_LAUNCH(h, (k_add_vec<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, y.as<T>(), x.as<T>(), nv);
     CUDA_TRY(cudaMemsetAsync(d2.data(), 0, 2 * sizeof(double), h.stream));
-    B200_LAUNCH(h, (k_norm<T>), cgrid(h, nv), kCBlock, 0, y.as<T>(), nv, 0, d2.as<double>());
-    const double hyp = std::sqrt(read_scalar(h, d2.as<double>()));
-    B200_LAUNCH(h, (k_scale<T>), cgrid(h, nv), kCBlock, 0, y.as<T>(), nv, 1.0 / hyp);
+    B200_LAUNCH(h, (k_norm<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, y.as<T>(), nv, 0, d2.as<double>());
+    const double hyp = std::sqrt(read_back(h, d2.as<double>()));
+    B200_LAUNCH(h, (k_scale<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, y.as<T>(), nv, 1.0 / hyp);
     CUDA_TRY(cudaMemsetAsync(d2.data(), 0, sizeof(double), h.stream));
-    B200_LAUNCH(h, (k_abs_diff<T>), cgrid(h, nv), kCBlock, 0, y.as<T>(), x.as<T>(), nv, 1, d2.as<double>());
-    const double diff = read_scalar(h, d2.as<double>());
+    B200_LAUNCH(h, (k_abs_diff<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, y.as<T>(), x.as<T>(), nv, 1, d2.as<double>());
+    const double diff = read_back(h, d2.as<double>());
     ++iter;
     if ((T)diff < (T)nv * (T)epsilon) break;
     B200_EXPECTS(iter < max_iterations, CUGRAPH_UNKNOWN_ERROR, "Eigenvector Centrality failed to converge.");
@@ -126,10 +105,10 @@ template <typename T>
 void normalize_by(handle_impl const& h, T* v, int32_t nv, int mode, dbuf& d2)
 {
   CUDA_TRY(cudaMemsetAsync(d2.data(), 0, 2 * sizeof(double), h.stream));
-  B200_LAUNCH(h, (k_norm<T>), cgrid(h, nv), kCBlock, 0, v, nv, mode, d2.as<double>());
-  const double norm = read_scalar(h, d2.as<double>() + (mode == 2 ? 1 : 0));
+  B200_LAUNCH(h, (k_norm<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, v, nv, mode, d2.as<double>());
+  const double norm = read_back(h, d2.as<double>() + (mode == 2 ? 1 : 0));
   B200_EXPECTS((T)norm > (T)0, CUGRAPH_UNKNOWN_ERROR, "Norm is required to be a positive value.");
-  B200_LAUNCH(h, (k_scale<T>), cgrid(h, nv), kCBlock, 0, v, nv, 1.0 / norm);
+  B200_LAUNCH(h, (k_scale<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, v, nv, 1.0 / norm);
 }
 
 template <typename T>
@@ -152,15 +131,12 @@ void hits_typed(handle_impl const& h, graph_impl& g, double epsilon, size_t max_
       if (do_expensive_check) {
         dbuf neg = make_dbuf<int>(1, h.stream);
         CUDA_TRY(cudaMemsetAsync(neg.data(), 0, sizeof(int), h.stream));
-        B200_LAUNCH(h, (k_count_negative<T>), cgrid(h, nv), kCBlock, 0, hubs_a.as<T>(), nv, neg.as<int>());
-        int hn = 0;
-        CUDA_TRY(cudaMemcpyAsync(&hn, neg.data(), sizeof(int), cudaMemcpyDeviceToHost, h.stream));
-        sync(h);
-        B200_EXPECTS(hn == 0, CUGRAPH_INVALID_INPUT, "Invalid input argument: initial guess values should be non-negative.");
+        B200_LAUNCH(h, (k_count_negative<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, hubs_a.as<T>(), (int64_t)nv, neg.as<int>());
+        B200_EXPECTS(read_back(h, neg.as<int>()) == 0, CUGRAPH_INVALID_INPUT, "Invalid input argument: initial guess values should be non-negative.");
       }
       normalize_by<T>(h, hubs_a.as<T>(), nv, 1, d2);
     } else {
-      B200_LAUNCH(h, (k_fill_vec<T>), cgrid(h, nv), kCBlock, 0, hubs_a.as<T>(), (int64_t)nv, (T)(1.0 / (double)nv));
+      B200_LAUNCH(h, (k_fill<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, hubs_a.as<T>(), (int64_t)nv, (T)(1.0 / (double)nv));
     }
     sweep_scratch_t sc_in, sc_out;
     sc_in.init(h, c_in);
@@ -174,8 +150,8 @@ void hits_typed(handle_impl const& h, graph_impl& g, double epsilon, size_t max_
       normalize_by<T>(h, curr, nv, 2, d2);
       normalize_by<T>(h, auth.as<T>(), nv, 2, d2);
       CUDA_TRY(cudaMemsetAsync(d2.data(), 0, sizeof(double), h.stream));
-      B200_LAUNCH(h, (k_abs_diff<T>), cgrid(h, nv), kCBlock, 0, curr, prev, nv, 0, d2.as<double>());
-      diff = (double)(T)read_scalar(h, d2.as<double>());
+      B200_LAUNCH(h, (k_abs_diff<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, curr, prev, nv, 0, d2.as<double>());
+      diff = (double)(T)read_back(h, d2.as<double>());
       std::swap(prev, curr);
       ++iter;
       if ((T)diff < tolerance) break;
@@ -217,7 +193,6 @@ cugraph_error_code_t cugraph_katz_centrality(const cugraph_resource_handle_t* ha
     auto* g       = G(graph);
     B200_EXPECTS(result != nullptr, CUGRAPH_INVALID_INPUT, "result out-pointer is NULL");
     *result = nullptr;
-    B200_EXPECTS(g->mg == nullptr, CUGRAPH_NOT_IMPLEMENTED, "multi-GPU Katz centrality is not implemented");
     B200_EXPECTS(alpha >= 0.0 && alpha <= 1.0, CUGRAPH_INVALID_INPUT, "Invalid input argument: alpha should be in [0.0, 1.0].");
     B200_EXPECTS(epsilon >= 0.0, CUGRAPH_INVALID_INPUT, "Invalid input argument: epsilon should be non-negative.");
     auto res = std::make_unique<centrality_result_impl>();
@@ -237,7 +212,6 @@ cugraph_error_code_t cugraph_eigenvector_centrality(const cugraph_resource_handl
     auto* g       = G(graph);
     B200_EXPECTS(result != nullptr, CUGRAPH_INVALID_INPUT, "result out-pointer is NULL");
     *result = nullptr;
-    B200_EXPECTS(g->mg == nullptr, CUGRAPH_NOT_IMPLEMENTED, "multi-GPU eigenvector centrality is not implemented");
     B200_EXPECTS(epsilon >= 0.0, CUGRAPH_INVALID_INPUT, "Invalid input argument: epsilon should be non-negative.");
     auto res = std::make_unique<centrality_result_impl>();
     if (g->weight_type == FLOAT32) eigenvector_typed<float>(h, *g, epsilon, max_iterations, *res);
@@ -256,7 +230,6 @@ cugraph_error_code_t cugraph_hits(const cugraph_resource_handle_t* handle, cugra
     auto* g       = G(graph);
     B200_EXPECTS(result != nullptr, CUGRAPH_INVALID_INPUT, "result out-pointer is NULL");
     *result = nullptr;
-    B200_EXPECTS(g->mg == nullptr, CUGRAPH_NOT_IMPLEMENTED, "multi-GPU HITS is not implemented");
     auto const* gv = V(initial_hubs_guess_vertices);
     auto const* gx = V(initial_hubs_guess_values);
     if (gv) {

@@ -8,23 +8,6 @@
 namespace b200 {
 namespace {
 
-constexpr int kCBlock = 256;
-inline int cgrid(handle_impl const& h, int64_t n) { return (int)std::min<int64_t>(std::max<int64_t>((n + kCBlock - 1) / kCBlock, 1), (int64_t)h.sm_count * 8); }
-
-__device__ __forceinline__ double block_sum(double v, double* smem)
-{
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) smem[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double t = 0.0;
-  if (threadIdx.x < 32) {
-    t = (threadIdx.x < (blockDim.x >> 5)) ? smem[threadIdx.x] : 0.0;
-    t = warp_sum(t);
-  }
-  __syncthreads();
-  return t;
-}
-
 // *out = max(*out, the warp's largest m); m >= 0, so the bits compare like unsigned integers
 __device__ __forceinline__ void warp_max_into(double m, double* out)
 {
@@ -45,9 +28,9 @@ __device__ __forceinline__ T scaled(T v, double inv)
 
 // out[0] += sum |a - b| ; optionally b <- a (the next sweep's input)
 template <typename T>
-__global__ void __launch_bounds__(kCBlock) k_abs_diff(T const* __restrict__ a, T* __restrict__ b, int32_t n, int copy, double* __restrict__ out)
+__global__ void __launch_bounds__(kBlock) k_abs_diff(T const* __restrict__ a, T* __restrict__ b, int32_t n, int copy, double* __restrict__ out)
 {
-  __shared__ double smem[kCBlock / 32];
+  __shared__ double smem[kBlock / 32];
   double d = 0.0;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     d += fabs((double)a[i] - (double)b[i]);
@@ -58,16 +41,16 @@ __global__ void __launch_bounds__(kCBlock) k_abs_diff(T const* __restrict__ a, T
 }
 
 template <typename T>
-__global__ void __launch_bounds__(kCBlock) k_add_vec(T* __restrict__ y, T const* __restrict__ add, int32_t n)
+__global__ void __launch_bounds__(kBlock) k_add_vec(T* __restrict__ y, T const* __restrict__ add, int32_t n)
 {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) y[i] += add[i];
 }
 
 // out[0] += sum v^2 (mode 0) | sum v (mode 1) ; out[1] = max v (mode 2, values are non-negative: integer compare of the bits)
 template <typename T>
-__global__ void __launch_bounds__(kCBlock) k_norm(T const* __restrict__ v, int32_t n, int mode, double* __restrict__ out)
+__global__ void __launch_bounds__(kBlock) k_norm(T const* __restrict__ v, int32_t n, int mode, double* __restrict__ out)
 {
-  __shared__ double smem[kCBlock / 32];
+  __shared__ double smem[kBlock / 32];
   double s = 0.0, m = 0.0;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const double x = (double)v[i];
@@ -83,7 +66,7 @@ __global__ void __launch_bounds__(kCBlock) k_norm(T const* __restrict__ v, int32
 }
 
 template <typename T>
-__global__ void __launch_bounds__(kCBlock) k_scale(T* __restrict__ v, int32_t n, double inv)
+__global__ void __launch_bounds__(kBlock) k_scale(T* __restrict__ v, int32_t n, double inv)
 {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) v[i] = scaled(v[i], inv);
 }

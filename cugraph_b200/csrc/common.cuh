@@ -90,11 +90,6 @@ inline size_t dtype_size(cugraph_data_type_id_t t)
 }
 
 // ---------------------------------------------------------------------------------------------
-// communicator (multi-GPU; defined in comm.cu)
-// ---------------------------------------------------------------------------------------------
-struct comm_impl;
-
-// ---------------------------------------------------------------------------------------------
 // schedule knobs (development / tests): environment variables read ONCE, when a handle is created.  Results never
 // depend on them.
 // ---------------------------------------------------------------------------------------------
@@ -147,14 +142,9 @@ struct handle_impl {
   tuning_t tune{};
   int device{0};
   cudaStream_t stream{nullptr};
-  bool borrowed_stream{false};        // stream belongs to the caller (torch): never destroyed here
-  cudaStream_t aux_stream{nullptr};  // overlap of independent kernels / collectives
-  cudaEvent_t ev_a{nullptr}, ev_b{nullptr};
+  bool borrowed_stream{false};  // stream belongs to the caller (torch): never destroyed here
   int sm_count{132};
   size_t l2_bytes{0};
-  comm_impl* comm{nullptr};  // not owned
-  int rank{0};
-  int size{1};
   mutable size_t launches{0};
   void* pinned{nullptr};  // 4 KiB pinned host scratch for scalar read-backs
 };
@@ -294,7 +284,15 @@ struct paths_result_impl {
 // ---------------------------------------------------------------------------------------------
 // launch helpers
 // ---------------------------------------------------------------------------------------------
-inline int ceil_div(int64_t a, int64_t b) { return static_cast<int>((a + b - 1) / b); }
+constexpr int kBlock = 256;  // threads per CTA of the element-wise kernels
+
+// CTAs of kBlock threads for n elements, per_thread elements each: at least one, never more than 2^20, and at most max_grid
+// (usually a multiple of h.sm_count) for kernels that gain nothing from more.  A kernel launched on such a grid strides over it.
+inline int grid_for(int64_t n, int per_thread = 1, int max_grid = 1 << 20)
+{
+  const int64_t b = (n + (int64_t)kBlock * per_thread - 1) / ((int64_t)kBlock * per_thread);
+  return (int)std::min<int64_t>(std::max<int64_t>(b, 1), std::min(max_grid, 1 << 20));
+}
 
 #ifndef B200_HOST_EMU
 #define B200_LAUNCH(h, kernel, grid, block, smem, ...)                           \
@@ -335,6 +333,57 @@ inline void check_last(const char* what)
 }
 
 inline void sync(handle_impl const& h) { CUDA_TRY(cudaStreamSynchronize(h.stream)); }
+
+// the value at d, once the work enqueued before it on the handle's stream has finished
+template <typename T>
+T read_back(handle_impl const& h, T const* d)
+{
+  T v{};
+  CUDA_TRY(cudaMemcpyAsync(&v, d, sizeof(T), cudaMemcpyDeviceToHost, h.stream));
+  sync(h);
+  return v;
+}
+
+// Element-wise kernels shared by the translation units.  A __global__ template instantiated in several of them is only
+// safe with internal linkage, so every translation unit gets its own copy.
+namespace {
+
+template <typename T>
+__global__ void k_fill(T* __restrict__ a, int64_t n, T v)
+{
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) a[i] = v;
+}
+
+template <typename T>
+__global__ void k_iota(T* __restrict__ a, int64_t n)
+{
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) a[i] = (T)i;
+}
+
+// *out += number of elements below 0
+template <typename T>
+__global__ void k_count_negative(T const* __restrict__ a, int64_t n, int* __restrict__ out)
+{
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    if (a[i] < (T)0) atomicAdd(out, 1);
+}
+
+// the sum of v over the CTA, valid in warp 0; smem holds one double per warp
+__device__ __forceinline__ double block_sum(double v, double* smem)
+{
+  v = warp_sum(v);
+  if ((threadIdx.x & 31) == 0) smem[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double t = 0.0;
+  if (threadIdx.x < 32) {
+    t = (threadIdx.x < (blockDim.x >> 5)) ? smem[threadIdx.x] : 0.0;
+    t = warp_sum(t);
+  }
+  __syncthreads();
+  return t;
+}
+
+}  // namespace
 
 // CUGRAPH_B200_BUILD_TRACE=1: print the time of every staging phase (stream-synchronised) to stderr
 struct phase_trace {

@@ -9,8 +9,6 @@
 namespace b200 {
 namespace {
 
-constexpr int kBlk = 256;
-
 __device__ __forceinline__ int find_root(int32_t* parent, int v)
 {
   int p = ((volatile int32_t*)parent)[v];
@@ -40,7 +38,7 @@ __device__ __forceinline__ void hook(int32_t* parent, int u, int v, int* changed
 
 // rows of degree >= 32 (a prefix of the degree-ordered rows): a warp per row; the others: a thread per row
 template <typename O>
-__global__ void __launch_bounds__(kBlk)
+__global__ void __launch_bounds__(kBlock)
 k_hook_hi(O const* __restrict__ off, int32_t const* __restrict__ idx, int32_t const* __restrict__ row_vertex, int32_t n_hi, int32_t* parent,
           int* changed)
 {
@@ -51,7 +49,7 @@ k_hook_hi(O const* __restrict__ off, int32_t const* __restrict__ idx, int32_t co
   }
 }
 template <typename O>
-__global__ void __launch_bounds__(kBlk)
+__global__ void __launch_bounds__(kBlock)
 k_hook_low(O const* __restrict__ off, int32_t const* __restrict__ idx, int32_t const* __restrict__ row_vertex, int32_t r0, int32_t r1,
            int32_t* parent, int* changed)
 {
@@ -64,10 +62,6 @@ __global__ void k_compress(int32_t* parent, int32_t n)
 {
   for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += gridDim.x * blockDim.x) parent[v] = find_root(parent, v);
 }
-__global__ void k_iota_i32(int32_t* a, int32_t n)
-{
-  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += gridDim.x * blockDim.x) a[v] = v;
-}
 
 template <typename O>
 void wcc_rounds(handle_impl const& h, csx_t const& c, int32_t nv, int32_t* parent)
@@ -75,20 +69,17 @@ void wcc_rounds(handle_impl const& h, csx_t const& c, int32_t nv, int32_t* paren
   dbuf d_changed = make_dbuf<int>(1, h.stream);
   const int32_t n_hi = c.degree_sorted ? c.seg[0] : 0;
   const int32_t n_ne = c.degree_sorted ? c.seg[kNumSeg - 2] : c.n_rows;
-  const int vgrid    = std::min((nv + kBlk - 1) / kBlk, h.sm_count * 8);
+  const int vgrid    = grid_for(nv, 1, h.sm_count * 8);
   while (true) {
     CUDA_TRY(cudaMemsetAsync(d_changed.data(), 0, sizeof(int), h.stream));
     if (n_hi > 0)
-      B200_LAUNCH(h, (k_hook_hi<O>), std::min((n_hi + 7) / 8, h.sm_count * 16), kBlk, 0, c.offsets.as<O>(), c.indices.as<int32_t>(),
+      B200_LAUNCH(h, (k_hook_hi<O>), grid_for((int64_t)n_hi * 32, 1, h.sm_count * 16), kBlock, 0, c.offsets.as<O>(), c.indices.as<int32_t>(),
                   c.row_vertex.as<int32_t>(), n_hi, parent, d_changed.as<int>());
     if (n_ne > n_hi)
-      B200_LAUNCH(h, (k_hook_low<O>), std::min((n_ne - n_hi + kBlk - 1) / kBlk, h.sm_count * 16), kBlk, 0, c.offsets.as<O>(),
+      B200_LAUNCH(h, (k_hook_low<O>), grid_for(n_ne - n_hi, 1, h.sm_count * 16), kBlock, 0, c.offsets.as<O>(),
                   c.indices.as<int32_t>(), c.row_vertex.as<int32_t>(), n_hi, n_ne, parent, d_changed.as<int>());
-    B200_LAUNCH(h, k_compress, vgrid, kBlk, 0, parent, nv);
-    int changed = 0;
-    CUDA_TRY(cudaMemcpyAsync(&changed, d_changed.data(), sizeof(int), cudaMemcpyDeviceToHost, h.stream));
-    sync(h);
-    if (!changed) break;
+    B200_LAUNCH(h, k_compress, vgrid, kBlock, 0, parent, nv);
+    if (!read_back(h, d_changed.as<int>())) break;
   }
 }
 
@@ -114,13 +105,12 @@ cugraph_error_code_t cugraph_weakly_connected_components(const cugraph_resource_
     auto* g       = G(graph);
     B200_EXPECTS(result != nullptr, CUGRAPH_INVALID_INPUT, "result out-pointer is NULL");
     *result = nullptr;
-    B200_EXPECTS(g->mg == nullptr, CUGRAPH_NOT_IMPLEMENTED, "multi-GPU weakly connected components are not implemented");
     B200_EXPECTS(g->is_symmetric, CUGRAPH_UNKNOWN_ERROR,
                  "Invalid input argument: input graph should be symmetric for weakly connected components.");
     const int32_t nv = g->n_vertices;
     dbuf parent      = make_dbuf<int32_t>(std::max(nv, 1), h.stream);
     if (nv > 0) {
-      B200_LAUNCH(h, k_iota_i32, std::min((nv + kBlk - 1) / kBlk, h.sm_count * 8), kBlk, 0, parent.as<int32_t>(), nv);
+      B200_LAUNCH(h, k_iota<int32_t>, grid_for(nv, 1, h.sm_count * 8), kBlock, 0, parent.as<int32_t>(), (int64_t)nv);
       csx_t const& c = *g->primary;  // symmetric: either orientation holds every edge in both directions
       if (c.offs64) wcc_rounds<int64_t>(h, c, nv, parent.as<int32_t>());
       else wcc_rounds<int32_t>(h, c, nv, parent.as<int32_t>());

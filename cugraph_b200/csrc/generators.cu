@@ -100,13 +100,13 @@ extern "C" cugraph_error_code_t cugraph_b200_generate_uniform(const cugraph_reso
                  "generate_uniform writes FLOAT32, FLOAT64 or INT32 arrays");
     B200_EXPECTS(hi > lo, CUGRAPH_INVALID_INPUT, "Invalid input argument: the range [lo, hi) is empty");
     if (ov->size == 0) return;
-    const int grid = (int)std::min<size_t>((ov->size + 255) / 256, (size_t)h.sm_count * 16);
+    const int grid = grid_for((int64_t)ov->size, 1, h.sm_count * 16);
     if (ov->type == FLOAT32)
-      B200_LAUNCH(h, (k_uniform_real<float>), grid, 256, 0, (float*)ov->data, (long long)ov->size, (unsigned long long)seed, lo, hi);
+      B200_LAUNCH(h, (k_uniform_real<float>), grid, kBlock, 0, (float*)ov->data, (long long)ov->size, (unsigned long long)seed, lo, hi);
     else if (ov->type == FLOAT64)
-      B200_LAUNCH(h, (k_uniform_real<double>), grid, 256, 0, (double*)ov->data, (long long)ov->size, (unsigned long long)seed, lo, hi);
+      B200_LAUNCH(h, (k_uniform_real<double>), grid, kBlock, 0, (double*)ov->data, (long long)ov->size, (unsigned long long)seed, lo, hi);
     else
-      B200_LAUNCH(h, k_uniform_int, grid, 256, 0, (int32_t*)ov->data, (long long)ov->size, (unsigned long long)seed, (long long)lo,
+      B200_LAUNCH(h, k_uniform_int, grid, kBlock, 0, (int32_t*)ov->data, (long long)ov->size, (unsigned long long)seed, (long long)lo,
                   (long long)hi);
     check_last("generate_uniform");
   });
@@ -134,8 +134,8 @@ extern "C" cugraph_error_code_t cugraph_b200_generate_rmat_edgelist(const cugrap
     if (num_edges == 0) return;
     const double ab = a + b;
     const float a_norm = (float)(ab > 0.0 ? a / ab : 0.0), c_norm = (float)((1.0 - ab) > 0.0 ? c / (1.0 - ab) : 0.0);
-    const int grid = (int)std::min<size_t>((num_edges + 255) / 256, (size_t)h.sm_count * 16);
-    B200_LAUNCH(h, k_rmat_edges, grid, 256, 0, (int)scale, (long long)num_edges, (unsigned long long)seed, (float)ab, a_norm, c_norm,
+    const int grid = grid_for((int64_t)num_edges, 1, h.sm_count * 16);
+    B200_LAUNCH(h, k_rmat_edges, grid, kBlock, 0, (int)scale, (long long)num_edges, (unsigned long long)seed, (float)ab, a_norm, c_norm,
                 clip_and_flip == TRUE ? 1 : 0, scramble_vertex_ids == TRUE ? 1 : 0, (int32_t*)sv->data, (int32_t*)dv->data);
     check_last("generate_rmat_edgelist");
   });

@@ -80,9 +80,6 @@ struct graph_impl {
   std::unique_ptr<csx_t> pull_alt;   // lazily built CSC with re-sorted rows (PageRank on a CSR graph)
   std::unique_ptr<csx_t> push_alt;   // lazily built CSR in vertex order (BFS/SSSP on a CSC graph)
   std::unique_ptr<csx_t> out_alt;    // lazily built CSR with rows re-sorted by out-degree (HITS' hub sweep on a CSC graph)
-
-  // multi-GPU (mg.cu): this rank's blocks of the 2D partition
-  void* mg{nullptr};
 };
 
 inline graph_impl* G(cugraph_graph_t* g)
@@ -148,15 +145,5 @@ std::unique_ptr<csx_t> build_binned_rows(handle_impl const& h, int32_t const* ma
                                          cugraph_data_type_id_t wtype, int64_t n, int32_t nv);
 // the vertex (row_vertex, or the physical row) of every edge of a csx, in edge order
 dbuf expand_majors(handle_impl const& h, csx_t const& c);
-
-// ---- multi-GPU hooks (mg.cu) ----
-struct mg_pr_args {
-  double alpha;
-  double epsilon;
-  size_t max_iterations;
-};
-void attach_comm(handle_impl* h, void* comm);
-void free_mg_graph(graph_impl* g);
-void mg_pagerank(handle_impl const& h, graph_impl& g, mg_pr_args const& a, centrality_result_impl& res);
 
 }  // namespace b200

@@ -107,23 +107,23 @@ __global__ void k_degree(int32_t const* major, int64_t n, int32_t* deg)
 
 __global__ void k_degree_keys(int32_t const* deg, int32_t nv, uint64_t* keys)
 {
-  for (int32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += gridDim.x * blockDim.x)
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < nv; i += (int64_t)gridDim.x * blockDim.x)
     keys[i] = ((uint64_t)(0x7fffffffu - (uint32_t)deg[i]) << 32) | (uint32_t)i;
 }
 
 __global__ void k_perm_from_keys(uint64_t const* keys, int32_t nv, int32_t* rank_of_int, int32_t* int_of_rank)
 {
-  for (int32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += gridDim.x * blockDim.x) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < nv; i += (int64_t)gridDim.x * blockDim.x) {
     int32_t r      = (int32_t)(keys[i] & 0xffffffffu);
     rank_of_int[i] = r;
-    int_of_rank[r] = i;
+    int_of_rank[r] = (int32_t)i;
   }
 }
 
 template <typename T>
 __global__ void k_gather_ext(T const* sorted_ext, int32_t const* rank_of_int, int32_t nv, T* ext_of_int)
 {
-  for (int32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += gridDim.x * blockDim.x)
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < nv; i += (int64_t)gridDim.x * blockDim.x)
     ext_of_int[i] = sorted_ext ? sorted_ext[rank_of_int[i]] : (T)rank_of_int[i];
 }
 
@@ -211,7 +211,7 @@ __global__ void k_segments(O const* offsets, int32_t n_rows, int32_t* seg /* kNu
 template <typename O>
 __global__ void k_check_sorted_degree(O const* offsets, int32_t n_rows, int* bad)
 {
-  for (int32_t r = blockIdx.x * blockDim.x + threadIdx.x; r + 1 < n_rows; r += gridDim.x * blockDim.x) {
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r + 1 < n_rows; r += (int64_t)gridDim.x * blockDim.x) {
     long long d0 = (long long)(offsets[r + 1] - offsets[r]);
     long long d1 = (long long)(offsets[r + 2] - offsets[r + 1]);
     if (d1 > d0) *bad = 1;
@@ -271,12 +271,6 @@ __global__ void k_expand_rows(O const* offsets, int32_t n_rows, int32_t const* r
 }
 
 template <typename T>
-__global__ void k_iota_t(int32_t n, T* out)
-{
-  for (int32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = (T)i;
-}
-
-template <typename T>
 __global__ void k_int_to_ext(int32_t const* in, int64_t n, T const* ext_of_int, T* out)
 {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -288,13 +282,7 @@ __global__ void k_int_to_ext(int32_t const* in, int64_t n, T const* ext_of_int, 
 template <typename T>
 __global__ void k_permute(T const* in, int32_t const* perm, int32_t n, T* out)
 {
-  for (int32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) out[i] = in[perm[i]];
-}
-
-template <typename T>
-__global__ void k_fill(T* a, int64_t n, T v)
-{
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) a[i] = v;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = in[perm[i]];
 }
 
 template <typename T>
@@ -342,10 +330,7 @@ int64_t unique_sorted(handle_impl const& h, T const* in, T* out, int64_t n)
   dbuf tmp(bytes, h.stream);
   CUDA_TRY(cub::DeviceSelect::Unique(tmp.data(), bytes, in, out, d_count.as<int64_t>(), n, h.stream));
   h.launches += 2;
-  int64_t cnt = 0;
-  CUDA_TRY(cudaMemcpyAsync(&cnt, d_count.data(), sizeof(int64_t), cudaMemcpyDeviceToHost, h.stream));
-  sync(h);
-  return cnt;
+  return read_back(h, d_count.as<int64_t>());
 }
 
 // ---------------------------------------------------------------- compressed-row construction
@@ -369,7 +354,7 @@ void build_csx_typed(handle_impl const& h, csx_t& out, int32_t const* major, int
     dbuf perm  = make_dbuf<uint32_t>(n, h.stream);
     dbuf perm2 = make_dbuf<uint32_t>(n, h.stream);
     B200_EXPECTS(n < (1ll << 32), CUGRAPH_INVALID_INPUT, "weighted graphs are limited to 2^32 edges per GPU");
-    B200_LAUNCH(h, k_iota64, grid_for(n, 4), kBlock, 0, n, perm.as<uint32_t>());
+    B200_LAUNCH(h, k_iota<uint32_t>, grid_for(n, 4), kBlock, 0, perm.as<uint32_t>(), n);
     if (dedupe && keep_min_weight) {
       // stable two-pass: order by weight first so that the run head after the key sort is the minimum
       using U = typename std::conditional<sizeof(W) == 4, uint32_t, uint64_t>::type;
@@ -456,12 +441,7 @@ void finish_binning_typed(handle_impl const& h, csx_t& c)
   for (int k = 0; k < kNumSeg; ++k) c.seg[k] = hseg[k];
   c.seg[kNumSeg] = c.n_rows;
   c.degree_sorted = true;
-  O nnz_hi = 0;
-  if (c.seg[0] > 0) {
-    CUDA_TRY(cudaMemcpyAsync(&nnz_hi, off + c.seg[0], sizeof(O), cudaMemcpyDeviceToHost, h.stream));
-    sync(h);
-  }
-  c.nnz_hi   = (int64_t)nnz_hi;
+  c.nnz_hi   = c.seg[0] > 0 ? (int64_t)read_back(h, off + c.seg[0]) : 0;
   c.n_chunks = (int32_t)((c.nnz_hi + kWarpChunk - 1) / kWarpChunk);
   c.chunk_first_row = make_dbuf<int32_t>((size_t)c.n_chunks + 1, h.stream);
   dbuf straddle     = make_dbuf<int32_t>((size_t)c.n_chunks + 1, h.stream);
@@ -472,9 +452,7 @@ void finish_binning_typed(handle_impl const& h, csx_t& c)
   B200_LAUNCH(h, k_split_flags, grid_for(c.n_chunks + 1), kBlock, 0, c.chunk_first_row.as<int32_t>(),
               straddle.as<int32_t>(), c.n_chunks, uniq.as<int32_t>());
   exclusive_scan_i32(h, uniq.as<int32_t>(), scan.as<int32_t>(), (int64_t)c.n_chunks + 1);
-  int32_t n_split = 0;
-  CUDA_TRY(cudaMemcpyAsync(&n_split, scan.as<int32_t>() + c.n_chunks, sizeof(int32_t), cudaMemcpyDeviceToHost, h.stream));
-  sync(h);
+  const int32_t n_split = read_back(h, scan.as<int32_t>() + c.n_chunks);
   c.n_split    = n_split;
   c.split_rows = make_dbuf<int32_t>((size_t)std::max(n_split, 1), h.stream);
   B200_LAUNCH(h, k_split_rows, grid_for(c.n_chunks + 1), kBlock, 0, c.chunk_first_row.as<int32_t>(),
@@ -525,11 +503,11 @@ staged_ids compute_ranks(handle_impl const& h, VT const* verts, int64_t n_verts,
   long long init[2] = {LLONG_MAX, LLONG_MIN};
   CUDA_TRY(cudaMemcpyAsync(mm.data(), init, sizeof(init), cudaMemcpyHostToDevice, h.stream));
   if (n > 0) {
-    B200_LAUNCH(h, (k_minmax<VT>), std::min(grid_for(n, 8), 2048), kBlock, 0, src, n, mm.as<long long>(), mm.as<long long>() + 1);
-    B200_LAUNCH(h, (k_minmax<VT>), std::min(grid_for(n, 8), 2048), kBlock, 0, dst, n, mm.as<long long>(), mm.as<long long>() + 1);
+    B200_LAUNCH(h, (k_minmax<VT>), grid_for(n, 8, 2048), kBlock, 0, src, n, mm.as<long long>(), mm.as<long long>() + 1);
+    B200_LAUNCH(h, (k_minmax<VT>), grid_for(n, 8, 2048), kBlock, 0, dst, n, mm.as<long long>(), mm.as<long long>() + 1);
   }
   if (n_verts > 0)
-    B200_LAUNCH(h, (k_minmax<VT>), std::min(grid_for(n_verts, 8), 2048), kBlock, 0, verts, n_verts, mm.as<long long>(),
+    B200_LAUNCH(h, (k_minmax<VT>), grid_for(n_verts, 8, 2048), kBlock, 0, verts, n_verts, mm.as<long long>(),
                 mm.as<long long>() + 1);
   long long hmm[2];
   CUDA_TRY(cudaMemcpyAsync(hmm, mm.data(), sizeof(hmm), cudaMemcpyDeviceToHost, h.stream));
@@ -561,9 +539,7 @@ staged_ids compute_ranks(handle_impl const& h, VT const* verts, int64_t n_verts,
     }
     if (n_verts > 0) B200_LAUNCH(h, (k_mark<VT>), grid_for(n_verts, 4), kBlock, 0, verts, n_verts, flags.as<int32_t>());
     exclusive_scan_i32(h, flags.as<int32_t>(), rank.as<int32_t>(), m + 1);
-    int32_t nv = 0;
-    CUDA_TRY(cudaMemcpyAsync(&nv, rank.as<int32_t>() + m, sizeof(int32_t), cudaMemcpyDeviceToHost, h.stream));
-    sync(h);
+    const int32_t nv = read_back(h, rank.as<int32_t>() + m);
     r.nv         = nv;
     r.sorted_ext = make_dbuf<VT>(nv, h.stream);
     B200_LAUNCH(h, (k_dense_sorted_ext<VT>), grid_for(m, 4), kBlock, 0, flags.as<int32_t>(), rank.as<int32_t>(), m,
@@ -683,7 +659,7 @@ void symmetrize_typed(handle_impl const& h, dbuf& src, dbuf& dst, dbuf& w, bool 
     using U = typename std::conditional<sizeof(W) == 4, uint32_t, uint64_t>::type;
     dbuf perm = make_dbuf<uint32_t>(n, h.stream), perm2 = make_dbuf<uint32_t>(n, h.stream);
     dbuf wk = make_dbuf<U>(n, h.stream), wk2 = make_dbuf<U>(n, h.stream);
-    B200_LAUNCH(h, k_iota64, grid_for(n, 4), kBlock, 0, n, perm.as<uint32_t>());
+    B200_LAUNCH(h, k_iota<uint32_t>, grid_for(n, 4), kBlock, 0, perm.as<uint32_t>(), n);
     B200_LAUNCH(h, (k_weight_keys<W, U>), grid_for(n, 4), kBlock, 0, w.as<W>(), n, wk.as<U>());
     sort_pairs<U, uint32_t>(h, wk.as<U>(), wk2.as<U>(), perm.as<uint32_t>(), perm2.as<uint32_t>(), n, 0, (int)sizeof(U) * 8);
     B200_LAUNCH(h, (k_gather<uint64_t>), grid_for(n, 4), kBlock, 0, comp.as<uint64_t>(), perm2.as<uint32_t>(), n, comp2.as<uint64_t>());
@@ -700,9 +676,7 @@ void symmetrize_typed(handle_impl const& h, dbuf& src, dbuf& dst, dbuf& w, bool 
   B200_LAUNCH(h, (k_sym_emit<W>), grid_for(n, 2), kBlock, 0, comp.as<uint64_t>(), weighted ? wsorted.as<W>() : (W const*)nullptr,
               n, bits, (int32_t const*)nullptr, 0, cnt.as<int32_t>(), (int32_t*)nullptr, (int32_t*)nullptr, (W*)nullptr);
   exclusive_scan_i32(h, cnt.as<int32_t>(), scan.as<int32_t>(), n + 1);
-  int32_t m = 0;
-  CUDA_TRY(cudaMemcpyAsync(&m, scan.as<int32_t>() + n, sizeof(int32_t), cudaMemcpyDeviceToHost, h.stream));
-  sync(h);
+  const int32_t m = read_back(h, scan.as<int32_t>() + n);
   dbuf os = make_dbuf<int32_t>(m, h.stream), od = make_dbuf<int32_t>(m, h.stream);
   dbuf ow;
   if (weighted) ow = make_dbuf<W>(m, h.stream);
@@ -960,9 +934,9 @@ dbuf reported_vertices(handle_impl const& h, graph_impl const& g)
   if (g.renumbered) {
     CUDA_TRY(cudaMemcpyAsync(out.data(), g.ext_of_int.data(), (size_t)g.n_vertices * es, cudaMemcpyDeviceToDevice, h.stream));
   } else if (g.vertex_type == INT32) {
-    B200_LAUNCH(h, (k_iota_t<int32_t>), grid_for(g.n_vertices), kBlock, 0, g.n_vertices, out.as<int32_t>());
+    B200_LAUNCH(h, k_iota<int32_t>, grid_for(g.n_vertices), kBlock, 0, out.as<int32_t>(), (int64_t)g.n_vertices);
   } else {
-    B200_LAUNCH(h, (k_iota_t<int64_t>), grid_for(g.n_vertices), kBlock, 0, g.n_vertices, out.as<int64_t>());
+    B200_LAUNCH(h, k_iota<int64_t>, grid_for(g.n_vertices), kBlock, 0, out.as<int64_t>(), (int64_t)g.n_vertices);
   }
   return out;
 }
@@ -997,10 +971,7 @@ dbuf collect_vertex_values(handle_impl const& h, graph_impl const& g, device_arr
   CUDA_TRY(cudaMemsetAsync(bad.data(), 0, sizeof(int), h.stream));
   B200_LAUNCH(h, (k_scatter_values<T>), grid_for((int64_t)verts->size), kBlock, 0, idx.as<int32_t>(), (T const*)vals->data,
               (int64_t)verts->size, out.as<T>(), bad.as<int>());
-  int hbad = 0;
-  CUDA_TRY(cudaMemcpyAsync(&hbad, bad.data(), sizeof(int), cudaMemcpyDeviceToHost, h.stream));
-  sync(h);
-  B200_EXPECTS(hbad == 0, CUGRAPH_INVALID_INPUT, "vertex list contains ids that are not vertices of the graph");
+  B200_EXPECTS(read_back(h, bad.as<int>()) == 0, CUGRAPH_INVALID_INPUT, "vertex list contains ids that are not vertices of the graph");
   return out;
 }
 

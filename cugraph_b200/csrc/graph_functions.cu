@@ -7,8 +7,6 @@
 namespace b200 {
 namespace {
 
-constexpr int kDBlock = 256;
-
 template <typename O>
 __global__ void k_row_lengths(O const* __restrict__ off, int32_t n, int32_t* __restrict__ out)
 {
@@ -42,19 +40,19 @@ void internal_degrees(handle_impl const& h, graph_impl const& g, bool want_major
 {
   csx_t const& c   = *g.primary;
   const int32_t nv = g.n_vertices;
-  const int grid   = std::min((std::max(nv, 1) + kDBlock - 1) / kDBlock, h.sm_count * 8);
+  const int grid   = grid_for(nv, 1, h.sm_count * 8);
   if (want_major) {
     major = make_dbuf<int32_t>(std::max(nv, 1), h.stream);
     if (nv > 0) {
-      if (c.offs64) B200_LAUNCH(h, (k_row_lengths<int64_t>), grid, kDBlock, 0, c.offsets.as<int64_t>(), nv, major.as<int32_t>());
-      else B200_LAUNCH(h, (k_row_lengths<int32_t>), grid, kDBlock, 0, c.offsets.as<int32_t>(), nv, major.as<int32_t>());
+      if (c.offs64) B200_LAUNCH(h, (k_row_lengths<int64_t>), grid, kBlock, 0, c.offsets.as<int64_t>(), nv, major.as<int32_t>());
+      else B200_LAUNCH(h, (k_row_lengths<int32_t>), grid, kBlock, 0, c.offsets.as<int32_t>(), nv, major.as<int32_t>());
     }
   }
   if (want_minor) {
     minor = make_dbuf<int32_t>(std::max(nv, 1), h.stream);
     CUDA_TRY(cudaMemsetAsync(minor.data(), 0, sizeof(int32_t) * std::max(nv, 1), h.stream));
     if (c.nnz > 0)
-      B200_LAUNCH(h, k_index_histogram, (int)std::min<long long>((c.nnz + kDBlock - 1) / kDBlock, (long long)h.sm_count * 16), kDBlock, 0,
+      B200_LAUNCH(h, k_index_histogram, grid_for(c.nnz, 1, h.sm_count * 16), kBlock, 0,
                   c.indices.as<int32_t>(), (long long)c.nnz, minor.as<int32_t>());
   }
 }
@@ -68,7 +66,6 @@ cugraph_error_code_t degrees_entry(const cugraph_resource_handle_t* handle, cugr
     auto* g       = G(graph);
     B200_EXPECTS(result != nullptr, CUGRAPH_INVALID_INPUT, "result out-pointer is NULL");
     *result = nullptr;
-    B200_EXPECTS(g->mg == nullptr, CUGRAPH_NOT_IMPLEMENTED, "multi-GPU degrees are not implemented");
     auto const* sv = V(source_vertices);
     if (sv) B200_EXPECTS(sv->type == g->vertex_type, CUGRAPH_INVALID_INPUT, "vertex type of graph and source_vertices must match");
     const int32_t nv = g->n_vertices;
@@ -99,11 +96,11 @@ cugraph_error_code_t degrees_entry(const cugraph_resource_handle_t* handle, cugr
     }
     auto pick = [&](dbuf const& deg) {
       dbuf out(std::max<size_t>(n, 1) * dtype_size(g->edge_type), h.stream);
-      const int grid = (int)std::min<size_t>((std::max<size_t>(n, 1) + kDBlock - 1) / kDBlock, (size_t)h.sm_count * 8);
+      const int grid = grid_for((int64_t)n, 1, h.sm_count * 8);
       if (g->edge_type == INT64)
-        B200_LAUNCH(h, (k_pick_degrees<int64_t>), grid, kDBlock, 0, deg.as<int32_t>(), sel.as<int32_t>(), (long long)n, out.as<int64_t>());
+        B200_LAUNCH(h, (k_pick_degrees<int64_t>), grid, kBlock, 0, deg.as<int32_t>(), sel.as<int32_t>(), (long long)n, out.as<int64_t>());
       else
-        B200_LAUNCH(h, (k_pick_degrees<int32_t>), grid, kDBlock, 0, deg.as<int32_t>(), sel.as<int32_t>(), (long long)n, out.as<int32_t>());
+        B200_LAUNCH(h, (k_pick_degrees<int32_t>), grid, kBlock, 0, deg.as<int32_t>(), sel.as<int32_t>(), (long long)n, out.as<int32_t>());
       return new device_array_impl{std::move(out), n, g->edge_type};
     };
     auto res      = std::make_unique<degrees_result_impl>();

@@ -4,7 +4,7 @@
 // per_v_transform_reduce_e's grouped ncclReduce, update_edge_src_dst_property.cuh:550-579 /
 // per_v_transform_reduce_e.cuh:3389-3407) are orchestrated by cugraph_b200/mg.py over
 // torch.distributed (NCCL on NVLink 5 / NVSwitch).  This file provides the device-side pieces behind
-// the C ABI: a resource handle bound to the caller's CUDA stream, rectangular edge blocks with the
+// the C ABI (the resource handle bound to the caller's CUDA stream is made in capi_basic.cu): rectangular edge blocks with the
 // same binned / column-blocked layout as the single-GPU graph, the block pull sweep and the fused
 // per-iteration vertex step, the transposed block sweep, the owner steps of Katz, eigenvector centrality and HITS, the BFS
 // pull step, the SSSP push relaxation and the WCC min-label round.  All calls only ENQUEUE work on the handle's stream (the
@@ -47,20 +47,6 @@ struct block_impl {
 
 namespace {
 
-__device__ __forceinline__ double block_sum2(double v, double* smem)
-{
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) smem[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double t = 0.0;
-  if (threadIdx.x < 32) {
-    t = (threadIdx.x < (blockDim.x >> 5)) ? smem[threadIdx.x] : 0.0;
-    t = warp_sum(t);
-  }
-  __syncthreads();
-  return t;
-}
-
 // owner slice, one PageRank iteration (pagerank_impl.cuh:225-251, 311-318 fused):
 //   init    = (dangling_prev * alpha + 1 - alpha) / V        (dangling_prev from totals_prev[1])
 //   pr_new  = first ? pr : y + init                          (kPersonalized = false, pers unused)
@@ -97,8 +83,8 @@ k_mg_vertex_step(T const* __restrict__ y, T* __restrict__ pr, T const* __restric
     x[i]  = (ow == (T)0) ? nv : nv / ow;
     pr[i] = nv;
   }
-  diff = block_sum2(diff, smem);
-  dang = block_sum2(dang, smem);
+  diff = block_sum(diff, smem);
+  dang = block_sum(dang, smem);
   if (threadIdx.x == 0) {
     atomicAdd(partial_out + 0, diff);
     atomicAdd(partial_out + 1, dang);
@@ -111,10 +97,10 @@ k_mg_vertex_step(T const* __restrict__ y, T* __restrict__ pr, T const* __restric
 
 // Katz: x_new = y + beta (y carries alpha from the sweep) ; out[0] += sum |x_new - x| ; out[1] += sum x_new^2 ; x = x_new
 template <typename T>
-__global__ void __launch_bounds__(kCBlock)
+__global__ void __launch_bounds__(kBlock)
 k_katz_step(T const* __restrict__ y, T* __restrict__ x, int32_t n, double beta, double* __restrict__ out)
 {
-  __shared__ double smem[kCBlock / 32];
+  __shared__ double smem[kBlock / 32];
   double d = 0.0, s = 0.0;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const T nv = (T)((double)y[i] + beta);
@@ -132,9 +118,9 @@ k_katz_step(T const* __restrict__ y, T* __restrict__ x, int32_t n, double beta, 
 
 // eigenvector, first half: y += x ; out[0] += sum y^2   (k_add_vec + k_norm mode 0)
 template <typename T>
-__global__ void __launch_bounds__(kCBlock) k_eig_add(T* __restrict__ y, T const* __restrict__ x, int32_t n, double* __restrict__ out)
+__global__ void __launch_bounds__(kBlock) k_eig_add(T* __restrict__ y, T const* __restrict__ x, int32_t n, double* __restrict__ out)
 {
-  __shared__ double smem[kCBlock / 32];
+  __shared__ double smem[kBlock / 32];
   double s = 0.0;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const T v = y[i] + x[i];
@@ -147,10 +133,10 @@ __global__ void __launch_bounds__(kCBlock) k_eig_add(T* __restrict__ y, T const*
 
 // eigenvector, second half: y *= 1 / sqrt(sumsq[0]) ; out[0] += sum |y - x| ; x = y   (k_scale + k_abs_diff)
 template <typename T>
-__global__ void __launch_bounds__(kCBlock)
+__global__ void __launch_bounds__(kBlock)
 k_eig_scale(T* __restrict__ y, T* __restrict__ x, int32_t n, double const* __restrict__ sumsq, double* __restrict__ out)
 {
-  __shared__ double smem[kCBlock / 32];
+  __shared__ double smem[kBlock / 32];
   const double inv = 1.0 / sqrt(sumsq[0]);
   double d         = 0.0;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -165,7 +151,7 @@ k_eig_scale(T* __restrict__ y, T* __restrict__ x, int32_t n, double const* __res
 
 // HITS: out[0] = max(out[0], max hubs), out[1] = max(out[1], max auth)   (k_norm mode 2 of both arrays)
 template <typename T>
-__global__ void __launch_bounds__(kCBlock) k_hits_max(T const* __restrict__ hubs, T const* __restrict__ auth, int32_t n, double* __restrict__ out)
+__global__ void __launch_bounds__(kBlock) k_hits_max(T const* __restrict__ hubs, T const* __restrict__ auth, int32_t n, double* __restrict__ out)
 {
   double mh = 0.0, ma = 0.0;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -179,11 +165,11 @@ __global__ void __launch_bounds__(kCBlock) k_hits_max(T const* __restrict__ hubs
 
 // HITS: hubs *= 1 / mx[0] ; auth *= 1 / mx[1] ; out[0] += sum |hubs - prev|   (two k_scale + k_abs_diff)
 template <typename T>
-__global__ void __launch_bounds__(kCBlock)
+__global__ void __launch_bounds__(kBlock)
 k_hits_scale(T* __restrict__ hubs, T* __restrict__ auth, T const* __restrict__ prev, int32_t n, double const* __restrict__ mx,
              double* __restrict__ out)
 {
-  __shared__ double smem[kCBlock / 32];
+  __shared__ double smem[kBlock / 32];
   const double inv_h = 1.0 / mx[0], inv_a = 1.0 / mx[1];
   double d = 0.0;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -257,23 +243,18 @@ k_block_bfs_pull_low(O const* __restrict__ off, int32_t const* __restrict__ idx,
   }
 }
 
-__global__ void k_fill_i64(long long* __restrict__ a, long long n, long long v)
-{
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) a[i] = v;
-}
-
 template <typename O>
 void block_bfs_pull(handle_impl const& h, csx_t const& c, uint8_t const* frontier, uint8_t const* visited, long long maxpart,
                     int grid_cols, int grid_c, long long* cand, int32_t n_row_slots)
 {
-  B200_LAUNCH(h, k_fill_i64, std::min((n_row_slots + 255) / 256 + 1, h.sm_count * 8), 256, 0, cand, (long long)n_row_slots, -1ll);
+  B200_LAUNCH(h, k_fill<long long>, grid_for(n_row_slots, 1, h.sm_count * 8), kBlock, 0, cand, (int64_t)n_row_slots, -1ll);
   const int32_t n_hi = c.degree_sorted ? c.seg[0] : 0;
   const int32_t n_ne = c.degree_sorted ? c.seg[kNumSeg - 2] : c.n_rows;  // rows with at least one edge
   if (n_hi > 0)
-    B200_LAUNCH(h, (k_block_bfs_pull_hi<O>), std::min((n_hi + 7) / 8, h.sm_count * 16), 256, 0, c.offsets.as<O>(),
+    B200_LAUNCH(h, (k_block_bfs_pull_hi<O>), grid_for((int64_t)n_hi * 32, 1, h.sm_count * 16), kBlock, 0, c.offsets.as<O>(),
                 c.indices.as<int32_t>(), c.row_vertex.as<int32_t>(), n_hi, frontier, visited, maxpart, grid_cols, grid_c, cand);
   if (n_ne > n_hi)
-    B200_LAUNCH(h, (k_block_bfs_pull_low<O>), std::min((n_ne - n_hi + 255) / 256, h.sm_count * 16), 256, 0, c.offsets.as<O>(),
+    B200_LAUNCH(h, (k_block_bfs_pull_low<O>), grid_for(n_ne - n_hi, 1, h.sm_count * 16), kBlock, 0, c.offsets.as<O>(),
                 c.indices.as<int32_t>(), c.row_vertex.as<int32_t>(), n_hi, n_ne, frontier, visited, maxpart, grid_cols, grid_c, cand);
 }
 
@@ -419,24 +400,36 @@ void block_sweep(handle_impl const& h, block_impl& b, bool transposed, bool use_
   if (b.y_complete[1 - o] == yv->data) b.y_complete[1 - o] = nullptr;  // this sweep wrote the other orientation's empty slots
 }
 
-// arguments of the owner steps: arrays of one floating type, each at least n_local long
-void check_owner_args(std::initializer_list<device_array_view_impl const*> vs, size_t n_local, void const* partial)
-{
-  B200_EXPECTS(partial != nullptr, CUGRAPH_INVALID_INPUT, "NULL argument");
-  cugraph_data_type_id_t t = (*vs.begin()) ? (*vs.begin())->type : FLOAT32;
-  for (auto const* v : vs) {
-    B200_EXPECTS(v != nullptr, CUGRAPH_INVALID_INPUT, "NULL argument");
-    B200_EXPECTS(v->type == t && (t == FLOAT32 || t == FLOAT64), CUGRAPH_INVALID_INPUT, "arrays must share one FLOAT32 / FLOAT64 type");
-    B200_EXPECTS(v->size >= n_local, CUGRAPH_INVALID_INPUT, "arrays shorter than n_local");
-  }
-}
-
 // f(float{}) for FLOAT32, else f(double{}): the launchers' dispatch on the floating type of their (checked) arrays
 template <typename F>
 void by_float_type(cugraph_data_type_id_t t, F&& f)
 {
   if (t == FLOAT32) f(float{});
   else f(double{});
+}
+
+// The frame of the owner steps (Katz, eigenvector, HITS, vertex sums and scaling).  Checks in this order: `partial` is
+// not NULL; the arrays `vs` are not NULL, share one FLOAT32 / FLOAT64 type and hold n_local elements; the device scalars
+// `ins` are not NULL.  Then, for n_local > 0, launch(h, T{}, n_local, grid) and the check of the launch.
+template <typename F>
+cugraph_error_code_t owner_step(cugraph_error_t** error, const char* what, const cugraph_resource_handle_t* handle,
+                                std::initializer_list<device_array_view_impl const*> vs, size_t n_local, void const* partial,
+                                std::initializer_list<void const*> ins, F&& launch)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(partial != nullptr, CUGRAPH_INVALID_INPUT, "NULL argument");
+    const cugraph_data_type_id_t t = (*vs.begin()) ? (*vs.begin())->type : FLOAT32;
+    for (auto const* v : vs) {
+      B200_EXPECTS(v != nullptr, CUGRAPH_INVALID_INPUT, "NULL argument");
+      B200_EXPECTS(v->type == t && (t == FLOAT32 || t == FLOAT64), CUGRAPH_INVALID_INPUT, "arrays must share one FLOAT32 / FLOAT64 type");
+      B200_EXPECTS(v->size >= n_local, CUGRAPH_INVALID_INPUT, "arrays shorter than n_local");
+    }
+    for (void const* p : ins) B200_EXPECTS(p != nullptr, CUGRAPH_INVALID_INPUT, "NULL argument");
+    if (n_local == 0) return;
+    by_float_type(t, [&](auto z) { launch(h, z, (int32_t)n_local, grid_for((int64_t)n_local, 1, h.sm_count * 8)); });
+    check_last(what);
+  });
 }
 
 // active rows -> queue (one read-back of its size and edge count) -> advance with `op`
@@ -447,12 +440,10 @@ void block_push_round(handle_impl const& h, block_push_t& p, T const* dist_cols,
   auto* cnt       = p.counts.as<block_queue_counts_t>();
   CUDA_TRY(cudaMemsetAsync(cnt, 0, sizeof(block_queue_counts_t), h.stream));
   if (p.n_ne > 0)
-    B200_LAUNCH(h, (k_block_active_rows<O, T>), std::min((p.n_ne + kBlock - 1) / kBlock, h.sm_count * 8), kBlock, 0,
+    B200_LAUNCH(h, (k_block_active_rows<O, T>), grid_for(p.n_ne, 1, h.sm_count * 8), kBlock, 0,
                 pc.offsets.as<O>(), pc.row_vertex.as<int32_t>(), p.n_ne, dist_cols, p.queue.as<int32_t>(), p.q_deg.as<int32_t>(),
                 cnt);
-  block_queue_counts_t hc{};
-  CUDA_TRY(cudaMemcpyAsync(&hc, cnt, sizeof(hc), cudaMemcpyDeviceToHost, h.stream));
-  sync(h);
+  const block_queue_counts_t hc = read_back(h, cnt);
   advance<O>(h, p.adv, pc.offsets.as<O>(), pc.indices.as<int32_t>(), p.queue.as<int32_t>(), hc.n, hc.edges, op,
              p.q_deg.as<int32_t>());
 }
@@ -461,7 +452,7 @@ void block_push_round(handle_impl const& h, block_push_t& p, T const* dist_cols,
 template <typename T, typename Op>
 void block_push_min(handle_impl const& h, block_impl const& b, block_push_t& p, long long* out, T const* active_cols, Op op)
 {
-  B200_LAUNCH(h, k_fill_i64, std::min((b.n_rows + 255) / 256 + 1, h.sm_count * 8), 256, 0, out, (long long)b.n_rows, LLONG_MAX);
+  B200_LAUNCH(h, k_fill<long long>, grid_for(b.n_rows, 1, h.sm_count * 8), kBlock, 0, out, (int64_t)b.n_rows, LLONG_MAX);
   if (p.csx->offs64) block_push_round<int64_t>(h, p, active_cols, op);
   else block_push_round<int32_t>(h, p, active_cols, op);
 }
@@ -513,11 +504,10 @@ void pagerank_vertex_step(handle_impl const& h, device_array_view_impl const* yv
                  (!persv || persv->size >= n_local),
                CUGRAPH_INVALID_INPUT, "arrays shorter than n_local");
   if (n_local == 0) return;
-  const int grid = (int)std::min<size_t>((n_local + 255) / 256, (size_t)h.sm_count * 8);
   by_float_type(yv->type, [&](auto z) {
     using T = decltype(z);
     auto* kernel = persv ? k_mg_vertex_step<T, true> : k_mg_vertex_step<T, false>;
-    B200_LAUNCH(h, kernel, grid, 256, 0, (T const*)yv->data, (T*)pv->data, (T const*)ov->data, (T*)xv->data,
+    B200_LAUNCH(h, kernel, grid_for((int64_t)n_local, 1, h.sm_count * 8), kBlock, 0, (T const*)yv->data, (T*)pv->data, (T const*)ov->data, (T*)xv->data,
                 persv ? (T const*)persv->data : nullptr, (int32_t)n_local, alpha, n_vertices_global, pers_sum,
                 first == TRUE ? 1 : 0, totals_prev, partial_out);
   });
@@ -525,53 +515,11 @@ void pagerank_vertex_step(handle_impl const& h, device_array_view_impl const* yv
 
 }  // namespace
 
-void attach_comm(handle_impl*, void*)
-{
-  throw capi_exception(CUGRAPH_NOT_IMPLEMENTED,
-                       "multi-GPU goes through cugraph_b200.mg (torch.distributed) + the cugraph_b200_block_* entry points");
-}
-
-void free_mg_graph(graph_impl*) {}
-
-void mg_pagerank(handle_impl const&, graph_impl&, mg_pr_args const&, centrality_result_impl&)
-{
-  throw capi_exception(CUGRAPH_NOT_IMPLEMENTED, "multi-GPU PageRank: use cugraph_b200.mg.MGGraph / mg.pagerank");
-}
-
 }  // namespace b200
 
 using namespace b200;
 
 extern "C" {
-
-cugraph_resource_handle_t* cugraph_b200_create_resource_handle_on_stream(void* cuda_stream)
-{
-  try {
-    auto* h = new handle_impl{};
-    h->tune = tuning_t::from_env();
-    CUDA_TRY(cudaGetDevice(&h->device));
-    h->stream         = reinterpret_cast<cudaStream_t>(cuda_stream);
-    h->borrowed_stream = true;
-    CUDA_TRY(cudaStreamCreateWithFlags(&h->aux_stream, cudaStreamNonBlocking));
-    register_stream(h->stream);
-    register_stream(h->aux_stream);
-    CUDA_TRY(cudaEventCreateWithFlags(&h->ev_a, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventCreateWithFlags(&h->ev_b, cudaEventDisableTiming));
-    cudaDeviceProp prop{};
-    CUDA_TRY(cudaGetDeviceProperties(&prop, h->device));
-    h->sm_count = prop.multiProcessorCount;
-    h->l2_bytes = static_cast<size_t>(prop.l2CacheSize);
-    CUDA_TRY(cudaMallocHost(&h->pinned, 4096));
-    cudaMemPool_t pool;
-    CUDA_TRY(cudaDeviceGetDefaultMemPool(&pool, h->device));
-    uint64_t threshold = UINT64_MAX;
-    CUDA_TRY(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &threshold));
-    return reinterpret_cast<cugraph_resource_handle_t*>(h);
-  } catch (std::exception const& e) {
-    std::fprintf(stderr, "cugraph_b200_create_resource_handle_on_stream: %s\n", e.what());
-    return nullptr;
-  }
-}
 
 size_t cugraph_b200_padded_elems(size_t n, size_t elem_size) { return padded_x_elems((int32_t)n, elem_size); }
 
@@ -647,18 +595,10 @@ cugraph_error_code_t cugraph_b200_katz_step(const cugraph_resource_handle_t* han
                                             cugraph_type_erased_device_array_view_t* x, size_t n_local, double beta,
                                             double* partial_out_device, cugraph_error_t** error)
 {
-  return guarded(error, [&] {
-    auto const& h = H(handle);
-    auto const* yv = V(y);
-    auto const* xv = V(x);
-    check_owner_args({yv, xv}, n_local, partial_out_device);
-    if (n_local == 0) return;
-    const int32_t n = (int32_t)n_local;
-    by_float_type(yv->type, [&](auto z) {
-      using T = decltype(z);
-      B200_LAUNCH(h, k_katz_step<T>, cgrid(h, n), kCBlock, 0, (T const*)yv->data, (T*)xv->data, n, beta, partial_out_device);
-    });
-    check_last("katz_step");
+  auto const *yv = V(y), *xv = V(x);
+  return owner_step(error, "katz_step", handle, {yv, xv}, n_local, partial_out_device, {}, [&](auto const& h, auto z, int32_t n, int grid) {
+    using T = decltype(z);
+    B200_LAUNCH(h, k_katz_step<T>, grid, kBlock, 0, (T const*)yv->data, (T*)xv->data, n, beta, partial_out_device);
   });
 }
 
@@ -667,19 +607,12 @@ cugraph_error_code_t cugraph_b200_eigenvector_add_step(const cugraph_resource_ha
                                                        const cugraph_type_erased_device_array_view_t* x, size_t n_local,
                                                        double* partial_out_device, cugraph_error_t** error)
 {
-  return guarded(error, [&] {
-    auto const& h = H(handle);
-    auto const* yv = V(y);
-    auto const* xv = V(x);
-    check_owner_args({yv, xv}, n_local, partial_out_device);
-    if (n_local == 0) return;
-    const int32_t n = (int32_t)n_local;
-    by_float_type(yv->type, [&](auto z) {
-      using T = decltype(z);
-      B200_LAUNCH(h, k_eig_add<T>, cgrid(h, n), kCBlock, 0, (T*)yv->data, (T const*)xv->data, n, partial_out_device);
-    });
-    check_last("eigenvector_add_step");
-  });
+  auto const *yv = V(y), *xv = V(x);
+  return owner_step(error, "eigenvector_add_step", handle, {yv, xv}, n_local, partial_out_device, {},
+                    [&](auto const& h, auto z, int32_t n, int grid) {
+                      using T = decltype(z);
+                      B200_LAUNCH(h, k_eig_add<T>, grid, kBlock, 0, (T*)yv->data, (T const*)xv->data, n, partial_out_device);
+                    });
 }
 
 cugraph_error_code_t cugraph_b200_eigenvector_scale_step(const cugraph_resource_handle_t* handle,
@@ -688,20 +621,13 @@ cugraph_error_code_t cugraph_b200_eigenvector_scale_step(const cugraph_resource_
                                                          const double* sumsq_device, double* partial_out_device,
                                                          cugraph_error_t** error)
 {
-  return guarded(error, [&] {
-    auto const& h = H(handle);
-    auto const* yv = V(y);
-    auto const* xv = V(x);
-    check_owner_args({yv, xv}, n_local, partial_out_device);
-    B200_EXPECTS(sumsq_device != nullptr, CUGRAPH_INVALID_INPUT, "NULL argument");
-    if (n_local == 0) return;
-    const int32_t n = (int32_t)n_local;
-    by_float_type(yv->type, [&](auto z) {
-      using T = decltype(z);
-      B200_LAUNCH(h, k_eig_scale<T>, cgrid(h, n), kCBlock, 0, (T*)yv->data, (T*)xv->data, n, sumsq_device, partial_out_device);
-    });
-    check_last("eigenvector_scale_step");
-  });
+  auto const *yv = V(y), *xv = V(x);
+  return owner_step(error, "eigenvector_scale_step", handle, {yv, xv}, n_local, partial_out_device, {sumsq_device},
+                    [&](auto const& h, auto z, int32_t n, int grid) {
+                      using T = decltype(z);
+                      B200_LAUNCH(h, k_eig_scale<T>, grid, kBlock, 0, (T*)yv->data, (T*)xv->data, n, sumsq_device,
+                                  partial_out_device);
+                    });
 }
 
 cugraph_error_code_t cugraph_b200_hits_max_step(const cugraph_resource_handle_t* handle,
@@ -709,19 +635,12 @@ cugraph_error_code_t cugraph_b200_hits_max_step(const cugraph_resource_handle_t*
                                                 const cugraph_type_erased_device_array_view_t* authorities, size_t n_local,
                                                 double* max_out_device, cugraph_error_t** error)
 {
-  return guarded(error, [&] {
-    auto const& h = H(handle);
-    auto const* hv = V(hubs);
-    auto const* av = V(authorities);
-    check_owner_args({hv, av}, n_local, max_out_device);
-    if (n_local == 0) return;
-    const int32_t n = (int32_t)n_local;
-    by_float_type(hv->type, [&](auto z) {
-      using T = decltype(z);
-      B200_LAUNCH(h, k_hits_max<T>, cgrid(h, n), kCBlock, 0, (T const*)hv->data, (T const*)av->data, n, max_out_device);
-    });
-    check_last("hits_max_step");
-  });
+  auto const *hv = V(hubs), *av = V(authorities);
+  return owner_step(error, "hits_max_step", handle, {hv, av}, n_local, max_out_device, {},
+                    [&](auto const& h, auto z, int32_t n, int grid) {
+                      using T = decltype(z);
+                      B200_LAUNCH(h, k_hits_max<T>, grid, kBlock, 0, (T const*)hv->data, (T const*)av->data, n, max_out_device);
+                    });
 }
 
 cugraph_error_code_t cugraph_b200_hits_scale_step(const cugraph_resource_handle_t* handle,
@@ -730,57 +649,35 @@ cugraph_error_code_t cugraph_b200_hits_scale_step(const cugraph_resource_handle_
                                                   const cugraph_type_erased_device_array_view_t* prev_hubs, size_t n_local,
                                                   const double* max_device, double* partial_out_device, cugraph_error_t** error)
 {
-  return guarded(error, [&] {
-    auto const& h = H(handle);
-    auto const* hv = V(hubs);
-    auto const* av = V(authorities);
-    auto const* pv = V(prev_hubs);
-    check_owner_args({hv, av, pv}, n_local, partial_out_device);
-    B200_EXPECTS(max_device != nullptr, CUGRAPH_INVALID_INPUT, "NULL argument");
-    if (n_local == 0) return;
-    const int32_t n = (int32_t)n_local;
-    by_float_type(hv->type, [&](auto z) {
-      using T = decltype(z);
-      B200_LAUNCH(h, k_hits_scale<T>, cgrid(h, n), kCBlock, 0, (T*)hv->data, (T*)av->data, (T const*)pv->data, n, max_device,
-                  partial_out_device);
-    });
-    check_last("hits_scale_step");
-  });
+  auto const *hv = V(hubs), *av = V(authorities), *pv = V(prev_hubs);
+  return owner_step(error, "hits_scale_step", handle, {hv, av, pv}, n_local, partial_out_device, {max_device},
+                    [&](auto const& h, auto z, int32_t n, int grid) {
+                      using T = decltype(z);
+                      B200_LAUNCH(h, k_hits_scale<T>, grid, kBlock, 0, (T*)hv->data, (T*)av->data, (T const*)pv->data, n,
+                                  max_device, partial_out_device);
+                    });
 }
 
 cugraph_error_code_t cugraph_b200_vertex_sum(const cugraph_resource_handle_t* handle,
                                              const cugraph_type_erased_device_array_view_t* v, size_t n_local, bool_t squares,
                                              double* partial_out_device, cugraph_error_t** error)
 {
-  return guarded(error, [&] {
-    auto const& h = H(handle);
-    auto const* vv = V(v);
-    check_owner_args({vv}, n_local, partial_out_device);
-    if (n_local == 0) return;
-    const int32_t n = (int32_t)n_local;
-    const int mode  = squares == TRUE ? 0 : 1;
-    by_float_type(vv->type, [&](auto z) {
-      using T = decltype(z);
-      B200_LAUNCH(h, k_norm<T>, cgrid(h, n), kCBlock, 0, (T const*)vv->data, n, mode, partial_out_device);
-    });
-    check_last("vertex_sum");
-  });
+  auto const* vv = V(v);
+  const int mode = squares == TRUE ? 0 : 1;
+  return owner_step(error, "vertex_sum", handle, {vv}, n_local, partial_out_device, {},
+                    [&](auto const& h, auto z, int32_t n, int grid) {
+                      using T = decltype(z);
+                      B200_LAUNCH(h, k_norm<T>, grid, kBlock, 0, (T const*)vv->data, n, mode, partial_out_device);
+                    });
 }
 
 cugraph_error_code_t cugraph_b200_vertex_scale(const cugraph_resource_handle_t* handle, cugraph_type_erased_device_array_view_t* v,
                                                size_t n_local, double inv, cugraph_error_t** error)
 {
-  return guarded(error, [&] {
-    auto const& h = H(handle);
-    auto const* vv = V(v);
-    check_owner_args({vv}, n_local, &inv);
-    if (n_local == 0) return;
-    const int32_t n = (int32_t)n_local;
-    by_float_type(vv->type, [&](auto z) {
-      using T = decltype(z);
-      B200_LAUNCH(h, k_scale<T>, cgrid(h, n), kCBlock, 0, (T*)vv->data, n, inv);
-    });
-    check_last("vertex_scale");
+  auto const* vv = V(v);
+  return owner_step(error, "vertex_scale", handle, {vv}, n_local, &inv, {}, [&](auto const& h, auto z, int32_t n, int grid) {
+    using T = decltype(z);
+    B200_LAUNCH(h, k_scale<T>, grid, kBlock, 0, (T*)vv->data, n, inv);
   });
 }
 

@@ -15,16 +15,6 @@
 namespace b200 {
 namespace {
 
-constexpr int kBlock = 256;
-inline int grid_for(int64_t n) { return (int)std::min<int64_t>(std::max<int64_t>((n + kBlock - 1) / kBlock, 1), 1 << 22); }
-
-template <typename T>
-__global__ void k_fill(T* a, int32_t n, T v)
-{
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) a[i] = v;
-}
-
 __global__ void k_out_degree(int32_t const* __restrict__ indices, long long nnz, int32_t* __restrict__ deg)
 {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < nnz; i += (long long)gridDim.x * blockDim.x)
@@ -41,22 +31,7 @@ __global__ void k_out_weight(int32_t const* __restrict__ indices, T const* __res
 template <typename S, typename T>
 __global__ void k_cast(S const* in, int32_t n, T* out)
 {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = (T)in[i];
-}
-
-__device__ __forceinline__ double block_sum(double v, double* smem)
-{
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) smem[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double t = 0.0;
-  if (threadIdx.x < 32) {
-    t = (threadIdx.x < (blockDim.x >> 5)) ? smem[threadIdx.x] : 0.0;
-    t = warp_sum(t);
-  }
-  __syncthreads();
-  return t;  // valid in warp 0
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = (T)in[i];
 }
 
 // fused vertex pass: diff += |new-old| ; dangling += new where out_w==0 ; x = new / (out_w or 1)
@@ -105,8 +80,8 @@ __global__ void k_personalize(int32_t const* __restrict__ pv, T const* __restric
                               T* __restrict__ y, pr_state_t const* __restrict__ st)
 {
   if (st->done) return;
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) y[pv[i]] = (T)((double)y[pv[i]] + st->pers_scale * ((double)pvals[i] / pers_sum));
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    y[pv[i]] = (T)((double)y[pv[i]] + st->pers_scale * ((double)pvals[i] / pers_sum));
 }
 
 template <typename T>
@@ -117,13 +92,6 @@ __global__ void k_sum(T const* a, int32_t n, double* out)
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) s += (double)a[i];
   s = block_sum(s, smem);
   if (threadIdx.x == 0) atomicAdd(out, s);
-}
-
-template <typename T>
-__global__ void k_count_negative(T const* a, int64_t n, int* out)
-{
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-    if (a[i] < (T)0) atomicAdd(out, 1);
 }
 
 struct pr_args {
@@ -172,14 +140,14 @@ void pagerank_typed(handle_impl const& h, graph_impl& g, pr_args const& a, centr
         dbuf sums = make_dbuf<double>(nv, h.stream);
         CUDA_TRY(cudaMemsetAsync(sums.data(), 0, sizeof(double) * nv, h.stream));
         if (c.nnz > 0)
-          B200_LAUNCH(h, (k_out_weight<T>), std::min(grid_for(c.nnz), h.sm_count * 16), kBlock, 0, c.indices.as<int32_t>(),
+          B200_LAUNCH(h, (k_out_weight<T>), grid_for(c.nnz, 1, h.sm_count * 16), kBlock, 0, c.indices.as<int32_t>(),
                       c.weights.as<T>(), (long long)c.nnz, sums.as<double>());
         B200_LAUNCH(h, (k_cast<double, T>), grid_for(nv), kBlock, 0, sums.as<double>(), nv, ow.as<T>());
       } else {
         dbuf deg = make_dbuf<int32_t>(nv, h.stream);
         CUDA_TRY(cudaMemsetAsync(deg.data(), 0, sizeof(int32_t) * nv, h.stream));
         if (c.nnz > 0)
-          B200_LAUNCH(h, k_out_degree, std::min(grid_for(c.nnz), h.sm_count * 16), kBlock, 0, c.indices.as<int32_t>(),
+          B200_LAUNCH(h, k_out_degree, grid_for(c.nnz, 1, h.sm_count * 16), kBlock, 0, c.indices.as<int32_t>(),
                       (long long)c.nnz, deg.as<int32_t>());
         B200_LAUNCH(h, (k_cast<int32_t, T>), grid_for(nv), kBlock, 0, deg.as<int32_t>(), nv, ow.as<T>());
       }
@@ -192,11 +160,8 @@ void pagerank_typed(handle_impl const& h, graph_impl& g, pr_args const& a, centr
   if (a.expensive && weighted && c.nnz > 0) {
     dbuf neg = make_dbuf<int>(1, h.stream);
     CUDA_TRY(cudaMemsetAsync(neg.data(), 0, sizeof(int), h.stream));
-    B200_LAUNCH(h, (k_count_negative<T>), std::min(grid_for(c.nnz), h.sm_count * 16), kBlock, 0, c.weights.as<T>(), c.nnz, neg.as<int>());
-    int hneg = 0;
-    CUDA_TRY(cudaMemcpyAsync(&hneg, neg.data(), sizeof(int), cudaMemcpyDeviceToHost, h.stream));
-    sync(h);
-    B200_EXPECTS(hneg == 0, CUGRAPH_UNKNOWN_ERROR, "Invalid input argument: input edge weights should have non-negative values.");
+    B200_LAUNCH(h, (k_count_negative<T>), grid_for(c.nnz, 1, h.sm_count * 16), kBlock, 0, c.weights.as<T>(), c.nnz, neg.as<int>());
+    B200_EXPECTS(read_back(h, neg.as<int>()) == 0, CUGRAPH_UNKNOWN_ERROR, "Invalid input argument: input edge weights should have non-negative values.");
   }
 
   // personalization (pagerank_impl.cuh:200-214): ids -> internal, sum must be positive
@@ -211,17 +176,18 @@ void pagerank_typed(handle_impl const& h, graph_impl& g, pr_args const& a, centr
     n_pers   = (int32_t)a.pers_v->size;
     pers_idx = make_dbuf<int32_t>(n_pers, h.stream);
     ext_to_int(h, g, a.pers_v->data, n_pers, pers_idx.as<int32_t>());
-    dbuf bad = make_dbuf<int>(1, h.stream);
-    CUDA_TRY(cudaMemsetAsync(bad.data(), 0, sizeof(int), h.stream));
-    B200_LAUNCH(h, (k_count_negative<int32_t>), grid_for(n_pers), kBlock, 0, pers_idx.as<int32_t>(), (int64_t)n_pers, bad.as<int>());
-    dbuf dsum = make_dbuf<double>(1, h.stream);
-    CUDA_TRY(cudaMemsetAsync(dsum.data(), 0, sizeof(double), h.stream));
-    B200_LAUNCH(h, (k_sum<T>), std::min(grid_for(n_pers), 1024), kBlock, 0, (T const*)a.pers_val->data, n_pers, dsum.as<double>());
-    int hbad = 0;
-    CUDA_TRY(cudaMemcpyAsync(&hbad, bad.data(), sizeof(int), cudaMemcpyDeviceToHost, h.stream));
-    CUDA_TRY(cudaMemcpyAsync(&pers_sum, dsum.data(), sizeof(double), cudaMemcpyDeviceToHost, h.stream));
-    sync(h);
-    B200_EXPECTS(hbad == 0, CUGRAPH_INVALID_INPUT, "Invalid input argument: peresonalization vertices have invalid vertex IDs.");
+    struct pers_check_t {  // both read back with one copy
+      double sum;
+      int n_invalid;
+    };
+    dbuf chk = make_dbuf<pers_check_t>(1, h.stream);
+    auto* dchk = chk.as<pers_check_t>();
+    CUDA_TRY(cudaMemsetAsync(dchk, 0, sizeof(pers_check_t), h.stream));
+    B200_LAUNCH(h, (k_count_negative<int32_t>), grid_for(n_pers), kBlock, 0, pers_idx.as<int32_t>(), (int64_t)n_pers, &dchk->n_invalid);
+    B200_LAUNCH(h, (k_sum<T>), grid_for(n_pers, 1, 1024), kBlock, 0, (T const*)a.pers_val->data, n_pers, &dchk->sum);
+    const pers_check_t hchk = read_back(h, dchk);
+    B200_EXPECTS(hchk.n_invalid == 0, CUGRAPH_INVALID_INPUT, "Invalid input argument: peresonalization vertices have invalid vertex IDs.");
+    pers_sum = hchk.sum;
     B200_EXPECTS(pers_sum > 0.0, CUGRAPH_UNKNOWN_ERROR, "Invalid input argument: sum of personalization valuese should be positive.");
   }
 
@@ -242,7 +208,7 @@ void pagerank_typed(handle_impl const& h, graph_impl& g, pr_args const& a, centr
   }
 
   tr.mark("pagerank: state setup");
-  const int vgrid = std::min(grid_for(nv), h.sm_count * 8);
+  const int vgrid = grid_for(nv, 1, h.sm_count * 8);
   const int max_it = (int)std::min<size_t>(a.max_iterations, 0x7fffffff);
   // prologue: x and dangling sum of the starting vector, init for sweep 1
   B200_LAUNCH(h, (k_vertex_pass<T>), vgrid, kBlock, 0, pr_a.as<T>(), (T const*)nullptr, out_w, x.as<T>(), nv, st);
@@ -254,10 +220,7 @@ void pagerank_typed(handle_impl const& h, graph_impl& g, pr_args const& a, centr
   int enqueued    = 0;
   int iters       = 0;
   const int batch = (a.epsilon > 0.0) ? 8 : 64;
-  if (max_it == 0) {
-    // the reference's loop body runs at least once (pagerank_impl.cuh:224-327: test after iter++)
-  }
-  while (true) {
+  while (true) {  // the reference's loop body runs at least once (pagerank_impl.cuh:224-327: test after iter++)
     int todo = std::min(batch, std::max(max_it, 1) - enqueued);
     for (int k = 0; k < todo; ++k) {
       pull_sweep<T>(h, c, nv, x.as<T>(), nxt, sc, a.alpha);
@@ -318,13 +281,8 @@ cugraph_error_code_t pagerank_entry(const cugraph_resource_handle_t* handle, cug
     if (!a.pre_w) a.pre_v = nullptr;
     if (!a.init_val) a.init_v = nullptr;
     auto res = std::make_unique<centrality_result_impl>();
-    if (g->mg) {
-      mg_pagerank(h, *g, mg_pr_args{a.alpha, a.epsilon, a.max_iterations}, *res);
-    } else if (g->weight_type == FLOAT32) {
-      pagerank_typed<float>(h, *g, a, *res);
-    } else {
-      pagerank_typed<double>(h, *g, a, *res);
-    }
+    if (g->weight_type == FLOAT32) pagerank_typed<float>(h, *g, a, *res);
+    else pagerank_typed<double>(h, *g, a, *res);
     bool converged = res->converged;
     *result        = reinterpret_cast<cugraph_centrality_result_t*>(res.release());
     // cpp/src/c_api/pagerank.cpp:306-313: the result object is still returned
@@ -446,7 +404,6 @@ cugraph_error_code_t cugraph_b200_time_pull_spmv(const cugraph_resource_handle_t
   return guarded(error, [&] {
     auto const& h = H(handle);
     auto* g       = G(graph);
-    B200_EXPECTS(g->mg == nullptr, CUGRAPH_NOT_IMPLEMENTED, "time_pull_spmv is single-GPU only");
     B200_EXPECTS(g->weight_type == FLOAT32, CUGRAPH_NOT_IMPLEMENTED, "time_pull_spmv: float32 graphs only");
     csx_t const& c = pull_view(h, *g);
     int32_t nv     = g->n_vertices;

@@ -1,4 +1,4 @@
-// Launch grids and CUB wrappers of the one-time staging passes, shared by graph_build.cu and sweep_layout.cu.  Everything
+// CUB wrappers of the one-time staging passes, shared by graph_build.cu and sweep_layout.cu.  Everything
 // lives in an anonymous namespace, as in advance.cuh: every translation unit gets its own instantiations.
 #pragma once
 #include "common.cuh"
@@ -8,20 +8,6 @@
 
 namespace b200 {
 namespace {
-
-constexpr int kBlock = 256;
-
-inline int grid_for(int64_t n, int per_thread = 1)
-{
-  int64_t b = (n + (int64_t)kBlock * per_thread - 1) / ((int64_t)kBlock * per_thread);
-  return (int)std::min<int64_t>(std::max<int64_t>(b, 1), 1 << 20);
-}
-
-__global__ void k_iota64(int64_t n, uint32_t* v)
-{
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-    v[i] = (uint32_t)i;
-}
 
 template <typename K, typename Val>
 void sort_pairs(handle_impl const& h, K const* kin, K* kout, Val const* vin, Val* vout, int64_t n, int begin_bit, int end_bit)
@@ -53,10 +39,7 @@ int64_t select_flagged(handle_impl const& h, std::common_type_t<In> in, uint8_t 
   dbuf tmp(bytes, h.stream);
   CUDA_TRY(cub::DeviceSelect::Flagged(tmp.data(), bytes, in, flags, out, d_count.as<int64_t>(), n, h.stream));
   h.launches += 2;
-  int64_t cnt = 0;
-  CUDA_TRY(cudaMemcpyAsync(&cnt, d_count.data(), sizeof(int64_t), cudaMemcpyDeviceToHost, h.stream));
-  sync(h);
-  return cnt;
+  return read_back(h, d_count.as<int64_t>());
 }
 
 inline int bits_for(int64_t n)

@@ -6,9 +6,6 @@
 namespace b200 {
 namespace {
 
-constexpr int kBlock = 256;
-inline int grid_for(int64_t n) { return (int)std::min<int64_t>(std::max<int64_t>((n + kBlock - 1) / kBlock, 1), 1 << 22); }
-
 // rows that may need an fp64 accumulator in a sweep: the piece stream covers every row
 inline int32_t acc_rows(csx_t const& c) { return std::max(c.n_rows, 1); }
 
@@ -16,26 +13,25 @@ inline int32_t acc_rows(csx_t const& c) { return std::max(c.n_rows, 1); }
 template <typename T>
 __global__ void k_fill_pattern(T* x, int32_t n)
 {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) x[i] = (T)(0.5 + (double)((unsigned)(i * 2654435761u) >> 16) / 65536.0);
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    x[i] = (T)(0.5 + (double)(((unsigned)i * 2654435761u) >> 16) / 65536.0);
 }
 
 // packed (relative difference bits << 32 | row): atomicMax keeps the worst row of each class
-template <typename O, typename T>
-__global__ void k_compare_rows(O const* __restrict__ off, int32_t const* __restrict__ row_vertex, T const* __restrict__ a,
-                               T const* __restrict__ b, int32_t n_rows, int32_t n_hi, double tol,
-                               unsigned long long* __restrict__ worst /*[2]*/, unsigned long long* __restrict__ n_bad /*[2]*/)
+template <typename T>
+__global__ void k_compare_rows(int32_t const* __restrict__ row_vertex, T const* __restrict__ a, T const* __restrict__ b,
+                               int32_t n_rows, int32_t n_hi, double tol, unsigned long long* __restrict__ worst /*[2]*/,
+                               unsigned long long* __restrict__ n_bad /*[2]*/)
 {
-  int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= n_rows) return;
-  const int v        = row_vertex ? row_vertex[r] : r;
-  const double va = (double)a[v], vb = (double)b[v];
-  const double den   = fmax(fabs(va), 1e-300);
-  const float rel    = (float)fmin(fabs(va - vb) / den, 1e30);
-  const int cls      = r < n_hi ? 0 : 1;
-  atomicMax(worst + cls, ((unsigned long long)__float_as_uint(rel) << 32) | (unsigned)r);
-  if (rel > tol) atomicAdd(n_bad + cls, 1ull);
-  (void)off;
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n_rows; r += (int64_t)gridDim.x * blockDim.x) {
+    const int v     = row_vertex ? row_vertex[r] : (int)r;
+    const double va = (double)a[v], vb = (double)b[v];
+    const double den = fmax(fabs(va), 1e-300);
+    const float rel  = (float)fmin(fabs(va - vb) / den, 1e30);
+    const int cls    = r < n_hi ? 0 : 1;
+    atomicMax(worst + cls, ((unsigned long long)__float_as_uint(rel) << 32) | (unsigned)r);
+    if (rel > tol) atomicAdd(n_bad + cls, 1ull);
+  }
 }
 
 }  // namespace
@@ -108,7 +104,7 @@ cugraph_error_code_t cugraph_b200_debug_compare_sweeps(const cugraph_resource_ha
     auto const& h = H(handle);
     auto* g       = G(graph);
     B200_EXPECTS(out != nullptr, CUGRAPH_INVALID_INPUT, "out is NULL");
-    B200_EXPECTS(g->mg == nullptr && g->weight_type == FLOAT32, CUGRAPH_NOT_IMPLEMENTED, "single-GPU float32 graphs only");
+    B200_EXPECTS(g->weight_type == FLOAT32, CUGRAPH_NOT_IMPLEMENTED, "single-GPU float32 graphs only");
     csx_t const& c = pull_view(h, *g);
     B200_EXPECTS(!c.offs64, CUGRAPH_NOT_IMPLEMENTED, "32-bit offsets only");
     const int32_t nv = g->n_vertices;
@@ -120,8 +116,7 @@ cugraph_error_code_t cugraph_b200_debug_compare_sweeps(const cugraph_resource_ha
     pull_sweep<float>(h, c, nv, x.as<float>(), y1.as<float>(), sc, 0.85);
     dbuf res = make_dbuf<unsigned long long>(4, h.stream);
     CUDA_TRY(cudaMemsetAsync(res.data(), 0, 4 * sizeof(unsigned long long), h.stream));
-    B200_LAUNCH(h, (k_compare_rows<int32_t, float>), grid_for(c.n_rows), kBlock, 0, c.offsets.as<int32_t>(),
-                c.row_vertex.as<int32_t>(), y0.as<float>(), y1.as<float>(), c.n_rows, c.seg[0], 1e-5,
+    B200_LAUNCH(h, (k_compare_rows<float>), grid_for(c.n_rows), kBlock, 0, c.row_vertex.as<int32_t>(), y0.as<float>(), y1.as<float>(), c.n_rows, c.seg[0], 1e-5,
                 res.as<unsigned long long>(), res.as<unsigned long long>() + 2);
     unsigned long long hres[4];
     CUDA_TRY(cudaMemcpyAsync(hres, res.data(), sizeof(hres), cudaMemcpyDeviceToHost, h.stream));

@@ -21,8 +21,7 @@ namespace {
 
 __global__ void k_hot_row_starts(int32_t const* __restrict__ off, int32_t n_cov, uint8_t* __restrict__ flag)
 {
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r < n_cov) flag[(size_t)off[r]] = 1;  // covered rows are never empty
+  for (int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; r < n_cov; r += (int64_t)gridDim.x * blockDim.x) flag[(size_t)off[r]] = 1;  // covered rows are never empty
 }
 
 __global__ void k_hot_heads(int32_t const* __restrict__ idx, long long nnz, int W, uint8_t* __restrict__ flag)
@@ -40,21 +39,21 @@ __global__ void k_hot_segment_info(int32_t const* __restrict__ head_pos, int32_t
                                    int32_t const* __restrict__ off, int32_t n_cov, int32_t* __restrict__ seg_row,
                                    int32_t* __restrict__ seg_pieces)
 {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k > n_segs) return;
-  if (k == n_segs) {
-    seg_pieces[k] = 0;
-    return;
+  for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k <= n_segs; k += (int64_t)gridDim.x * blockDim.x) {
+    if (k == n_segs) {
+      seg_pieces[k] = 0;
+      continue;
+    }
+    const long long start = head_pos[k];
+    const long long end   = (k + 1 < n_segs) ? (long long)head_pos[k + 1] : nnz;
+    int lo = 0, hi = n_cov;  // last row r with off[r] <= start
+    while (hi - lo > 1) {
+      const int mid = lo + ((hi - lo) >> 1);
+      if ((long long)off[mid] <= start) lo = mid; else hi = mid;
+    }
+    seg_row[k]    = lo;
+    seg_pieces[k] = (int)((end - start + kHotPieceEntries - 1) / kHotPieceEntries);
   }
-  const long long start = head_pos[k];
-  const long long end   = (k + 1 < n_segs) ? (long long)head_pos[k + 1] : nnz;
-  int lo = 0, hi = n_cov;  // last row r with off[r] <= start
-  while (hi - lo > 1) {
-    const int mid = lo + ((hi - lo) >> 1);
-    if ((long long)off[mid] <= start) lo = mid; else hi = mid;
-  }
-  seg_row[k]    = lo;
-  seg_pieces[k] = (int)((end - start + kHotPieceEntries - 1) / kHotPieceEntries);
 }
 
 __host__ __device__ __forceinline__ int piece_kind(int len)
@@ -70,33 +69,33 @@ __global__ void k_hot_emit_pieces(int32_t const* __restrict__ head_pos, int32_t 
                                   int32_t* __restrict__ piece_start, int32_t* __restrict__ piece_len,
                                   int32_t* __restrict__ piece_row)
 {
-  const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= n_segs) return;
-  const long long start = head_pos[k];
-  const long long end   = (k + 1 < n_segs) ? (long long)head_pos[k + 1] : nnz;
-  const int row         = seg_row[k];
-  const int bb          = (row / band_rows) * B + idx[start] / W;  // (band, block)
-  int p                 = piece_off[k];
-  for (long long s = start; s < end; s += kHotPieceEntries, ++p) {
-    const int len  = (int)((end - s < kHotPieceEntries) ? end - s : kHotPieceEntries);
-    piece_key[p]   = (uint32_t)(bb * kNumKinds + piece_kind(len));
-    piece_start[p] = (int32_t)s;
-    piece_len[p]   = len;
-    piece_row[p]   = row;
+  for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n_segs; k += (int64_t)gridDim.x * blockDim.x) {
+    const long long start = head_pos[k];
+    const long long end   = (k + 1 < n_segs) ? (long long)head_pos[k + 1] : nnz;
+    const int row         = seg_row[k];
+    const int bb          = (row / band_rows) * B + idx[start] / W;  // (band, block)
+    int p                 = piece_off[k];
+    for (long long s = start; s < end; s += kHotPieceEntries, ++p) {
+      const int len  = (int)((end - s < kHotPieceEntries) ? end - s : kHotPieceEntries);
+      piece_key[p]   = (uint32_t)(bb * kNumKinds + piece_kind(len));
+      piece_start[p] = (int32_t)s;
+      piece_len[p]   = len;
+      piece_row[p]   = row;
+    }
   }
 }
 
 __global__ void k_hot_class_starts(uint32_t const* __restrict__ sorted_key, int32_t n_pieces, int n_keys,
                                    int32_t* __restrict__ class_start)
 {
-  const int key = blockIdx.x * blockDim.x + threadIdx.x;
-  if (key > n_keys) return;
-  int lo = 0, hi = n_pieces;  // first piece with sorted_key >= key
-  while (lo < hi) {
-    const int mid = lo + ((hi - lo) >> 1);
-    if (sorted_key[mid] < (uint32_t)key) lo = mid + 1; else hi = mid;
+  for (int64_t key = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; key <= n_keys; key += (int64_t)gridDim.x * blockDim.x) {
+    int lo = 0, hi = n_pieces;  // first piece with sorted_key >= key
+    while (lo < hi) {
+      const int mid = lo + ((hi - lo) >> 1);
+      if (sorted_key[mid] < (uint32_t)key) lo = mid + 1; else hi = mid;
+    }
+    class_start[key] = lo;
   }
-  class_start[key] = lo;
 }
 
 struct sweep_fill_t {  // build-time companion of a chunk: its pieces start at piece_begin, its (band, block, kind) run ends at piece_end
@@ -360,26 +359,27 @@ __global__ void k_tail_run_bounds(int32_t const* __restrict__ off, int32_t row_l
   below[d] = lo;
 }
 
-// one thread per lane of a tile
+// one thread per lane of a tile, striding over the grid
 template <typename T>
 __global__ void k_tail_fill(tail_run_t const* __restrict__ runs, int n_runs, int32_t const* __restrict__ off,
                             int32_t const* __restrict__ idx, T const* __restrict__ w, int32_t pad_col,
                             int32_t* __restrict__ ids_out, T* __restrict__ w_out)
 {
-  const long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (t >= (long long)runs[n_runs].first_tile * kTailTile) return;
-  const int tile = (int)(t / kTailTile), lane = (int)(t % kTailTile);
-  int r = 0;
-  while (tile >= runs[r + 1].first_tile) ++r;
-  const tail_run_t R = runs[r];
-  const int d        = R.degree;
-  const int row      = R.first_row + (tile - R.first_tile) * kTailTile + lane;
-  const bool live    = row < runs[r + 1].first_row;
-  const long long e0 = live ? (long long)off[row] : 0;
-  const long long o  = R.id_off + (long long)(tile - R.first_tile) * kTailTile * d + lane;
-  for (int k = 0; k < d; ++k) {
-    ids_out[o + (long long)k * kTailTile] = live ? idx[e0 + k] : pad_col;
-    if (w_out) w_out[o + (long long)k * kTailTile] = live ? w[e0 + k] : (T)0;
+  const long long n_lanes = (long long)runs[n_runs].first_tile * kTailTile;
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < n_lanes; t += (int64_t)gridDim.x * blockDim.x) {
+    const int tile = (int)(t / kTailTile), lane = (int)(t % kTailTile);
+    int r = 0;
+    while (tile >= runs[r + 1].first_tile) ++r;
+    const tail_run_t R = runs[r];
+    const int d        = R.degree;
+    const int row      = R.first_row + (tile - R.first_tile) * kTailTile + lane;
+    const bool live    = row < runs[r + 1].first_row;
+    const long long e0 = live ? (long long)off[row] : 0;
+    const long long o  = R.id_off + (long long)(tile - R.first_tile) * kTailTile * d + lane;
+    for (int k = 0; k < d; ++k) {
+      ids_out[o + (long long)k * kTailTile] = live ? idx[e0 + k] : pad_col;
+      if (w_out) w_out[o + (long long)k * kTailTile] = live ? w[e0 + k] : (T)0;
+    }
   }
 }
 
@@ -460,13 +460,7 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   const int32_t n_str = c.seg[sweep_stream_bin(h, c)];              // rows of the stream; the tail is swept by k_sweep_tail
   if (n_str <= 0) return nullptr;                                   // no row reaches the bound: the plain sweep fits better
   const int B         = (int)(((int64_t)nv + W - 1) / W);
-  int64_t nnz = 0;  // edges of the stream rows: a prefix of indices (rows are degree-descending)
-  {
-    int32_t off_str;
-    CUDA_TRY(cudaMemcpyAsync(&off_str, c.offsets.as<int32_t>() + n_str, sizeof(int32_t), cudaMemcpyDeviceToHost, h.stream));
-    sync(h);
-    nnz = (int64_t)off_str;
-  }
+  const int64_t nnz   = read_back(h, c.offsets.as<int32_t>() + n_str);  // edges of the stream rows: a prefix of indices (rows are degree-descending)
   auto L              = std::make_unique<sweep_layout_t>();
   L->W = W; L->B = B; L->n_cov = n_cov; L->n_str = n_str; L->nnz = c.nnz;
   int32_t const* idx = c.indices.as<int32_t>();
@@ -481,7 +475,7 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   dbuf flag = make_dbuf<uint8_t>(nnz, h.stream);
   CUDA_TRY(cudaMemsetAsync(flag.data(), 0, nnz, h.stream));
   B200_LAUNCH(h, k_hot_row_starts, grid_for(n_str), kBlock, 0, c.offsets.as<int32_t>(), n_str, flag.as<uint8_t>());
-  B200_LAUNCH(h, k_hot_heads, std::min(grid_for(nnz, 4), h.sm_count * 32), kBlock, 0, idx, (long long)nnz, W, flag.as<uint8_t>());
+  B200_LAUNCH(h, k_hot_heads, grid_for(nnz, 4, h.sm_count * 32), kBlock, 0, idx, (long long)nnz, W, flag.as<uint8_t>());
   dbuf head_pos = make_dbuf<int32_t>(nnz, h.stream);
   const int64_t n_segs64 = select_flagged<int32_t, thrust::counting_iterator<int32_t>>(
     h, thrust::counting_iterator<int32_t>(0), flag.as<uint8_t>(), head_pos.as<int32_t>(), nnz);
@@ -495,9 +489,7 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   B200_LAUNCH(h, k_hot_segment_info, grid_for((int64_t)n_segs + 1), kBlock, 0, head_pos.as<int32_t>(), n_segs,
               (long long)nnz, c.offsets.as<int32_t>(), n_str, seg_row.as<int32_t>(), seg_pieces.as<int32_t>());
   exclusive_scan_i32(h, seg_pieces.as<int32_t>(), piece_off.as<int32_t>(), (int64_t)n_segs + 1);
-  int32_t n_pieces = 0;
-  CUDA_TRY(cudaMemcpyAsync(&n_pieces, piece_off.as<int32_t>() + n_segs, sizeof(int32_t), cudaMemcpyDeviceToHost, h.stream));
-  sync(h);
+  const int32_t n_pieces = read_back(h, piece_off.as<int32_t>() + n_segs);
   seg_pieces.release();
   L->n_pieces = n_pieces;
   dbuf piece_key = make_dbuf<uint32_t>(n_pieces, h.stream), piece_key2 = make_dbuf<uint32_t>(n_pieces, h.stream);
@@ -514,7 +506,7 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   // 3. order pieces by (band, block, kind)
   const int n_keys = n_bands * B * kNumKinds;
   dbuf perm = make_dbuf<uint32_t>(n_pieces, h.stream), perm2 = make_dbuf<uint32_t>(n_pieces, h.stream);
-  B200_LAUNCH(h, k_iota64, grid_for(n_pieces, 4), kBlock, 0, (int64_t)n_pieces, perm.as<uint32_t>());
+  B200_LAUNCH(h, k_iota<uint32_t>, grid_for(n_pieces, 4), kBlock, 0, perm.as<uint32_t>(), (int64_t)n_pieces);
   sort_pairs<uint32_t, uint32_t>(h, piece_key.as<uint32_t>(), piece_key2.as<uint32_t>(), perm.as<uint32_t>(),
                                  perm2.as<uint32_t>(), n_pieces, 0, bits_for(n_keys + 1));
   dbuf class_start = make_dbuf<int32_t>((size_t)n_keys + 1, h.stream);

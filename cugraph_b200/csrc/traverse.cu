@@ -9,9 +9,8 @@
 //  * the advance writes straight into per-vertex slots guarded by a visited bitmap (BFS) or an
 //    atomicMin on the distance word (SSSP); there is no emit-buffer + per-level radix sort/unique
 //    (transform_reduce_if_v_frontier_outgoing_e_by_dst.cuh:225-600).
-//  * load balance: a CTA scans the degrees of 256 frontier vertices and strides over the summed
-//    edge range (owner found by binary search in shared memory); vertices above kLargeDegree go to
-//    a second queue that the whole grid expands edge-parallel.
+//  * load balance: the merge-path advance (advance.cuh, DESIGN §3.4) cuts the summed edge range of a queue into tiles of
+//    equal size, whatever the mix of degrees; a CTA finds the queue entries of its tile and strides over its edges.
 //  * bottom-up BFS steps process 32 consecutive vertices per warp: one visited-word load, early
 //    exit on the first parent in the frontier bitmap (neighbours are sorted by internal id, i.e.
 //    hubs first), the next-frontier word is assembled with a ballot — no atomics.
@@ -30,12 +29,8 @@
 namespace b200 {
 namespace {
 
-inline int grid_for(int64_t n) { return (int)std::min<int64_t>(std::max<int64_t>((n + kBlock - 1) / kBlock, 1), 1 << 22); }
-
 struct frontier_counters_t {
   int n_small;              // entries appended to the next queue
-  int n_large;              // unused (kept for the layout of the 2-int reset)
-  int n_far;                // unused (kept for the layout)
   int n_conv;               // bitmap -> queue conversion cursor
   unsigned long long m_f;   // sum of degrees of the vertices appended (direction-optimising heuristic)
   unsigned long long packed;  // SSSP with 32-bit offsets: (sum of degrees << 32) | entries appended — ONE atomic per append
@@ -181,61 +176,56 @@ k_bfs_bottomup(O const* __restrict__ off, int32_t const* __restrict__ idx, uint3
 
 __global__ void k_queue_to_bitmap(int32_t const* __restrict__ q, int n, uint32_t* __restrict__ bm)
 {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) atomicOr(bm + (q[i] >> 5), 1u << (q[i] & 31));
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) atomicOr(bm + (q[i] >> 5), 1u << (q[i] & 31));
 }
 
 __global__ void k_bitmap_to_queue(uint32_t const* __restrict__ bm, int n_words, int32_t* __restrict__ q, int* counter)
 {
-  int w = blockIdx.x * blockDim.x + threadIdx.x;
-  uint32_t word = (w < n_words) ? bm[w] : 0u;
-  int c         = __popc(word);
-  // warp-level exclusive scan of counts, one atomic per warp
-  int lane = threadIdx.x & 31;
-  int incl = c;
+  // the whole CTA takes each step, so that every warp stays converged for its shuffles
+  for (int64_t w0 = blockIdx.x * (int64_t)blockDim.x; w0 < n_words; w0 += (int64_t)gridDim.x * blockDim.x) {
+    const int w   = (int)(w0 + threadIdx.x);
+    uint32_t word = (w < n_words) ? bm[w] : 0u;
+    int c         = __popc(word);
+    // warp-level exclusive scan of counts, one atomic per warp
+    int lane = threadIdx.x & 31;
+    int incl = c;
 #pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int y = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += y;
+    for (int o = 1; o < 32; o <<= 1) {
+      int y = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += y;
+    }
+    int total = __shfl_sync(0xffffffffu, incl, 31);
+    int base  = 0;
+    if (lane == 31 && total) base = atomicAdd(counter, total);
+    base = __shfl_sync(0xffffffffu, base, 31) + incl - c;
+    while (word) {
+      int b     = __ffs(word) - 1;
+      q[base++] = (w << 5) + b;
+      word &= word - 1;
+    }
   }
-  int total = __shfl_sync(0xffffffffu, incl, 31);
-  int base  = 0;
-  if (lane == 31 && total) base = atomicAdd(counter, total);
-  base = __shfl_sync(0xffffffffu, base, 31) + incl - c;
-  while (word) {
-    int b     = __ffs(word) - 1;
-    q[base++] = (w << 5) + b;
-    word &= word - 1;
-  }
-}
-
-template <typename T>
-__global__ void k_fill(T* a, int64_t n, T v)
-{
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) a[i] = v;
 }
 
 template <typename O>
 __global__ void k_bfs_seed(int32_t const* __restrict__ src, int n, uint32_t* visited, int32_t* dist, int32_t* q,
                            frontier_counters_t* cnt, O const* __restrict__ off)
 {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  int v        = src[i];
-  uint32_t bit = 1u << (v & 31);
-  uint32_t old = atomicOr(visited + (v >> 5), bit);
-  if (old & bit) return;  // duplicate source
-  dist[v]     = 0;
-  int pos     = atomicAdd(&cnt->n_small, 1);
-  q[pos]      = v;
-  unsigned d  = (unsigned)((long long)off[v + 1] - (long long)off[v]);
-  atomicAdd(&cnt->m_f, (unsigned long long)d);
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    int v        = src[i];
+    uint32_t bit = 1u << (v & 31);
+    uint32_t old = atomicOr(visited + (v >> 5), bit);
+    if (old & bit) continue;  // duplicate source
+    dist[v]     = 0;
+    int pos     = atomicAdd(&cnt->n_small, 1);
+    q[pos]      = v;
+    unsigned d  = (unsigned)((long long)off[v + 1] - (long long)off[v]);
+    atomicAdd(&cnt->m_f, (unsigned long long)d);
+  }
 }
 
 __global__ void k_widen_dist(int32_t const* in, int32_t n, int64_t* out)
 {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = in[i] == INT_MAX ? LLONG_MAX : (int64_t)in[i];
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = in[i] == INT_MAX ? LLONG_MAX : (int64_t)in[i];
 }
 
 template <typename O>
@@ -253,8 +243,8 @@ void run_bfs(handle_impl const& h, csx_t const& c, int32_t nv, int32_t const* so
   frontier_counters_t* dc = cnt.as<frontier_counters_t>();
   CUDA_TRY(cudaMemsetAsync(visited.data(), 0, sizeof(uint32_t) * n_words, h.stream));
   CUDA_TRY(cudaMemsetAsync(cnt.data(), 0, sizeof(frontier_counters_t), h.stream));
-  B200_LAUNCH(h, (k_fill<int32_t>), std::min(grid_for(nv), h.sm_count * 32), kBlock, 0, dist, (int64_t)nv, INT_MAX);
-  if (pred) B200_LAUNCH(h, (k_fill<int32_t>), std::min(grid_for(nv), h.sm_count * 32), kBlock, 0, pred, (int64_t)nv, -1);
+  B200_LAUNCH(h, (k_fill<int32_t>), grid_for(nv, 1, h.sm_count * 32), kBlock, 0, dist, (int64_t)nv, INT_MAX);
+  if (pred) B200_LAUNCH(h, (k_fill<int32_t>), grid_for(nv, 1, h.sm_count * 32), kBlock, 0, pred, (int64_t)nv, -1);
   B200_LAUNCH(h, (k_bfs_seed<O>), grid_for(n_sources), kBlock, 0, sources, n_sources, visited.as<uint32_t>(), dist,
               qa.as<int32_t>(), dc, off);
   frontier_counters_t* hc = reinterpret_cast<frontier_counters_t*>(h.pinned);
@@ -301,7 +291,7 @@ void run_bfs(handle_impl const& h, csx_t const& c, int32_t nv, int32_t const* so
         if (n_f > 0) B200_LAUNCH(h, k_queue_to_bitmap, grid_for(n_f), kBlock, 0, cur, n_f, fbm.as<uint32_t>());
         frontier_is_bitmap = true;
       }
-      int grid = std::min(grid_for((int64_t)n_words * 32), h.sm_count * 16);
+      int grid = grid_for((int64_t)n_words * 32, 1, h.sm_count * 16);
       B200_LAUNCH(h, (k_bfs_bottomup<O>), grid, kBlock, 0, off, idx, visited.as<uint32_t>(), fbm.as<uint32_t>(),
                   nbm.as<uint32_t>(), dist, pred, level, nv, dc);
       std::swap(fbm, nbm);
@@ -375,11 +365,11 @@ struct dist_packed {
 
 __global__ void k_unpack_dist(unsigned long long const* __restrict__ p, int n, float* __restrict__ dist, int32_t* __restrict__ pred)
 {
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= n) return;
-  const unsigned long long x = p[v];
-  dist[v]                    = __uint_as_float((unsigned)(x >> 32));
-  pred[v]                    = (int32_t)(unsigned)(x & 0xffffffffu);
+  for (int64_t v = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; v < n; v += (int64_t)gridDim.x * blockDim.x) {
+    const unsigned long long x = p[v];
+    dist[v]                    = __uint_as_float((unsigned)(x >> 32));
+    pred[v]                    = (int32_t)(unsigned)(x & 0xffffffffu);
+  }
 }
 
 template <typename O, typename T, typename DA>
@@ -519,12 +509,12 @@ __global__ void k_split_near(O const* __restrict__ off, int32_t const* __restric
                              T hi, int32_t* stamp, int round, int32_t* near_out, int32_t* near_deg_out,
                              frontier_counters_t* cnt)
 {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int v = q_in[i];
-  if (dist.get(v) < hi) {
-    stamp[v] = round;
-    enqueue_counted(off, v, near_out, near_deg_out, cnt);
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int v = q_in[i];
+    if (dist.get(v) < hi) {
+      stamp[v] = round;
+      enqueue_counted(off, v, near_out, near_deg_out, cnt);
+    }
   }
 }
 
@@ -784,10 +774,7 @@ void sssp_windows(handle_impl const& h, csx_t const& c, int32_t nv, int32_t sour
   dbuf wsum = make_dbuf<double>(2, h.stream);
   CUDA_TRY(cudaMemsetAsync(wsum.data(), 0, 2 * sizeof(double), h.stream));
   B200_LAUNCH(h, (k_sum_weights<T>), h.sm_count * 8, kBlock, 0, w, (long long)c.nnz, wsum.as<double>());
-  double hsum = 0.0;
-  CUDA_TRY(cudaMemcpyAsync(&hsum, wsum.data(), sizeof(double), cudaMemcpyDeviceToHost, h.stream));
-  sync(h);
-  const double avg_w   = hsum / (double)c.nnz;
+  const double avg_w   = read_back(h, wsum.as<double>()) / (double)c.nnz;
   const double avg_deg = (double)c.nnz / (double)nv;
   const double delta_scale = h.tune.sssp_delta_scale;  // tuning knob (results do not depend on it)
   T delta = (T)(32.0 * avg_w / std::max(avg_deg, 1e-30) * delta_scale);
@@ -825,14 +812,10 @@ void sssp_windows(handle_impl const& h, csx_t const& c, int32_t nv, int32_t sour
   int32_t *near_deg = la.as<int32_t>(), *next_near_deg = lb.as<int32_t>();  // degrees of the queue entries
   int n_near = 1, round = 1, window = 1;
   // the seed kernel wrote the source's degree next to it: read it back (the first advance needs the edge count)
-  int32_t seed_deg = 0;
-  CUDA_TRY(cudaMemcpyAsync(&seed_deg, near_deg, sizeof(int32_t), cudaMemcpyDeviceToHost, h.stream));
-  sync(h);
-  unsigned long long near_edges = (unsigned long long)(unsigned)seed_deg;
+  unsigned long long near_edges = (unsigned long long)(unsigned)read_back(h, near_deg);
   advance_scratch_t adv;
   adv.init(h, nv, (int64_t)c.nnz);
   T lo = (T)0, hi = delta;
-  const int full_grid = h.sm_count * 8;
   const bool trace    = h.tune.sssp_trace;
   unsigned long long tr_edges = 0;
   int tr_rounds = 0, tr_splits = 0;
@@ -911,12 +894,12 @@ void sssp_windows(handle_impl const& h, csx_t const& c, int32_t nv, int32_t sour
     *hmin_pinned = inf;
     CUDA_TRY(cudaMemcpyAsync(dwin.data(), hwin, sizeof(sssp_window_t<T>), cudaMemcpyHostToDevice, h.stream));
     CUDA_TRY(cudaMemcpyAsync(dmin.data(), hmin_pinned, sizeof(T), cudaMemcpyHostToDevice, h.stream));
-    B200_LAUNCH(h, (k_min_beyond<T, DA>), std::min(grid_for(nv), h.sm_count * 64), kBlock, 0, dist, nv, hi, unreached, dmin.as<T>());
+    B200_LAUNCH(h, (k_min_beyond<T, DA>), grid_for(nv, 1, h.sm_count * 64), kBlock, 0, dist, nv, hi, unreached, dmin.as<T>());
     B200_LAUNCH(h, (k_next_window<T>), 1, 1, 0, dmin.as<T>(), delta, dwin.as<sssp_window_t<T>>());
     ++round;
     ++window;
     CUDA_TRY(cudaMemsetAsync(cnt.data(), 0, sizeof(frontier_counters_t), h.stream));
-    B200_LAUNCH(h, (k_select_window<O, T, DA>), std::min(grid_for((nv + kSelectPer - 1) / kSelectPer), h.sm_count * 8), kBlock, 0, off, dist, nv, dwin.as<sssp_window_t<T>>(),
+    B200_LAUNCH(h, (k_select_window<O, T, DA>), grid_for(nv, kSelectPer, h.sm_count * 8), kBlock, 0, off, dist, nv, dwin.as<sssp_window_t<T>>(),
                 stamp.as<int32_t>(), round, near, near_deg, dc);
     CUDA_TRY(cudaMemcpyAsync(hc, cnt.data(), sizeof(frontier_counters_t), cudaMemcpyDeviceToHost, h.stream));
     CUDA_TRY(cudaMemcpyAsync(hwin, dwin.data(), sizeof(sssp_window_t<T>), cudaMemcpyDeviceToHost, h.stream));
@@ -936,23 +919,22 @@ void run_sssp(handle_impl const& h, csx_t const& c, int32_t nv, int32_t source, 
   int32_t const* idx = c.indices.as<int32_t>();
   T const* w         = c.weights.as<T>();
   const T unreached  = std::numeric_limits<T>::max();
-  const int full_grid = h.sm_count * 8;
-  if (pred) B200_LAUNCH(h, (k_fill<int32_t>), std::min(grid_for(nv), h.sm_count * 32), kBlock, 0, pred, (int64_t)nv, -1);
+  if (pred) B200_LAUNCH(h, (k_fill<int32_t>), grid_for(nv, 1, h.sm_count * 32), kBlock, 0, pred, (int64_t)nv, -1);
   if (c.nnz == 0) {
-    B200_LAUNCH(h, (k_fill<T>), std::min(grid_for(nv), h.sm_count * 32), kBlock, 0, dist, (int64_t)nv, unreached);
+    B200_LAUNCH(h, (k_fill<T>), grid_for(nv, 1, h.sm_count * 32), kBlock, 0, dist, (int64_t)nv, unreached);
     B200_LAUNCH(h, (k_fill<T>), 1, 1, 0, dist + source, (int64_t)1, (T)0);
     return;
   }
   if (pred && std::is_same<T, float>::value) {  // float with predecessors: (distance, predecessor) in one word
     dbuf packed = make_dbuf<unsigned long long>(nv, h.stream);
-    B200_LAUNCH(h, (k_fill<unsigned long long>), std::min(grid_for(nv), h.sm_count * 32), kBlock, 0, packed.as<unsigned long long>(),
+    B200_LAUNCH(h, (k_fill<unsigned long long>), grid_for(nv, 1, h.sm_count * 32), kBlock, 0, packed.as<unsigned long long>(),
                 (int64_t)nv, dist_packed::pack(0x7f7fffffu, -1));
     sssp_windows<O, float, dist_packed>(h, c, nv, source, cutoff_d, dist_packed{packed.as<unsigned long long>()});
     B200_LAUNCH(h, k_unpack_dist, grid_for(nv), kBlock, 0, packed.as<unsigned long long>(), nv, reinterpret_cast<float*>(dist), pred);
     check_last("sssp");
     return;
   }
-  B200_LAUNCH(h, (k_fill<T>), std::min(grid_for(nv), h.sm_count * 32), kBlock, 0, dist, (int64_t)nv, unreached);
+  B200_LAUNCH(h, (k_fill<T>), grid_for(nv, 1, h.sm_count * 32), kBlock, 0, dist, (int64_t)nv, unreached);
   sssp_windows<O, T, dist_plain<T>>(h, c, nv, source, cutoff_d, dist_plain<T>{dist});
   if (pred) {
     if (sizeof(O) == 4) {
@@ -965,7 +947,7 @@ void run_sssp(handle_impl const& h, csx_t const& c, int32_t nv, int32_t source, 
     dbuf flags = make_dbuf<int>(2, h.stream);
     int* hflags = reinterpret_cast<int*>(reinterpret_cast<char*>(h.pinned) + 512);
     CUDA_TRY(cudaMemsetAsync(flags.data(), 0, 2 * sizeof(int), h.stream));
-    B200_LAUNCH(h, (k_sssp_count_orphans<T>), std::min(grid_for(nv), full_grid), kBlock, 0, dist, pred, nv, source, unreached,
+    B200_LAUNCH(h, (k_sssp_count_orphans<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, dist, pred, nv, source, unreached,
                 flags.as<int>());
     CUDA_TRY(cudaMemcpyAsync(hflags, flags.data(), 2 * sizeof(int), cudaMemcpyDeviceToHost, h.stream));
     sync(h);
@@ -1015,37 +997,37 @@ __global__ void k_scatter_to_internal(int32_t const* __restrict__ int_of_pos, D 
                                       int32_t const* __restrict__ pred_int_pos, int32_t n, long long* __restrict__ dist_int,
                                       int32_t* __restrict__ pred_int)
 {
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= n) return;
-  const int v = int_of_pos[p];
-  if (v < 0) return;
-  dist_int[v] = (long long)dist_pos[p];
-  pred_int[v] = pred_int_pos[p];
+  for (int64_t p = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; p < n; p += (int64_t)gridDim.x * blockDim.x) {
+    const int v = int_of_pos[p];
+    if (v < 0) continue;
+    dist_int[v] = (long long)dist_pos[p];
+    pred_int[v] = pred_int_pos[p];
+  }
 }
 
 __global__ void k_paths_max_len(int32_t const* __restrict__ dest, int32_t n_dest, long long const* __restrict__ dist,
                                 int32_t const* __restrict__ pred, int32_t nv, long long unreachable, long long* __restrict__ out)
 {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_dest) return;
-  const int v = dest[i];
-  if (v < 0 || v >= nv || pred[v] < 0 || dist[v] >= unreachable) return;
-  atomicMax(reinterpret_cast<unsigned long long*>(out), (unsigned long long)dist[v]);
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n_dest; i += (int64_t)gridDim.x * blockDim.x) {
+    const int v = dest[i];
+    if (v < 0 || v >= nv || pred[v] < 0 || dist[v] >= unreachable) continue;
+    atomicMax(reinterpret_cast<unsigned long long*>(out), (unsigned long long)dist[v]);
+  }
 }
 
 __global__ void k_paths_walk(int32_t const* __restrict__ dest, int32_t n_dest, long long const* __restrict__ dist,
                              int32_t const* __restrict__ pred, int32_t nv, long long unreachable, long long len,
                              int32_t* __restrict__ paths)
 {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_dest) return;
-  int v = dest[i];
-  if (v < 0 || v >= nv) return;
-  long long d = dist[v];
-  if (d >= unreachable || d >= len) return;  // not reached: the row stays invalid
-  for (; d >= 0 && v >= 0; --d) {
-    paths[(long long)i * len + d] = v;
-    v = pred[v];
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n_dest; i += (int64_t)gridDim.x * blockDim.x) {
+    int v = dest[i];
+    if (v < 0 || v >= nv) continue;
+    long long d = dist[v];
+    if (d >= unreachable || d >= len) continue;  // not reached: the row stays invalid
+    for (; d >= 0 && v >= 0; --d) {
+      paths[i * len + d] = v;
+      v = pred[v];
+    }
   }
 }
 
@@ -1090,7 +1072,6 @@ cugraph_error_code_t cugraph_bfs(const cugraph_resource_handle_t* handle, cugrap
     B200_EXPECTS(sources != nullptr, CUGRAPH_INVALID_INPUT, "sources is NULL");
     auto const* s = V(sources);
     B200_EXPECTS(s->type == g->vertex_type, CUGRAPH_INVALID_INPUT, "vertex type of graph and sources must match");
-    B200_EXPECTS(g->mg == nullptr, CUGRAPH_NOT_IMPLEMENTED, "multi-GPU BFS is not implemented");
     B200_EXPECTS(g->is_symmetric || direction_optimizing == FALSE, CUGRAPH_UNKNOWN_ERROR,
                  "Invalid input argument: input graph should be symmetric for direction optimizing BFS.");
     const int32_t nv = g->n_vertices;
@@ -1142,7 +1123,6 @@ cugraph_error_code_t cugraph_sssp(const cugraph_resource_handle_t* handle, cugra
     auto* g       = G(graph);
     B200_EXPECTS(result != nullptr, CUGRAPH_INVALID_INPUT, "result out-pointer is NULL");
     *result = nullptr;
-    B200_EXPECTS(g->mg == nullptr, CUGRAPH_NOT_IMPLEMENTED, "multi-GPU SSSP is not implemented");
     B200_EXPECTS(g->weighted, CUGRAPH_INVALID_INPUT, "SSSP requires a weighted graph");
     const int32_t nv = g->n_vertices;
     // external source id -> internal
@@ -1152,9 +1132,7 @@ cugraph_error_code_t cugraph_sssp(const cugraph_resource_handle_t* handle, cugra
     if (g->vertex_type == INT64) CUDA_TRY(cudaMemcpyAsync(src_ext.data(), &s64, 8, cudaMemcpyHostToDevice, h.stream));
     else CUDA_TRY(cudaMemcpyAsync(src_ext.data(), &s32, 4, cudaMemcpyHostToDevice, h.stream));
     ext_to_int(h, *g, src_ext.data(), 1, src_int.as<int32_t>());
-    int32_t src = -1;
-    CUDA_TRY(cudaMemcpyAsync(&src, src_int.data(), sizeof(int32_t), cudaMemcpyDeviceToHost, h.stream));
-    sync(h);
+    const int32_t src = read_back(h, src_int.as<int32_t>());
     B200_EXPECTS(src >= 0 && (g->vertex_type == INT64 || source <= (size_t)INT_MAX), CUGRAPH_INVALID_INPUT,
                  "Invalid input argument: source vertex is invalid.");
     csx_t const& c = push_view(h, *g);
@@ -1231,10 +1209,7 @@ cugraph_error_code_t cugraph_extract_paths(const cugraph_resource_handle_t* hand
     if (nd > 0)
       B200_LAUNCH(h, k_paths_max_len, grid_for((int64_t)nd), kBlock, 0, dest_int.as<int32_t>(), (int32_t)nd, dist_int.as<long long>(),
                   pred_int.as<int32_t>(), nv, unreachable, d_max.as<long long>());
-    long long hmax = 0;
-    CUDA_TRY(cudaMemcpyAsync(&hmax, d_max.data(), sizeof(long long), cudaMemcpyDeviceToHost, h.stream));
-    sync(h);
-    const long long len = hmax + 1;
+    const long long len = read_back(h, d_max.as<long long>()) + 1;
     const size_t total  = nd * (size_t)len;
     dbuf paths_int      = make_dbuf<int32_t>(std::max<size_t>(total, 1), h.stream);
     if (total > 0) {
