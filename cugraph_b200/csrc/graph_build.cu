@@ -310,17 +310,7 @@ __global__ void k_copy_cast(void const* in, cugraph_data_type_id_t in_type, int6
   }
 }
 
-// ---------------------------------------------------------------- CUB wrappers
-template <typename K>
-void sort_keys(handle_impl const& h, K const* in, K* out, int64_t n, int begin_bit, int end_bit)
-{
-  size_t bytes = 0;
-  CUDA_TRY(cub::DeviceRadixSort::SortKeys(nullptr, bytes, in, out, n, begin_bit, end_bit, h.stream));
-  dbuf tmp(bytes, h.stream);
-  CUDA_TRY(cub::DeviceRadixSort::SortKeys(tmp.data(), bytes, in, out, n, begin_bit, end_bit, h.stream));
-  h.launches += 4;
-}
-
+// ---------------------------------------------------------------- CUB wrappers (sort_keys: staging.cuh)
 template <typename T>
 int64_t unique_sorted(handle_impl const& h, T const* in, T* out, int64_t n)
 {

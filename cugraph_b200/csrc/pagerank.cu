@@ -8,6 +8,7 @@
 // `done` flag between batches; kernels of iterations past convergence are no-ops, so the iteration
 // count and result are exactly those of a check-every-iteration loop.
 #include "graph.cuh"
+#include "staging.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -84,6 +85,13 @@ __global__ void k_personalize(int32_t const* __restrict__ pv, T const* __restric
     y[pv[i]] = (T)((double)y[pv[i]] + st->pers_scale * ((double)pvals[i] / pers_sum));
 }
 
+// entries equal to their predecessor in a sorted array
+__global__ void k_count_repeats(int32_t const* __restrict__ sorted, int32_t n, int* __restrict__ out)
+{
+  for (int64_t i = 1 + blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    if (sorted[i] == sorted[i - 1]) atomicAdd(out, 1);
+}
+
 template <typename T>
 __global__ void k_sum(T const* a, int32_t n, double* out)
 {
@@ -157,6 +165,13 @@ void pagerank_typed(handle_impl const& h, graph_impl& g, pr_args const& a, centr
     out_w = c.out_w.as<T>();
   }
   tr.mark("pagerank: pull view + out-weights");
+  // the expensive input checks of pagerank_impl.cuh:90-175, in its order
+  if (a.expensive && a.pre_w) {
+    dbuf neg = make_dbuf<int>(1, h.stream);
+    CUDA_TRY(cudaMemsetAsync(neg.data(), 0, sizeof(int), h.stream));
+    B200_LAUNCH(h, (k_count_negative<T>), grid_for(nv), kBlock, 0, out_w, (int64_t)nv, neg.as<int>());
+    B200_EXPECTS(read_back(h, neg.as<int>()) == 0, CUGRAPH_UNKNOWN_ERROR, "Invalid input argument: outgoing edge weight sum values should be non-negative.");
+  }
   if (a.expensive && weighted && c.nnz > 0) {
     dbuf neg = make_dbuf<int>(1, h.stream);
     CUDA_TRY(cudaMemsetAsync(neg.data(), 0, sizeof(int), h.stream));
@@ -176,17 +191,31 @@ void pagerank_typed(handle_impl const& h, graph_impl& g, pr_args const& a, centr
     n_pers   = (int32_t)a.pers_v->size;
     pers_idx = make_dbuf<int32_t>(n_pers, h.stream);
     ext_to_int(h, g, a.pers_v->data, n_pers, pers_idx.as<int32_t>());
-    struct pers_check_t {  // both read back with one copy
+    struct pers_check_t {  // all read back with one copy
       double sum;
       int n_invalid;
+      int n_negative;   // the expensive check only, as the two below
+      int n_repeated;
     };
     dbuf chk = make_dbuf<pers_check_t>(1, h.stream);
     auto* dchk = chk.as<pers_check_t>();
     CUDA_TRY(cudaMemsetAsync(dchk, 0, sizeof(pers_check_t), h.stream));
     B200_LAUNCH(h, (k_count_negative<int32_t>), grid_for(n_pers), kBlock, 0, pers_idx.as<int32_t>(), (int64_t)n_pers, &dchk->n_invalid);
     B200_LAUNCH(h, (k_sum<T>), grid_for(n_pers, 1, 1024), kBlock, 0, (T const*)a.pers_val->data, n_pers, &dchk->sum);
+    dbuf sorted;
+    if (a.expensive) {
+      B200_LAUNCH(h, (k_count_negative<T>), grid_for(n_pers), kBlock, 0, (T const*)a.pers_val->data, (int64_t)n_pers,
+                  &dchk->n_negative);
+      // without this check a repeated vertex reaches k_personalize, whose read-modify-writes of y then race
+      sorted = make_dbuf<int32_t>(n_pers, h.stream);
+      sort_keys<int32_t>(h, pers_idx.as<int32_t>(), sorted.as<int32_t>(), n_pers, 0, 32);
+      B200_LAUNCH(h, k_count_repeats, grid_for(n_pers), kBlock, 0, sorted.as<int32_t>(), n_pers, &dchk->n_repeated);
+    }
     const pers_check_t hchk = read_back(h, dchk);
     B200_EXPECTS(hchk.n_invalid == 0, CUGRAPH_INVALID_INPUT, "Invalid input argument: peresonalization vertices have invalid vertex IDs.");
+    B200_EXPECTS(hchk.n_negative == 0, CUGRAPH_UNKNOWN_ERROR, "Invalid input argument: peresonalization values should be non-negative.");
+    B200_EXPECTS(hchk.n_repeated == 0, CUGRAPH_UNKNOWN_ERROR,
+                 "Invalid input argument: personalization vertices should not contain duplicate entries.");
     pers_sum = hchk.sum;
     B200_EXPECTS(pers_sum > 0.0, CUGRAPH_UNKNOWN_ERROR, "Invalid input argument: sum of personalization valuese should be positive.");
   }

@@ -1,4 +1,5 @@
-// CUB wrappers of the one-time staging passes, shared by graph_build.cu and sweep_layout.cu.  Everything
+// CUB wrappers of the one-time staging passes, shared by graph_build.cu and sweep_layout.cu (and PageRank's expensive input
+// check, pagerank.cu).  Everything
 // lives in an anonymous namespace, as in advance.cuh: every translation unit gets its own instantiations.
 #pragma once
 #include "common.cuh"
@@ -8,6 +9,16 @@
 
 namespace b200 {
 namespace {
+
+template <typename K>
+void sort_keys(handle_impl const& h, K const* in, K* out, int64_t n, int begin_bit, int end_bit)
+{
+  size_t bytes = 0;
+  CUDA_TRY(cub::DeviceRadixSort::SortKeys(nullptr, bytes, in, out, n, begin_bit, end_bit, h.stream));
+  dbuf tmp(bytes, h.stream);
+  CUDA_TRY(cub::DeviceRadixSort::SortKeys(tmp.data(), bytes, in, out, n, begin_bit, end_bit, h.stream));
+  h.launches += 4;
+}
 
 template <typename K, typename Val>
 void sort_pairs(handle_impl const& h, K const* kin, K* kout, Val const* vin, Val* vout, int64_t n, int begin_bit, int end_bit)
