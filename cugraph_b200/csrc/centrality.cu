@@ -1,11 +1,13 @@
 // Katz centrality and HITS on the pull sweep — the sibling algorithms that run on the same primitive as PageRank
 // (per_v_transform_reduce_incoming_e / _outgoing_e with reduce_op::plus; reference cpp/src/centrality/katz_centrality_impl.cuh:34-196,
-// cpp/src/link_analysis/hits_impl.cuh:29-206, C API cpp/src/c_api/katz.cpp, cpp/src/c_api/hits.cpp).  Both are host loops
-// over pull_sweep (sweep.cu: the shared-memory piece stream when the graph has one) plus small vector passes; their
-// per-iteration convergence test reads one scalar back, as the reference does.
+// cpp/src/link_analysis/hits_impl.cuh:29-206, C API cpp/src/c_api/katz.cpp, cpp/src/c_api/hits.cpp).  Each is a host loop
+// over pull_sweep (sweep.cu: the shared-memory piece stream when the graph has one) and the owner-step kernels of
+// centrality_ops.cuh over all vertices: the single-GPU form of its MGGraph loop (mg.py), without the collectives.  Each
+// iteration reads its scalars back once, for the convergence test.
 #include "centrality_ops.cuh"
 #include "graph.cuh"
 
+#include <array>
 #include <cmath>
 #include <limits>
 
@@ -25,22 +27,23 @@ void katz_typed(handle_impl const& h, graph_impl& g, double alpha, double beta, 
   dbuf x = make_sweep_x<T>(h, nv), y = make_dbuf<T>(std::max(nv, 1), h.stream);  // x: zeros (katz_centrality_impl.cuh:88-93)
   sweep_scratch_t sc;
   sc.init(h, c);
+  // the sweep adds beta before its one rounding to T (adding it in the step would round twice), so the step adds 0
   sc.set_init(h, beta);
-  dbuf d_diff = make_dbuf<double>(1, h.stream);
-  size_t iter = 0;
+  dbuf d2      = make_dbuf<double>(2, h.stream);  // diff, sum x^2
+  size_t iter  = 0;
+  double sumsq = 0.0;
   while (nv > 0) {
     pull_sweep<T>(h, c, nv, x.as<T>(), y.as<T>(), sc, alpha);
-    CUDA_TRY(cudaMemsetAsync(d_diff.data(), 0, sizeof(double), h.stream));
-    B200_LAUNCH(h, (k_abs_diff<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, y.as<T>(), x.as<T>(), nv, 1, d_diff.as<double>());
-    const double diff = read_back(h, d_diff.as<double>());
+    CUDA_TRY(cudaMemsetAsync(d2.data(), 0, 2 * sizeof(double), h.stream));
+    B200_LAUNCH(h, (k_katz_step<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, y.as<T>(), x.as<T>(), nv, 0.0, d2.as<double>());
+    const std::array<double, 2> r = read_back(h, d2.as<std::array<double, 2>>());
+    sumsq                         = r[1];
     ++iter;
-    if ((T)diff < (T)epsilon) break;
+    if ((T)r[0] < (T)epsilon) break;
     B200_EXPECTS(iter < max_iterations, CUGRAPH_UNKNOWN_ERROR, "Katz Centrality failed to converge.");
   }
-  if (nv > 0) {  // x holds the final values (copied by k_abs_diff)
-    CUDA_TRY(cudaMemsetAsync(d_diff.data(), 0, sizeof(double), h.stream));
-    B200_LAUNCH(h, (k_norm<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, x.as<T>(), nv, 0, d_diff.as<double>());
-    const double l2 = std::sqrt(read_back(h, d_diff.as<double>()));
+  if (nv > 0) {  // x holds the final values, and sumsq their sum of squares (from the last step)
+    const double l2 = std::sqrt(sumsq);
     B200_EXPECTS(l2 > 0.0, CUGRAPH_UNKNOWN_ERROR, "L2 norm of the computed Katz Centrality values should be positive.");
     B200_LAUNCH(h, (k_scale<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, x.as<T>(), nv, 1.0 / l2);
   }
@@ -65,18 +68,15 @@ void eigenvector_typed(handle_impl const& h, graph_impl& g, double epsilon, size
   if (nv > 0) B200_LAUNCH(h, (k_fill<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, x.as<T>(), (int64_t)nv, (T)(1.0 / (double)nv));
   sweep_scratch_t sc;
   sc.init(h, c);
-  dbuf d2     = make_dbuf<double>(2, h.stream);
+  dbuf d2     = make_dbuf<double>(2, h.stream);  // sum y^2, diff
   size_t iter = 0;
   while (nv > 0) {
     pull_sweep<T>(h, c, nv, x.as<T>(), y.as<T>(), sc, 1.0);
-    B200_LAUNCH(h, (k_add_vec<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, y.as<T>(), x.as<T>(), nv);
     CUDA_TRY(cudaMemsetAsync(d2.data(), 0, 2 * sizeof(double), h.stream));
-    B200_LAUNCH(h, (k_norm<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, y.as<T>(), nv, 0, d2.as<double>());
-    const double hyp = std::sqrt(read_back(h, d2.as<double>()));
-    B200_LAUNCH(h, (k_scale<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, y.as<T>(), nv, 1.0 / hyp);
-    CUDA_TRY(cudaMemsetAsync(d2.data(), 0, sizeof(double), h.stream));
-    B200_LAUNCH(h, (k_abs_diff<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, y.as<T>(), x.as<T>(), nv, 1, d2.as<double>());
-    const double diff = read_back(h, d2.as<double>());
+    B200_LAUNCH(h, (k_eig_add<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, y.as<T>(), x.as<T>(), nv, d2.as<double>());
+    B200_LAUNCH(h, (k_eig_scale<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, y.as<T>(), x.as<T>(), nv, d2.as<double>(),
+                d2.as<double>() + 1);
+    const double diff = read_back(h, d2.as<double>() + 1);
     ++iter;
     if ((T)diff < (T)nv * (T)epsilon) break;
     B200_EXPECTS(iter < max_iterations, CUGRAPH_UNKNOWN_ERROR, "Eigenvector Centrality failed to converge.");
@@ -101,12 +101,13 @@ struct hits_result_impl {
   size_t number_of_iterations{0};
 };
 
+// v /= sum v (the initial guess, and both results with `normalize`)
 template <typename T>
-void normalize_by(handle_impl const& h, T* v, int32_t nv, int mode, dbuf& d2)
+void normalize_by(handle_impl const& h, T* v, int32_t nv, dbuf& d)
 {
-  CUDA_TRY(cudaMemsetAsync(d2.data(), 0, 2 * sizeof(double), h.stream));
-  B200_LAUNCH(h, (k_norm<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, v, nv, mode, d2.as<double>());
-  const double norm = read_back(h, d2.as<double>() + (mode == 2 ? 1 : 0));
+  CUDA_TRY(cudaMemsetAsync(d.data(), 0, sizeof(double), h.stream));
+  B200_LAUNCH(h, (k_norm<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, v, nv, 1, d.as<double>());
+  const double norm = read_back(h, d.as<double>());
   B200_EXPECTS((T)norm > (T)0, CUGRAPH_UNKNOWN_ERROR, "Norm is required to be a positive value.");
   B200_LAUNCH(h, (k_scale<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, v, nv, 1.0 / norm);
 }
@@ -119,7 +120,7 @@ void hits_typed(handle_impl const& h, graph_impl& g, double epsilon, size_t max_
   csx_t const& c_in  = pull_view(h, g);       // rows = destinations: authorities <- hubs
   csx_t const& c_out = out_sweep_view(h, g);  // rows = sources: hubs <- authorities
   dbuf hubs_a = make_sweep_x<T>(h, nv), hubs_b = make_sweep_x<T>(h, nv), auth = make_sweep_x<T>(h, nv);
-  dbuf d2 = make_dbuf<double>(2, h.stream);
+  dbuf d3 = make_dbuf<double>(3, h.stream);  // hub max, authority max, diff
   B200_EXPECTS(epsilon >= 0.0, CUGRAPH_INVALID_INPUT, "Invalid input argument: epsilon should be non-negative.");
   double diff = std::numeric_limits<T>::max();
   size_t iter = max_iterations;
@@ -134,7 +135,7 @@ void hits_typed(handle_impl const& h, graph_impl& g, double epsilon, size_t max_
         B200_LAUNCH(h, (k_count_negative<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, hubs_a.as<T>(), (int64_t)nv, neg.as<int>());
         B200_EXPECTS(read_back(h, neg.as<int>()) == 0, CUGRAPH_INVALID_INPUT, "Invalid input argument: initial guess values should be non-negative.");
       }
-      normalize_by<T>(h, hubs_a.as<T>(), nv, 1, d2);
+      normalize_by<T>(h, hubs_a.as<T>(), nv, d3);
     } else {
       B200_LAUNCH(h, (k_fill<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, hubs_a.as<T>(), (int64_t)nv, (T)(1.0 / (double)nv));
     }
@@ -147,19 +148,21 @@ void hits_typed(handle_impl const& h, graph_impl& g, double epsilon, size_t max_
     while (true) {
       pull_sweep<T>(h, c_in, nv, prev, auth.as<T>(), sc_in, 1.0, false);
       pull_sweep<T>(h, c_out, nv, auth.as<T>(), curr, sc_out, 1.0, false);
-      normalize_by<T>(h, curr, nv, 2, d2);
-      normalize_by<T>(h, auth.as<T>(), nv, 2, d2);
-      CUDA_TRY(cudaMemsetAsync(d2.data(), 0, sizeof(double), h.stream));
-      B200_LAUNCH(h, (k_abs_diff<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, curr, prev, nv, 0, d2.as<double>());
-      diff = (double)(T)read_back(h, d2.as<double>());
+      CUDA_TRY(cudaMemsetAsync(d3.data(), 0, 3 * sizeof(double), h.stream));
+      B200_LAUNCH(h, (k_hits_max<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, curr, auth.as<T>(), nv, d3.as<double>());
+      B200_LAUNCH(h, (k_hits_scale<T>), grid_for(nv, 1, h.sm_count * 8), kBlock, 0, curr, auth.as<T>(), prev, nv, d3.as<double>(),
+                  d3.as<double>() + 2);
+      const std::array<double, 3> r = read_back(h, d3.as<std::array<double, 3>>());
+      B200_EXPECTS((T)r[0] > (T)0 && (T)r[1] > (T)0, CUGRAPH_UNKNOWN_ERROR, "Norm is required to be a positive value.");
+      diff = (double)(T)r[2];
       std::swap(prev, curr);
       ++iter;
       if ((T)diff < tolerance) break;
       B200_EXPECTS(iter < max_iterations, CUGRAPH_UNKNOWN_ERROR, "HITS failed to converge.");
     }
     if (normalize) {
-      normalize_by<T>(h, prev, nv, 1, d2);
-      normalize_by<T>(h, auth.as<T>(), nv, 1, d2);
+      normalize_by<T>(h, prev, nv, d3);
+      normalize_by<T>(h, auth.as<T>(), nv, d3);
     }
     res.hubs        = new device_array_impl{to_reported_order(h, g, prev, sizeof(T)), (size_t)nv, g.weight_type};
     res.authorities = new device_array_impl{to_reported_order(h, g, auth.data(), sizeof(T)), (size_t)nv, g.weight_type};

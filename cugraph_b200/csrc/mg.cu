@@ -91,98 +91,6 @@ k_mg_vertex_step(T const* __restrict__ y, T* __restrict__ pr, T const* __restric
   }
 }
 
-// ---- owner steps of the multi-GPU Katz, eigenvector and HITS iterations over this rank's n_local slice.  Each adds its
-// partial scalars into a device double[] that the launcher all-reduces; the arithmetic is that of the single-GPU drivers
-// (centrality.cu) through the same helpers (centrality_ops.cuh), with their passes fused.
-
-// Katz: x_new = y + beta (y carries alpha from the sweep) ; out[0] += sum |x_new - x| ; out[1] += sum x_new^2 ; x = x_new
-template <typename T>
-__global__ void __launch_bounds__(kBlock)
-k_katz_step(T const* __restrict__ y, T* __restrict__ x, int32_t n, double beta, double* __restrict__ out)
-{
-  __shared__ double smem[kBlock / 32];
-  double d = 0.0, s = 0.0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const T nv = (T)((double)y[i] + beta);
-    d += fabs((double)nv - (double)x[i]);
-    s += (double)nv * (double)nv;
-    x[i] = nv;
-  }
-  d = block_sum(d, smem);
-  s = block_sum(s, smem);
-  if (threadIdx.x == 0) {
-    if (d != 0.0) atomicAdd(out, d);
-    if (s != 0.0) atomicAdd(out + 1, s);
-  }
-}
-
-// eigenvector, first half: y += x ; out[0] += sum y^2   (k_add_vec + k_norm mode 0)
-template <typename T>
-__global__ void __launch_bounds__(kBlock) k_eig_add(T* __restrict__ y, T const* __restrict__ x, int32_t n, double* __restrict__ out)
-{
-  __shared__ double smem[kBlock / 32];
-  double s = 0.0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const T v = y[i] + x[i];
-    y[i]      = v;
-    s += (double)v * (double)v;
-  }
-  s = block_sum(s, smem);
-  if (threadIdx.x == 0 && s != 0.0) atomicAdd(out, s);
-}
-
-// eigenvector, second half: y *= 1 / sqrt(sumsq[0]) ; out[0] += sum |y - x| ; x = y   (k_scale + k_abs_diff)
-template <typename T>
-__global__ void __launch_bounds__(kBlock)
-k_eig_scale(T* __restrict__ y, T* __restrict__ x, int32_t n, double const* __restrict__ sumsq, double* __restrict__ out)
-{
-  __shared__ double smem[kBlock / 32];
-  const double inv = 1.0 / sqrt(sumsq[0]);
-  double d         = 0.0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const T v = scaled(y[i], inv);
-    d += fabs((double)v - (double)x[i]);
-    y[i] = v;
-    x[i] = v;
-  }
-  d = block_sum(d, smem);
-  if (threadIdx.x == 0 && d != 0.0) atomicAdd(out, d);
-}
-
-// HITS: out[0] = max(out[0], max hubs), out[1] = max(out[1], max auth)   (k_norm mode 2 of both arrays)
-template <typename T>
-__global__ void __launch_bounds__(kBlock) k_hits_max(T const* __restrict__ hubs, T const* __restrict__ auth, int32_t n, double* __restrict__ out)
-{
-  double mh = 0.0, ma = 0.0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const double h = (double)hubs[i], a = (double)auth[i];
-    mh = h > mh ? h : mh;
-    ma = a > ma ? a : ma;
-  }
-  warp_max_into(mh, out);
-  warp_max_into(ma, out + 1);
-}
-
-// HITS: hubs *= 1 / mx[0] ; auth *= 1 / mx[1] ; out[0] += sum |hubs - prev|   (two k_scale + k_abs_diff)
-template <typename T>
-__global__ void __launch_bounds__(kBlock)
-k_hits_scale(T* __restrict__ hubs, T* __restrict__ auth, T const* __restrict__ prev, int32_t n, double const* __restrict__ mx,
-             double* __restrict__ out)
-{
-  __shared__ double smem[kBlock / 32];
-  const double inv_h = 1.0 / mx[0], inv_a = 1.0 / mx[1];
-  double d = 0.0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    const T h = scaled(hubs[i], inv_h);
-    hubs[i]   = h;
-    auth[i]   = scaled(auth[i], inv_a);
-    d += fabs((double)h - (double)prev[i]);
-  }
-  d = block_sum(d, smem);
-  if (threadIdx.x == 0 && d != 0.0) atomicAdd(out, d);
-}
-
-
 // the global code of a column slot: (owner rank) * maxpart + local id, owner rank = (col / maxpart) * grid_cols + grid_c
 __device__ __forceinline__ long long column_code(int col, long long maxpart, int grid_cols, int grid_c)
 {
@@ -408,9 +316,10 @@ void by_float_type(cugraph_data_type_id_t t, F&& f)
   else f(double{});
 }
 
-// The frame of the owner steps (Katz, eigenvector, HITS, vertex sums and scaling).  Checks in this order: `partial` is
-// not NULL; the arrays `vs` are not NULL, share one FLOAT32 / FLOAT64 type and hold n_local elements; the device scalars
-// `ins` are not NULL.  Then, for n_local > 0, launch(h, T{}, n_local, grid) and the check of the launch.
+// The frame of the owner steps (Katz, eigenvector, HITS, vertex sums and scaling; their kernels, in centrality_ops.cuh,
+// are those of the single-GPU drivers).  Checks in this order: `partial` is not NULL; the arrays `vs` are not NULL, share
+// one FLOAT32 / FLOAT64 type and hold n_local elements; the device scalars `ins` are not NULL.  Then, for n_local > 0,
+// launch(h, T{}, n_local, grid) and the check of the launch.
 template <typename F>
 cugraph_error_code_t owner_step(cugraph_error_t** error, const char* what, const cugraph_resource_handle_t* handle,
                                 std::initializer_list<device_array_view_impl const*> vs, size_t n_local, void const* partial,

@@ -7,6 +7,7 @@
 // advances the device-resident loop state.  The host enqueues iterations in batches and only reads the
 // `done` flag between batches; kernels of iterations past convergence are no-ops, so the iteration
 // count and result are exactly those of a check-every-iteration loop.
+#include "centrality_ops.cuh"
 #include "graph.cuh"
 #include "staging.cuh"
 
@@ -90,16 +91,6 @@ __global__ void k_count_repeats(int32_t const* __restrict__ sorted, int32_t n, i
 {
   for (int64_t i = 1 + blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     if (sorted[i] == sorted[i - 1]) atomicAdd(out, 1);
-}
-
-template <typename T>
-__global__ void k_sum(T const* a, int32_t n, double* out)
-{
-  __shared__ double smem[8];
-  double s = 0.0;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) s += (double)a[i];
-  s = block_sum(s, smem);
-  if (threadIdx.x == 0) atomicAdd(out, s);
 }
 
 struct pr_args {
@@ -201,7 +192,7 @@ void pagerank_typed(handle_impl const& h, graph_impl& g, pr_args const& a, centr
     auto* dchk = chk.as<pers_check_t>();
     CUDA_TRY(cudaMemsetAsync(dchk, 0, sizeof(pers_check_t), h.stream));
     B200_LAUNCH(h, (k_count_negative<int32_t>), grid_for(n_pers), kBlock, 0, pers_idx.as<int32_t>(), (int64_t)n_pers, &dchk->n_invalid);
-    B200_LAUNCH(h, (k_sum<T>), grid_for(n_pers, 1, 1024), kBlock, 0, (T const*)a.pers_val->data, n_pers, &dchk->sum);
+    B200_LAUNCH(h, (k_norm<T>), grid_for(n_pers, 1, 1024), kBlock, 0, (T const*)a.pers_val->data, n_pers, 1, &dchk->sum);
     dbuf sorted;
     if (a.expensive) {
       B200_LAUNCH(h, (k_count_negative<T>), grid_for(n_pers), kBlock, 0, (T const*)a.pers_val->data, (int64_t)n_pers,

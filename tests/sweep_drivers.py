@@ -16,7 +16,7 @@ The bound.  Every driver iterates a non-negative map (weights and values are non
   S <= |y*| (every term is non-negative, and the constant term the sweep adds is too), so a sweep adds at most
       delta = 2 (5u + d_max 2^-52)
   of componentwise relative error.
-- A vector pass adds its roundings: a scaling (T)((double)v * (1/s)) u + 2e, k_add_vec u, PageRank's x = pr / out_w u.
+- A vector pass adds its roundings: a scaling (T)((double)v * (1/s)) u + 2e, the eigenvector add y + x u, PageRank's x = pr / out_w u.
   An fp64 sum of n non-negative terms (norms, maxima are exact, differences, the dangling sum, the personalization sum) is
   off by at most n e relatively, in any order of the atomics.
 - Propagation.  A non-negative linear map does not expand the componentwise relative error of its input, nor does adding a
