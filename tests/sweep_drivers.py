@@ -466,9 +466,9 @@ def check_pagerank(h, g, graph, steps=30, alpha=0.85, pers=None, guess=None, out
 
 
 def personalizations(graph, seed=0):
-    """tests/mg_pagerank_sim.cases: one hub, a sink, a vertex without in-edges, an isolated id, a share with zeros among
+    """tests/mg_pagerank_ref.cases: one hub, a sink, a vertex without in-edges, an isolated id, a share with zeros among
     the values — as (internal ids, values)"""
-    from tests.mg_pagerank_sim import cases
+    from tests.mg_pagerank_ref import cases
     V = graph.V
     share = np.random.default_rng(seed).choice(V, size=max(V // 8, 2), replace=False)   # the draw of cases(): its zeros too
     out = {}

@@ -1,14 +1,14 @@
 """Multi-GPU Katz, eigenvector centrality and HITS on the CPU, over the emulated library (tests/emu_py.py).
 
-- All ranks of a 2D partition in one process (tests/mg_centrality_sim.py) through the real block sweeps and owner steps:
-  grids 1x2, 2x1, 2x2 and 4x2 on a directed RMAT-8 and on a graph with isolated ids, sources, sinks and duplicate edges,
-  against the oracle and single-GPU cugraph_katz_centrality / _eigenvector_centrality / cugraph_hits; a tiny graph that
-  leaves blocks without edges; weighted float32 / float64 blocks (float64: the oracle's iteration count, rtol 1e-9) and
-  64-bit-offset blocks; HITS from an initial guess; non-convergence.
+- Every rank of a grid in one process (tests/mg_world.py) running cugraph_b200.mg.MGGraph.katz_centrality /
+  .eigenvector_centrality / .hits: grids 1x2, 2x1, 2x2 and 4x2 on a directed RMAT-8 and on a graph with isolated ids,
+  sources, sinks and duplicate edges, against the oracle and single-GPU cugraph_katz_centrality / _eigenvector_centrality /
+  cugraph_hits on the vertices that appear in edges; a tiny graph that leaves blocks without edges; weighted float32 /
+  float64 blocks (float64: the oracle's iteration count, rtol 1e-9) and 64-bit-offset blocks; HITS from an initial
+  guess; non-convergence on every rank.
 - The owner-step entry points' error paths.
-- World sizes 2, 4 and 8 over gloo running cugraph_b200.mg.MGGraph.katz_centrality / .eigenvector_centrality / .hits (the
-  real orchestration), with an initial guess given by ranks that do not own those vertices and the non-convergence error
-  on every rank."""
+- World sizes 2, 4 and 8 over gloo running the same drivers (the real process groups), with an initial guess given by
+  ranks that do not own those vertices and the non-convergence error on every rank."""
 import ctypes as C
 import os
 import sys
@@ -20,8 +20,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import oracle  # noqa: E402
-from tests import mg_centrality_sim as sim  # noqa: E402
+from tests import mg_centrality_ref as refs  # noqa: E402
 from tests import mg_procs  # noqa: E402
+from tests import mg_world  # noqa: E402
 from tests.emu_py import surface  # noqa: E402, F401
 
 GRIDS = [(1, 2), (2, 1), (2, 2), (4, 2)]
@@ -31,106 +32,105 @@ EIG_TOL = dict(rtol=2e-3, atol=1e-8)
 HITS_TOL = dict(rtol=2e-3, atol=1e-9)
 
 
-def check_all(s, d, V, R, Cc, w=None, dtype=np.float32, device="cpu", single=True):
-    """the three algorithms on one grid against the oracle (and single GPU for float32)"""
-    grid = sim.Grid(s, d, V, R, Cc, w=w, dtype=dtype, device=device)
-    try:
-        f64 = dtype == np.float64
-        alpha = sim.katz_alpha(d, V) * (0.5 if w is not None else 1.0)
-        got, it = sim.katz(grid, alpha, epsilon=1e-6, max_iterations=200)
-        ref, it_ref = oracle.katz(s, d, V, w, alpha=alpha, epsilon=1e-6, dtype=dtype)
-        if f64:
-            assert it == it_ref
-            np.testing.assert_allclose(got, ref, rtol=1e-9)
-        else:
-            np.testing.assert_allclose(got, ref, rtol=KATZ_RTOL)
-        if single:
-            sg, _ = sim.single_gpu("katz", s, d, V, w=w, alpha=alpha, epsilon=1e-6, max_iterations=200)
-            np.testing.assert_allclose(got, sg, rtol=KATZ_RTOL)
+def check_all(s, d, V, world, w=None, dtype=np.float32, device="cpu", single=True):
+    """the three algorithms on one grid against the oracle (and single GPU for float32), all on the vertices that appear
+    in edges; returns the number of ranks whose block has no edges"""
+    ids, remap = mg_world.present(s, d, V)
+    rs, rd, n = remap[s], remap[d], ids.size
+    f64 = dtype == np.float64
+    alpha = refs.katz_alpha(d, V) * (0.5 if w is not None else 1.0)
+    runs = [("katz", dict(alpha=alpha, epsilon=1e-6, max_iterations=200)),
+            ("eigenvector", dict(epsilon=1e-6, max_iterations=500)), ("hits", dict(epsilon=1e-6, max_iterations=500))]
+    got, empty = refs.mg_centrality(s, d, V, world, runs, w=w, dtype=dtype, device=device)
+    assert not any(isinstance(r, str) for r in got), got                # an error message
+    (katz, kst), (eig, est), (hb, au, hst) = got
 
-        got, it = sim.eigenvector(grid, epsilon=1e-6, max_iterations=500)
-        ref, it_ref = oracle.eigenvector(s, d, V, w, epsilon=1e-6)
-        if f64:
-            assert it == it_ref
-            np.testing.assert_allclose(got, ref, rtol=1e-9)
-        else:
-            assert abs(it - it_ref) <= 1
-            np.testing.assert_allclose(got, ref, **EIG_TOL)
-        if single:
-            sg, _ = sim.single_gpu("eigenvector", s, d, V, w=w, epsilon=1e-6, max_iterations=500)
-            np.testing.assert_allclose(got, sg, **EIG_TOL)
+    got, it = katz[ids], kst["iterations"]
+    want, it_ref = oracle.katz(rs, rd, n, w, alpha=alpha, epsilon=1e-6, dtype=dtype)
+    if f64:
+        assert it == it_ref
+        np.testing.assert_allclose(got, want, rtol=1e-9)
+    else:
+        np.testing.assert_allclose(got, want, rtol=KATZ_RTOL)
+    if single:
+        sg, _ = refs.single_gpu("katz", rs, rd, n, w=w, alpha=alpha, epsilon=1e-6, max_iterations=200)
+        np.testing.assert_allclose(got, sg, rtol=KATZ_RTOL)
 
-        hb, au, it, _ = sim.hits(grid, epsilon=1e-6, max_iterations=500)
-        rh, ra, it_ref, _ = oracle.hits(s, d, V, epsilon=1e-6)
-        if f64:
-            assert it == it_ref
-            np.testing.assert_allclose(hb, rh, rtol=1e-9, atol=1e-15)
-            np.testing.assert_allclose(au, ra, rtol=1e-9, atol=1e-15)
-        else:
-            assert abs(it - it_ref) <= 1
-            np.testing.assert_allclose(hb, rh, **HITS_TOL)
-            np.testing.assert_allclose(au, ra, **HITS_TOL)
-        if single:
-            sh, sa = sim.single_gpu("hits", s, d, V, w=w, epsilon=1e-6, max_iterations=500)
-            np.testing.assert_allclose(hb, sh, **HITS_TOL)
-            np.testing.assert_allclose(au, sa, **HITS_TOL)
-        return grid.empty_blocks
-    finally:
-        grid.free()
+    got, it = eig[ids], est["iterations"]
+    want, it_ref = oracle.eigenvector(rs, rd, n, w, epsilon=1e-6)
+    if f64:
+        assert it == it_ref
+        np.testing.assert_allclose(got, want, rtol=1e-9)
+    else:
+        assert abs(it - it_ref) <= 1
+        np.testing.assert_allclose(got, want, **EIG_TOL)
+    if single:
+        sg, _ = refs.single_gpu("eigenvector", rs, rd, n, w=w, epsilon=1e-6, max_iterations=500)
+        np.testing.assert_allclose(got, sg, **EIG_TOL)
+
+    hb, au, it = hb[ids], au[ids], hst["iterations"]
+    rh, ra, it_ref, _ = oracle.hits(rs, rd, n, epsilon=1e-6)
+    if f64:
+        assert it == it_ref
+        np.testing.assert_allclose(hb, rh, rtol=1e-9, atol=1e-15)
+        np.testing.assert_allclose(au, ra, rtol=1e-9, atol=1e-15)
+    else:
+        assert abs(it - it_ref) <= 1
+        np.testing.assert_allclose(hb, rh, **HITS_TOL)
+        np.testing.assert_allclose(au, ra, **HITS_TOL)
+    if single:
+        sh, sa = refs.single_gpu("hits", rs, rd, n, w=w, epsilon=1e-6, max_iterations=500)
+        np.testing.assert_allclose(hb, sh, **HITS_TOL)
+        np.testing.assert_allclose(au, sa, **HITS_TOL)
+    return empty
 
 
 @pytest.mark.parametrize("R,Cc", GRIDS, ids=GRID_IDS)
-def test_mg_centrality_simulated_emulated(surface, R, Cc):
-    check_all(*sim.rmat_graph(8), R, Cc)
-    check_all(*sim.odd_graph(), R, Cc)
+def test_mg_centrality_simulated_emulated(surface, monkeypatch, R, Cc):
+    world = mg_world.grid_world(monkeypatch, R, Cc)
+    check_all(*refs.rmat_graph(8), world)
+    check_all(*refs.odd_graph(), world)
 
 
-def test_mg_centrality_empty_blocks_emulated(surface):
-    assert check_all(*sim.tiny_graph(), 4, 2, single=False) > 0
+def test_mg_centrality_empty_blocks_emulated(surface, monkeypatch):
+    assert check_all(*refs.tiny_graph(), mg_world.grid_world(monkeypatch, 4, 2), single=False) > 0
 
 
 @pytest.mark.parametrize("wdtype", [np.float32, np.float64], ids=["f32", "f64"])
-def test_mg_centrality_weighted_blocks_emulated(surface, wdtype):
-    s, d, V = sim.odd_graph()
+def test_mg_centrality_weighted_blocks_emulated(surface, monkeypatch, wdtype):
+    s, d, V = refs.odd_graph()
     w = np.random.default_rng(2).uniform(0.5, 1.0, s.size).astype(wdtype)
-    check_all(s, d, V, 2, 2, w=w, dtype=wdtype, single=wdtype == np.float32)
+    check_all(s, d, V, mg_world.grid_world(monkeypatch, 2, 2), w=w, dtype=wdtype, single=wdtype == np.float32)
 
 
 def test_mg_centrality_offs64_emulated(surface, monkeypatch):
     """CUGRAPH_B200_OFFS64_MIN_EDGES=0: the blocks and their column-major copies get 64-bit offsets (the plain sweep)"""
     monkeypatch.setenv("CUGRAPH_B200_OFFS64_MIN_EDGES", "0")
-    s, d, V = sim.rmat_graph(8)
+    s, d, V = refs.rmat_graph(8)
     w = np.random.default_rng(3).uniform(0.5, 1.0, s.size)
-    check_all(s, d, V, 2, 2, w=w, dtype=np.float64, single=False)
+    check_all(s, d, V, mg_world.grid_world(monkeypatch, 2, 2), w=w, dtype=np.float64, single=False)
 
 
-def test_mg_hits_initial_guess_emulated(surface):
-    s, d, V = sim.odd_graph()
+def test_mg_hits_initial_guess_emulated(surface, monkeypatch):
+    s, d, V = refs.odd_graph()
     guess = np.random.default_rng(4).uniform(0.0, 2.0, V)
     guess[::3] = 0.0
-    grid = sim.Grid(s, d, V, 2, 2)
-    try:
-        hb, au, it, _ = sim.hits(grid, epsilon=1e-6, max_iterations=500, initial_hubs=guess)
-    finally:
-        grid.free()
-    rh, ra, it_ref, _ = oracle.hits(s, d, V, epsilon=1e-6, initial_hubs=guess)
-    assert abs(it - it_ref) <= 1
-    np.testing.assert_allclose(hb, rh, **HITS_TOL)
-    np.testing.assert_allclose(au, ra, **HITS_TOL)
+    ids, remap = mg_world.present(s, d, V)
+    runs = [("hits", dict(epsilon=1e-6, max_iterations=500, initial_hubs_guess=(ids, guess[ids])))]
+    ((hb, au, st),), _ = refs.mg_centrality(s, d, V, mg_world.grid_world(monkeypatch, 2, 2), runs)
+    rh, ra, it_ref, _ = oracle.hits(remap[s], remap[d], ids.size, epsilon=1e-6, initial_hubs=guess[ids])
+    assert abs(st["iterations"] - it_ref) <= 1
+    np.testing.assert_allclose(hb[ids], rh, **HITS_TOL)
+    np.testing.assert_allclose(au[ids], ra, **HITS_TOL)
 
 
-def test_mg_centrality_nonconvergence_emulated(surface):
-    s, d, V = sim.rmat_graph(8)
-    grid = sim.Grid(s, d, V, 2, 2)
-    try:
-        with pytest.raises(RuntimeError, match="Katz Centrality failed to converge"):
-            sim.katz(grid, sim.katz_alpha(d, V), epsilon=1e-12, max_iterations=3)
-        with pytest.raises(RuntimeError, match="Eigenvector Centrality failed to converge"):
-            sim.eigenvector(grid, epsilon=1e-12, max_iterations=3)
-        with pytest.raises(RuntimeError, match="HITS failed to converge"):
-            sim.hits(grid, epsilon=1e-12, max_iterations=3)
-    finally:
-        grid.free()
+def test_mg_centrality_nonconvergence_emulated(surface, monkeypatch):
+    s, d, V = refs.rmat_graph(8)
+    runs = [("katz", dict(alpha=refs.katz_alpha(d, V), epsilon=1e-12, max_iterations=3)),
+            ("eigenvector", dict(epsilon=1e-12, max_iterations=3)), ("hits", dict(epsilon=1e-12, max_iterations=3))]
+    errors, _ = refs.mg_centrality(s, d, V, mg_world.grid_world(monkeypatch, 2, 2), runs)   # the same on every rank
+    for e, msg in zip(errors, ("Katz Centrality", "Eigenvector Centrality", "HITS")):
+        assert isinstance(e, str) and f"{msg} failed to converge" in e, e
 
 
 def test_owner_step_errors_emulated(surface):
@@ -169,7 +169,7 @@ def test_owner_step_errors_emulated(surface):
 # ---------------------------------------------------------------------------------------------------------- gloo runs
 def _gloo_graph():
     """the odd graph with scattered 64-bit external ids (isolated ids are not vertices of an MG graph)"""
-    s, d, V = sim.odd_graph(seed=11)
+    s, d, V = refs.odd_graph(seed=11)
     ids = np.random.default_rng(11).choice(10**9, size=V, replace=False).astype(np.int64) + 10**10
     return ids, s, d, V
 
@@ -187,7 +187,7 @@ def _gloo_worker(rank, world):
     n = s.size
     lo, hi = rank * n // world, (rank + 1) * n // world
     g = mg.MGGraph(torch.from_numpy(ids[s[lo:hi]]), torch.from_numpy(ids[d[lo:hi]]))
-    alpha = sim.katz_alpha(d, V)
+    alpha = refs.katz_alpha(d, V)
     out = {}
     v, x = mg.katz_centrality(g, alpha, epsilon=1e-6, max_iterations=200)
     out["katz"] = (v.numpy(), x.numpy(), g.last_katz_stats)
@@ -239,7 +239,7 @@ def test_mg_centrality_emulated_gloo(world):
         assert cnt == n
         return out
 
-    alpha = sim.katz_alpha(d, V)
+    alpha = refs.katz_alpha(d, V)
     ref, _ = oracle.katz(rs, rd, n, alpha=alpha, epsilon=1e-6, dtype=np.float32)
     np.testing.assert_allclose(by_id("katz", 1), ref, rtol=KATZ_RTOL)
     ref, _ = oracle.eigenvector(rs, rd, n, epsilon=1e-6)

@@ -1,11 +1,11 @@
 """Multi-GPU Katz, eigenvector centrality and HITS on the GPU.
 
-- All ranks of a 2D partition on ONE GPU (tests/mg_centrality_sim.py) through the real block sweeps and owner steps: grids
-  1x2, 2x1, 2x2 and 4x2 on directed RMAT-14 and RMAT-16, against the oracle and single-GPU cugraph_katz_centrality /
-  _eigenvector_centrality / cugraph_hits (iterations within one of single GPU's); weighted float32 / float64 blocks and
-  64-bit-offset blocks.
-- A world-size-1 NCCL process group running cugraph_b200.mg.MGGraph.katz_centrality / .eigenvector_centrality / .hits (the
-  1x1 grid): the real orchestration and the real stream ordering on the device.
+- Every rank of a grid on ONE GPU in one process (tests/mg_world.py) running cugraph_b200.mg.MGGraph.katz_centrality /
+  .eigenvector_centrality / .hits: grids 1x2, 2x1, 2x2 and 4x2 on directed RMAT-14 and RMAT-16, against the oracle and
+  single-GPU cugraph_katz_centrality / _eigenvector_centrality / cugraph_hits on the vertices that appear in edges
+  (iterations within one of single GPU's); weighted float32 / float64 blocks and 64-bit-offset blocks.
+- A world-size-1 NCCL process group running the same drivers (the 1x1 grid): the real collectives and the real stream
+  ordering on the device.
 - 2 and 4 GPUs over NCCL (skipped when fewer GPUs are visible)."""
 import ctypes as C
 import os
@@ -18,27 +18,26 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import oracle  # noqa: E402
+from tests import mg_centrality_ref as refs  # noqa: E402
 from tests import mg_procs  # noqa: E402
-from tests import mg_centrality_sim as sim  # noqa: E402
+from tests import mg_world  # noqa: E402
 from tests.test_mg_centrality_cpu import EIG_TOL, HITS_TOL, KATZ_RTOL, check_all  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
 
-def _iterations_match_single_gpu(s, d, V, R, Cc):
-    """iteration counts within one of single GPU's on the same graph"""
+def _iterations_match_single_gpu(s, d, V, world):
+    """iteration counts within one of single GPU's on the graph's vertices"""
     import torch
     from cugraph_b200 import _capi
     from tests.gpu_util import make_graph
-    grid = sim.Grid(s, d, V, R, Cc, device="cuda")
-    try:
-        alpha = sim.katz_alpha(d, V)
-        _, it_k = sim.katz(grid, alpha, epsilon=1e-6, max_iterations=200)
-        _, it_e = sim.eigenvector(grid, epsilon=1e-6, max_iterations=500)
-        _, _, it_h, _ = sim.hits(grid, epsilon=1e-6, max_iterations=500)
-    finally:
-        grid.free()
-    h, g = make_graph(s, d, store_transposed=True, vertices=np.arange(V, dtype=np.int32))
+    alpha = refs.katz_alpha(d, V)
+    runs = [("katz", dict(alpha=alpha, epsilon=1e-6, max_iterations=200)),
+            ("eigenvector", dict(epsilon=1e-6, max_iterations=500)), ("hits", dict(epsilon=1e-6, max_iterations=500))]
+    ((_, kst), (_, est), (_, _, hst)), _ = refs.mg_centrality(s, d, V, world, runs, device="cuda")
+    it_k, it_e, it_h = kst["iterations"], est["iterations"], hst["iterations"]
+    ids, remap = mg_world.present(s, d, V)
+    h, g = make_graph(remap[s], remap[d], store_transposed=True, vertices=np.arange(ids.size, dtype=np.int32))
     L, res, err = _capi.lib(), C.c_void_p(), C.c_void_p()
     _capi.check(L.cugraph_katz_centrality(h.ptr, g.ptr, None, alpha, 1.0, 1e-6, 200, 0, C.byref(res), C.byref(err)), err, "katz")
     sg_k = L.cugraph_centrality_result_get_num_iterations(res)
@@ -54,36 +53,37 @@ def _iterations_match_single_gpu(s, d, V, R, Cc):
 
 
 @pytest.mark.parametrize("R,Cc", [(1, 2), (2, 1), (2, 2), (4, 2)], ids=["1x2", "2x1", "2x2", "4x2"])
-def test_mg_centrality_simulated_on_one_gpu(R, Cc):
+def test_mg_centrality_simulated_on_one_gpu(monkeypatch, R, Cc):
+    world = mg_world.grid_world(monkeypatch, R, Cc)
     for scale in (14, 16):
-        s, d, V = sim.rmat_graph(scale)
-        check_all(s, d, V, R, Cc, device="cuda")
-        _iterations_match_single_gpu(s, d, V, R, Cc)
-    check_all(*sim.odd_graph(), R, Cc, device="cuda")
+        s, d, V = refs.rmat_graph(scale)
+        check_all(s, d, V, world, device="cuda")
+        _iterations_match_single_gpu(s, d, V, world)
+    check_all(*refs.odd_graph(), world, device="cuda")
 
 
 @pytest.mark.parametrize("wdtype", [np.float32, np.float64], ids=["f32", "f64"])
-def test_mg_centrality_weighted_blocks_on_one_gpu(wdtype):
-    s, d, V = sim.rmat_graph(14)
+def test_mg_centrality_weighted_blocks_on_one_gpu(monkeypatch, wdtype):
+    s, d, V = refs.rmat_graph(14)
     w = np.random.default_rng(2).uniform(0.5, 1.0, s.size).astype(wdtype)
-    check_all(s, d, V, 2, 2, w=w, dtype=wdtype, device="cuda", single=wdtype == np.float32)
+    check_all(s, d, V, mg_world.grid_world(monkeypatch, 2, 2), w=w, dtype=wdtype, device="cuda", single=wdtype == np.float32)
 
 
 def test_mg_centrality_offs64_on_one_gpu(monkeypatch):
     monkeypatch.setenv("CUGRAPH_B200_OFFS64_MIN_EDGES", "0")
-    s, d, V = sim.rmat_graph(14)
-    check_all(s, d, V, 2, 2, device="cuda", single=False)
+    s, d, V = refs.rmat_graph(14)
+    check_all(s, d, V, mg_world.grid_world(monkeypatch, 2, 2), device="cuda", single=False)
 
 
 # ------------------------------------------------------------------------------------------------- NCCL process groups
 def _nccl_worker(rank, world):
     import torch
     from cugraph_b200 import mg
-    s, d, V = sim.rmat_graph(14)
+    s, d, V = refs.rmat_graph(14)
     E = s.size
     lo, hi = rank * E // world, (rank + 1) * E // world
     g = mg.MGGraph(torch.as_tensor(s[lo:hi]).cuda(), torch.as_tensor(d[lo:hi]).cuda())
-    alpha = sim.katz_alpha(d, V)
+    alpha = refs.katz_alpha(d, V)
     out = {}
     v, x = mg.katz_centrality(g, alpha, epsilon=1e-6, max_iterations=200)
     out["katz"] = (v.cpu().numpy(), x.cpu().numpy(), g.last_katz_stats)
@@ -101,7 +101,7 @@ def _nccl_worker(rank, world):
 
 def _run_nccl(world):
     res = mg_procs.run(_nccl_worker, world, backend="nccl", timeout=600)
-    s, d, V = sim.rmat_graph(14)
+    s, d, V = refs.rmat_graph(14)
     present = np.unique(np.concatenate([s, d]))
     remap = np.full(V, -1)
     remap[present] = np.arange(present.size)
@@ -114,7 +114,7 @@ def _run_nccl(world):
         assert sum(r[key][0].size for r in res) == n
         return out
 
-    ref, _ = oracle.katz(rs, rd, n, alpha=sim.katz_alpha(d, V), epsilon=1e-6, dtype=np.float32)
+    ref, _ = oracle.katz(rs, rd, n, alpha=refs.katz_alpha(d, V), epsilon=1e-6, dtype=np.float32)
     np.testing.assert_allclose(by_id("katz", 1), ref, rtol=KATZ_RTOL)
     ref, _ = oracle.eigenvector(rs, rd, n, epsilon=1e-6)
     np.testing.assert_allclose(by_id("eig", 1), ref, **EIG_TOL)

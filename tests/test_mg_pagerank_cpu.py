@@ -1,14 +1,14 @@
 """Multi-GPU PageRank with personalization, an initial guess and precomputed out-weights on the CPU, over the emulated
 library (tests/emu_py.py).
 
-- All ranks of a 2D partition in one process (tests/mg_pagerank_sim.py) through the real block sweeps and owner steps:
-  grids 1x2, 2x1, 2x2 and 4x2 on a directed RMAT-8 and on a graph with isolated ids, sources, sinks and duplicate edges,
-  weighted and unweighted, float32 and float64, against the fp64 oracle at equal iteration count.
+- Every rank of a grid in one process (tests/mg_world.py) running cugraph_b200.mg.MGGraph.pagerank: grids 1x2, 2x1, 2x2
+  and 4x2 on a directed RMAT-8 and on a graph with isolated ids, sources, sinks and duplicate edges, weighted and
+  unweighted, float32 and float64, against the fp64 oracle on the graph's vertices at equal iteration count.
 - The personalized owner step's entry point: its arithmetic and its error paths.
-- World sizes 2, 4 and 8 over gloo running cugraph_b200.mg.MGGraph.pagerank (the real orchestration): personalization
-  from one rank, from a rank that owns none of its vertices and split across ranks; the reference's two personalized C-API
-  goldens with the personalization given by rank 0 only; an initial guess and precomputed out-weights; every input error
-  raised on every rank with the same type and message; FailedToConvergeError on every rank."""
+- World sizes 2, 4 and 8 over gloo running MGGraph.pagerank (the real process groups): personalization from one rank,
+  from a rank that owns none of its vertices and split across ranks; the reference's two personalized C-API goldens with
+  the personalization given by rank 0 only; an initial guess and precomputed out-weights; every input error raised on
+  every rank with the same type and message; FailedToConvergeError on every rank."""
 import ctypes as C
 import os
 import sys
@@ -19,9 +19,10 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from tests import mg_centrality_sim as graphs  # noqa: E402
-from tests import mg_pagerank_sim as sim  # noqa: E402
+from tests import mg_centrality_ref as graphs  # noqa: E402
+from tests import mg_pagerank_ref as refs  # noqa: E402
 from tests import mg_procs  # noqa: E402
+from tests import mg_world  # noqa: E402
 from tests.emu_py import surface  # noqa: E402, F401
 
 GRIDS = [(1, 2), (2, 1), (2, 2), (4, 2)]
@@ -29,39 +30,40 @@ GRID_IDS = ["1x2", "2x1", "2x2", "4x2"]
 ITERS = 20
 
 
-def check_all(s, d, V, R, Cc, w=None, dtype=np.float32, device="cpu", iters=ITERS, single=False):
+def check_all(s, d, V, world, w=None, dtype=np.float32, device="cpu", iters=ITERS, single=False):
     """plain and personalized runs, doubled out-weights and a converged initial guess on one grid against the oracle (and,
-    with `single`, against single-GPU personalized PageRank)"""
-    grid = sim.Grid(s, d, V, R, Cc, w=w, dtype=dtype, device=device)
-    tol = sim.F64_TOL if dtype == np.float64 else sim.F32_TOL
-    ow = sim.out_weights(s, V, w)
-    try:
-        plain, it, conv = sim.pagerank(grid, ow, max_iterations=iters)
-        assert it == iters and not conv
-        ref, _, _ = sim.oracle_pagerank(s, d, V, w, max_iterations=iters)
-        np.testing.assert_allclose(plain, ref, **tol)
-        for name, pv in sim.cases(s, d, V).items():
-            got, _, _ = sim.pagerank(grid, ow, max_iterations=iters, personalization=pv)
-            ref, _, _ = sim.oracle_pagerank(s, d, V, w, max_iterations=iters, personalization=pv)
-            np.testing.assert_allclose(got, ref, **tol, err_msg=name)
-            if single:
-                sg = single_gpu(s, d, V, w, pv, iters)
-                np.testing.assert_allclose(got, sg, **tol, err_msg=name)
-        got, _, _ = sim.pagerank(grid, ow, max_iterations=iters, personalization=np.ones(V))
-        np.testing.assert_allclose(got, plain, **tol)               # teleport to every vertex alike = plain PageRank
-        got, _, _ = sim.pagerank(grid, 2.0 * ow, max_iterations=iters)
-        ref, _, _ = sim.oracle_pagerank(s, d, V, w, max_iterations=iters, out_w=2.0 * ow)
-        np.testing.assert_allclose(got, ref, **tol)
-        pv = sim.cases(s, d, V)["share_with_zeros"]
-        for pers in (None, pv):
-            conv_ref, _, _ = sim.oracle_pagerank(s, d, V, w, epsilon=1e-12, max_iterations=1000, personalization=pers)
-            got, it, conv = sim.pagerank(grid, ow, epsilon=1e-5, max_iterations=100, personalization=pers,
-                                         initial_guess=conv_ref)
-            assert it == 1 and conv
-            np.testing.assert_allclose(got, conv_ref, rtol=1e-5, atol=1e-12)
-        return grid.empty_blocks
-    finally:
-        grid.free()
+    with `single`, against single-GPU personalized PageRank), all on the vertices that appear in edges"""
+    tol = refs.F64_TOL if dtype == np.float64 else refs.F32_TOL
+    ids, remap = mg_world.present(s, d, V)
+    rs, rd, n = remap[s], remap[d], ids.size
+    ow = refs.out_weights(rs, n, w)
+    # dense over the vertices; the isolated id's case personalizes no vertex of the graph
+    pers = {name: pv[ids] for name, pv in refs.cases(s, d, V).items() if pv[ids].any()}
+    share = pers["share_with_zeros"]
+    conv_ref = {k: refs.oracle_pagerank(rs, rd, n, w, epsilon=1e-12, max_iterations=1000, personalization=pv)[0]
+                for k, pv in (("plain", None), ("share", share))}
+    fixed = dict(alpha=0.85, epsilon=0.0, max_iterations=iters)
+    runs = [fixed] + [dict(fixed, personalization=(ids, pv)) for pv in pers.values()]
+    runs += [dict(fixed, personalization=(ids, np.ones(n))), dict(fixed, precomputed_out_weights=(ids, 2.0 * ow))]
+    runs += [dict(alpha=0.85, epsilon=1e-5, max_iterations=100, initial_guess=(ids, conv_ref["plain"])),
+             dict(alpha=0.85, epsilon=1e-5, max_iterations=100, initial_guess=(ids, conv_ref["share"]),
+                  personalization=(ids, share))]
+    got = [(x[ids], it, conv) for x, it, conv in refs.mg_pagerank(s, d, V, world, runs, w=w, dtype=dtype, device=device)]
+    plain, it, conv = got[0]
+    assert it == iters and not conv
+    np.testing.assert_allclose(plain, refs.oracle_pagerank(rs, rd, n, w, max_iterations=iters)[0], **tol)
+    for (name, pv), (x, _, _) in zip(pers.items(), got[1:]):
+        want, _, _ = refs.oracle_pagerank(rs, rd, n, w, max_iterations=iters, personalization=pv)
+        np.testing.assert_allclose(x, want, **tol, err_msg=name)
+        if single:
+            np.testing.assert_allclose(x, single_gpu(rs, rd, n, w, pv, iters), **tol, err_msg=name)
+    ones, doubled, from_plain, from_share = got[len(pers) + 1:]
+    np.testing.assert_allclose(ones[0], plain, **tol)               # teleport to every vertex alike = plain PageRank
+    want, _, _ = refs.oracle_pagerank(rs, rd, n, w, max_iterations=iters, out_w=2.0 * ow)
+    np.testing.assert_allclose(doubled[0], want, **tol)
+    for (x, it, conv), k in ((from_plain, "plain"), (from_share, "share")):
+        assert it == 1 and conv
+        np.testing.assert_allclose(x, conv_ref[k], rtol=1e-5, atol=1e-12)
 
 
 def single_gpu(s, d, V, w, pv, iters):
@@ -79,22 +81,23 @@ def single_gpu(s, d, V, w, pv, iters):
 
 
 @pytest.mark.parametrize("R,Cc", GRIDS, ids=GRID_IDS)
-def test_mg_pagerank_simulated_emulated(surface, R, Cc):
-    check_all(*graphs.rmat_graph(8), R, Cc)
-    check_all(*graphs.odd_graph(), R, Cc)
+def test_mg_pagerank_simulated_emulated(surface, monkeypatch, R, Cc):
+    world = mg_world.grid_world(monkeypatch, R, Cc)
+    check_all(*graphs.rmat_graph(8), world)
+    check_all(*graphs.odd_graph(), world)
 
 
 @pytest.mark.parametrize("wdtype", [np.float32, np.float64], ids=["f32", "f64"])
-def test_mg_pagerank_weighted_emulated(surface, wdtype):
+def test_mg_pagerank_weighted_emulated(surface, monkeypatch, wdtype):
     s, d, V = graphs.odd_graph()
     w = np.random.default_rng(2).uniform(0.5, 1.0, s.size).astype(wdtype)
-    check_all(s, d, V, 2, 2, w=w, dtype=wdtype)
+    check_all(s, d, V, mg_world.grid_world(monkeypatch, 2, 2), w=w, dtype=wdtype)
 
 
-def test_mg_pagerank_float64_rmat_emulated(surface):
+def test_mg_pagerank_float64_rmat_emulated(surface, monkeypatch):
     s, d, V = graphs.rmat_graph(8)
     w = np.random.default_rng(3).uniform(0.5, 1.0, s.size)
-    check_all(s, d, V, 4, 2, w=w, dtype=np.float64)
+    check_all(s, d, V, mg_world.grid_world(monkeypatch, 4, 2), w=w, dtype=np.float64)
 
 
 def test_personalized_vertex_step_emulated(surface):
@@ -297,7 +300,7 @@ def check_gloo(res, ids, s, d, V, golden, tol):
         return out
 
     def ref(**kw):
-        return sim.oracle_pagerank(rs, rd, n, max_iterations=ITERS, **kw)[0]
+        return refs.oracle_pagerank(rs, rd, n, max_iterations=ITERS, **kw)[0]
 
     np.testing.assert_allclose(by_id("plain"), ref(), **tol)
     np.testing.assert_allclose(by_id("share_rank0"), ref(personalization=dense(inp["share"])), **tol)

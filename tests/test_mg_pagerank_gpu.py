@@ -1,11 +1,11 @@
 """Multi-GPU PageRank with personalization, an initial guess and precomputed out-weights on the GPU.
 
-- All ranks of a 2D partition on ONE GPU (tests/mg_pagerank_sim.py) through the real block sweeps and owner steps: grids
-  1x2, 2x1, 2x2 and 4x2 on directed RMAT-14 and RMAT-16, float32 and float64, against the fp64 oracle and against
-  single-GPU personalized PageRank with the same personalization at equal iteration count; converging runs within one
-  iteration of single GPU's.
-- A world-size-1 NCCL process group running cugraph_b200.mg.MGGraph.pagerank (the 1x1 grid): the real orchestration and
-  the real stream ordering on the device.
+- Every rank of a grid on ONE GPU in one process (tests/mg_world.py) running cugraph_b200.mg.MGGraph.pagerank: grids 1x2,
+  2x1, 2x2 and 4x2 on directed RMAT-14 and RMAT-16, float32 and float64, against the fp64 oracle and against single-GPU
+  personalized PageRank with the same personalization at equal iteration count, on the vertices that appear in edges;
+  converging runs within one iteration of single GPU's.
+- A world-size-1 NCCL process group running MGGraph.pagerank (the 1x1 grid): the real collectives and the real stream
+  ordering on the device.
 - 2 and 4 GPUs over NCCL (skipped when fewer GPUs are visible)."""
 import os
 import sys
@@ -16,15 +16,16 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from tests import mg_centrality_sim as graphs  # noqa: E402
-from tests import mg_pagerank_sim as sim  # noqa: E402
+from tests import mg_centrality_ref as graphs  # noqa: E402
+from tests import mg_pagerank_ref as refs  # noqa: E402
 from tests import mg_procs  # noqa: E402
+from tests import mg_world  # noqa: E402
 from tests.test_mg_pagerank_cpu import ITERS, _gloo_graph, _gloo_worker, check_all, check_gloo  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
 
-def _converging_runs_match_single_gpu(s, d, V, R, Cc):
+def _converging_runs_match_single_gpu(s, d, V, world):
     """iteration counts at epsilon 1e-6 within one of single GPU's, plain and personalized"""
     import ctypes as C
 
@@ -32,18 +33,15 @@ def _converging_runs_match_single_gpu(s, d, V, R, Cc):
     from cugraph_b200 import _capi
     from cugraph_b200.mg import _views
     from tests.gpu_util import make_graph
-    pv = sim.cases(s, d, V)["share_with_zeros"]
-    grid = sim.Grid(s, d, V, R, Cc, device="cuda")
-    try:
-        ow = sim.out_weights(s, V)
-        _, it_plain, conv_plain = sim.pagerank(grid, ow, epsilon=1e-6, max_iterations=500)
-        _, it_pers, conv_pers = sim.pagerank(grid, ow, epsilon=1e-6, max_iterations=500, personalization=pv)
-    finally:
-        grid.free()
-    h, g = make_graph(s, d, store_transposed=True, vertices=np.arange(V, dtype=np.int32))
+    ids, remap = mg_world.present(s, d, V)
+    rs, rd, n = remap[s], remap[d], ids.size
+    pv = refs.cases(s, d, V)["share_with_zeros"][ids]
+    runs = [dict(epsilon=1e-6, max_iterations=500), dict(epsilon=1e-6, max_iterations=500, personalization=(ids, pv))]
+    (_, it_plain, conv_plain), (_, it_pers, conv_pers) = refs.mg_pagerank(s, d, V, world, runs, device="cuda")
+    h, g = make_graph(rs, rd, store_transposed=True, vertices=np.arange(n, dtype=np.int32))
     L, err = _capi.lib(), C.c_void_p()
-    ids = np.flatnonzero(pv != 0).astype(np.int32)
-    pids, pvals = torch.as_tensor(ids).cuda(), torch.as_tensor(pv[ids].astype(np.float32)).cuda()
+    nz = np.flatnonzero(pv != 0).astype(np.int32)
+    pids, pvals = torch.as_tensor(nz).cuda(), torch.as_tensor(pv[nz].astype(np.float32)).cuda()
     iters = []
     with _views(pids, pvals) as (vi, vv):
         for name, pers in (("cugraph_pagerank_allow_nonconvergence", []),
@@ -60,32 +58,33 @@ def _converging_runs_match_single_gpu(s, d, V, R, Cc):
 
 
 @pytest.mark.parametrize("R,Cc", [(1, 2), (2, 1), (2, 2), (4, 2)], ids=["1x2", "2x1", "2x2", "4x2"])
-def test_mg_pagerank_simulated_on_one_gpu(R, Cc):
+def test_mg_pagerank_simulated_on_one_gpu(monkeypatch, R, Cc):
+    world = mg_world.grid_world(monkeypatch, R, Cc)
     for scale in (14, 16):
         s, d, V = graphs.rmat_graph(scale)
-        check_all(s, d, V, R, Cc, device="cuda", single=True)
-        _converging_runs_match_single_gpu(s, d, V, R, Cc)
-    check_all(*graphs.odd_graph(), R, Cc, device="cuda", single=True)
+        check_all(s, d, V, world, device="cuda", single=True)
+        _converging_runs_match_single_gpu(s, d, V, world)
+    check_all(*graphs.odd_graph(), world, device="cuda", single=True)
 
 
 @pytest.mark.parametrize("wdtype", [np.float32, np.float64], ids=["f32", "f64"])
-def test_mg_pagerank_weighted_on_one_gpu(wdtype):
+def test_mg_pagerank_weighted_on_one_gpu(monkeypatch, wdtype):
     s, d, V = graphs.rmat_graph(14)
     w = np.random.default_rng(2).uniform(0.5, 1.0, s.size).astype(wdtype)
-    check_all(s, d, V, 2, 2, w=w, dtype=wdtype, device="cuda", single=True)
+    check_all(s, d, V, mg_world.grid_world(monkeypatch, 2, 2), w=w, dtype=wdtype, device="cuda", single=True)
 
 
-def test_mg_pagerank_float64_rmat16_on_one_gpu():
+def test_mg_pagerank_float64_rmat16_on_one_gpu(monkeypatch):
     s, d, V = graphs.rmat_graph(16)
     w = np.random.default_rng(3).uniform(0.5, 1.0, s.size)
-    check_all(s, d, V, 4, 2, w=w, dtype=np.float64, device="cuda", single=True)
+    check_all(s, d, V, mg_world.grid_world(monkeypatch, 4, 2), w=w, dtype=np.float64, device="cuda", single=True)
 
 
 # ------------------------------------------------------------------------------------------------- NCCL process groups
 def _run_nccl(world, golden):
     res = mg_procs.run(_gloo_worker, world, golden["c_api"], "cuda", backend="nccl", timeout=600)
     ids, s, d, V = _gloo_graph()
-    check_gloo(res, ids, s, d, V, golden["c_api"], sim.F32_TOL)
+    check_gloo(res, ids, s, d, V, golden["c_api"], refs.F32_TOL)
     assert ITERS == res[0]["plain"][2]
 
 

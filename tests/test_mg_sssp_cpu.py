@@ -1,11 +1,10 @@
 """Multi-GPU SSSP on the CPU, over the emulated library (tests/emu_py.py).
 
-- All ranks of a 2D partition in one process (tests/mg_sssp_sim.py) through the real block entry points: grids 1x2, 2x1, 2x2
-  and 4x2, float32 and float64, with and without predecessors, with a cutoff, on 64-bit-offset blocks, and on the
-  zero-weight graph.  Distances bit-exact vs the oracle and vs single-GPU cugraph_sssp; predecessors valid and a tree.
-- World sizes 2, 4 and 8 over gloo running cugraph_b200.mg.MGGraph.sssp (the real orchestration: process groups,
-  collectives, windows, the predecessor look-up at the owners), on a graph with unreachable vertices and a weighted chain
-  that takes many windows, and once with everything in one window.
+- Every rank of a grid in one process (tests/mg_world.py) running cugraph_b200.mg.MGGraph.sssp: grids 1x2, 2x1, 2x2 and
+  4x2, float32 and float64, with and without predecessors, with a cutoff, on 64-bit-offset blocks, and on the zero-weight
+  graph.  Distances bit-exact vs the oracle and vs single-GPU cugraph_sssp; predecessors valid and a tree.
+- World sizes 2, 4 and 8 over gloo running MGGraph.sssp (the real process groups), on a graph with unreachable vertices
+  and a weighted chain that takes many windows, and once with everything in one window.
 - The error paths of MGGraph.sssp and of the two C entry points."""
 import ctypes as C
 import math
@@ -19,7 +18,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from tests import mg_procs  # noqa: E402
-from tests import mg_sssp_sim as sim  # noqa: E402
+from tests import mg_sssp_ref as refs  # noqa: E402
+from tests import mg_world  # noqa: E402
 from tests.emu_py import surface  # noqa: E402, F401
 
 SCALE = 8
@@ -27,40 +27,39 @@ SCALE = 8
 
 @pytest.mark.parametrize("wdtype", [np.float32, np.float64], ids=["f32", "f64"])
 @pytest.mark.parametrize("R,Cc", [(1, 2), (2, 1), (2, 2), (4, 2)], ids=["1x2", "2x1", "2x2", "4x2"])
-def test_mg_sssp_simulated_emulated(surface, R, Cc, wdtype):
-    s, d, w, V = sim.rmat_graph(SCALE, wdtype)
-    for src in sim.sources(s, V):
-        single = sim.single_gpu_sssp(s, d, w, V, src)
-        dist, pred, stats = sim.simulate(s, d, w, V, R, Cc, src)
-        sim.check(s, d, w, V, src, dist, pred, single=single)
-        assert stats["windows"] > 1
-        dist, pred, _ = sim.simulate(s, d, w, V, R, Cc, src, predecessors=False)
-        assert pred is None
-        sim.check(s, d, w, V, src, dist, None, single=single)
-    src = sim.sources(s, V)[0]
-    reach = single[single < np.finfo(wdtype).max]
+def test_mg_sssp_simulated_emulated(surface, monkeypatch, R, Cc, wdtype):
+    world = mg_world.grid_world(monkeypatch, R, Cc)
+    s, d, w, V = refs.rmat_graph(SCALE, wdtype)
+    srcs = refs.sources(s, V)
+    single = {src: refs.single_gpu_sssp(s, d, w, V, src) for src in srcs}
+    reach = single[srcs[-1]][single[srcs[-1]] < np.finfo(wdtype).max]
     co = float(np.quantile(reach, 0.3))
-    dist, pred, _ = sim.simulate(s, d, w, V, R, Cc, src, cutoff=co)
-    sim.check(s, d, w, V, src, dist, pred, cutoff=co, single=sim.single_gpu_sssp(s, d, w, V, src, cutoff=co))
+    runs = [(src, math.inf, preds) for src in srcs for preds in (True, False)] + [(srcs[0], co, True)]
+    res = refs.mg_sssp(s, d, w, V, world, runs)
+    for (src, _, _), (dist, pred, stats) in zip(runs, res[:-1]):
+        refs.check(s, d, w, V, src, dist, pred, single=single[src])
+        assert stats["windows"] > 1
+    dist, pred, _ = res[-1]
+    refs.check(s, d, w, V, srcs[0], dist, pred, cutoff=co, single=refs.single_gpu_sssp(s, d, w, V, srcs[0], cutoff=co))
 
 
 @pytest.mark.parametrize("wdtype", [np.float32, np.float64], ids=["f32", "f64"])
 def test_mg_sssp_simulated_offs64_emulated(surface, monkeypatch, wdtype):
     """CUGRAPH_B200_OFFS64_MIN_EDGES=0: the blocks and their push copies get 64-bit offsets"""
     monkeypatch.setenv("CUGRAPH_B200_OFFS64_MIN_EDGES", "0")
-    s, d, w, V = sim.rmat_graph(SCALE, wdtype)
-    src = sim.sources(s, V)[0]
-    dist, pred, _ = sim.simulate(s, d, w, V, 2, 2, src)
+    s, d, w, V = refs.rmat_graph(SCALE, wdtype)
+    src = refs.sources(s, V)[0]
+    (dist, pred, _), = refs.mg_sssp(s, d, w, V, mg_world.grid_world(monkeypatch, 2, 2), [(src, math.inf, True)])
     monkeypatch.delenv("CUGRAPH_B200_OFFS64_MIN_EDGES")
-    sim.check(s, d, w, V, src, dist, pred, single=sim.single_gpu_sssp(s, d, w, V, src))
+    refs.check(s, d, w, V, src, dist, pred, single=refs.single_gpu_sssp(s, d, w, V, src))
 
 
 @pytest.mark.parametrize("wdtype", [np.float32, np.float64], ids=["f32", "f64"])
-def test_mg_sssp_zero_weights_emulated(surface, wdtype):
-    s, d, w, V = sim.zero_weight_graph(wdtype)
-    for src in (0, 7):
-        dist, pred, _ = sim.simulate(s, d, w, V, 2, 2, src)
-        sim.check(s, d, w, V, src, dist, pred, single=sim.single_gpu_sssp(s, d, w, V, src))
+def test_mg_sssp_zero_weights_emulated(surface, monkeypatch, wdtype):
+    s, d, w, V = refs.zero_weight_graph(wdtype)
+    res = refs.mg_sssp(s, d, w, V, mg_world.grid_world(monkeypatch, 2, 2), [(src, math.inf, True) for src in (0, 7)])
+    for src, (dist, pred, _) in zip((0, 7), res):
+        refs.check(s, d, w, V, src, dist, pred, single=refs.single_gpu_sssp(s, d, w, V, src))
 
 
 # ---------------------------------------------------------------------------------------------------- C entry point errors

@@ -1,11 +1,11 @@
 """Multi-GPU weakly connected components on the CPU, over the emulated library (tests/emu_py.py).
 
-- All ranks of a 2D partition in one process (tests/mg_wcc_sim.py) through the real block entry point: grids 1x2, 2x1, 2x2
-  and 4x2 on the components graph and a symmetrised RMAT-8, a tiny graph that leaves blocks without edges, 64-bit-offset
-  blocks and push copies, and weighted float32 / float64 blocks.  Partition = the oracle's and single-GPU WCC's; every
-  label a vertex of its own component that carries its own label.
+- Every rank of a grid in one process (tests/mg_world.py) running cugraph_b200.mg.MGGraph.weakly_connected_components:
+  grids 1x2, 2x1, 2x2 and 4x2 on the components graph and a symmetrised RMAT-8, a tiny graph that leaves blocks without
+  edges, 64-bit-offset blocks and push copies, and weighted float32 / float64 blocks.  Partition = the oracle's and
+  single-GPU WCC's; every label a vertex of its own component that carries its own label.
 - cugraph_b200_block_wcc_min called directly against a numpy min: every column active, a few, none.
-- World sizes 2, 4 and 8 over gloo running cugraph_b200.mg.MGGraph.weakly_connected_components (the real orchestration).
+- World sizes 2, 4 and 8 over gloo running MGGraph.weakly_connected_components (the real process groups).
 - The error paths of the entry point."""
 import ctypes as C
 import os
@@ -18,7 +18,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from tests import mg_procs  # noqa: E402
-from tests import mg_wcc_sim as sim  # noqa: E402
+from tests import mg_wcc_ref as refs  # noqa: E402
+from tests import mg_world  # noqa: E402
 from tests.emu_py import surface  # noqa: E402, F401
 
 GRIDS = [(1, 2), (2, 1), (2, 2), (4, 2)]
@@ -26,41 +27,43 @@ GRID_IDS = ["1x2", "2x1", "2x2", "4x2"]
 
 
 @pytest.mark.parametrize("R,Cc", GRIDS, ids=GRID_IDS)
-def test_mg_wcc_simulated_emulated(surface, R, Cc):
-    s, d, V, path_len = sim.components_graph()
-    labels, stats = sim.simulate(s, d, V, R, Cc)
-    sim.check(s, d, V, labels, single=sim.single_gpu_wcc(s, d, V))
+def test_mg_wcc_simulated_emulated(surface, monkeypatch, R, Cc):
+    world = mg_world.grid_world(monkeypatch, R, Cc)
+    s, d, V, path_len = refs.components_graph()
+    labels, stats, _ = refs.mg_wcc(s, d, V, world)
+    refs.check(s, d, V, labels, single=refs.single_gpu_wcc(s, d, V))
     assert stats["rounds"] >= path_len // 2, stats
-    s, d, V = sim.rmat_graph(8)
-    labels, _ = sim.simulate(s, d, V, R, Cc)
-    sim.check(s, d, V, labels, single=sim.single_gpu_wcc(s, d, V))
+    s, d, V = refs.rmat_graph(8)
+    labels, _, _ = refs.mg_wcc(s, d, V, world)
+    refs.check(s, d, V, labels, single=refs.single_gpu_wcc(s, d, V))
 
 
-def test_mg_wcc_empty_blocks_emulated(surface):
+def test_mg_wcc_empty_blocks_emulated(surface, monkeypatch):
     """three edges over eight blocks: most ranks' blocks have no edges"""
     s = np.array([0, 1, 5, 9, 9, 2], np.int32)
     d = np.array([1, 0, 9, 5, 2, 9], np.int32)
     V = 12
-    labels, stats = sim.simulate(s, d, V, 4, 2)
-    assert stats["empty_blocks"] > 0
-    sim.check(s, d, V, labels, single=sim.single_gpu_wcc(s, d, V))
+    labels, _, empty = refs.mg_wcc(s, d, V, mg_world.grid_world(monkeypatch, 4, 2))
+    assert empty > 0
+    refs.check(s, d, V, labels, single=refs.single_gpu_wcc(s, d, V))
 
 
 def test_mg_wcc_simulated_offs64_emulated(surface, monkeypatch):
     """CUGRAPH_B200_OFFS64_MIN_EDGES=0: the blocks and their push copies get 64-bit offsets"""
     monkeypatch.setenv("CUGRAPH_B200_OFFS64_MIN_EDGES", "0")
-    s, d, V, _ = sim.components_graph()
-    labels, _ = sim.simulate(s, d, V, 2, 2)
+    s, d, V, _ = refs.components_graph()
+    labels, _, _ = refs.mg_wcc(s, d, V, mg_world.grid_world(monkeypatch, 2, 2))
     monkeypatch.delenv("CUGRAPH_B200_OFFS64_MIN_EDGES")
-    sim.check(s, d, V, labels, single=sim.single_gpu_wcc(s, d, V))
+    refs.check(s, d, V, labels, single=refs.single_gpu_wcc(s, d, V))
 
 
 @pytest.mark.parametrize("wdtype", [np.float32, np.float64], ids=["f32", "f64"])
-def test_mg_wcc_weighted_blocks_emulated(surface, wdtype):
-    s, d, V, _ = sim.components_graph()
-    want, _ = sim.simulate(s, d, V, 2, 2)
+def test_mg_wcc_weighted_blocks_emulated(surface, monkeypatch, wdtype):
+    world = mg_world.grid_world(monkeypatch, 2, 2)
+    s, d, V, _ = refs.components_graph()
+    want, _, _ = refs.mg_wcc(s, d, V, world)
     w = np.random.default_rng(1).random(s.size).astype(wdtype)
-    got, _ = sim.simulate(s, d, V, 2, 2, w=w)
+    got, _, _ = refs.mg_wcc(s, d, V, world, w=w)
     assert np.array_equal(got, want)
 
 
@@ -167,7 +170,7 @@ def test_block_wcc_entry_errors_emulated(surface):
 # ---------------------------------------------------------------------------------------------------------- gloo runs
 def _gloo_graph():
     """the components graph with scattered 64-bit external ids (isolated ids are not vertices of an MG graph)"""
-    s, d, V, path_len = sim.components_graph(seed=9)
+    s, d, V, path_len = refs.components_graph(seed=9)
     ids = np.random.default_rng(9).choice(10**9, size=V, replace=False).astype(np.int64) + 10**10
     return ids, s, d, V, path_len
 
@@ -198,7 +201,7 @@ def test_mg_wcc_emulated_gloo(world):
         n += r["verts"].size
     assert n == present.size
     ref = oracle.wcc(s, d, V)
-    assert sim.same_partition(labels[present], ref[present])
+    assert refs.same_partition(labels[present], ref[present])
     assert np.array_equal(ref[labels[present]], ref[present])
     assert np.array_equal(labels[labels[present]], labels[present])
     stats = [r["stats"] for r in res]

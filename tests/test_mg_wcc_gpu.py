@@ -1,10 +1,10 @@
 """Multi-GPU weakly connected components on the GPU.
 
-- All ranks of a 2D partition on ONE GPU (tests/mg_wcc_sim.py) through the real block kernels: grids 1x2, 2x1, 2x2 and 4x2
-  on symmetrised RMAT-14 and RMAT-16 and on the components graph, on 64-bit-offset blocks, and on weighted float32 /
-  float64 blocks.
-- A world-size-1 NCCL process group running cugraph_b200.mg.MGGraph.weakly_connected_components (the 1x1 grid): the real
-  orchestration and the real stream ordering on the device.
+- Every rank of a grid on ONE GPU in one process (tests/mg_world.py) running
+  cugraph_b200.mg.MGGraph.weakly_connected_components: grids 1x2, 2x1, 2x2 and 4x2 on symmetrised RMAT-14 and RMAT-16
+  and on the components graph, on 64-bit-offset blocks, and on weighted float32 / float64 blocks.
+- A world-size-1 NCCL process group running MGGraph.weakly_connected_components (the 1x1 grid): the real collectives and
+  the real stream ordering on the device.
 - 2 and 4 GPUs over NCCL (skipped when fewer GPUs are visible).
 Partition = the oracle's and single-GPU cugraph_weakly_connected_components'; every label a vertex of its own component
 that carries its own label."""
@@ -18,44 +18,47 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from tests import mg_procs  # noqa: E402
-from tests import mg_wcc_sim as sim  # noqa: E402
+from tests import mg_wcc_ref as refs  # noqa: E402
+from tests import mg_world  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("R,Cc", [(1, 2), (2, 1), (2, 2), (4, 2)], ids=["1x2", "2x1", "2x2", "4x2"])
-def test_mg_wcc_simulated_on_one_gpu(R, Cc):
+def test_mg_wcc_simulated_on_one_gpu(monkeypatch, R, Cc):
+    world = mg_world.grid_world(monkeypatch, R, Cc)
     for scale in (14, 16):
-        s, d, V = sim.rmat_graph(scale)
-        labels, _ = sim.simulate(s, d, V, R, Cc, device="cuda")
-        sim.check(s, d, V, labels, single=sim.single_gpu_wcc(s, d, V))
-    s, d, V, path_len = sim.components_graph()
-    labels, stats = sim.simulate(s, d, V, R, Cc, device="cuda")
-    sim.check(s, d, V, labels, single=sim.single_gpu_wcc(s, d, V))
+        s, d, V = refs.rmat_graph(scale)
+        labels, _, _ = refs.mg_wcc(s, d, V, world, device="cuda")
+        refs.check(s, d, V, labels, single=refs.single_gpu_wcc(s, d, V))
+    s, d, V, path_len = refs.components_graph()
+    labels, stats, _ = refs.mg_wcc(s, d, V, world, device="cuda")
+    refs.check(s, d, V, labels, single=refs.single_gpu_wcc(s, d, V))
     assert stats["rounds"] >= path_len // 2, stats
 
 
 def test_mg_wcc_simulated_offs64_on_one_gpu(monkeypatch):
     monkeypatch.setenv("CUGRAPH_B200_OFFS64_MIN_EDGES", "0")
-    s, d, V = sim.rmat_graph(14)
-    labels, _ = sim.simulate(s, d, V, 2, 2, device="cuda")
+    s, d, V = refs.rmat_graph(14)
+    labels, _, _ = refs.mg_wcc(s, d, V, mg_world.grid_world(monkeypatch, 2, 2), device="cuda")
     monkeypatch.delenv("CUGRAPH_B200_OFFS64_MIN_EDGES")
-    sim.check(s, d, V, labels, single=sim.single_gpu_wcc(s, d, V))
+    refs.check(s, d, V, labels, single=refs.single_gpu_wcc(s, d, V))
 
 
 @pytest.mark.parametrize("wdtype", [np.float32, np.float64], ids=["f32", "f64"])
-def test_mg_wcc_weighted_blocks_on_one_gpu(wdtype):
-    s, d, V = sim.rmat_graph(14)
-    want, _ = sim.simulate(s, d, V, 2, 2, device="cuda")
+def test_mg_wcc_weighted_blocks_on_one_gpu(monkeypatch, wdtype):
+    world = mg_world.grid_world(monkeypatch, 2, 2)
+    s, d, V = refs.rmat_graph(14)
+    want, _, _ = refs.mg_wcc(s, d, V, world, device="cuda")
     w = np.random.default_rng(1).random(s.size).astype(wdtype)
-    got, _ = sim.simulate(s, d, V, 2, 2, w=w, device="cuda")
+    got, _, _ = refs.mg_wcc(s, d, V, world, w=w, device="cuda")
     assert np.array_equal(got, want)
 
 
 # ------------------------------------------------------------------------------------------------- NCCL process groups
 def _graphs():
-    s, d, V = sim.rmat_graph(14)
-    cs, cd, cV, _ = sim.components_graph()
+    s, d, V = refs.rmat_graph(14)
+    cs, cd, cV, _ = refs.components_graph()
     return [(s, d, V), (cs, cd, cV)]
 
 
@@ -86,7 +89,7 @@ def _run_nccl(world):
             n += v.size
             assert st == res[0][i][2]                   # every rank ran the same rounds
         assert n == present.size
-        sim.check(s, d, V, labels, single=sim.single_gpu_wcc(s, d, V))
+        refs.check(s, d, V, labels, single=refs.single_gpu_wcc(s, d, V))
 
 
 def test_mg_wcc_nccl_world_size_1():
