@@ -127,6 +127,8 @@ def lib():
     _sig(L.cugraph_b200_create_resource_handle_on_stream, vp, [vp])
     _sig(L.cugraph_b200_padded_elems, sz, [sz, sz])
     _sig(L.cugraph_b200_block_create, i32, [vp, sz, sz, vp, vp, vp, pvp, pvp])
+    _sig(L.cugraph_b200_block_stage_edges, i32, [vp, sz, sz, vp, vp, vp, vp, i32, i32, C.POINTER(sz), pvp])
+    _sig(L.cugraph_b200_block_degrees, i32, [vp, vp, vp, vp, pvp])
     _sig(L.cugraph_b200_block_free, None, [vp])
     _sig(L.cugraph_b200_block_span, sz, [vp])
     _sig(L.cugraph_b200_block_pull_sweep, i32, [vp, vp, vp, vp, dbl, pvp])

@@ -145,5 +145,10 @@ std::unique_ptr<csx_t> build_binned_rows(handle_impl const& h, int32_t const* ma
                                          cugraph_data_type_id_t wtype, int64_t n, int32_t nv);
 // the vertex (row_vertex, or the physical row) of every edge of a csx, in edge order
 dbuf expand_majors(handle_impl const& h, csx_t const& c);
+// multi-GPU staging of one edge block (cugraph_b200_block_stage_edges): the n edges (rows, cols[, reversed][, w]) in
+// slot coordinates, rewritten in place; returns how many are left
+int64_t stage_block_edges(handle_impl const& h, int32_t n_rows, int32_t n_cols, int32_t* rows, int32_t* cols,
+                          uint8_t const* reversed, void* w, cugraph_data_type_id_t wtype, int64_t n, bool drop_multi_edges,
+                          bool symmetrize);
 
 }  // namespace b200

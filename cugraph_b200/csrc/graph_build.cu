@@ -691,6 +691,144 @@ void symmetrize_ranks(handle_impl const& h, dbuf& src, dbuf& dst, dbuf& w, cugra
 }
 
 // ---------------------------------------------------------------------------------------------
+// staging of one multi-GPU edge block.  Edge u -> v sits at position (row = slot of v, col = slot of u); with symmetrize the
+// caller has also shuffled a reversed copy (flag 1) of every non-self-loop edge v -> u to that position, so the position
+// holds the whole group of the unordered pair {u, v}.  The same rules as single-GPU staging then apply locally:
+// multi-edges -> the minimum weight per (row, col, flag) (weight-key sort, stable key sort, run heads, as build_csx_typed);
+// symmetrize -> symmetrize_typed's pairing, the i-th lightest flag-0 edge with the i-th lightest flag-1 edge, emitting
+// only the orientation stored here (the position (row = u, col = v) sees the same group from the other side and emits
+// the other one, with the bit-identical averaged weight).
+// ---------------------------------------------------------------------------------------------
+namespace {
+
+__global__ void k_block_stage_keys(int32_t const* rows, int32_t const* cols, uint8_t const* rev, int64_t n, int bits,
+                                   uint64_t* keys)
+{
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const uint64_t pos = ((uint64_t)(uint32_t)rows[i] << bits) | (uint32_t)cols[i];
+    keys[i]            = (pos << 1) | (rev && rev[i] ? 1ull : 0ull);
+  }
+}
+
+// keep[i] and the weight of element i of the sorted group of its position: a flag-0 edge always stays, averaged with the
+// flag-1 edge of the same rank when there is one; a flag-1 edge stays when it has no flag-0 partner
+template <typename W>
+__global__ void k_block_pair(uint64_t const* keys, W const* w, int64_t n, uint8_t* keep, W* w_out)
+{
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const uint64_t pos = keys[i] >> 1;
+    const int64_t r0 = lb64(keys, n, pos << 1), r1 = lb64(keys, n, (pos << 1) | 1ull), r2 = lb64(keys, n, (pos << 1) + 2ull);
+    if (keys[i] & 1ull) {
+      keep[i] = (i - r1) >= (r1 - r0) ? 1 : 0;
+      if (w) w_out[i] = w[i];
+    } else {
+      const int64_t j = i - r0;
+      keep[i]         = 1;
+      if (w) w_out[i] = j < r2 - r1 ? (W)((w[i] + w[r1 + j]) / (W)2) : w[i];
+    }
+  }
+}
+
+__global__ void k_block_unpack(uint64_t const* keys, int64_t n, int bits, int32_t* rows, int32_t* cols)
+{
+  const uint64_t mask = (1ull << bits) - 1ull;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    rows[i] = (int32_t)(keys[i] >> (bits + 1));
+    cols[i] = (int32_t)((keys[i] >> 1) & mask);
+  }
+}
+
+template <typename W>
+int64_t stage_block_typed(handle_impl const& h, int bits, int32_t* rows, int32_t* cols, uint8_t const* rev, W* w, int64_t n,
+                          bool drop_multi_edges, bool symmetrize)
+{
+  const int key_bits = 2 * bits + 1;
+  dbuf keys = make_dbuf<uint64_t>(n, h.stream), keys2 = make_dbuf<uint64_t>(n, h.stream);
+  B200_LAUNCH(h, k_block_stage_keys, grid_for(n, 4), kBlock, 0, rows, cols, symmetrize ? rev : nullptr, n, bits,
+              keys.as<uint64_t>());
+  dbuf ws;  // the weights in key order
+  if (w == nullptr) {
+    sort_keys<uint64_t>(h, keys.as<uint64_t>(), keys2.as<uint64_t>(), n, 0, key_bits);
+  } else {
+    // stable two-pass: by weight first, so that every group of equal keys is in ascending weight
+    B200_EXPECTS(n < (1ll << 32), CUGRAPH_INVALID_INPUT, "weighted graphs are limited to 2^32 edges per GPU");
+    using U   = typename std::conditional<sizeof(W) == 4, uint32_t, uint64_t>::type;
+    dbuf perm = make_dbuf<uint32_t>(n, h.stream), perm2 = make_dbuf<uint32_t>(n, h.stream);
+    dbuf wk = make_dbuf<U>(n, h.stream), wk2 = make_dbuf<U>(n, h.stream);
+    B200_LAUNCH(h, k_iota<uint32_t>, grid_for(n, 4), kBlock, 0, perm.as<uint32_t>(), n);
+    B200_LAUNCH(h, (k_weight_keys<W, U>), grid_for(n, 4), kBlock, 0, w, n, wk.as<U>());
+    sort_pairs<U, uint32_t>(h, wk.as<U>(), wk2.as<U>(), perm.as<uint32_t>(), perm2.as<uint32_t>(), n, 0, (int)sizeof(U) * 8);
+    wk.release();
+    wk2.release();
+    B200_LAUNCH(h, (k_gather<uint64_t>), grid_for(n, 4), kBlock, 0, keys.as<uint64_t>(), perm2.as<uint32_t>(), n,
+                keys2.as<uint64_t>());
+    sort_pairs<uint64_t, uint32_t>(h, keys2.as<uint64_t>(), keys.as<uint64_t>(), perm2.as<uint32_t>(), perm.as<uint32_t>(), n,
+                                   0, key_bits);
+    std::swap(keys, keys2);
+    ws = make_dbuf<W>(n, h.stream);
+    B200_LAUNCH(h, (k_gather<W>), grid_for(n, 4), kBlock, 0, w, perm.as<uint32_t>(), n, ws.as<W>());
+  }
+  // keys2 holds the sorted keys, ws their weights; each pass below selects the flagged ones into keys / wsel, then swaps
+  int64_t m = n;
+  dbuf flag = make_dbuf<uint8_t>(n, h.stream);
+  auto select = [&](dbuf const& wsrc) {
+    const int64_t k = select_flagged<uint64_t>(h, keys2.as<uint64_t>(), flag.as<uint8_t>(), keys.as<uint64_t>(), m);
+    std::swap(keys, keys2);
+    if (w != nullptr) {
+      dbuf wsel = make_dbuf<W>(k, h.stream);
+      select_flagged<W>(h, wsrc.as<W>(), flag.as<uint8_t>(), wsel.as<W>(), m);
+      ws = std::move(wsel);
+    }
+    m = k;
+  };
+  if (drop_multi_edges) {
+    B200_LAUNCH(h, k_run_heads, grid_for(m, 4), kBlock, 0, keys2.as<uint64_t>(), m, flag.as<uint8_t>());
+    select(ws);
+  }
+  if (symmetrize && m > 0) {
+    dbuf wp;
+    if (w != nullptr) wp = make_dbuf<W>(m, h.stream);
+    B200_LAUNCH(h, (k_block_pair<W>), grid_for(m, 2), kBlock, 0, keys2.as<uint64_t>(), w ? ws.as<W>() : (W const*)nullptr, m,
+                flag.as<uint8_t>(), w ? wp.as<W>() : (W*)nullptr);
+    select(wp);
+  }
+  if (m > 0) {
+    B200_LAUNCH(h, k_block_unpack, grid_for(m, 4), kBlock, 0, keys2.as<uint64_t>(), m, bits, rows, cols);
+    if (w != nullptr) CUDA_TRY(cudaMemcpyAsync(w, ws.data(), m * sizeof(W), cudaMemcpyDeviceToDevice, h.stream));
+  }
+  check_last("stage_block_edges");
+  sync(h);
+  return m;
+}
+
+}  // namespace
+
+int64_t stage_block_edges(handle_impl const& h, int32_t n_rows, int32_t n_cols, int32_t* rows, int32_t* cols,
+                          uint8_t const* reversed, void* w, cugraph_data_type_id_t wtype, int64_t n, bool drop_multi_edges,
+                          bool symmetrize)
+{
+  const int bits = bits_for(std::max<int64_t>(std::max(n_rows, n_cols), 2));
+  B200_EXPECTS(2 * bits + 1 <= 64, CUGRAPH_INVALID_INPUT, "too many slots to stage");
+  B200_EXPECTS(!symmetrize || 2 * n < (1ll << 31), CUGRAPH_INVALID_INPUT, "symmetrize: edge list too large for one GPU pass");
+  if (n == 0) return 0;
+  // every slot in range: [min, max] of the rows and of the columns in one read-back
+  dbuf mm = make_dbuf<long long>(4, h.stream);
+  long long init[4] = {LLONG_MAX, LLONG_MIN, LLONG_MAX, LLONG_MIN};
+  CUDA_TRY(cudaMemcpyAsync(mm.data(), init, sizeof(init), cudaMemcpyHostToDevice, h.stream));
+  B200_LAUNCH(h, (k_minmax<int32_t>), grid_for(n, 8, 2048), kBlock, 0, rows, n, mm.as<long long>(), mm.as<long long>() + 1);
+  B200_LAUNCH(h, (k_minmax<int32_t>), grid_for(n, 8, 2048), kBlock, 0, cols, n, mm.as<long long>() + 2,
+              mm.as<long long>() + 3);
+  long long hmm[4];
+  CUDA_TRY(cudaMemcpyAsync(hmm, mm.data(), sizeof(hmm), cudaMemcpyDeviceToHost, h.stream));
+  sync(h);
+  B200_EXPECTS(hmm[0] >= 0 && hmm[1] < n_rows && hmm[2] >= 0 && hmm[3] < n_cols, CUGRAPH_INVALID_INPUT,
+               "edge slots out of range of the block");
+  if (w == nullptr || wtype == FLOAT32)
+    return stage_block_typed<float>(h, bits, rows, cols, reversed, (float*)w, n, drop_multi_edges, symmetrize);
+  return stage_block_typed<double>(h, bits, rows, cols, reversed, (double*)w, n, drop_multi_edges, symmetrize);
+}
+
+// ---------------------------------------------------------------------------------------------
 // the staging entry point used by capi_graph.cu
 // ---------------------------------------------------------------------------------------------
 template <typename VT>

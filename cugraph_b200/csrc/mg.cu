@@ -401,6 +401,21 @@ struct block_wcc_op {
   }
 };
 
+// the block's edge counts per row slot (from the offsets, through row_vertex) and per column slot (a histogram)
+template <typename O>
+__global__ void __launch_bounds__(kBlock)
+k_block_degrees(O const* __restrict__ off, int32_t const* __restrict__ row_vertex, int32_t n_phys, int32_t const* __restrict__ idx,
+                long long nnz, long long* __restrict__ row_deg, long long* __restrict__ col_deg)
+{
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < nnz || i < n_phys; i += (long long)gridDim.x * blockDim.x) {
+    if (i < n_phys) {
+      const long long d = (long long)off[i + 1] - (long long)off[i];
+      if (d) row_deg[row_vertex[i]] = d;   // a row slot with edges lies below n_rows
+    }
+    if (i < nnz) atomicAdd((unsigned long long*)(col_deg + idx[i]), 1ull);
+  }
+}
+
 // the two PageRank owner-step entry points: argument checks and the launch (pv == nullptr: uniform teleport)
 void pagerank_vertex_step(handle_impl const& h, device_array_view_impl const* yv, device_array_view_impl const* pv,
                           device_array_view_impl const* ov, device_array_view_impl const* xv,
@@ -462,6 +477,62 @@ cugraph_error_code_t cugraph_b200_block_create(const cugraph_resource_handle_t* 
     prepare_pull_sweep(h, *b->csx, b->n_span, b->wtype == FLOAT64 ? 8 : 4);
     sync(h);
     *block = reinterpret_cast<cugraph_b200_block_t*>(b.release());
+  });
+}
+
+cugraph_error_code_t cugraph_b200_block_stage_edges(const cugraph_resource_handle_t* handle, size_t n_rows, size_t n_cols,
+                                                    cugraph_type_erased_device_array_view_t* rows,
+                                                    cugraph_type_erased_device_array_view_t* cols,
+                                                    const cugraph_type_erased_device_array_view_t* reversed,
+                                                    cugraph_type_erased_device_array_view_t* weights, bool_t drop_multi_edges,
+                                                    bool_t symmetrize, size_t* n_out, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(rows && cols && n_out, CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto const* r = V(rows);
+    auto const* c = V(cols);
+    auto const* f = V(reversed);
+    auto const* w = V(weights);
+    B200_EXPECTS(r->type == INT32 && c->type == INT32 && r->size == c->size, CUGRAPH_INVALID_INPUT,
+                 "block rows / cols must be INT32 arrays of equal size");
+    B200_EXPECTS(f == nullptr || (dtype_size(f->type) == 1 && f->size == r->size), CUGRAPH_INVALID_INPUT,
+                 "reversed must hold one byte flag per edge");
+    B200_EXPECTS(w == nullptr || ((w->type == FLOAT32 || w->type == FLOAT64) && w->size == r->size), CUGRAPH_INVALID_INPUT,
+                 "block weights must be FLOAT32 / FLOAT64 with one value per edge");
+    B200_EXPECTS(n_rows < (1u << 31) && n_cols < (1u << 31), CUGRAPH_INVALID_INPUT, "block too large");
+    *n_out = (size_t)stage_block_edges(h, (int32_t)n_rows, (int32_t)n_cols, (int32_t*)r->data, (int32_t*)c->data,
+                                       f ? (uint8_t const*)f->data : nullptr, w ? w->data : nullptr, w ? w->type : FLOAT32,
+                                       (int64_t)r->size, drop_multi_edges == TRUE, symmetrize == TRUE);
+  });
+}
+
+cugraph_error_code_t cugraph_b200_block_degrees(const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+                                                cugraph_type_erased_device_array_view_t* row_counts,
+                                                cugraph_type_erased_device_array_view_t* col_counts, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(block && row_counts && col_counts, CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto const* b  = reinterpret_cast<block_impl const*>(block);
+    auto const* rv = V(row_counts);
+    auto const* cv = V(col_counts);
+    B200_EXPECTS(rv->type == INT64 && cv->type == INT64, CUGRAPH_INVALID_INPUT, "row_counts / col_counts must be INT64");
+    B200_EXPECTS(rv->size >= (size_t)b->n_rows && cv->size >= (size_t)b->n_cols, CUGRAPH_INVALID_INPUT,
+                 "count arrays shorter than the block's slots");
+    CUDA_TRY(cudaMemsetAsync(rv->data, 0, (size_t)b->n_rows * sizeof(long long), h.stream));
+    CUDA_TRY(cudaMemsetAsync(cv->data, 0, (size_t)b->n_cols * sizeof(long long), h.stream));
+    csx_t const& c   = *b->csx;
+    const long long n = std::max<long long>(c.nnz, c.n_rows);
+    if (n == 0) return;
+    const int grid = grid_for(n, 1, h.sm_count * 8);
+    if (c.offs64)
+      B200_LAUNCH(h, k_block_degrees<int64_t>, grid, kBlock, 0, c.offsets.as<int64_t>(), c.row_vertex.as<int32_t>(), c.n_rows,
+                  c.indices.as<int32_t>(), (long long)c.nnz, (long long*)rv->data, (long long*)cv->data);
+    else
+      B200_LAUNCH(h, k_block_degrees<int32_t>, grid, kBlock, 0, c.offsets.as<int32_t>(), c.row_vertex.as<int32_t>(), c.n_rows,
+                  c.indices.as<int32_t>(), (long long)c.nnz, (long long*)rv->data, (long long*)cv->data);
+    check_last("block_degrees");
   });
 }
 

@@ -157,6 +157,12 @@ def _unique_big(tensors, chunk=1 << 29):
 # ----------------------------------------------------------------------------------------------
 # 2D partition
 # ----------------------------------------------------------------------------------------------
+# the most shuffled edges per GPU that cugraph_b200_block_stage_edges takes (single-GPU staging's bounds): 2n < 2^31 with
+# symmetrize, n < 2^32 with weights
+STAGE_MAX_SYMMETRIZED = (1 << 30) - 1
+STAGE_MAX_WEIGHTED = (1 << 32) - 1
+
+
 @dataclass
 class Partition:
     groups: Groups
@@ -167,19 +173,47 @@ class Partition:
     n_local: int
     maxpart: int
     n_global: int
+    reversed: object = None   # uint8 per local edge with symmetrize: 1 = the reversed copy of an edge v -> u, else None
 
 
-def partition_edges(src: torch.Tensor, dst: torch.Tensor, weights=None, groups: Groups | None = None) -> Partition:
+def partition_edges(src: torch.Tensor, dst: torch.Tensor, weights=None, groups: Groups | None = None, *, vertices=None,
+                    drop_self_loops=False, drop_multi_edges=False, symmetrize=False) -> Partition:
     """Shuffle this rank's share of the edge list into the 2D partition and renumber.
-    Edge (u -> v) is stored on GPU (r(owner(v)), c(owner(u)))  (graph_partition_utils.cuh:101-128)."""
+    Edge (u -> v) is stored on GPU (r(owner(v)), c(owner(u)))  (graph_partition_utils.cuh:101-128).
+    vertices: external ids (the edge ids' dtype) that are vertices also without an edge, sent to their owners with the
+    referenced ids; drop_self_loops: edges u -> u are dropped first; symmetrize: a reversed copy v -> u of every other edge
+    travels with it, flagged in Partition.reversed (MGGraph stages the block from them).  drop_multi_edges changes nothing
+    here; with it or symmetrize, the size bounds of cugraph_b200_block_stage_edges are checked on the shuffled edges.  Every
+    rank raises the same error, after the one MAX all-reduce that also gives maxpart: TypeError for a `vertices` dtype that
+    differs from the edge ids' on some rank, ValueError for a rank with too many shuffled edges to stage."""
     g = groups or make_groups()
     P, Cc = g.world, g.C
+    bad_vertices = 0
+    if vertices is not None:
+        vertices = torch.as_tensor(vertices)
+        if vertices.dtype != src.dtype:
+            bad_vertices, vertices = 1, None     # sent as none; every rank raises after the all-reduce below
+        else:
+            vertices = torch.unique(vertices.to(src.device).reshape(-1))
+    if drop_self_loops:
+        keep = src != dst
+        src, dst = src[keep], dst[keep]
+        weights = weights[keep] if weights is not None else None
+    rev = None
+    if symmetrize:
+        other = src != dst
+        n_rev = int(other.sum().item())
+        src, dst = torch.cat([src, dst[other]]), torch.cat([dst, src[other]])
+        weights = torch.cat([weights, weights[other]]) if weights is not None else None
+        rev = torch.cat([torch.zeros(src.numel() - n_rev, dtype=torch.uint8, device=src.device),
+                         torch.ones(n_rev, dtype=torch.uint8, device=src.device)])
     so, do = vertex_owner(src, P), vertex_owner(dst, P)
     target = (do // Cc) * Cc + (so % Cc)
-    payload = [src, dst] + ([weights] if weights is not None else [])
+    payload = [src, dst] + ([weights] if weights is not None else []) + ([rev] if rev is not None else [])
     recv, _, _, _ = exchange(payload, target, P)
     src_e, dst_e = recv[0], recv[1]
     w_e = recv[2] if weights is not None else None
+    rev_e = recv[-1] if rev is not None else None
     # vertices referenced here -> their owners, together with how often each is a SOURCE here; the owner
     # numbers its vertices by descending global out-degree so that hot sources get the lowest local ids
     # (the column-blocked sweep keeps the lowest column ids in shared memory) — the role of the
@@ -187,8 +221,12 @@ def partition_edges(src: torch.Tensor, dst: torch.Tensor, weights=None, groups: 
     u = _unique_big([src_e, dst_e])
     ks = torch.searchsorted(u, src_e)
     cnt = torch.bincount(ks, minlength=u.numel()).to(torch.int64)
-    ou = vertex_owner(u, P)
-    (recv_ids, recv_cnt), order, sc, rc = exchange([u, cnt], ou, P)
+    ids, ids_cnt = u, cnt
+    if vertices is not None:   # listed vertices travel with the referenced ids, as sources of no edge
+        ids = torch.cat([u, vertices])
+        ids_cnt = torch.cat([cnt, torch.zeros(vertices.numel(), dtype=torch.int64, device=cnt.device)])
+    ou = vertex_owner(ids, P)
+    (recv_ids, recv_cnt), order, sc, rc = exchange([ids, ids_cnt], ou, P)
     mine, inv = torch.unique(recv_ids, return_inverse=True)   # sorted external ids owned by this rank
     n_local = int(mine.numel())
     deg = torch.zeros(n_local, dtype=torch.int64, device=src.device).index_add_(0, inv, recv_cnt)
@@ -202,18 +240,26 @@ def partition_edges(src: torch.Tensor, dst: torch.Tensor, weights=None, groups: 
     lid = torch.empty_like(back)
     lid[order] = back                                   # lid[k] = local id (at its owner) of u[k]
     t = torch.tensor([n_local, n_local], dtype=torch.int64, device=src.device)
-    mx = t[:1].clone()
+    n_e = src_e.numel()
+    too_many = int((symmetrize and n_e > STAGE_MAX_SYMMETRIZED) or
+                   ((symmetrize or drop_multi_edges) and weights is not None and n_e > STAGE_MAX_WEIGHTED))
+    mx = torch.tensor([n_local, bad_vertices, too_many], dtype=torch.int64, device=src.device)   # input errors ride along
     dist.all_reduce(mx, op=dist.ReduceOp.MAX)
+    if int(mx[1].item()):
+        raise TypeError("MGGraph: vertices must have the dtype of the edge ids on every rank")
+    if int(mx[2].item()):
+        raise ValueError("MGGraph: too many edges on one GPU to stage (symmetrize needs 2n < 2^31, weighted multi-edge "
+                         "removal n < 2^32 shuffled edges per GPU)")
     tot = t[1:].clone()
     dist.all_reduce(tot, op=dist.ReduceOp.SUM)
-    maxpart = max(int(mx.item()), 1)
+    maxpart = max(int(mx[0].item()), 1)
     kd = torch.searchsorted(u, dst_e)
     rows = ((ou[kd] % Cc) * maxpart + lid[kd]).to(torch.int32)
     # columns are partition-major (slot = r_u * maxpart + lid): exactly the layout all_gather_into_tensor produces, so the
     # gathered x is consumed in place (an interleaved order put all hot sources into the first column block but cost a
     # strided 4 * n_cols-byte transpose copy per iteration; every partition's hot sources still lead ITS column range)
     cols = ((ou[ks] // Cc) * maxpart + lid[ks]).to(torch.int32)
-    return Partition(g, rows, cols, w_e, mine, n_local, maxpart, int(tot.item()))
+    return Partition(g, rows, cols, w_e, mine, n_local, maxpart, int(tot.item()), rev_e)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -241,20 +287,41 @@ def _global_count(mask):
 
 
 class MGGraph:
-    """This rank's edge block of a 2D-partitioned graph (pull orientation: rows = destinations)."""
+    """This rank's edge block of a 2D-partitioned graph (pull orientation: rows = destinations).
 
-    def __init__(self, src, dst, weights=None, groups: Groups | None = None, dtype=torch.float32):
+    src, dst (and weights) are this rank's share of the edge list, in external ids.  The keyword options are those of the
+    single-GPU constructor (cugraph_graph_create_sg), applied in the reference's order, and must be the same on every rank
+    (not checked: with drop_self_loops or symmetrize differing between ranks the shuffle's collectives do not match):
+      vertices: external ids, in the edge ids' dtype, that are vertices of the graph also without an edge (any rank may pass
+        any ids, or None; duplicates are merged).  The vertices are these and the endpoints of the edges left after
+        self-loop removal.
+      drop_self_loops: edges u -> u are dropped.
+      drop_multi_edges: one edge per (u, v) is kept, the one of MINIMUM weight, whatever order the edges arrive in.  Single
+        GPU keeps the minimum only for a graph declared symmetric and otherwise the first copy in input order.
+      symmetrize: single GPU's pairing rule: the edges between u and v are grouped, the i-th lightest u -> v edge paired with
+        the i-th lightest v -> u edge becomes one undirected edge of the averaged weight (W)((a + b) / 2), unpaired edges keep
+        their weight; every undirected edge is stored in both directions, a self-loop once.
+    Errors raise on every rank: TypeError for a `vertices` dtype other than the edge ids' on any rank, ValueError for a rank
+    with more shuffled edges than staging takes (see partition_edges), and a CugraphError when staging fails on some rank
+    (that rank's own error, CugraphRuntimeError on the others; with drop_multi_edges or symmetrize only: one all-reduce of
+    the outcome).  With every option at its default the construction is the plain shuffle of the edges as given."""
+
+    def __init__(self, src, dst, weights=None, groups: Groups | None = None, dtype=torch.float32, *, vertices=None,
+                 drop_self_loops=False, drop_multi_edges=False, symmetrize=False):
         from cugraph_b200 import _capi
         from cugraph_b200.pylibcugraph.resource_handle import ResourceHandle
         assert src.is_cuda or _capi.emulated(), "MGGraph needs CUDA tensors"
         self.lib = _capi.lib()
         self._capi = _capi
         self.dtype = dtype if weights is None else weights.dtype
-        self.part = partition_edges(src, dst, weights, groups)
+        self.part = partition_edges(src, dst, weights, groups, vertices=vertices, drop_self_loops=drop_self_loops,
+                                    drop_multi_edges=drop_multi_edges, symmetrize=symmetrize)
         p = self.part
         g = p.groups
         self.handle = ResourceHandle(stream=torch.cuda.current_stream().cuda_stream)
         self.n_rows, self.n_cols = g.C * p.maxpart, g.R * p.maxpart
+        if drop_multi_edges or symmetrize:
+            self._stage_edges(drop_multi_edges, symmetrize)
         es = 4 if self.dtype == torch.float32 else 8
         blk = C.c_void_p()
         with _views(p.rows, p.cols, p.weights) as (rv, cv, wv):
@@ -277,9 +344,52 @@ class MGGraph:
         self.last_sssp_stats = None
         self.last_wcc_stats = None
         self.last_katz_stats = self.last_eigenvector_stats = self.last_hits_stats = None
+        self._degrees = None                                   # (in, out) of the owned slice, made by the first degrees()
         self.device = src.device
         p.rows = p.cols = p.weights = None  # the block owns its own copy
         torch.cuda.synchronize()
+
+    def _stage_edges(self, drop_multi_edges, symmetrize):
+        """multi-edge removal and symmetrization of this rank's shuffled edges, on the device (cugraph_b200_block_stage_edges,
+        in place): every copy of u -> v, and with symmetrize every reversed copy of v -> u, is on this rank already"""
+        p = self.part
+        n_out = C.c_size_t()
+        failure = None
+        try:
+            with _views(p.rows, p.cols, p.reversed, p.weights) as (rv, cv, fv, wv):
+                self._call("cugraph_b200_block_stage_edges", self.n_rows, self.n_cols, rv.ptr, cv.ptr, fv.ptr, wv.ptr,
+                           1 if drop_multi_edges else 0, 1 if symmetrize else 0, C.byref(n_out))
+        except self._capi.CugraphError as e:   # e.g. out of memory on this rank alone: the others must not go on
+            failure = e
+        failed = torch.tensor([0 if failure is None else 1], dtype=torch.int64, device=p.rows.device)
+        dist.all_reduce(failed, op=dist.ReduceOp.MAX)
+        if failure is not None:
+            raise failure
+        if int(failed.item()):
+            raise self._capi.CugraphRuntimeError(self._capi.UNKNOWN_ERROR, "staging the edges failed on another rank",
+                                                 "MGGraph")
+        m = n_out.value
+        p.rows, p.cols = p.rows[:m], p.cols[:m]
+        p.weights = p.weights[:m] if p.weights is not None else None
+        p.reversed = None
+
+    def degrees(self):
+        """(vertices, in_degrees, out_degrees) of the vertices this rank owns: edge counts of the staged graph, in the
+        vertices' dtype (single-GPU cugraph_degrees').  The first call counts the block's rows and columns
+        (cugraph_b200_block_degrees) and reduce-scatters them in the row and the column group; later calls reuse the result."""
+        p, g = self.part, self.part.groups
+        if self._degrees is None:
+            rows = torch.empty(self.n_rows, dtype=torch.int64, device=self.device)
+            cols = torch.empty(self.n_cols, dtype=torch.int64, device=self.device)
+            with _views(rows, cols) as (vr, vc):
+                self._call("cugraph_b200_block_degrees", self.block, vr.ptr, vc.ptr)
+            deg_in = torch.empty(p.maxpart, dtype=torch.int64, device=self.device)
+            deg_out = torch.empty(p.maxpart, dtype=torch.int64, device=self.device)
+            reduce_scatter_into(deg_in, rows, g.row_group)
+            reduce_scatter_into(deg_out, cols, g.col_group)                   # partition-major, as out_w
+            dt = p.vertices.dtype
+            self._degrees = (deg_in[:p.n_local].to(dt), deg_out[:p.n_local].to(dt))
+        return p.vertices, self._degrees[0].clone(), self._degrees[1].clone()
 
     def __del__(self):
         try:
@@ -620,8 +730,8 @@ class MGGraph:
     # ------------------------------------------------------------------------------------------
     def weakly_connected_components(self):
         """Returns (vertices, labels) of the vertices this rank owns: a vertex's label is the external id of one member of
-        its component (the same member on every rank), in the vertices' dtype.  The graph must be symmetric: the caller
-        passes both directions of every edge (not checked).  Sets last_wcc_stats = dict(rounds)."""
+        its component (the same member on every rank), in the vertices' dtype.  The graph must be symmetric (not checked):
+        construct it with symmetrize=True, or pass both directions of every edge.  Sets last_wcc_stats = dict(rounds)."""
         p, g = self.part, self.part.groups
         dev, mp = self.device, p.maxpart
         label_own = torch.full((mp,), INT64_MAX, dtype=torch.int64, device=dev)
@@ -930,8 +1040,13 @@ def sssp(graph: MGGraph, source, cutoff=math.inf, compute_predecessors=True):
 
 def weakly_connected_components(graph: MGGraph):
     """(vertices, labels) of the vertices owned by this rank (the MG contract of pylibcugraph.weakly_connected_components;
-    the graph must be symmetric)."""
+    the graph must be symmetric: MGGraph(..., symmetrize=True))."""
     return graph.weakly_connected_components()
+
+
+def degrees(graph: MGGraph):
+    """(vertices, in_degrees, out_degrees) of the vertices owned by this rank (the MG contract of pylibcugraph.degrees)."""
+    return graph.degrees()
 
 
 def katz_centrality(graph: MGGraph, alpha, beta=1.0, epsilon=1e-6, max_iterations=100):

@@ -48,6 +48,30 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_create(
   const cugraph_resource_handle_t* handle, size_t n_rows, size_t n_cols,
   const cugraph_type_erased_device_array_view_t* rows, const cugraph_type_erased_device_array_view_t* cols,
   const cugraph_type_erased_device_array_view_t* weights, cugraph_b200_block_t** block, cugraph_error_t** error);
+/* Staging of this GPU's share of a multi-GPU edge list before cugraph_b200_block_create: the rules of single-GPU staging
+ * (drop_multi_edges, symmetrize of cugraph_graph_create_sg) applied to the n edges (rows[i], cols[i]) in the block's slot
+ * coordinates, rows[i] < n_rows and cols[i] < n_cols (else CUGRAPH_INVALID_INPUT), with optional FLOAT32 / FLOAT64 weights.
+ *   drop_multi_edges: one edge per (row, col, reversed flag) is kept, the one of MINIMUM weight.
+ *   symmetrize: reversed (one byte per edge, nonzero = a reversed copy; NULL = none) marks the copies u -> v of edges v -> u
+ *   that the caller has shuffled to the position (row = v, col = u) of the original u -> v (none for a self-loop).  Per
+ *   position, the i-th lightest original is paired with the i-th lightest reversed copy and becomes one edge of weight
+ *   (W)((a + b) / 2); unpaired edges keep their weight.  Only this position's orientation is emitted: the position of the
+ *   reversed pair sees the same group from the other side and emits the other one, with a bit-identical weight.  Without
+ *   symmetrize the flags are ignored.
+ * The staged edges are written in place into the first *n_out entries of rows, cols and weights (*n_out <= n), ordered by
+ * (row, col).  Symmetrize needs 2n < 2^31 (single-GPU staging's bound, kept although this pass has no 32-bit output
+ * positions), weights n < 2^32 (32-bit permutations).  Synchronises the handle's stream. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_stage_edges(
+  const cugraph_resource_handle_t* handle, size_t n_rows, size_t n_cols, cugraph_type_erased_device_array_view_t* rows,
+  cugraph_type_erased_device_array_view_t* cols, const cugraph_type_erased_device_array_view_t* reversed,
+  cugraph_type_erased_device_array_view_t* weights, bool_t drop_multi_edges, bool_t symmetrize, size_t* n_out,
+  cugraph_error_t** error);
+/* The block's edge counts: row_counts[row slot] (INT64, at least n_rows) = the edges of that row, col_counts[column slot]
+ * (INT64, at least n_cols) = the edges of that column; the first n_rows / n_cols entries are overwritten.  Summed over the
+ * row group (rows) and the column group (columns) they are the in- and out-degrees of the owned vertices.  Asynchronous. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_degrees(
+  const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block, cugraph_type_erased_device_array_view_t* row_counts,
+  cugraph_type_erased_device_array_view_t* col_counts, cugraph_error_t** error);
 CUGRAPH_EXPORT void cugraph_b200_block_free(cugraph_b200_block_t* block);
 CUGRAPH_EXPORT size_t cugraph_b200_block_span(const cugraph_b200_block_t* block);
 /* y[row] = alpha * sum over the block's edges (row, col) of x[col] * w; rows without edges get 0.  The FIRST sweep of a block
