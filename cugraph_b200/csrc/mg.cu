@@ -7,7 +7,7 @@
 // the C ABI (the resource handle bound to the caller's CUDA stream is made in capi_basic.cu): rectangular edge blocks with the
 // same binned / column-blocked layout as the single-GPU graph, the block pull sweep and the fused
 // per-iteration vertex step, the transposed block sweep, the owner steps of Katz, eigenvector centrality and HITS, the BFS
-// pull step, the SSSP push relaxation and the WCC min-label round.  All calls only ENQUEUE work on the handle's stream (the
+// pull step, the SSSP push relaxation, the WCC min-label round and the two sides of an extract_paths round.  All calls only ENQUEUE work on the handle's stream (the
 // SSSP and WCC calls read back one queue size; the first transposed sweep of a block builds its column-major copy).
 #include "advance.cuh"
 #include "centrality_ops.cuh"
@@ -416,6 +416,91 @@ k_block_degrees(O const* __restrict__ off, int32_t const* __restrict__ row_verte
   }
 }
 
+// ---- one position round of multi-GPU extract_paths (the MG walk of k_paths_walk, traverse.cu; reference: the gather rounds
+// of extract_bfs_paths_impl.cuh:129-238).  An entry (row, pos, code) asks the owner of `code` (owner rank * maxpart + local
+// id) for that vertex's external id, to be written at paths[row][pos], and for its predecessor's code, which continues the
+// walk at pos - 1.  The launcher sends the requests' local ids to their owners and brings the answers back in request order.
+
+// owner side: answers[2i] = external id, answers[2i + 1] = predecessor code (-1 = none) of local id lids[i]; (-1, -1) for a
+// local id outside [0, n_local)
+template <typename V>
+__global__ void __launch_bounds__(kBlock)
+k_paths_answer(int32_t const* __restrict__ lids, long long n, V const* __restrict__ vertices, long long const* __restrict__ pred_code,
+               int32_t n_local, long long* __restrict__ answers)
+{
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int32_t l = lids[i];
+    const bool ok   = l >= 0 && l < n_local;
+    answers[2 * i]     = ok ? (long long)vertices[l] : -1ll;
+    answers[2 * i + 1] = ok ? pred_code[l] : -1ll;
+  }
+}
+
+// whether an entry lies inside the paths matrix (entries outside it are dropped unwritten)
+__device__ __forceinline__ bool paths_in_matrix(int32_t row, int32_t pos, long long n_paths_rows, long long len)
+{
+  return row >= 0 && row < n_paths_rows && pos >= 0 && pos < len;
+}
+
+// the owner rank of the request that follows an answered entry, -1 when its walk ends here: the position is 0, there is no
+// predecessor, or the code names no rank
+__device__ __forceinline__ int paths_next_rank(long long code, int32_t pos, long long maxpart, int world)
+{
+  if (pos <= 0 || code < 0) return -1;
+  const long long q = code / maxpart;
+  return q < world ? (int)q : -1;
+}
+
+// requester side, first pass: counts[q] = the next requests that go to rank q
+__global__ void __launch_bounds__(kBlock)
+k_paths_count(long long const* __restrict__ answers, int32_t const* __restrict__ rows, int32_t const* __restrict__ pos, long long n,
+              long long n_paths_rows, long long len, long long maxpart, int world, long long* __restrict__ counts)
+{
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int32_t p = pos[i];
+    if (!paths_in_matrix(rows[i], p, n_paths_rows, len)) continue;
+    const int q = paths_next_rank(answers[2 * i + 1], p, maxpart, world);
+    if (q >= 0) atomicAdd((unsigned long long*)(counts + q), 1ull);
+  }
+}
+
+// warp-aggregated append to one of several counters: the active lanes with the same key claim consecutive slots of it
+__device__ __forceinline__ int warp_append_keyed(int* counters, int key)
+{
+  const unsigned peers = __match_any_sync(__activemask(), key);
+  const int leader     = __ffs((int)peers) - 1;
+  const int lane       = threadIdx.x & 31;
+  int base             = 0;
+  if (lane == leader) base = atomicAdd(counters + key, __popc(peers));
+  base = __shfl_sync(peers, base, leader);
+  return base + __popc(peers & ((1u << lane) - 1u));
+}
+
+// requester side, second pass: paths[row][pos] = the answered external id; the entries that go on are placed in rank
+// order (bucket q starts at counts[0] + ... + counts[q - 1]; cursor[q] starts at 0) as (local id, row, pos - 1)
+template <typename V>
+__global__ void __launch_bounds__(kBlock)
+k_paths_advance(long long const* __restrict__ answers, int32_t const* __restrict__ rows, int32_t const* __restrict__ pos, long long n,
+                V* __restrict__ paths, long long n_paths_rows, long long len, long long maxpart, int world,
+                long long const* __restrict__ counts, int* __restrict__ cursor, int32_t* __restrict__ next_lid,
+                int32_t* __restrict__ next_row, int32_t* __restrict__ next_pos)
+{
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int32_t r = rows[i], p = pos[i];
+    if (!paths_in_matrix(r, p, n_paths_rows, len)) continue;
+    const long long code = answers[2 * i + 1];
+    paths[r * len + p]   = (V)answers[2 * i];
+    const int q          = paths_next_rank(code, p, maxpart, world);
+    if (q < 0) continue;
+    long long at = 0;
+    for (int k = 0; k < q; ++k) at += counts[k];
+    at += warp_append_keyed(cursor, q);
+    next_lid[at] = (int32_t)(code - (long long)q * maxpart);
+    next_row[at] = r;
+    next_pos[at] = p - 1;
+  }
+}
+
 // the two PageRank owner-step entry points: argument checks and the launch (pv == nullptr: uniform teleport)
 void pagerank_vertex_step(handle_impl const& h, device_array_view_impl const* yv, device_array_view_impl const* pv,
                           device_array_view_impl const* ov, device_array_view_impl const* xv,
@@ -808,6 +893,98 @@ cugraph_error_code_t cugraph_b200_block_wcc_min(const cugraph_resource_handle_t*
     auto* cand        = (long long*)cv->data;
     block_push_min(h, *b, p, cand, label, block_wcc_op{p.csx->row_vertex.as<int32_t>(), label, cand});
     check_last("block_wcc_min");
+  });
+}
+
+// answers[2i], answers[2i + 1] = external id and predecessor code of local id lids[i].  Asynchronous.
+cugraph_error_code_t cugraph_b200_paths_answer(const cugraph_resource_handle_t* handle,
+                                               const cugraph_type_erased_device_array_view_t* lids,
+                                               const cugraph_type_erased_device_array_view_t* vertices,
+                                               const cugraph_type_erased_device_array_view_t* pred_codes, size_t n_local,
+                                               cugraph_type_erased_device_array_view_t* answers, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(lids && vertices && pred_codes && answers, CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto const* lv = V(lids);
+    auto const* vv = V(vertices);
+    auto const* cv = V(pred_codes);
+    auto const* av = V(answers);
+    B200_EXPECTS(lv->type == INT32, CUGRAPH_INVALID_INPUT, "lids must be INT32");
+    B200_EXPECTS(vv->type == INT32 || vv->type == INT64, CUGRAPH_INVALID_INPUT, "vertices must be INT32 / INT64");
+    B200_EXPECTS(cv->type == INT64 && av->type == INT64, CUGRAPH_INVALID_INPUT, "pred_codes / answers must be INT64");
+    B200_EXPECTS(n_local < (1u << 31) && vv->size >= n_local && cv->size >= n_local, CUGRAPH_INVALID_INPUT,
+                 "vertices / pred_codes shorter than n_local");
+    B200_EXPECTS(av->size >= 2 * lv->size, CUGRAPH_INVALID_INPUT, "answers must hold two entries per local id");
+    const long long n = (long long)lv->size;
+    if (n == 0) return;
+    const int grid = grid_for(n, 1, h.sm_count * 8);
+    if (vv->type == INT32)
+      B200_LAUNCH(h, k_paths_answer<int32_t>, grid, kBlock, 0, (int32_t const*)lv->data, n, (int32_t const*)vv->data,
+                  (long long const*)cv->data, (int32_t)n_local, (long long*)av->data);
+    else
+      B200_LAUNCH(h, k_paths_answer<int64_t>, grid, kBlock, 0, (int32_t const*)lv->data, n, (int64_t const*)vv->data,
+                  (long long const*)cv->data, (int32_t)n_local, (long long*)av->data);
+    check_last("paths_answer");
+  });
+}
+
+// paths[row][pos] = the answered ids; the entries that go on, grouped by owner rank, into next_*, and counts[rank].
+// Asynchronous.
+cugraph_error_code_t cugraph_b200_paths_advance(const cugraph_resource_handle_t* handle,
+                                                const cugraph_type_erased_device_array_view_t* answers,
+                                                const cugraph_type_erased_device_array_view_t* rows,
+                                                const cugraph_type_erased_device_array_view_t* positions,
+                                                cugraph_type_erased_device_array_view_t* paths, size_t max_path_length,
+                                                size_t maxpart, int world, cugraph_type_erased_device_array_view_t* next_lids,
+                                                cugraph_type_erased_device_array_view_t* next_rows,
+                                                cugraph_type_erased_device_array_view_t* next_positions,
+                                                cugraph_type_erased_device_array_view_t* counts, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(answers && rows && positions && paths && next_lids && next_rows && next_positions && counts,
+                 CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto const* av = V(answers);
+    auto const* rv = V(rows);
+    auto const* pv = V(positions);
+    auto const* xv = V(paths);
+    auto const* nl = V(next_lids);
+    auto const* nr = V(next_rows);
+    auto const* np = V(next_positions);
+    auto const* cv = V(counts);
+    const size_t n = rv->size;
+    B200_EXPECTS(rv->type == INT32 && pv->type == INT32 && pv->size == n, CUGRAPH_INVALID_INPUT,
+                 "rows / positions must be INT32 arrays of equal size");
+    B200_EXPECTS(av->type == INT64 && av->size >= 2 * n, CUGRAPH_INVALID_INPUT, "answers must hold two INT64 entries per row");
+    B200_EXPECTS(xv->type == INT32 || xv->type == INT64, CUGRAPH_INVALID_INPUT, "paths must be INT32 / INT64");
+    B200_EXPECTS(max_path_length > 0 && xv->size % max_path_length == 0, CUGRAPH_INVALID_INPUT,
+                 "paths must hold whole rows of max_path_length entries");
+    B200_EXPECTS(nl->type == INT32 && nr->type == INT32 && np->type == INT32 && nl->size >= n && nr->size >= n && np->size >= n,
+                 CUGRAPH_INVALID_INPUT, "next_lids / next_rows / next_positions must be INT32 arrays of at least n entries");
+    B200_EXPECTS(world > 0 && cv->type == INT64 && cv->size >= (size_t)world, CUGRAPH_INVALID_INPUT,
+                 "counts must be INT64 with one entry per rank");
+    B200_EXPECTS(maxpart > 0 && maxpart < (1u << 31), CUGRAPH_INVALID_INPUT, "bad maxpart");
+    auto* cnt   = (long long*)cv->data;
+    dbuf cursor = make_dbuf<int>((size_t)world, h.stream);
+    CUDA_TRY(cudaMemsetAsync(cnt, 0, sizeof(long long) * (size_t)world, h.stream));
+    CUDA_TRY(cudaMemsetAsync(cursor.data(), 0, sizeof(int) * (size_t)world, h.stream));
+    if (n == 0) return;
+    const long long len = (long long)max_path_length, n_paths_rows = (long long)(xv->size / max_path_length);
+    const int grid      = grid_for((int64_t)n, 1, h.sm_count * 8);
+    auto const* ans     = (long long const*)av->data;
+    auto const* r       = (int32_t const*)rv->data;
+    auto const* p       = (int32_t const*)pv->data;
+    B200_LAUNCH(h, k_paths_count, grid, kBlock, 0, ans, r, p, (long long)n, n_paths_rows, len, (long long)maxpart, world, cnt);
+    if (xv->type == INT32)
+      B200_LAUNCH(h, k_paths_advance<int32_t>, grid, kBlock, 0, ans, r, p, (long long)n, (int32_t*)xv->data, n_paths_rows, len,
+                  (long long)maxpart, world, (long long const*)cnt, cursor.as<int>(), (int32_t*)nl->data, (int32_t*)nr->data,
+                  (int32_t*)np->data);
+    else
+      B200_LAUNCH(h, k_paths_advance<int64_t>, grid, kBlock, 0, ans, r, p, (long long)n, (int64_t*)xv->data, n_paths_rows, len,
+                  (long long)maxpart, world, (long long const*)cnt, cursor.as<int>(), (int32_t*)nl->data, (int32_t*)nr->data,
+                  (int32_t*)np->data);
+    check_last("paths_advance");
   });
 }
 

@@ -12,9 +12,11 @@ per iteration on equal-sized (padded) vertex partitions, the dangling / converge
 one 2-element all_reduce and never touch the host unless epsilon > 0, and the local sweep is the
 same column-blocked shared-memory kernel as on one GPU (C-ABI: cugraph_b200_block_*).
 
-BFS moves byte flags per level (one max-reduce-scatter of candidate predecessors); SSSP runs Δ-windows of rounds, each an
-all-gather of the frontier's distances, the block's push relaxation on the device and one min-reduce-scatter of INT64
-(distance, predecessor) keys (see MGGraph.sssp); WCC propagates the smallest vertex code per round, with one
+BFS moves byte flags per level (one max-reduce-scatter of candidate predecessors), from one source or a set of sources
+given by every rank; extract_paths walks the BFS predecessors one path position per round, each an all-to-all-v of local
+ids to their owners and one of (external id, predecessor code) answers back (see MGGraph.extract_paths); SSSP runs
+Δ-windows of rounds, each an all-gather of the frontier's distances, the block's push relaxation on the device and one
+min-reduce-scatter of INT64 (distance, predecessor) keys (see MGGraph.sssp); WCC propagates the smallest vertex code per round, with one
 min-reduce-scatter of INT64 labels (see MGGraph.weakly_connected_components); Katz, eigenvector centrality and HITS iterate
 the block sweep like PageRank, HITS also in the transposed orientation, with owner-step kernels between the collectives
 (see MGGraph.katz_centrality).
@@ -343,6 +345,7 @@ class MGGraph:
         self._id_order = None                                  # (local ids by external id, sorted external ids)
         self.last_sssp_stats = None
         self.last_wcc_stats = None
+        self.last_paths_stats = None
         self.last_katz_stats = self.last_eigenvector_stats = self.last_hits_stats = None
         self._degrees = None                                   # (in, out) of the owned slice, made by the first degrees()
         self.device = src.device
@@ -551,8 +554,17 @@ class MGGraph:
     # Distances are the BFS levels (bit-exact vs single-GPU); a predecessor is any frontier neighbour, as in the reference.
     # ------------------------------------------------------------------------------------------
     def bfs(self, source, depth_limit=-1, compute_predecessors=True):
-        """source: external vertex id (the same value on every rank).  Returns (vertices, distances, predecessors) of the
-        vertices this rank owns: int32 distances (INT32_MAX = unreachable), predecessors as external ids (-1 = none)."""
+        """BFS from one source or from a set of sources.  Returns (vertices, distances, predecessors) of the vertices this
+        rank owns: int32 distances (INT32_MAX = unreachable), predecessors as external ids (-1 = none), or None when not
+        requested.
+          source a Python / NumPy integer or a 0-d tensor: one external vertex id, the same value on every rank;
+            ValueError on every rank when it is not a vertex.
+          source a 1-D tensor or array: external ids given by THIS rank (possibly none; ranks may give different or
+            overlapping ids).  The BFS starts from the union of every rank's ids, each at distance 0 without a predecessor,
+            as cugraph_bfs does with several sources; with no id on any rank every vertex is unreached.  Every rank raises
+            the same error (one all-reduce): TypeError for ids in a dtype other than the edge ids' on some rank,
+            CugraphValueError for an id that is not a vertex.
+        Every rank must pass the same form, a scalar or an array (not checked: the collectives would not match)."""
         p, g = self.part, self.part.groups
         dev, mp = self.device, p.maxpart
         imax = torch.iinfo(torch.int32).max
@@ -561,11 +573,17 @@ class MGGraph:
         visited = torch.zeros(mp, dtype=torch.uint8, device=dev)
         visited[p.n_local:] = 1                                  # padding slots never take part
         frontier = torch.zeros(mp, dtype=torch.uint8, device=dev)
-        lid = self._source_lid(source, "bfs")
-        if lid >= 0:
-            dist_own[lid] = 0
-            visited[lid] = 1
-            frontier[lid] = 1
+        if _is_scalar(source):
+            lid = self._source_lid(source, "bfs")
+            if lid >= 0:
+                dist_own[lid] = 0
+                visited[lid] = 1
+                frontier[lid] = 1
+        else:
+            lids = self._sources_to_owners(source)
+            dist_own[lids] = 0
+            visited[lids] = 1
+            frontier[lids] = 1
         f_cols = torch.zeros(self.n_cols, dtype=torch.uint8, device=dev)
         v_rows = torch.zeros(self.n_rows, dtype=torch.uint8, device=dev)
         cand = torch.full((self.n_rows,), -1, dtype=torch.int64, device=dev)
@@ -608,6 +626,25 @@ class MGGraph:
             raise ValueError(f"{what} source {source} is not a vertex of the graph")
         return lid
 
+    def _sources_to_owners(self, sources):
+        """the local ids of the sources, from every rank, that this rank owns (duplicates kept): each rank's ids travel to
+        their owners in one all-to-all-v; one all-reduce of the error counts, and every rank raises the same error"""
+        from cugraph_b200 import _capi as capi
+        p, g, dev = self.part, self.part.groups, self.device
+        s = torch.as_tensor(sources)
+        bad_type = int(s.dtype != p.vertices.dtype)
+        s = s.to(dev).reshape(-1).to(torch.int64) if not bad_type else torch.zeros(0, dtype=torch.int64, device=dev)
+        (req,), _, _, _ = exchange([s], vertex_owner(s, g.world), g.world)
+        lid, hit = self._owned_lids(req)
+        errs = torch.stack([torch.tensor(bad_type, dtype=torch.int64, device=dev), (~hit).sum().to(torch.int64)])
+        dist.all_reduce(errs)
+        bad_type, invalid = errs.tolist()
+        if bad_type:
+            raise TypeError("MGGraph.bfs: sources must have the dtype of the edge ids on every rank")
+        if invalid:
+            raise capi.CugraphValueError(capi.INVALID_INPUT, "Found invalid vertex in the input sources", "MGGraph.bfs")
+        return lid
+
     def _codes_to_external(self, codes):
         """predecessor codes (owner rank * maxpart + local id, -1 = none) -> external ids, answered by the owners (one
         all-to-all-v there and back)"""
@@ -624,6 +661,111 @@ class MGGraph:
         pred = torch.full((codes.numel(),), -1, dtype=verts.dtype, device=dev)
         pred[has] = got
         return pred
+
+    # ------------------------------------------------------------------------------------------
+    # multi-GPU extract_paths: single GPU's walk (k_paths_max_len / k_paths_walk, traverse.cu) spread over the owners, one
+    # path position per round, as the reference gathers one position per round over all destinations
+    # (extract_bfs_paths_impl.cuh:129-238).  Set-up, once per call: the owned predecessors become codes (owner rank * maxpart
+    # + local id; one all-to-all-v to their owners and back, the inverse of _codes_to_external); every destination asks its
+    # owner for (distance, predecessor code) (one all-to-all-v there and back); ONE MAX all-reduce gives max_path_length;
+    # cugraph_b200_paths_advance writes every destination into its own column and groups the walks that go on by the owner
+    # of their next vertex.  Then exactly max_path_length - 1 rounds on every rank, a fixed count that needs no termination
+    # all-reduce.  One round: an all-to-all of the per-rank request counts (read back together with the counts sent), an
+    # all-to-all-v of the requested local ids to their owners, cugraph_b200_paths_answer there, an all-to-all-v of the
+    # (external id, predecessor code) answers back in request order, and cugraph_b200_paths_advance.
+    # ------------------------------------------------------------------------------------------
+    def extract_paths(self, distances, predecessors, destinations):
+        """Paths from the BFS sources to `destinations` (single-GPU cugraph_extract_paths' semantics).  distances (int32) and
+        predecessors (external ids) are the n_local entries MGGraph.bfs returned on this rank; destinations are external ids
+        given by this rank, any ids (owned by any rank, or not vertices at all), possibly none.  Returns (paths,
+        max_path_length): paths[i] ([len(destinations), max_path_length], the vertices' dtype) holds the path from the source
+        to destinations[i] in columns 0 .. distance, -1 elsewhere; a source gives [source, -1, ...]; an unreached destination,
+        an id that is not a vertex, or a distance >= max_path_length gives a row of -1; a predecessor that is not a vertex ends
+        the walk.  max_path_length = 1 + the largest distance among the destinations of EVERY rank that have a predecessor
+        (the same on every rank).  Every rank raises the same error (one all-reduce): ValueError when distances or
+        predecessors do not hold n_local entries (or are None), or a rank has 2^31 or more destinations; TypeError for
+        distances that are not int32.  Sets last_paths_stats = dict(rounds)."""
+        p, g, dev, mp = self.part, self.part.groups, self.device, self.part.maxpart
+        n, P = p.n_local, g.world
+        imax = torch.iinfo(torch.int32).max
+        dst = torch.as_tensor(destinations).to(dev).reshape(-1).to(torch.int64)
+        m = dst.numel()
+        if distances is not None:
+            distances = torch.as_tensor(distances).to(dev).reshape(-1)
+        if predecessors is not None:
+            predecessors = torch.as_tensor(predecessors).to(dev).reshape(-1)
+        bad_size = int(distances is None or predecessors is None or distances.numel() != n or predecessors.numel() != n
+                       or m > imax)
+        bad_type = int(not bad_size and distances.dtype != torch.int32)
+        errs = torch.tensor([bad_size, bad_type], dtype=torch.int64, device=dev)
+        dist.all_reduce(errs)
+        bad_size, bad_type = errs.tolist()
+        if bad_size:
+            raise ValueError("MGGraph.extract_paths: distances and predecessors must be the n_local entries MGGraph.bfs "
+                             "returned on every rank, and each rank may give fewer than 2^31 destinations")
+        if bad_type:
+            raise TypeError("MGGraph.extract_paths: distances must be int32 on every rank")
+        # owned predecessors -> codes, answered by the predecessors' owners (-1: none, or not a vertex)
+        pred = predecessors.to(torch.int64)
+        has = pred != -1
+        ask = pred[has]
+        (req,), order, sc, rc = exchange([ask], vertex_owner(ask, P), P)
+        lid, hit = self._owned_lids(req)
+        ans = torch.where(hit, g.rank * mp + lid, -1)
+        back = torch.empty(sum(sc), dtype=torch.int64, device=dev)
+        dist.all_to_all_single(back, ans, output_split_sizes=sc, input_split_sizes=rc)
+        got = torch.empty_like(back)
+        got[order] = back
+        pred_code = torch.full((n,), -1, dtype=torch.int64, device=dev)
+        pred_code[has] = got
+        # destinations -> (distance, predecessor code) from their owners; INT32_MAX / -1 for an id that is not a vertex
+        d_own = distances.to(torch.int64)
+        (req,), order, sc, rc = exchange([dst], vertex_owner(dst, P), P)
+        lid, hit = self._owned_lids(req)
+        ans = torch.full((req.numel(), 2), -1, dtype=torch.int64, device=dev)
+        ans[:, 0] = imax
+        ans[hit, 0] = d_own[lid[hit]]
+        ans[hit, 1] = pred_code[lid[hit]]
+        back = torch.empty(2 * sum(sc), dtype=torch.int64, device=dev)
+        dist.all_to_all_single(back, ans.reshape(-1), output_split_sizes=[2 * k for k in sc],
+                               input_split_sizes=[2 * k for k in rc])
+        got = torch.empty((m, 2), dtype=torch.int64, device=dev)
+        got[order] = back.view(-1, 2)
+        d_dst, c_dst = got[:, 0], got[:, 1]
+        mx = torch.zeros(1, dtype=torch.int64, device=dev)
+        if m:
+            mx = torch.maximum(mx, torch.where((d_dst < imax) & (c_dst >= 0), d_dst, 0).max())
+        dist.all_reduce(mx, op=dist.ReduceOp.MAX)
+        length = int(mx.item()) + 1
+        paths = torch.full((m, length), -1, dtype=p.vertices.dtype, device=dev)
+        rows = ((d_dst >= 0) & (d_dst < length)).nonzero().reshape(-1)
+        answers = torch.stack([dst[rows], c_dst[rows]], 1).reshape(-1)
+        cap = max(rows.numel(), 1)       # a walk never splits: no round has more entries than the first
+        cur = [rows.to(torch.int32), d_dst[rows].to(torch.int32)]
+        bufs = [[torch.empty(cap, dtype=torch.int32, device=dev) for _ in range(3)] for _ in range(2)]
+        counts = torch.empty(2 * P, dtype=torch.int64, device=dev)   # [sent to each rank, received from each rank]
+
+        def advance(answers, rows, pos, nxt):
+            with _views(answers, rows, pos, paths.view(-1), *nxt, counts) as vs:
+                self._call("cugraph_b200_paths_advance", *[v.ptr for v in vs[:4]], length, mp, P, *[v.ptr for v in vs[4:]])
+
+        advance(answers, cur[0], cur[1], bufs[0])
+        for k in range(length - 1):
+            lids_out, rows_k, pos_k = bufs[k % 2]
+            dist.all_to_all_single(counts[P:], counts[:P])
+            both = counts.tolist()
+            sc, rc = both[:P], both[P:]
+            ns, nr = sum(sc), sum(rc)
+            lids_in = torch.empty(nr, dtype=torch.int32, device=dev)
+            dist.all_to_all_single(lids_in, lids_out[:ns], output_split_sizes=rc, input_split_sizes=sc)
+            answers = torch.empty(2 * nr, dtype=torch.int64, device=dev)
+            with _views(lids_in, p.vertices, pred_code, answers) as (vl, vv, vc, va):
+                self._call("cugraph_b200_paths_answer", vl.ptr, vv.ptr, vc.ptr, n, va.ptr)
+            back = torch.empty(2 * ns, dtype=torch.int64, device=dev)
+            dist.all_to_all_single(back, answers, output_split_sizes=[2 * x for x in sc], input_split_sizes=[2 * x for x in rc])
+            advance(back, rows_k[:ns], pos_k[:ns], bufs[(k + 1) % 2])
+        self.last_paths_stats = dict(rounds=length - 1)
+        return paths, length
 
     # ------------------------------------------------------------------------------------------
     # multi-GPU SSSP.  The reference's MG SSSP (sssp_impl.cuh:301-375) gathers the distances of the frontier's sources over
@@ -870,6 +1012,22 @@ class MGGraph:
         self.last_eigenvector_stats = dict(iterations=it)
         return p.vertices, x[:p.n_local].clone()
 
+    def _owned_lids(self, ids):
+        """(local ids, hit) of int64 external ids sent to this rank as their owner: hit[i] says whether ids[i] is a vertex
+        of the graph, and then lid[i] is its local id (lid[i] is 0 where it is not)"""
+        p, n = self.part, self.part.n_local
+        if n == 0 or ids.numel() == 0:
+            return (torch.zeros(ids.numel(), dtype=torch.int64, device=ids.device),
+                    torch.zeros(ids.numel(), dtype=torch.bool, device=ids.device))
+        if self._id_order is None:   # sorted once per graph: a sort of the owned ids costs milliseconds at scale
+            vid = p.vertices.to(torch.int64)
+            order = torch.argsort(vid)
+            self._id_order = (order, vid[order])
+        order, sv = self._id_order
+        pos = torch.searchsorted(sv, ids).clamp(max=n - 1)
+        hit = sv[pos] == ids
+        return torch.where(hit, order[pos], 0), hit
+
     def _pairs_to_owners(self, pairs, dtype):
         """(vertex ids, values) given by this rank (None: nothing) for any vertices -> the pairs of the vertices this rank
         owns, from every rank, with one all-to-all-v (every rank must call it).  Returns (local ids, values in `dtype`,
@@ -888,19 +1046,8 @@ class MGGraph:
             else:
                 mismatch = 1
         (rv, rx), _, _, _ = exchange([gv, gx], vertex_owner(gv, g.world), g.world)
-        n = p.n_local
-        if n > 0 and rv.numel() > 0:
-            if self._id_order is None:   # sorted once per graph: a sort of the owned ids costs milliseconds at scale
-                vid = p.vertices.to(torch.int64)
-                order = torch.argsort(vid)
-                self._id_order = (order, vid[order])
-            order, sv = self._id_order
-            pos = torch.searchsorted(sv, rv).clamp(max=n - 1)
-            hit = sv[pos] == rv
-            lid, val = order[pos[hit]], rx[hit]
-        else:
-            hit = torch.zeros(rv.numel(), dtype=torch.bool, device=dev)
-            lid, val = torch.zeros(0, dtype=torch.int64, device=dev), rx[:0]
+        lid, hit = self._owned_lids(rv)
+        lid, val = lid[hit], rx[hit]
         srt = torch.sort(lid).values
         counts = torch.stack([torch.tensor(mismatch, dtype=torch.float64, device=dev),
                               torch.tensor(gv.numel(), dtype=torch.float64, device=dev),
@@ -985,6 +1132,13 @@ class MGGraph:
         return p.vertices, prev[:p.n_local].clone(), auth[:p.n_local].clone()
 
 
+def _is_scalar(x):
+    """a Python / NumPy integer or a 0-d tensor / array: MGGraph.bfs's one-source form"""
+    if isinstance(x, (torch.Tensor, np.ndarray)):
+        return x.ndim == 0
+    return isinstance(x, (int, np.integer))
+
+
 def _np_type(dtype):
     """the numpy scalar type of a block dtype: convergence tests compare in it, as the single-GPU drivers compare in T"""
     return np.float32 if dtype == torch.float32 else np.float64
@@ -1027,9 +1181,16 @@ def wcc_owner_step(label_own, cand_own):
     return changed
 
 
-def bfs(graph: MGGraph, source, depth_limit=-1, compute_predecessors=True):
-    """(vertices, distances, predecessors) of the vertices owned by this rank (the MG contract of pylibcugraph.bfs)."""
-    return graph.bfs(source, depth_limit, compute_predecessors)
+def bfs(graph: MGGraph, sources, depth_limit=-1, compute_predecessors=True):
+    """(vertices, distances, predecessors) of the vertices owned by this rank (the MG contract of pylibcugraph.bfs).
+    sources: one external id, the same on every rank, or a 1-D tensor / array of this rank's source ids (see MGGraph.bfs)."""
+    return graph.bfs(sources, depth_limit, compute_predecessors)
+
+
+def extract_paths(graph: MGGraph, distances, predecessors, destinations):
+    """(paths, max_path_length) for this rank's destinations from this rank's part of a BFS result (the MG contract of
+    pylibcugraph.extract_paths; see MGGraph.extract_paths)."""
+    return graph.extract_paths(distances, predecessors, destinations)
 
 
 def sssp(graph: MGGraph, source, cutoff=math.inf, compute_predecessors=True):

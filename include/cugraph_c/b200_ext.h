@@ -4,8 +4,8 @@
  *  - multi-GPU: the reference receives NCCL communicators inside a raft::handle_t built by raft-dask / MPI
  *    (python/pylibcugraph/pylibcugraph/comms/comms_wrapper.pyx:10-32, cpp/tests/utilities/mg_utilities.cpp:37-55) and keeps
  *    the 2D-partitioned blocks inside graph_t.  raft is not part of this build: cugraph_graph_create_mg and the multi-GPU
- *    algorithm entry points return CUGRAPH_NOT_IMPLEMENTED; multi-GPU PageRank, BFS, SSSP, WCC, Katz, eigenvector centrality
- *    and HITS are driven by the launcher (cugraph_b200/mg.py, one process per GPU over torch.distributed / NCCL) on top of
+ *    algorithm entry points return CUGRAPH_NOT_IMPLEMENTED; multi-GPU PageRank, BFS, extract_paths, SSSP, WCC, Katz,
+ *    eigenvector centrality and HITS are driven by the launcher (cugraph_b200/mg.py, one process per GPU over torch.distributed / NCCL) on top of
  *    the cugraph_b200_block_* and owner-step device pieces declared below.
  *  - profiling hooks used by bench.py to time the dominant kernel on the handle's stream.
  */
@@ -221,6 +221,34 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_wcc_min(
   const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
   const cugraph_type_erased_device_array_view_t* label_cols,
   cugraph_type_erased_device_array_view_t* cand_rows, cugraph_error_t** error);
+
+/* One position round of multi-GPU extract_paths (the role of the gather rounds of
+ * cpp/src/traversal/extract_bfs_paths_impl.cuh:129-238).  An entry (row, pos, code) of a requester asks the owner of the
+ * vertex code (owner rank * maxpart + local id, as in cugraph_b200_block_bfs_pull) for that vertex's external id, written at
+ * paths[row][pos], and for its predecessor's code, which continues the walk at pos - 1.  The launcher sends the local ids to
+ * their owners and brings the answers back in request order.
+ *   paths_answer (owner side): for every local id lids[i] (INT32), answers[2i] = vertices[lids[i]] (INT32 / INT64 external
+ *     ids, widened) and answers[2i + 1] = pred_codes[lids[i]] (INT64, -1 = none); (-1, -1) for an id outside [0, n_local).
+ *     vertices and pred_codes hold at least n_local entries, answers (INT64) at least 2 * len(lids).
+ *   paths_advance (requester side): entry i is (rows[i], positions[i]) (INT32, equal sizes) with answers[2i], answers[2i + 1]
+ *     as above.  paths (INT32 / INT64, whole rows of max_path_length entries) gets paths[row][pos] = answers[2i] for every
+ *     entry inside it; entries outside it are dropped.  An entry with pos > 0 and a code >= 0 of a rank q < world goes on as
+ *     (local id = code - q * maxpart, row, pos - 1) into next_lids / next_rows / next_positions (INT32, at least as many
+ *     entries as rows), grouped by q in rank order, and counts[q] (INT64, at least world entries, overwritten) receives the
+ *     size of group q.  One pass over the entries counts the groups, a second writes the paths and appends every entry to
+ *     its group at a per-rank cursor (warp-aggregated atomics); the order inside a group is not fixed.
+ * Both are asynchronous; wrong types or sizes return CUGRAPH_INVALID_INPUT. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_paths_answer(
+  const cugraph_resource_handle_t* handle, const cugraph_type_erased_device_array_view_t* lids,
+  const cugraph_type_erased_device_array_view_t* vertices, const cugraph_type_erased_device_array_view_t* pred_codes,
+  size_t n_local, cugraph_type_erased_device_array_view_t* answers, cugraph_error_t** error);
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_paths_advance(
+  const cugraph_resource_handle_t* handle, const cugraph_type_erased_device_array_view_t* answers,
+  const cugraph_type_erased_device_array_view_t* rows, const cugraph_type_erased_device_array_view_t* positions,
+  cugraph_type_erased_device_array_view_t* paths, size_t max_path_length, size_t maxpart, int world,
+  cugraph_type_erased_device_array_view_t* next_lids, cugraph_type_erased_device_array_view_t* next_rows,
+  cugraph_type_erased_device_array_view_t* next_positions, cugraph_type_erased_device_array_view_t* counts,
+  cugraph_error_t** error);
 
 /* Debug hook: one sweep as PageRank would run it on this graph (the shared-memory piece stream when the graph has one)
  * against the plain sweep (an independent implementation) on the same pseudo-random x.  out[0..3] = degree >= 32 rows
