@@ -116,6 +116,7 @@ def lib():
     _sig(L.cugraph_hits_result_get_number_of_iterations, sz, [vp])
     _sig(L.cugraph_hits_result_free, None, [vp])
     _sig(L.cugraph_weakly_connected_components, i32, [vp, vp, i32, pvp, pvp])
+    _sig(L.cugraph_strongly_connected_components, i32, [vp, vp, i32, pvp, pvp])
     _sig(L.cugraph_labeling_result_get_vertices, vp, [vp])
     _sig(L.cugraph_labeling_result_get_labels, vp, [vp])
     _sig(L.cugraph_labeling_result_free, None, [vp])

@@ -178,3 +178,12 @@ def weakly_connected_components(G: Graph, directed=None, connection=None, return
     h, g = G._plc_graph(False)
     verts, labels = plc.weakly_connected_components(h, g, None, None, None, None, False)
     return _frame(vertex=_host(verts), labels=_host(labels))
+
+
+def strongly_connected_components(G: Graph, directed=None, connection=None, return_labels=None):
+    """cugraph.strongly_connected_components (components/connectivity.py): 'vertex', 'labels'.  The graph must be directed:
+    an undirected Graph is symmetric, and the library rejects symmetric graphs here as the reference does."""
+    plc = _plc()
+    h, g = G._plc_graph(False)
+    verts, labels = plc.strongly_connected_components(h, g, None, None, None, None, False)
+    return _frame(vertex=_host(verts), labels=_host(labels))

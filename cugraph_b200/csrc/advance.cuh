@@ -1,5 +1,6 @@
 // The load-balanced frontier advance (merge-path partition of a queue's edges into equal tiles) and the small device
-// helpers around it.  Shared by the single-GPU traversals (traverse.cu: BFS top-down levels, SSSP rounds) and the multi-GPU
+// helpers around it.  Shared by the single-GPU traversals (traverse.cu: BFS top-down levels, SSSP rounds), strongly
+// connected components (scc.cu: trim, reach and colouring rounds) and the multi-GPU
 // block relaxation (mg.cu: cugraph_b200_block_sssp_relax / _pred), which advance over a queue of physical rows of a block's
 // push copy.  Everything lives in an anonymous namespace: every translation unit gets its own instantiations.
 #pragma once
@@ -24,6 +25,14 @@ __device__ __forceinline__ int warp_append(int* counter)
   if (lane == leader) base = atomicAdd(counter, __popc(mask));
   base = __shfl_sync(mask, base, leader);
   return base + __popc(mask & ((1u << lane) - 1u));
+}
+
+// the active lanes of a diverged warp add their values to *target with one atomic
+__device__ __forceinline__ void warp_add_u64(unsigned long long* target, unsigned v)
+{
+  unsigned mask = __activemask();
+  unsigned sum  = __reduce_add_sync(mask, v);
+  if ((threadIdx.x & 31) == __ffs(mask) - 1) atomicAdd(target, (unsigned long long)sum);
 }
 
 // ------------------------------------------------------------------------------------------

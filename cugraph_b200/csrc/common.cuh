@@ -109,7 +109,7 @@ struct tuning_t {
   unsigned long long advance_split_edges{1ull << 31};  // CUGRAPH_B200_ADVANCE_SPLIT_EDGES: frontiers with this many edges are advanced in halves (tests lower it)
   long long offs64_min_edges{1ll << 31};  // CUGRAPH_B200_OFFS64_MIN_EDGES: a csx with this many edges stores 64-bit offsets, in [0, 2^31]
                                           // (tests: 0; lazily built views follow the handle passed to the algorithm)
-  bool bfs_trace{false}, sssp_trace{false}, build_trace{false};  // CUGRAPH_B200_{BFS,SSSP,BUILD}_TRACE
+  bool bfs_trace{false}, sssp_trace{false}, build_trace{false}, scc_trace{false};  // CUGRAPH_B200_{BFS,SSSP,BUILD,SCC}_TRACE
   static tuning_t from_env()
   {
     tuning_t t;
@@ -131,6 +131,7 @@ struct tuning_t {
     t.bfs_trace   = get("CUGRAPH_B200_BFS_TRACE") != nullptr;
     t.sssp_trace  = get("CUGRAPH_B200_SSSP_TRACE") != nullptr;
     t.build_trace = get("CUGRAPH_B200_BUILD_TRACE") != nullptr;
+    t.scc_trace   = get("CUGRAPH_B200_SCC_TRACE") != nullptr;
     return t;
   }
 };
@@ -267,7 +268,7 @@ inline cugraph_type_erased_device_array_t* wrap_array(dbuf&& b, size_t n, cugrap
   return reinterpret_cast<cugraph_type_erased_device_array_t*>(a);
 }
 
-// result objects (reference cpp/src/c_api/centrality_result.hpp:14-19, paths_result.hpp:12-16)
+// result objects (reference cpp/src/c_api/centrality_result.hpp:14-19, paths_result.hpp:12-16, labeling_result.hpp)
 struct centrality_result_impl {
   device_array_impl* vertices{nullptr};
   device_array_impl* values{nullptr};
@@ -279,6 +280,12 @@ struct paths_result_impl {
   device_array_impl* vertices{nullptr};
   device_array_impl* distances{nullptr};
   device_array_impl* predecessors{nullptr};
+};
+
+// weakly / strongly connected components (components.cu, scc.cu)
+struct labeling_result_impl {
+  device_array_impl* vertices{nullptr};
+  device_array_impl* labels{nullptr};
 };
 
 // ---------------------------------------------------------------------------------------------

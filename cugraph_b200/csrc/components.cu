@@ -83,11 +83,6 @@ void wcc_rounds(handle_impl const& h, csx_t const& c, int32_t nv, int32_t* paren
   }
 }
 
-struct labeling_result_impl {
-  device_array_impl* vertices{nullptr};
-  device_array_impl* labels{nullptr};
-};
-
 }  // namespace
 }  // namespace b200
 

@@ -80,6 +80,7 @@ struct graph_impl {
   std::unique_ptr<csx_t> pull_alt;   // lazily built CSC with re-sorted rows (PageRank on a CSR graph)
   std::unique_ptr<csx_t> push_alt;   // lazily built CSR in vertex order (BFS/SSSP on a CSC graph)
   std::unique_ptr<csx_t> out_alt;    // lazily built CSR with rows re-sorted by out-degree (HITS' hub sweep on a CSC graph)
+  std::unique_ptr<csx_t> in_alt;     // lazily built CSC in vertex order (SCC's backward advances on a CSR graph)
 };
 
 inline graph_impl* G(cugraph_graph_t* g)
@@ -91,6 +92,7 @@ inline graph_impl* G(cugraph_graph_t* g)
 // Accessors that build the missing orientation on demand (graph_build.cu).
 csx_t const& pull_view(handle_impl const& h, graph_impl& g);  // rows = destinations, indices = sources
 csx_t const& push_view(handle_impl const& h, graph_impl& g);  // rows = sources, vertex-indexed offsets
+csx_t const& in_view(handle_impl const& h, graph_impl& g);    // rows = destinations, vertex-indexed offsets
 csx_t const& out_sweep_view(handle_impl const& h, graph_impl& g);  // rows = sources, binned for the sweep kernels (HITS)
 
 // ---- the pull sweep (sweep.cu): y[row] = init + alpha * sum_{(col -> row)} x[col] * w(col, row) for every row of a csx

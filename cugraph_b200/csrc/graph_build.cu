@@ -1016,6 +1016,25 @@ csx_t const& push_view(handle_impl const& h, graph_impl& g)
   return *g.push_alt;
 }
 
+// rows = destinations, indices = sources, physical row r = vertex r (the mirror image of push_view): the primary
+// orientation of a CSC graph, a transpose of a CSR graph built once.  The graph's own storage is never changed.
+csx_t const& in_view(handle_impl const& h, graph_impl& g)
+{
+  if (g.store_transposed || g.is_symmetric) return *g.primary;
+  if (!g.in_alt) {
+    csx_t const& p = *g.primary;  // CSR: rows = sources, indices = destinations
+    dbuf maj       = expand_majors(h, p);
+    auto c         = std::make_unique<csx_t>();
+    build_csx(h, *c, p.indices.as<int32_t>(), maj.as<int32_t>(), g.weighted ? p.weights.data() : nullptr,
+              g.weight_type, p.nnz, g.n_vertices, nullptr, nullptr, false, false);
+    c->degree_sorted = false;
+    for (int k = 0; k <= kNumSeg; ++k) c->seg[k] = 0;
+    sync(h);
+    g.in_alt = std::move(c);
+  }
+  return *g.in_alt;
+}
+
 // ---------------------------------------------------------------------------------------------
 // id translation
 // ---------------------------------------------------------------------------------------------

@@ -36,13 +36,6 @@ struct frontier_counters_t {
   unsigned long long packed;  // SSSP with 32-bit offsets: (sum of degrees << 32) | entries appended — ONE atomic per append
 };
 
-__device__ __forceinline__ void warp_add_u64(unsigned long long* target, unsigned v)
-{
-  unsigned mask = __activemask();
-  unsigned sum  = __reduce_add_sync(mask, v);
-  if ((threadIdx.x & 31) == __ffs(mask) - 1) atomicAdd(target, (unsigned long long)sum);
-}
-
 // every edge of the graph, edge-balanced (the same k_tile_owners / k_advance as advance(), advance.cuh): the row offsets are the scan of the identity queue
 template <typename Op>
 void advance_all_edges(handle_impl const& h, int32_t const* off, int32_t const* idx, int32_t n_vertices, long long nnz, Op op)

@@ -188,10 +188,9 @@ def _ensure_wcc_args(graph, offsets, indices, weights, labels):
     return kind
 
 
-def weakly_connected_components(resource_handle, graph, offsets, indices, weights, labels, do_expensive_check):
-    """weakly_connected_components.pyx:107-290.  Either `graph`, or the CSR arrays `offsets` / `indices` [/ `weights`] of a
-    symmetric graph (the legacy form: a graph is built from them with renumber=False).  Returns (vertices, labels); with a
-    `labels` array the labels are written into it (vertex order) and None is returned."""
+def _labeling(fn_name, resource_handle, graph, offsets, indices, weights, labels, do_expensive_check, is_symmetric):
+    """the legacy CSR form (a graph built from offsets / indices [/ weights] with renumber=False), the C call and the result
+    plumbing shared by weakly_connected_components and strongly_connected_components"""
     from cugraph_b200.pylibcugraph.graph_properties import GraphProperties
     from cugraph_b200.pylibcugraph.graphs import SGGraph
     from cugraph_b200.pylibcugraph.resource_handle import ResourceHandle
@@ -199,14 +198,13 @@ def weakly_connected_components(resource_handle, graph, offsets, indices, weight
     if kind == "csr_arrays":
         if resource_handle is None:
             resource_handle = ResourceHandle()
-        graph = SGGraph(resource_handle, GraphProperties(is_symmetric=True, is_multigraph=False), offsets, indices, weights,
-                        store_transposed=False, renumber=False, do_expensive_check=True, input_array_format="CSR")
+        graph = SGGraph(resource_handle, GraphProperties(is_symmetric=is_symmetric, is_multigraph=False), offsets, indices,
+                        weights, store_transposed=False, renumber=False, do_expensive_check=True, input_array_format="CSR")
     res, err = C.c_void_p(), C.c_void_p()
     resource_handle.order_after_caller()
     L = _capi.lib()
-    code = L.cugraph_weakly_connected_components(resource_handle.ptr, graph.ptr, int(bool(do_expensive_check)), C.byref(res),
-                                                 C.byref(err))
-    _capi.check(code, err, "cugraph_weakly_connected_components")
+    code = getattr(L, fn_name)(resource_handle.ptr, graph.ptr, int(bool(do_expensive_check)), C.byref(res), C.byref(err))
+    _capi.check(code, err, fn_name)
     verts = copy_to_torch(resource_handle, L.cugraph_labeling_result_get_vertices(res))
     labs = copy_to_torch(resource_handle, L.cugraph_labeling_result_get_labels(res))
     L.cugraph_labeling_result_free(res)
@@ -218,11 +216,21 @@ def weakly_connected_components(resource_handle, graph, offsets, indices, weight
     return (verts, labs)
 
 
+def weakly_connected_components(resource_handle, graph, offsets, indices, weights, labels, do_expensive_check):
+    """weakly_connected_components.pyx:107-290.  Either `graph`, or the CSR arrays `offsets` / `indices` [/ `weights`] of a
+    symmetric graph (the legacy form: a graph is built from them with renumber=False).  Returns (vertices, labels); with a
+    `labels` array the labels are written into it (vertex order) and None is returned."""
+    return _labeling("cugraph_weakly_connected_components", resource_handle, graph, offsets, indices, weights, labels,
+                     do_expensive_check, is_symmetric=True)
+
+
 def strongly_connected_components(resource_handle, graph, offsets, indices, weights, labels, do_expensive_check):
-    """Not part of this build (SURVEY.md §8: outside the hot path and its "next" rows); the argument rules are the
-    reference's, so that its input-validation tests behave the same."""
-    _ensure_wcc_args(graph, offsets, indices, weights, labels)
-    raise NotImplementedError("strongly_connected_components is not part of this hot-path build")
+    """strongly_connected_components.pyx:107-270.  Either `graph` (not symmetric), or the CSR arrays `offsets` / `indices`
+    [/ `weights`] of a directed graph (the legacy form: a graph is built from them with is_symmetric=False,
+    is_multigraph=False, store_transposed=False, renumber=False).  Returns (vertices, labels); with a `labels` array the
+    labels are written into it (vertex order) and None is returned.  Weights are ignored."""
+    return _labeling("cugraph_strongly_connected_components", resource_handle, graph, offsets, indices, weights, labels,
+                     do_expensive_check, is_symmetric=False)
 
 
 def generate_rmat_edgelist(resource_handle, random_state, scale, num_edges, a, b, c, clip_and_flip, scramble_vertex_ids,

@@ -7,7 +7,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "cugraph_b200", "csrc")
 OUT = os.path.join(ROOT, "cugraph_b200", "lib", "libcugraph_c_emu.so")
-SRCS = [os.path.join(CSRC, f) for f in ("capi_basic.cu", "capi_graph.cu", "graph_build.cu", "sweep_layout.cu", "sweep.cu", "pagerank.cu", "traverse.cu", "mg.cu", "generators.cu", "centrality.cu", "components.cu", "graph_functions.cu")] + \
+SRCS = [os.path.join(CSRC, f) for f in ("capi_basic.cu", "capi_graph.cu", "graph_build.cu", "sweep_layout.cu", "sweep.cu", "pagerank.cu", "traverse.cu", "mg.cu", "generators.cu", "centrality.cu", "components.cu", "scc.cu", "graph_functions.cu")] + \
     [os.path.join(ROOT, "emu", "emu_debug.cpp")]
 
 

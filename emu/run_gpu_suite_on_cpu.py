@@ -17,4 +17,8 @@ with emulated_python_surface():
     sys.exit(pytest.main([os.path.join(ROOT, "tests"), "-q", "-m", "gpu", "--deselect", "tests/test_mg_gpu.py",
                           "--deselect", "tests/test_reference_c_tests_gpu.py",
                           "--deselect", "tests/test_zz_late_additions_gpu.py::test_reference_c_test_program_on_gpu",
+                          # SCC at GPU sizes (RMAT-16/18, 10^5-vertex chains and cycles); tests/test_scc_cpu.py runs the same checks smaller
+                          *[a for t in ("rmat", "rmat_scrambled_int64_and_renumber_false", "random_both_orientations", "offs64",
+                                        "loops_multi_edges_and_wcc", "inputs", "phase_shapes") for a in ("--deselect", f"tests/test_scc_gpu.py::test_scc_{t}_gpu")],
+                          "--deselect", "tests/test_scc_gpu.py::test_reference_scc_c_test_gpu",
                           "-p", "no:cacheprovider"] + sys.argv[1:]))
