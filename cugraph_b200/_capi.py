@@ -139,6 +139,7 @@ def lib():
     _sig(L.cugraph_b200_block_sssp_relax, i32, [vp, vp, vp, dbl, sz, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_block_sssp_pred, i32, [vp, vp, vp, vp, sz, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_block_wcc_min, i32, [vp, vp, vp, vp, pvp])
+    _sig(L.cugraph_b200_block_scc_push, i32, [vp, vp, i32, i32, vp, vp, vp, sz, i32, i32, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_paths_answer, i32, [vp, vp, vp, vp, sz, vp, pvp])
     _sig(L.cugraph_b200_paths_advance, i32, [vp, vp, vp, vp, vp, sz, sz, i32, vp, vp, vp, vp, pvp])
     _sig(L.cugraph_b200_pagerank_vertex_step, i32, [vp, vp, vp, vp, vp, sz, dbl, dbl, i32, vp, vp, pvp])

@@ -32,9 +32,18 @@ struct block_push_t {
   bool sweep_ready{false};
 };
 
+// a queue over the block's own physical rows (row slots as sources: the backward push of multi-GPU SCC), built on first use
+struct block_rows_queue_t {
+  int32_t n_ne{0};     // physical rows with at least one edge (a prefix)
+  dbuf queue, q_deg;   // as in block_push_t
+  dbuf counts;         // block_queue_counts_t
+  advance_scratch_t adv;
+};
+
 struct block_impl {
   std::unique_ptr<csx_t> csx;
   std::unique_ptr<block_push_t> push;  // lazily built (multi-GPU SSSP, WCC and transposed sweeps)
+  std::unique_ptr<block_rows_queue_t> rows_queue;  // lazily built (multi-GPU SCC's backward push)
   int32_t n_rows{0}, n_cols{0}, n_span{0};
   bool weighted{false};
   cugraph_data_type_id_t wtype{FLOAT32};
@@ -400,6 +409,81 @@ struct block_wcc_op {
     if (l < cand[nbr]) atomicMin(cand + nbr, l);  // a stale read is larger than the current value: never skips a win
   }
 };
+
+// ---- one round of multi-GPU strongly connected components on this GPU's edge block (MGGraph.strongly_connected_components).
+// Forward (along u -> v) the sources are the column slots, and the push copy advances the active ones into row slots.
+// Backward (along v -> u) the sources are the row slots, and the block's own rows (rows = destinations, neighbours =
+// sources) advance the active ones into column slots.  An edge counts when its source is active (value != INT64_MIN), its
+// two ends are different vertices (their global codes differ: self-loops are never live edges) and the source's key equals
+// the destination's (subproblem or colour).  It then raises out[dst] to the source's value (max) or adds one to it (count).
+constexpr int kSccPushMax = 0, kSccPushCount = 1;
+
+// an SCC push value over the source slots; INT64_MIN = inactive (the launcher's values use the whole range above it)
+struct scc_value_t {
+  long long v;
+};
+__device__ __forceinline__ bool column_active(scc_value_t x) { return x.v != LLONG_MIN; }
+
+struct block_scc_op {
+  int32_t const* src_of;     // source slot of a physical row (column slot forward, row slot backward)
+  long long const* key_src;  // over source slots
+  long long const* val_src;
+  long long const* key_dst;  // over destination slots
+  int maxpart;                // < 2^31: 32-bit divisions (a 64-bit one is a call, whose frame spilled)
+  int grid_cols, grid_r, grid_c;
+  bool transposed;
+  int mode;
+  long long* out;            // over destination slots
+  __device__ __forceinline__ void edge(int r, long long, int nbr) const
+  {
+    const int s = src_of[r];
+    if (key_src[s] != key_dst[nbr]) return;
+    const int col = transposed ? nbr : s, row = transposed ? s : nbr;
+    // equal codes = equal owner ranks ((col / maxpart) * grid_cols + grid_c for the column, grid_r * grid_cols +
+    // row / maxpart for the row, as column_code) and equal local ids
+    const int cq = col / maxpart, rq = row / maxpart;
+    if (col - cq * maxpart == row - rq * maxpart && (long long)cq * grid_cols + grid_c == (long long)grid_r * grid_cols + rq)
+      return;
+    if (mode == kSccPushCount) {
+      atomicAdd((unsigned long long*)(out + nbr), 1ull);
+    } else {
+      const long long v = val_src[s];
+      if (v > out[nbr]) atomicMax(out + nbr, v);  // a stale read is smaller than the current value: never skips a win
+    }
+  }
+};
+
+// the queue over the block's own rows, built on first use (block_push_t's queue, for the primary rows)
+block_rows_queue_t& rows_queue(handle_impl const& h, block_impl& b)
+{
+  if (!b.rows_queue) {
+    auto q         = std::make_unique<block_rows_queue_t>();
+    csx_t const& c = *b.csx;
+    q->n_ne        = c.degree_sorted ? c.seg[kNumSeg - 2] : c.n_rows;
+    q->queue       = make_dbuf<int32_t>((size_t)std::max(c.n_rows, 1), h.stream);
+    q->q_deg       = make_dbuf<int32_t>((size_t)c.n_rows + 1, h.stream);
+    q->counts      = make_dbuf<block_queue_counts_t>(1, h.stream);
+    q->adv.init(h, c.n_rows, c.nnz);
+    sync(h);
+    b.rows_queue = std::move(q);
+  }
+  return *b.rows_queue;
+}
+
+// active rows of the block itself -> queue (one read-back of its size and edge count) -> advance with `op` (the mirror of
+// block_push_round over the primary rows)
+template <typename O>
+void block_rows_round(handle_impl const& h, csx_t const& c, block_rows_queue_t& q, scc_value_t const* vals, block_scc_op op)
+{
+  auto* cnt = q.counts.as<block_queue_counts_t>();
+  CUDA_TRY(cudaMemsetAsync(cnt, 0, sizeof(block_queue_counts_t), h.stream));
+  if (q.n_ne > 0)
+    B200_LAUNCH(h, (k_block_active_rows<O, scc_value_t>), grid_for(q.n_ne, 1, h.sm_count * 8), kBlock, 0, c.offsets.as<O>(),
+                c.row_vertex.as<int32_t>(), q.n_ne, vals, q.queue.as<int32_t>(), q.q_deg.as<int32_t>(), cnt);
+  const block_queue_counts_t hc = read_back(h, cnt);
+  advance<O>(h, q.adv, c.offsets.as<O>(), c.indices.as<int32_t>(), q.queue.as<int32_t>(), hc.n, hc.edges, op,
+             q.q_deg.as<int32_t>());
+}
 
 // the block's edge counts per row slot (from the offsets, through row_vertex) and per column slot (a histogram)
 template <typename O>
@@ -893,6 +977,57 @@ cugraph_error_code_t cugraph_b200_block_wcc_min(const cugraph_resource_handle_t*
     auto* cand        = (long long*)cv->data;
     block_push_min(h, *b, p, cand, label, block_wcc_op{p.csx->row_vertex.as<int32_t>(), label, cand});
     check_last("block_wcc_min");
+  });
+}
+
+// out_dst[dst slot] = max of val_src (mode 0, from INT64_MIN) or the count (mode 1, from 0) over the dst slot's live edges from
+// active sources with an equal key; forward (transposed = FALSE) from column to row slots, backward from row to column slots
+cugraph_error_code_t cugraph_b200_block_scc_push(const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+                                                 bool_t transposed, int mode,
+                                                 const cugraph_type_erased_device_array_view_t* key_src,
+                                                 const cugraph_type_erased_device_array_view_t* val_src,
+                                                 const cugraph_type_erased_device_array_view_t* key_dst, size_t maxpart,
+                                                 int grid_rows, int grid_cols, int grid_r, int grid_c,
+                                                 cugraph_type_erased_device_array_view_t* out_dst, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(block && key_src && val_src && key_dst && out_dst, CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto* b        = reinterpret_cast<block_impl*>(block);
+    auto const* ks = V(key_src);
+    auto const* vs = V(val_src);
+    auto const* kd = V(key_dst);
+    auto const* ov = V(out_dst);
+    const bool tr  = transposed == TRUE;
+    B200_EXPECTS(ks->type == INT64 && vs->type == INT64 && kd->type == INT64 && ov->type == INT64, CUGRAPH_INVALID_INPUT,
+                 "key_src / val_src / key_dst / out_dst must be INT64");
+    const size_t n_src = (size_t)(tr ? b->n_rows : b->n_cols), n_dst = (size_t)(tr ? b->n_cols : b->n_rows);
+    B200_EXPECTS(ks->size >= n_src && vs->size >= n_src && kd->size >= n_dst && ov->size >= n_dst, CUGRAPH_INVALID_INPUT,
+                 "key / value / output arrays shorter than the block's source / destination slots");
+    B200_EXPECTS(maxpart > 0 && maxpart < (1u << 31) && grid_rows > 0 && grid_cols > 0 && grid_r >= 0 && grid_r < grid_rows &&
+                   grid_c >= 0 &&
+                   grid_c < grid_cols,
+                 CUGRAPH_INVALID_INPUT, "bad grid position");
+    B200_EXPECTS(mode == kSccPushMax || mode == kSccPushCount, CUGRAPH_INVALID_INPUT, "mode must be 0 (max) or 1 (count)");
+    auto* out = (long long*)ov->data;
+    B200_LAUNCH(h, k_fill<long long>, grid_for((int64_t)n_dst, 1, h.sm_count * 8), kBlock, 0, out, (int64_t)n_dst,
+                mode == kSccPushMax ? LLONG_MIN : 0ll);
+    auto const* vals = (scc_value_t const*)vs->data;
+    if (tr) {
+      block_rows_queue_t& q = rows_queue(h, *b);
+      csx_t const& c        = *b->csx;
+      const block_scc_op op{c.row_vertex.as<int32_t>(), (long long const*)ks->data, (long long const*)vs->data,
+                            (long long const*)kd->data, (int)maxpart, grid_cols, grid_r, grid_c, true, mode, out};
+      if (c.offs64) block_rows_round<int64_t>(h, c, q, vals, op);
+      else block_rows_round<int32_t>(h, c, q, vals, op);
+    } else {
+      block_push_t& p = push_copy(h, *b);
+      const block_scc_op op{p.csx->row_vertex.as<int32_t>(), (long long const*)ks->data, (long long const*)vs->data,
+                            (long long const*)kd->data, (int)maxpart, grid_cols, grid_r, grid_c, false, mode, out};
+      if (p.csx->offs64) block_push_round<int64_t>(h, p, vals, op);
+      else block_push_round<int32_t>(h, p, vals, op);
+    }
+    check_last("block_scc_push");
   });
 }
 

@@ -1,4 +1,4 @@
-"""Multi-GPU PageRank, BFS, SSSP, weakly connected components, Katz, eigenvector centrality and HITS: 2D edge partition over one process per GPU (torch.distributed, NCCL on NVLink 5).
+"""Multi-GPU PageRank, BFS, SSSP, weakly and strongly connected components, Katz, eigenvector centrality and HITS: 2D edge partition over one process per GPU (torch.distributed, NCCL on NVLink 5).
 
 What the reference does (SURVEY.md §8e): P = R x C GPUs, vertex -> GPU by hash
 (cpp/include/cugraph/utilities/graph_partition_utils.cuh:30-43, 101-128), every GPU holds the edge
@@ -17,7 +17,9 @@ given by every rank; extract_paths walks the BFS predecessors one path position 
 ids to their owners and one of (external id, predecessor code) answers back (see MGGraph.extract_paths); SSSP runs
 Δ-windows of rounds, each an all-gather of the frontier's distances, the block's push relaxation on the device and one
 min-reduce-scatter of INT64 (distance, predecessor) keys (see MGGraph.sssp); WCC propagates the smallest vertex code per round, with one
-min-reduce-scatter of INT64 labels (see MGGraph.weakly_connected_components); Katz, eigenvector centrality and HITS iterate
+min-reduce-scatter of INT64 labels (see MGGraph.weakly_connected_components); SCC runs single GPU's Multistep phases as
+rounds of block pushes in both directions, forward through the block's column-major copy and backward through its own rows
+(see _SccRun); Katz, eigenvector centrality and HITS iterate
 the block sweep like PageRank, HITS also in the transposed orientation, with owner-step kernels between the collectives
 (see MGGraph.katz_centrality).
 
@@ -316,6 +318,7 @@ class MGGraph:
         self.lib = _capi.lib()
         self._capi = _capi
         self.dtype = dtype if weights is None else weights.dtype
+        self.symmetrize = symmetrize   # strongly_connected_components rejects symmetric graphs, as on one GPU
         self.part = partition_edges(src, dst, weights, groups, vertices=vertices, drop_self_loops=drop_self_loops,
                                     drop_multi_edges=drop_multi_edges, symmetrize=symmetrize)
         p = self.part
@@ -345,6 +348,7 @@ class MGGraph:
         self._id_order = None                                  # (local ids by external id, sorted external ids)
         self.last_sssp_stats = None
         self.last_wcc_stats = None
+        self.last_scc_stats = None
         self.last_paths_stats = None
         self.last_katz_stats = self.last_eigenvector_stats = self.last_hits_stats = None
         self._degrees = None                                   # (in, out) of the owned slice, made by the first degrees()
@@ -897,6 +901,33 @@ class MGGraph:
         return p.vertices, self._codes_to_external(label_own[:p.n_local])
 
     # ------------------------------------------------------------------------------------------
+    # multi-GPU strongly connected components: single GPU's Multistep (scc.cu) with the owners' state in torch and every
+    # round a push over the block (cugraph_b200_block_scc_push); see _SccRun.
+    # ------------------------------------------------------------------------------------------
+    def strongly_connected_components(self):
+        """Returns (vertices, labels) of the vertices this rank owns: a vertex's label is the external id of the member of
+        its strongly connected component with the smallest code (owner rank * maxpart + local id), in the vertices' dtype.
+        That is the rule of weakly_connected_components, so labels depend on no schedule, every rank agrees on them, and a
+        graph that holds every edge in both directions gets weakly_connected_components' labels on the same grid.  Weights
+        are ignored, self-loops are never live edges, multi-edges count once per edge.  A graph built with symmetrize=True is
+        rejected on every rank (CugraphRuntimeError, single GPU's message).  Sets last_scc_stats = dict(trim_rounds,
+        fw_rounds, bw_rounds, outer_rounds, colour_rounds, reach_rounds), the same on every rank."""
+        if self.symmetrize:
+            raise self._fail("MGGraph.strongly_connected_components",
+                             "Invalid input argument: call weakly_connected_components instead for symmetric graphs.")
+        run = _SccRun(self)
+        try:
+            run.trim()
+            if run.resolved < self.part.n_global:
+                run.forward_backward()
+            run.colouring()
+            labels = run.labels()
+        finally:
+            run.close()
+        self.last_scc_stats = run.stats
+        return self.part.vertices, self._codes_to_external(labels)
+
+    # ------------------------------------------------------------------------------------------
     # multi-GPU Katz, eigenvector centrality and HITS: the single-GPU drivers of centrality.cu with the sweep spread over the
     # grid.  A sweep y = A x over the owners' x is: x all-gathered inside the column group over the block's source slots,
     # the block's pull sweep, ONE reduce-scatter of the partial y inside the row group.  HITS' hub sweep y = A^T x runs the
@@ -1181,6 +1212,161 @@ def wcc_owner_step(label_own, cand_own):
     return changed
 
 
+INT64_MIN = torch.iinfo(torch.int64).min
+SCC_PUSH_MAX, SCC_PUSH_COUNT = 0, 1   # the modes of cugraph_b200_block_scc_push
+
+
+class _SccRun:
+    """One call of MGGraph.strongly_connected_components: single GPU's Multistep (scc.cu), phase by phase.
+
+    Owner state over the maxpart slots (int64 or bool; padding slots are never live): `live`, `sub` (subproblem of a live
+    vertex, -1 otherwise), `comp` (a member code of a resolved vertex's SCC), the live in- and out-degree counts and the
+    colour.  One round: the active sources' values (INT64_MIN = inactive) are all-gathered over the block's source slots
+    (forward: column slots, in the column group; backward: row slots, in the row group); cugraph_b200_block_scc_push pushes
+    them over the edges whose source and destination keys agree; ONE reduce-scatter (MAX or SUM) brings the result to the
+    destinations' owners (forward: row group; backward: column group); a torch owner step; one all-reduce of the number of
+    changed vertices ends the loop on every rank at once.  The keys (subproblem or colour, over the source and the
+    destination slots) change only between phases and colouring rounds and are gathered then.
+      1. trim: live in- / out-degrees by a count push in both orientations; vertices with a zero count are peeled, and their
+         edges, pushed in both orientations as counts, are the next round's decrements.  Vertices without edges are peeled
+         at once: singletons.
+      2. forward-backward from the live vertex with the largest in-degree x out-degree, ties to the smallest code (two
+         all-reduces): FW and BW reach inside the pivot's subproblem; FW ∩ BW is resolved, FW\\BW, BW\\FW and the rest
+         become subproblems 1, 2 and 3.
+      3. colouring until nothing is live: the largest code flows forward inside a subproblem (max push), the roots (colour
+         = own code) reach backward among the vertices of their colour, the reached vertices are resolved, every other live
+         vertex takes its colour as its subproblem.  An outer round that resolves nothing raises on every rank.
+    Labels: the smallest member code of every SCC, by one all-to-all-v of (comp, code) to comp's owner and one back."""
+
+    def __init__(self, graph):
+        self.G = graph
+        p, g = graph.part, graph.part.groups
+        self.p, self.g, self.mp = p, g, p.maxpart
+        dev, mp, i64 = graph.device, p.maxpart, torch.int64
+        self.code = torch.full((mp,), -1, dtype=i64, device=dev)
+        self.code[:p.n_local] = g.rank * mp + torch.arange(p.n_local, dtype=i64, device=dev)
+        self.live = self.code >= 0
+        self.sub = torch.full((mp,), -1, dtype=i64, device=dev)
+        self.comp = self.code.clone()
+        self.deg_in = torch.empty(mp, dtype=i64, device=dev)
+        self.deg_out = torch.empty(mp, dtype=i64, device=dev)
+        self.got = torch.empty(mp, dtype=i64, device=dev)
+        self.got2 = torch.empty(mp, dtype=i64, device=dev)
+        nc, nr = graph.n_cols, graph.n_rows
+        self.key_c, self.val_c, self.out_c = (torch.zeros(nc, dtype=i64, device=dev) for _ in range(3))
+        self.key_r, self.val_r, self.out_r = (torch.zeros(nr, dtype=i64, device=dev) for _ in range(3))
+        self._views = _views(self.key_c, self.val_c, self.out_c, self.key_r, self.val_r, self.out_r)
+        self.vkc, self.vvc, self.voc, self.vkr, self.vvr, self.vor = self._views.__enter__()
+        self.resolved = 0
+        self.stats = dict(trim_rounds=0, fw_rounds=0, bw_rounds=0, outer_rounds=0, colour_rounds=0, reach_rounds=0)
+
+    def close(self):
+        self._views.__exit__(None, None, None)
+
+    def push(self, backward, mode, val_own, out_own):
+        """out_own = the owners' reduced push of val_own (INT64_MIN = inactive source) along the edges, or against them"""
+        G, g = self.G, self.g
+        op = dist.ReduceOp.MAX if mode == SCC_PUSH_MAX else dist.ReduceOp.SUM
+        if backward:
+            all_gather_into(self.val_r, val_own, g.row_group)
+            G._call("cugraph_b200_block_scc_push", G.block, 1, mode, self.vkr.ptr, self.vvr.ptr, self.vkc.ptr, self.mp, g.R,
+                    g.C, g.r, g.c, self.voc.ptr)
+            reduce_scatter_into(out_own, self.out_c, g.col_group, op=op)
+        else:
+            all_gather_into(self.val_c, val_own, g.col_group)
+            G._call("cugraph_b200_block_scc_push", G.block, 0, mode, self.vkc.ptr, self.vvc.ptr, self.vkr.ptr, self.mp, g.R,
+                    g.C, g.r, g.c, self.vor.ptr)
+            reduce_scatter_into(out_own, self.out_r, g.row_group, op=op)
+        return out_own
+
+    def gather_keys(self, key_own):
+        all_gather_into(self.key_c, key_own, self.g.col_group)
+        all_gather_into(self.key_r, key_own, self.g.row_group)
+
+    def resolve(self, done, member):
+        """done (a mask of live vertices) is resolved with comp = member; returns the global count (one all-reduce)"""
+        self.comp = torch.where(done, member, self.comp)
+        self.live &= ~done
+        self.sub = torch.where(self.live, self.sub, -1)
+        n = _global_count(done)
+        self.resolved += n
+        return n
+
+    def trim(self):
+        self.key_c.zero_()
+        self.key_r.zero_()
+        self.push(False, SCC_PUSH_COUNT, torch.where(self.live, 0, INT64_MIN), self.deg_in)
+        self.push(True, SCC_PUSH_COUNT, torch.where(self.live, 0, INT64_MIN), self.deg_out)
+        self.sub = torch.where(self.live, 0, -1)
+        rounds = 0
+        peel = self.live & ((self.deg_in == 0) | (self.deg_out == 0))
+        while self.resolve(peel, self.code):
+            val = torch.where(peel, 0, INT64_MIN)
+            self.deg_in -= self.push(False, SCC_PUSH_COUNT, val, self.got)
+            self.deg_out -= self.push(True, SCC_PUSH_COUNT, val, self.got2)
+            peel = self.live & ((self.deg_in == 0) | (self.deg_out == 0))
+            rounds += 1
+        self.stats["trim_rounds"] = rounds
+
+    def reach(self, backward, mark):
+        """mark |= the vertices reached from mark (along the edges, or against them) with the source's key; returns the
+        rounds"""
+        frontier, rounds = mark, 0
+        while True:
+            got = self.push(backward, SCC_PUSH_MAX, torch.where(frontier, 0, INT64_MIN), self.got)
+            frontier = self.live & ~mark & (got != INT64_MIN)
+            mark |= frontier
+            rounds += 1
+            if _global_count(frontier) == 0:
+                return rounds
+
+    def forward_backward(self):
+        score = torch.where(self.live, self.deg_in * self.deg_out, -1).max().reshape(1)
+        dist.all_reduce(score, op=dist.ReduceOp.MAX)
+        pivot = torch.where(self.live & (self.deg_in * self.deg_out == score), self.code, INT64_MAX).min().reshape(1)
+        dist.all_reduce(pivot, op=dist.ReduceOp.MIN)
+        self.gather_keys(self.sub)
+        fw, bw = self.code == pivot, self.code == pivot
+        self.stats["fw_rounds"] = self.reach(False, fw)
+        self.stats["bw_rounds"] = self.reach(True, bw)
+        self.sub = torch.where(fw, 1, torch.where(bw, 2, 3))
+        self.resolve(self.live & fw & bw, pivot)
+
+    def colouring(self):
+        st = self.stats
+        while self.resolved < self.p.n_global:
+            self.gather_keys(self.sub)
+            colour = torch.where(self.live, self.code, -1)
+            frontier = self.live
+            while True:
+                got = self.push(False, SCC_PUSH_MAX, torch.where(frontier, colour, INT64_MIN), self.got)
+                frontier = self.live & (got > colour)
+                colour = torch.where(frontier, got, colour)
+                st["colour_rounds"] += 1
+                if _global_count(frontier) == 0:
+                    break
+            self.gather_keys(colour)
+            roots = self.live & (colour == self.code)
+            st["reach_rounds"] += self.reach(True, roots)
+            self.sub = colour
+            if self.resolve(roots, colour) == 0:
+                raise MGGraph._fail("MGGraph.strongly_connected_components",
+                                    "strongly_connected_components: a colouring round resolved no vertex")
+            st["outer_rounds"] += 1
+
+    def labels(self):
+        """the smallest member code of every owned vertex's SCC"""
+        p, g, mp = self.p, self.g, self.mp
+        comp, code = self.comp[:p.n_local], self.code[:p.n_local]
+        (lid, member), order, sc, rc = exchange([comp % mp, code], torch.div(comp, mp, rounding_mode="floor"), g.world)
+        low = torch.full((mp,), INT64_MAX, dtype=torch.int64, device=comp.device).scatter_reduce_(0, lid, member, "amin")
+        back = torch.empty(sum(sc), dtype=torch.int64, device=comp.device)
+        dist.all_to_all_single(back, low[lid].contiguous(), output_split_sizes=sc, input_split_sizes=rc)
+        label = torch.empty_like(back)
+        label[order] = back
+        return label
+
+
 def bfs(graph: MGGraph, sources, depth_limit=-1, compute_predecessors=True):
     """(vertices, distances, predecessors) of the vertices owned by this rank (the MG contract of pylibcugraph.bfs).
     sources: one external id, the same on every rank, or a 1-D tensor / array of this rank's source ids (see MGGraph.bfs)."""
@@ -1203,6 +1389,12 @@ def weakly_connected_components(graph: MGGraph):
     """(vertices, labels) of the vertices owned by this rank (the MG contract of pylibcugraph.weakly_connected_components;
     the graph must be symmetric: MGGraph(..., symmetrize=True))."""
     return graph.weakly_connected_components()
+
+
+def strongly_connected_components(graph: MGGraph):
+    """(vertices, labels) of the vertices owned by this rank (the MG contract of pylibcugraph.strongly_connected_components;
+    see MGGraph.strongly_connected_components)."""
+    return graph.strongly_connected_components()
 
 
 def degrees(graph: MGGraph):

@@ -222,6 +222,26 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_wcc_min(
   const cugraph_type_erased_device_array_view_t* label_cols,
   cugraph_type_erased_device_array_view_t* cand_rows, cugraph_error_t** error);
 
+/* One round of multi-GPU strongly connected components on this GPU's edge block (any phase of Multistep: trim, reach,
+ * colouring).  The block may be unweighted or weighted; weights are ignored.
+ *   transposed = FALSE (forward, along u -> v): sources are the column slots (key_src, val_src: at least n_cols entries),
+ *     destinations the row slots (key_dst, out_dst: at least n_rows); the edges are pushed through the block's column-major
+ *     copy (shared with cugraph_b200_block_sssp_relax / _wcc_min / the transposed sweep).
+ *   transposed = TRUE (backward, along v -> u): sources are the row slots, destinations the column slots; the edges are
+ *     pushed through the block's own rows, with a queue built by the first backward call and kept.
+ * All arrays are INT64.  out_dst is first filled with INT64_MIN (mode 0, max) or 0 (mode 1, count).  Then, for every edge
+ * whose source is active (val_src[src] != INT64_MIN), whose two ends are different vertices (the codes of the column slot,
+ * ((col / maxpart) * grid_cols + grid_c) * maxpart + col % maxpart, and of the row slot,
+ * (grid_r * grid_cols + row / maxpart) * maxpart + row % maxpart, differ) and with key_src[src] == key_dst[dst]:
+ *   mode 0: out_dst[dst] = max(out_dst[dst], val_src[src]);   mode 1: out_dst[dst] += 1  (multi-edges count once each).
+ * NULL arguments, other dtypes, short arrays, a grid position outside grid_rows x grid_cols and other modes return
+ * CUGRAPH_INVALID_INPUT.  Asynchronous, apart from one read-back of the number of active sources and their edge count. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_scc_push(
+  const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block, bool_t transposed, int mode,
+  const cugraph_type_erased_device_array_view_t* key_src, const cugraph_type_erased_device_array_view_t* val_src,
+  const cugraph_type_erased_device_array_view_t* key_dst, size_t maxpart, int grid_rows, int grid_cols, int grid_r,
+  int grid_c, cugraph_type_erased_device_array_view_t* out_dst, cugraph_error_t** error);
+
 /* One position round of multi-GPU extract_paths (the role of the gather rounds of
  * cpp/src/traversal/extract_bfs_paths_impl.cuh:129-238).  An entry (row, pos, code) of a requester asks the owner of the
  * vertex code (owner rank * maxpart + local id, as in cugraph_b200_block_bfs_pull) for that vertex's external id, written at
