@@ -118,12 +118,23 @@ size_t padded_x_elems(int32_t n_vertices, size_t elem_size);
 // an x buffer of padded_x_elems() elements, zero-filled; only [0, n_vertices) is to be written afterwards
 template <typename T>
 dbuf make_sweep_x(handle_impl const& h, int32_t n_vertices);
+// PageRank's vertex pass, done by the sweep where it writes each row (x_next == nullptr: none).  For the value `val` of vertex
+// v: x_next[v] = val / out_w[v] (val where out_w[v] is 0), st->dangling += val where out_w[v] is 0, and with y_old
+// st->diff += |val - y_old[v]|.  The sums are fp64 partials added with one atomic per warp, read by a later launch.
+// x_next is a second buffer from make_sweep_x: the sweep still reads x while it writes rows.  With an epilogue y may be
+// nullptr: the sweep then writes x_next alone (PageRank at epsilon = 0, whose y is read only after the last iteration).
+template <typename T>
+struct sweep_epilogue_t {
+  T const* out_w{nullptr};
+  T* x_next{nullptr};
+  T const* y_old{nullptr};
+};
 // The piece stream (sweep.cuh) when the graph has one, else the plain sweep (spmv.cuh).  x holds padded_x_elems() elements
 // and does not overlap y.  use_weights = false: plain neighbour sums on a weighted graph (HITS).  covered_rows_only: the
 // rows without edges may keep what y holds (multi-GPU blocks, whose unvarying term is 0).
 template <typename T>
 void pull_sweep(handle_impl const& h, csx_t const& c, int32_t n_vertices, T const* x, T* y, sweep_scratch_t& sc, double alpha,
-                bool use_weights = true, bool covered_rows_only = false);
+                bool use_weights = true, bool covered_rows_only = false, sweep_epilogue_t<T> const& epi = {});
 // build now what pull_sweep would build on its first call for elements of `elem_size` bytes (the piece stream, if c gets one)
 void prepare_pull_sweep(handle_impl const& h, csx_t const& c, int32_t n_vertices, size_t elem_size);
 

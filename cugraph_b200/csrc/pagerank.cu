@@ -2,11 +2,12 @@
 // Replaces cpp/src/link_analysis/pagerank_impl.cuh:40-330 (driver) and cpp/src/c_api/pagerank.cpp.
 //
 // Per iteration the reference runs ~6 V-sized thrust passes and 2 blocking scalar read-backs
-// (pagerank_impl.cuh:225-318).  Here an iteration is: pull sweep (sweep.cu) -> [personalization
-// scatter] -> ONE fused vertex pass (diff, dangling sum, next x = pr/out_w) -> 1-thread finalize that
-// advances the device-resident loop state.  The host enqueues iterations in batches and only reads the
-// `done` flag between batches; kernels of iterations past convergence are no-ops, so the iteration
-// count and result are exactly those of a check-every-iteration loop.
+// (pagerank_impl.cuh:225-318).  Here an iteration is: pull sweep (sweep.cu), whose row epilogue does the vertex pass
+// (diff, dangling sum, next x = pr/out_w) where it writes each row, into the other of two x buffers -> 1-thread finalize
+// that advances the device-resident loop state.  Personalized calls add their scatter after the sweep and so keep the
+// separate vertex pass.  The host enqueues iterations in batches and only reads the `done` flag between batches; kernels
+// of iterations past convergence are no-ops, so the iteration count and result are exactly those of a check-every-iteration
+// loop.
 #include "centrality_ops.cuh"
 #include "graph.cuh"
 #include "staging.cuh"
@@ -36,7 +37,8 @@ __global__ void k_cast(S const* in, int32_t n, T* out)
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = (T)in[i];
 }
 
-// fused vertex pass: diff += |new-old| ; dangling += new where out_w==0 ; x = new / (out_w or 1)
+// fused vertex pass: diff += |new-old| ; dangling += new where out_w==0 ; x = new / (out_w or 1).  The prologue's, and the
+// iterations' of personalized calls; the others have the sweep's row epilogue do it (sweep_epilogue_t)
 template <typename T>
 __global__ void __launch_bounds__(kBlock)
 k_vertex_pass(T const* __restrict__ pr_new, T const* __restrict__ pr_old, T const* __restrict__ out_w,
@@ -211,9 +213,14 @@ void pagerank_typed(handle_impl const& h, graph_impl& g, pr_args const& a, centr
     B200_EXPECTS(pers_sum > 0.0, CUGRAPH_UNKNOWN_ERROR, "Invalid input argument: sum of personalization valuese should be positive.");
   }
 
-  // state
+  // state.  Two x buffers: the sweep's row epilogue writes the next x while the sweep still reads this one.  A personalized
+  // call adds its scatter to y after the sweep, so its next x is made by a vertex pass after that, into the same buffer: it
+  // needs one.  (Folding the scatter into the epilogue would need a dense V-sized personalization vector read per row,
+  // about what the vertex pass costs.)
+  const bool fused = n_pers == 0;
   dbuf pr_a = make_dbuf<T>(nv, h.stream), pr_b = make_dbuf<T>(nv, h.stream);
-  dbuf x    = make_sweep_x<T>(h, nv);
+  dbuf x = make_sweep_x<T>(h, nv), x_alt;
+  if (fused) x_alt = make_sweep_x<T>(h, nv);
   sweep_scratch_t sc;
   sc.init(h, c);
   pr_state_t* st = sc.st();
@@ -236,6 +243,8 @@ void pagerank_typed(handle_impl const& h, graph_impl& g, pr_args const& a, centr
 
   T* cur = pr_a.as<T>();
   T* nxt = pr_b.as<T>();
+  T* xc  = x.as<T>();
+  T* xn  = fused ? x_alt.as<T>() : nullptr;
   pr_state_t* hst = reinterpret_cast<pr_state_t*>(h.pinned);
   int enqueued    = 0;
   int iters       = 0;
@@ -243,11 +252,20 @@ void pagerank_typed(handle_impl const& h, graph_impl& g, pr_args const& a, centr
   while (true) {  // the reference's loop body runs at least once (pagerank_impl.cuh:224-327: test after iter++)
     int todo = std::min(batch, std::max(max_it, 1) - enqueued);
     for (int k = 0; k < todo; ++k) {
-      pull_sweep<T>(h, c, nv, x.as<T>(), nxt, sc, a.alpha);
-      if (n_pers > 0)
+      if (fused) {
+        // diff only where it is read: epsilon = 0 never stops on it and last_diff is not returned.  Nor, then, is y read
+        // before the result: at epsilon = 0 the run ends after exactly max(max_it, 1) iterations, and only the last one
+        // writes y (4 bytes per vertex less in every other sweep); the others write the next x alone
+        const bool last = enqueued + 1 >= std::max(max_it, 1);
+        sweep_epilogue_t<T> epi{out_w, xn, a.epsilon > 0.0 ? cur : nullptr};
+        pull_sweep<T>(h, c, nv, xc, a.epsilon > 0.0 || last ? nxt : nullptr, sc, a.alpha, true, false, epi);
+        std::swap(xc, xn);
+      } else {
+        pull_sweep<T>(h, c, nv, xc, nxt, sc, a.alpha);
         B200_LAUNCH(h, (k_personalize<T>), grid_for(n_pers), kBlock, 0, pers_idx.as<int32_t>(), (T const*)a.pers_val->data,
                     n_pers, pers_sum, nxt, st);
-      B200_LAUNCH(h, (k_vertex_pass<T>), vgrid, kBlock, 0, nxt, cur, out_w, x.as<T>(), nv, st);
+        B200_LAUNCH(h, (k_vertex_pass<T>), vgrid, kBlock, 0, nxt, cur, out_w, xc, nv, st);
+      }
       B200_LAUNCH(h, k_finalize, 1, 1, 0, st, a.alpha, a.epsilon, nv, n_pers > 0 ? 1 : 0, 1, max_it);
       std::swap(cur, nxt);
       ++enqueued;

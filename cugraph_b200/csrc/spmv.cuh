@@ -48,6 +48,76 @@ inline double ld_stream(const double* p) { return *p; }
 #endif
 
 // ------------------------------------------------------------------------------------------
+// PageRank's row epilogue (sweep_epilogue_t, graph.cuh) as the kernels see it: x_next == nullptr = none; the sums go to the
+// loop state, which k_finalize reads in a later launch (no kernel waits on another CTA)
+// ------------------------------------------------------------------------------------------
+template <typename T>
+struct row_epi_t {
+  T const* __restrict__ out_w;
+  T* __restrict__ x_next;
+  T const* __restrict__ y_old;  // or nullptr: no diff
+  pr_state_t* __restrict__ st;
+};
+
+struct epi_sums_t {  // a lane's partial sums
+  double dangling{0.0}, diff{0.0};
+};
+
+// what the epilogue of vertex v reads: loaded apart from its use, so that a kernel can issue the loads with its own
+template <typename T>
+struct epi_in_t {
+  T ow, old;
+};
+
+template <typename T>
+__device__ __forceinline__ epi_in_t<T> epi_load(row_epi_t<T> const& e, int v)
+{
+  epi_in_t<T> p{(T)0, (T)0};
+  if (e.x_next) {
+    p.ow = e.out_w[v];
+    if (e.y_old) p.old = e.y_old[v];
+  }
+  return p;
+}
+
+// y[v] = val (y == nullptr: only with an epilogue, whose x_next is then the only output), and the epilogue of v when
+// there is one
+template <typename T>
+__device__ __forceinline__ void store_row(T* __restrict__ y, row_epi_t<T> const& e, int v, T val, epi_in_t<T> const& p,
+                                          epi_sums_t& s)
+{
+  if (y) y[v] = val;
+  if (e.x_next) {
+    e.x_next[v] = p.ow == (T)0 ? val : val / p.ow;
+    if (p.ow == (T)0) s.dangling += (double)val;
+    if (e.y_old) s.diff += fabs((double)val - (double)p.old);
+  }
+}
+template <typename T>
+__device__ __forceinline__ void store_row(T* __restrict__ y, row_epi_t<T> const& e, int v, T val, epi_sums_t& s)
+{
+  store_row(y, e, v, val, epi_load(e, v), s);
+}
+
+// one thread's sums into the loop state (a zero sum adds nothing: no atomic)
+template <typename T>
+__device__ __forceinline__ void epi_commit(row_epi_t<T> const& e, epi_sums_t const& s)
+{
+  if (s.dangling != 0.0) atomicAdd(&e.st->dangling, s.dangling);
+  if (s.diff != 0.0) atomicAdd(&e.st->diff, s.diff);
+}
+
+// the warp's sums, one atomic each; every lane of the warp calls it
+template <typename T>
+__device__ __forceinline__ void epi_flush(row_epi_t<T> const& e, epi_sums_t s)
+{
+  if (!e.x_next) return;
+  s.dangling = warp_sum(s.dangling);
+  if (e.y_old) s.diff = warp_sum(s.diff);
+  if ((threadIdx.x & 31) == 0) epi_commit(e, s);
+}
+
+// ------------------------------------------------------------------------------------------
 // degree >= 32 prefix: one warp per 1024-edge chunk
 // ------------------------------------------------------------------------------------------
 template <typename O, typename T, bool WEIGHTED>
@@ -55,7 +125,7 @@ __global__ void __launch_bounds__(256)
 k_spmv_hi(O const* __restrict__ offsets, int32_t const* __restrict__ indices, T const* __restrict__ weights,
           T const* __restrict__ x, T* __restrict__ y, int32_t const* __restrict__ row_vertex,
           int32_t const* __restrict__ chunk_first_row, int32_t n_chunks, long long nnz_hi,
-          double* __restrict__ acc_hi, double alpha, pr_state_t const* __restrict__ st)
+          double* __restrict__ acc_hi, double alpha, pr_state_t const* __restrict__ st, row_epi_t<T> epi)
 {
   if (st->done) return;
   const int lane = threadIdx.x & 31;
@@ -68,6 +138,7 @@ k_spmv_hi(O const* __restrict__ offsets, int32_t const* __restrict__ indices, T 
   long long row_beg  = (long long)offsets[r];
   long long row_end  = (long long)offsets[r + 1];
   long long e        = e0;
+  epi_sums_t sums;  // lane 0's: it writes the rows
   while (e < e1) {
     const long long seg_end = row_end < e1 ? row_end : e1;
     double acc              = 0.0;
@@ -94,8 +165,7 @@ k_spmv_hi(O const* __restrict__ offsets, int32_t const* __restrict__ indices, T 
     if (lane == 0) {
       const bool whole = (row_beg >= e0) && (row_end <= e1);
       if (whole) {
-        const int v = row_vertex ? row_vertex[r] : r;
-        y[v]        = (T)(acc * alpha + init);
+        store_row(y, epi, row_vertex ? row_vertex[r] : r, (T)(acc * alpha + init), sums);
       } else {
         atomicAdd(acc_hi + r, acc);
       }
@@ -107,21 +177,23 @@ k_spmv_hi(O const* __restrict__ offsets, int32_t const* __restrict__ indices, T 
       row_end = (long long)offsets[r + 1];
     }
   }
+  if (epi.x_next && lane == 0) epi_commit(epi, sums);
 }
 
 // rows that straddle chunk boundaries: fold the fp64 partials
 template <typename T>
 __global__ void k_spmv_hi_finish(int32_t const* __restrict__ split_rows, int32_t n_split, double* __restrict__ acc_hi,
                                  T* __restrict__ y, int32_t const* __restrict__ row_vertex, double alpha,
-                                 pr_state_t const* __restrict__ st)
+                                 pr_state_t const* __restrict__ st, row_epi_t<T> epi)
 {
   if (st->done) return;
   int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n_split) return;
-  int r     = split_rows[k];
-  int v     = row_vertex ? row_vertex[r] : r;
-  y[v]      = (T)(acc_hi[r] * alpha + st->init);
+  int r = split_rows[k];
+  epi_sums_t sums;
+  store_row(y, epi, row_vertex ? row_vertex[r] : r, (T)(acc_hi[r] * alpha + st->init), sums);
   acc_hi[r] = 0.0;
+  if (epi.x_next) epi_commit(epi, sums);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -141,7 +213,7 @@ template <typename O, typename T, bool WEIGHTED>
 __global__ void __launch_bounds__(256)
 k_spmv_low(O const* __restrict__ offsets, int32_t const* __restrict__ indices, T const* __restrict__ weights,
            T const* __restrict__ x, T* __restrict__ y, int32_t const* __restrict__ row_vertex, low_bins_t bins,
-           double alpha, pr_state_t const* __restrict__ st)
+           double alpha, pr_state_t const* __restrict__ st, row_epi_t<T> epi)
 {
   if (st->done) return;
   int b = 0;
@@ -150,9 +222,11 @@ k_spmv_low(O const* __restrict__ offsets, int32_t const* __restrict__ indices, T
     if ((int)blockIdx.x >= bins.block_begin[k]) b = k;
   const double init = st->init;
   const int blk     = blockIdx.x - bins.block_begin[b];
-  if (b == kNumSeg - 2) {  // empty rows
+  epi_sums_t sums;
+  if (b == kNumSeg - 2) {  // empty rows (b is the block's: the whole warp gets here)
     int r = bins.row_begin[b] + blk * 256 + threadIdx.x;
-    if (r < bins.row_begin[b + 1]) y[row_vertex ? row_vertex[r] : r] = (T)init;
+    if (r < bins.row_begin[b + 1]) store_row(y, epi, row_vertex ? row_vertex[r] : r, (T)init, sums);
+    epi_flush(epi, sums);
     return;
   }
   const int g   = low_bin_lanes(b);
@@ -185,7 +259,8 @@ k_spmv_low(O const* __restrict__ offsets, int32_t const* __restrict__ indices, T
           (((double)v[4] + (double)v[5]) + ((double)v[6] + (double)v[7]));
   }
   for (int o = g >> 1; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if (in && sub == 0) y[row_vertex ? row_vertex[r] : r] = (T)(acc * alpha + init);
+  if (in && sub == 0) store_row(y, epi, row_vertex ? row_vertex[r] : r, (T)(acc * alpha + init), sums);
+  epi_flush(epi, sums);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -210,7 +285,7 @@ inline low_bins_t make_low_bins(csx_t const& c)
 
 template <typename O, typename T>
 void launch_pull_sweep(handle_impl const& h, csx_t const& c, T const* x, T* y, double* acc_hi, double alpha,
-                       pr_state_t const* st, bool use_weights = true)
+                       pr_state_t const* st, bool use_weights = true, row_epi_t<T> const& epi = {})
 {
   O const* off        = c.offsets.as<O>();
   int32_t const* idx  = c.indices.as<int32_t>();
@@ -222,14 +297,14 @@ void launch_pull_sweep(handle_impl const& h, csx_t const& c, T const* x, T* y, d
   if (c.n_chunks > 0) {
     int grid = (c.n_chunks + kWarpsPerCta - 1) / kWarpsPerCta;
     B200_LAUNCH(h, hi_kernel, grid, 256, 0, off, idx, w, x, y, rv, c.chunk_first_row.as<int32_t>(), c.n_chunks,
-                (long long)c.nnz_hi, acc_hi, alpha, st);
+                (long long)c.nnz_hi, acc_hi, alpha, st, epi);
     if (c.n_split > 0)
       B200_LAUNCH(h, (k_spmv_hi_finish<T>), (c.n_split + 255) / 256, 256, 0, c.split_rows.as<int32_t>(), c.n_split,
-                  acc_hi, y, rv, alpha, st);
+                  acc_hi, y, rv, alpha, st, epi);
   }
   low_bins_t bins = make_low_bins(c);
   int lblocks     = bins.block_begin[kNumSeg - 1];
-  B200_LAUNCH(h, low_kernel, lblocks, 256, 0, off, idx, w, x, y, rv, bins, alpha, st);
+  B200_LAUNCH(h, low_kernel, lblocks, 256, 0, off, idx, w, x, y, rv, bins, alpha, st, epi);
 }
 
 }  // namespace b200

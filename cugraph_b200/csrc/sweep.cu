@@ -70,23 +70,29 @@ dbuf make_sweep_x(handle_impl const& h, int32_t n_vertices)
 
 template <typename T>
 void pull_sweep(handle_impl const& h, csx_t const& c, int32_t n_vertices, T const* x, T* y, sweep_scratch_t& sc, double alpha,
-                bool use_weights, bool covered_rows_only)
+                bool use_weights, bool covered_rows_only, sweep_epilogue_t<T> const& epi)
 {
   double* acc = sc.acc.as<double>();
+  B200_EXPECTS(!epi.x_next || (epi.out_w && !covered_rows_only && epi.x_next != x), CUGRAPH_UNKNOWN_ERROR,
+               "internal: a row epilogue needs out_w, every row and an x_next apart from x");
+  B200_EXPECTS(y || (epi.x_next && !epi.y_old), CUGRAPH_UNKNOWN_ERROR, "internal: a sweep without y needs an epilogue");
+  const row_epi_t<T> e{epi.out_w, epi.x_next, epi.y_old, sc.st()};
   if (sweep_layout_t const* L = sweep_layout(h, c, n_vertices, sizeof(T)))
-    launch_sweep<T>(h, c, *L, x, y, acc, alpha, sc.st(), use_weights, covered_rows_only);
+    launch_sweep<T>(h, c, *L, x, y, acc, alpha, sc.st(), use_weights, covered_rows_only, e);
   else if (c.offs64)  // the plain sweep writes every row
-    launch_pull_sweep<int64_t, T>(h, c, x, y, acc, alpha, sc.st(), use_weights);
+    launch_pull_sweep<int64_t, T>(h, c, x, y, acc, alpha, sc.st(), use_weights, e);
   else
-    launch_pull_sweep<int32_t, T>(h, c, x, y, acc, alpha, sc.st(), use_weights);
+    launch_pull_sweep<int32_t, T>(h, c, x, y, acc, alpha, sc.st(), use_weights, e);
 }
 
 void prepare_pull_sweep(handle_impl const& h, csx_t const& c, int32_t nv, size_t es) { sweep_layout(h, c, nv, es); }
 
 template dbuf make_sweep_x<float>(handle_impl const&, int32_t);
 template dbuf make_sweep_x<double>(handle_impl const&, int32_t);
-template void pull_sweep(handle_impl const&, csx_t const&, int32_t, float const*, float*, sweep_scratch_t&, double, bool, bool);
-template void pull_sweep(handle_impl const&, csx_t const&, int32_t, double const*, double*, sweep_scratch_t&, double, bool, bool);
+template void pull_sweep(handle_impl const&, csx_t const&, int32_t, float const*, float*, sweep_scratch_t&, double, bool, bool,
+                         sweep_epilogue_t<float> const&);
+template void pull_sweep(handle_impl const&, csx_t const&, int32_t, double const*, double*, sweep_scratch_t&, double, bool, bool,
+                         sweep_epilogue_t<double> const&);
 
 }  // namespace b200
 

@@ -603,15 +603,29 @@ __global__ void __launch_bounds__(kSweepThreads, 1) k_sweep(sweep_args_t<T> a)
   }
 }
 
+// the epilogue of rows r, r + 1 of a float sweep without row_vertex, their out_w given: y_old read, x_next written as float2
+__device__ __forceinline__ void epi_row_pair(row_epi_t<float> const& e, int r, float v0, float v1, float2 ow, epi_sums_t& s)
+{
+  *reinterpret_cast<float2*>(e.x_next + r) = make_float2(ow.x == 0.f ? v0 : v0 / ow.x, ow.y == 0.f ? v1 : v1 / ow.y);
+  if (ow.x == 0.f) s.dangling += (double)v0;
+  if (ow.y == 0.f) s.dangling += (double)v1;
+  if (e.y_old) {
+    const float2 o = *reinterpret_cast<float2 const*>(e.y_old + r);
+    s.diff += fabs((double)v0 - (double)o.x) + fabs((double)v1 - (double)o.y);
+  }
+}
+
 // y[row] = acc * alpha + init for the rows [row_lo, n_rows): acc for the stream rows (< n_cov, the caller passes n_str), init
-// for the empty rows behind them; clears their accumulators and the n_phases cursors.  row_lo is a multiple of kBandRowAlign.  A warp handles 256 consecutive rows in four steps of 64: every step is one 512-byte load + one 512-byte store of
-// accumulators and one 256-byte store of y per warp (lane = two rows), all four loads issued before the first use.
-// (Eight CONSECUTIVE rows per thread looked the same on paper and ran at 2.3 TB/s: every warp-wide 128-bit access then
-// touched sixteen 128-byte lines for a quarter of their bytes.)
+// for the empty rows behind them (and the row epilogue of each, if any); clears their accumulators and the n_phases
+// cursors.  row_lo is a multiple of kBandRowAlign.  A warp handles 64 kFinishSteps consecutive rows in steps of 64: every
+// step is one 512-byte load + one 512-byte store of accumulators and one 256-byte store of y per warp (lane = two rows),
+// all loads issued before the first use, the epilogue's out_w among them.  (Eight CONSECUTIVE rows per thread looked the
+// same on paper and ran at 2.3 TB/s: every warp-wide 128-bit access then touched sixteen 128-byte lines for a quarter of
+// their bytes.)
 template <typename T, int kFinishSteps>
 __global__ void __launch_bounds__(256)
 k_sweep_finish(double* __restrict__ acc, int row_lo, int n_cov, int n_rows, T* __restrict__ y, int32_t const* __restrict__ row_vertex,
-               double alpha, int* __restrict__ cursor, int n_phases, pr_state_t const* __restrict__ st)
+               double alpha, int* __restrict__ cursor, int n_phases, pr_state_t const* __restrict__ st, row_epi_t<T> epi)
 {
   static_assert(kBandRowAlign % (64 * kFinishSteps) == 0, "a warp's rows must not straddle a band bound");
   if (st->done) return;
@@ -621,13 +635,26 @@ k_sweep_finish(double* __restrict__ acc, int row_lo, int n_cov, int n_rows, T* _
   const int base = row_lo + (t >> 5) * (64 * kFinishSteps) + 2 * lane;  // first of this lane's two rows in step 0
   if (base - 2 * lane >= n_rows) return;
   const double init = st->init;
+  epi_sums_t sums;
   double2 q[kFinishSteps];
+  T ow[kFinishSteps][2];  // the epilogue's out_w of the lane's two rows
 #pragma unroll
   for (int k = 0; k < kFinishSteps; ++k) {
     const int r = base + 64 * k;
     q[k]        = make_double2(0.0, 0.0);
     if (r + 1 < n_cov) q[k] = *reinterpret_cast<double2*>(acc + r);
     else if (r < n_cov) q[k].x = acc[r];
+    ow[k][0] = ow[k][1] = (T)0;
+    if (epi.x_next) {
+      if (sizeof(T) == 4 && !row_vertex && r + 1 < n_rows) {
+        const float2 o = *reinterpret_cast<float2 const*>(epi.out_w + r);
+        ow[k][0]       = (T)o.x;
+        ow[k][1]       = (T)o.y;
+      } else {
+        if (r < n_rows) ow[k][0] = epi.out_w[row_vertex ? row_vertex[r] : r];
+        if (r + 1 < n_rows) ow[k][1] = epi.out_w[row_vertex ? row_vertex[r + 1] : r + 1];
+      }
+    }
   }
 #pragma unroll
   for (int k = 0; k < kFinishSteps; ++k) {
@@ -635,13 +662,25 @@ k_sweep_finish(double* __restrict__ acc, int row_lo, int n_cov, int n_rows, T* _
     if (r + 1 < n_cov) *reinterpret_cast<double2*>(acc + r) = make_double2(0.0, 0.0);
     else if (r < n_cov) acc[r] = 0.0;
     const T v0 = (T)(q[k].x * alpha + init), v1 = (T)(q[k].y * alpha + init);
-    if (!row_vertex && r + 1 < n_rows && sizeof(T) == 4) {
-      *reinterpret_cast<float2*>(y + r) = make_float2((float)v0, (float)v1);
-    } else {
-      if (r < n_rows) y[row_vertex ? row_vertex[r] : r] = v0;
-      if (r + 1 < n_rows) y[row_vertex ? row_vertex[r + 1] : r + 1] = v1;
+    bool paired = false;
+    if constexpr (sizeof(T) == 4) {
+      if (!row_vertex && r + 1 < n_rows) {
+        if (y) *reinterpret_cast<float2*>(y + r) = make_float2(v0, v1);
+        if (epi.x_next) epi_row_pair(epi, r, v0, v1, make_float2((float)ow[k][0], (float)ow[k][1]), sums);
+        paired = true;
+      }
+    }
+    if (!paired) {
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        if (r + j < n_rows) {
+          const int v = row_vertex ? row_vertex[r + j] : r + j;
+          store_row(y, epi, v, j ? v1 : v0, epi_in_t<T>{ow[k][j], epi.y_old ? epi.y_old[v] : (T)0}, sums);
+        }
+      }
     }
   }
+  epi_flush(epi, sums);  // the early return above is the whole warp's
 }
 
 // The tail rows [n_str, n_cov) from the tail layout (sweep_layout.cuh), then y = init for the empty rows [n_cov, empty_hi).  Its
@@ -687,6 +726,7 @@ struct tail_args_t {
   pr_state_t const* __restrict__ st;
   int n_runs, empty_hi, W;
   double alpha;
+  row_epi_t<T> epi;
 };
 
 struct tail_unit_t {  // warp-uniform; d = 0: no unit
@@ -724,17 +764,21 @@ __device__ __forceinline__ void tail_load(int (&q)[kTailUnitEntries], tail_unit_
 }
 
 // the unit's rows, in-degree D: a row's entries in batches of 8, gathered, then summed as an fp64 tree (the order of
-// k_spmv_low), the batches added in order
-template <typename T, bool WEIGHTED, int D>
+// k_spmv_low), the batches added in order; EPI: with the row epilogue (a.epi)
+template <typename T, bool WEIGHTED, int D, bool EPI>
 __device__ __forceinline__ void tail_rows(int const (&q)[kTailUnitEntries], tail_unit_t const& u, tail_args_t<T> const& a,
                                           T const* __restrict__ sx, double init, unsigned long long pol, unsigned long long keep,
-                                          int lane)
+                                          int lane, epi_sums_t& sums)
 {
   constexpr int U = tail_unit_tiles(D);
   T const* wp       = WEIGHTED ? a.w + u.base + lane : nullptr;  // entry j: wp[32 j]
 #pragma unroll
   for (int t = 0; t < U; ++t) {
     if (t < u.n_tiles) {
+      const int row = u.row0 + t * kTailTile + lane;
+      const int v   = row < u.row_end ? (a.row_vertex ? a.row_vertex[row] : row) : -1;
+      // the epilogue's loads are issued with the gathers: after the sum they would be one more round trip per tile
+      const epi_in_t<T> p = EPI && v >= 0 ? epi_load(a.epi, v) : epi_in_t<T>{(T)0, (T)0};
       double s = 0.0;
 #pragma unroll
       for (int k0 = 0; k0 < D; k0 += kTailBatch) {
@@ -752,22 +796,26 @@ __device__ __forceinline__ void tail_rows(int const (&q)[kTailUnitEntries], tail
         }
         s += ((b[0] + b[1]) + (b[2] + b[3])) + ((b[4] + b[5]) + (b[6] + b[7]));
       }
-      const int row = u.row0 + t * kTailTile + lane;
-      if (row < u.row_end) a.y[a.row_vertex ? a.row_vertex[row] : row] = (T)(s * a.alpha + init);
+      if (v >= 0) {
+        if constexpr (EPI) store_row(a.y, a.epi, v, (T)(s * a.alpha + init), p, sums);
+        else a.y[v] = (T)(s * a.alpha + init);
+      }
     }
   }
 }
 
-template <typename T, bool WEIGHTED, int D = 1>
+template <typename T, bool WEIGHTED, bool EPI, int D = 1>
 __device__ __forceinline__ void tail_process(int const (&q)[kTailUnitEntries], tail_unit_t const& u, tail_args_t<T> const& a,
                                              T const* __restrict__ sx, double init, unsigned long long pol,
-                                             unsigned long long keep, int lane)
+                                             unsigned long long keep, int lane, epi_sums_t& sums)
 {
-  if (u.d == D) tail_rows<T, WEIGHTED, D>(q, u, a, sx, init, pol, keep, lane);
-  else if constexpr (D < kTailMaxDegree) tail_process<T, WEIGHTED, D + 1>(q, u, a, sx, init, pol, keep, lane);
+  if (u.d == D) tail_rows<T, WEIGHTED, D, EPI>(q, u, a, sx, init, pol, keep, lane, sums);
+  else if constexpr (D < kTailMaxDegree) tail_process<T, WEIGHTED, EPI, D + 1>(q, u, a, sx, init, pol, keep, lane, sums);
 }
 
-template <typename T, bool WEIGHTED>
+// EPI: with the row epilogue (a.epi.x_next set).  A template argument, not a run-time test: the kernel runs at the register
+// limit, and sweeps without an epilogue (Katz, HITS, ...) keep the code they had.
+template <typename T, bool WEIGHTED, bool EPI>
 __global__ void __launch_bounds__(kTailThreads, 1) k_sweep_tail(tail_args_t<T> a)
 {
   B200_DYN_SMEM(smem_raw);
@@ -783,6 +831,10 @@ __global__ void __launch_bounds__(kTailThreads, 1) k_sweep_tail(tail_args_t<T> a
   }
   if ((int)threadIdx.x <= a.n_runs) s_run[threadIdx.x] = a.runs[threadIdx.x];
   const double init = a.st->init;
+  // the lane's epilogue sums over all its units and empty rows, flushed once per warp at the end.  In registers: 8 KiB of
+  // them in shared memory took the kernel past the 196 KiB shared-memory carve-out, and the L1 that serves its gathers shrank
+  // from 60 to 28 KiB (the whole sweep 8 % slower, epilogue or not)
+  epi_sums_t sums;
   __syncthreads();  // the barrier is initialised before anybody waits on it, the run table is in place
   // unit i is processed while the ids of unit i+1 and the draw of unit i+2 are in flight
   const int ra = draw_issue(a.cursor, 1, lane, true), rb = draw_issue(a.cursor, 1, lane, true);
@@ -794,28 +846,76 @@ __global__ void __launch_bounds__(kTailThreads, 1) k_sweep_tail(tail_args_t<T> a
   while (A.d > 0) {
     tail_load(qb, B, a.ids, pol, lane);
     const int rc = draw_issue(a.cursor, 1, lane, B.d > 0);
-    tail_process<T, WEIGHTED>(qa, A, a, sx, init, pol, keep, lane);
+    tail_process<T, WEIGHTED, EPI>(qa, A, a, sx, init, pol, keep, lane, sums);
     if (B.d == 0) break;
     const tail_unit_t C = tail_unit(s_run, a.n_runs, draw_get(rc));
     tail_load(qa, C, a.ids, pol, lane);
     const int rd = draw_issue(a.cursor, 1, lane, C.d > 0);
-    tail_process<T, WEIGHTED>(qb, B, a, sx, init, pol, keep, lane);
+    tail_process<T, WEIGHTED, EPI>(qb, B, a, sx, init, pol, keep, lane, sums);
     A = C;
     B = tail_unit(s_run, a.n_runs, draw_get(rd));
   }
+  // the empty rows: y = init, and with an epilogue x_next = init / out_w (about half of RMAT's vertices).  Without
+  // row_vertex in 16-byte vectors, kEmptyBatch of them in flight per thread (a row at a time measured ~1 % slower)
   const int stride = gridDim.x * blockDim.x;
-  for (int r = a.runs[a.n_runs].first_row + (int)(blockIdx.x * blockDim.x + threadIdx.x); r < a.empty_hi; r += stride)
-    a.y[a.row_vertex ? a.row_vertex[r] : r] = (T)init;
+  const int tid    = (int)(blockIdx.x * blockDim.x + threadIdx.x);
+  const int lo     = a.runs[a.n_runs].first_row;
+  if constexpr (!EPI) {
+    for (int r = lo + tid; r < a.empty_hi; r += stride) a.y[a.row_vertex ? a.row_vertex[r] : r] = (T)init;
+  } else if (a.row_vertex) {
+    for (int r = lo + tid; r < a.empty_hi; r += stride) store_row(a.y, a.epi, a.row_vertex[r], (T)init, sums);
+  } else {
+    constexpr int kV = 16 / sizeof(T), kEmptyBatch = 4;
+    const int v_lo = (lo + kV - 1) / kV, v_hi = a.empty_hi / kV;  // whole vectors [v_lo, v_hi)
+    const int s_hi = v_lo < v_hi ? v_lo * kV : a.empty_hi;         // rows before them; the rest from v_hi * kV on
+    for (int r = lo + tid; r < s_hi; r += stride) store_row(a.y, a.epi, r, (T)init, sums);
+    for (int r = (v_lo < v_hi ? v_hi * kV : a.empty_hi) + tid; r < a.empty_hi; r += stride) store_row(a.y, a.epi, r, (T)init, sums);
+    const T fill = (T)init;
+    for (int i0 = v_lo + tid; i0 < v_hi; i0 += kEmptyBatch * stride) {
+      uint4 ow[kEmptyBatch], old[kEmptyBatch];
+#pragma unroll
+      for (int j = 0; j < kEmptyBatch; ++j) {
+        const int i = i0 + j * stride;
+        if (i < v_hi) {
+          ow[j] = reinterpret_cast<uint4 const*>(a.epi.out_w)[i];
+          if (a.epi.y_old) old[j] = reinterpret_cast<uint4 const*>(a.epi.y_old)[i];
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < kEmptyBatch; ++j) {
+        const int i = i0 + j * stride;
+        if (i < v_hi) {
+          T w[kV], o[kV], yv[kV], xv[kV];
+          std::memcpy(w, &ow[j], 16);
+          if (a.epi.y_old) std::memcpy(o, &old[j], 16);
+#pragma unroll
+          for (int k = 0; k < kV; ++k) {
+            yv[k] = fill;
+            xv[k] = w[k] == (T)0 ? fill : fill / w[k];
+            if (w[k] == (T)0) sums.dangling += (double)fill;
+            if (a.epi.y_old) sums.diff += fabs((double)fill - (double)o[k]);
+          }
+          uint4 qy, qx;
+          std::memcpy(&qy, yv, 16);
+          std::memcpy(&qx, xv, 16);
+          if (a.y) reinterpret_cast<uint4*>(a.y)[i] = qy;
+          reinterpret_cast<uint4*>(a.epi.x_next)[i] = qx;
+        }
+      }
+    }
+  }
+  if constexpr (EPI) epi_flush(a.epi, sums);
 }
 
 // x must hold padded_x_elems() elements, zero behind n_vertices (slices are copied whole)
 template <typename T>
 void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L, T const* x, T* y, double* acc, double alpha,
-                  pr_state_t const* st, bool use_weights, bool covered_rows_only)
+                  pr_state_t const* st, bool use_weights, bool covered_rows_only, row_epi_t<T> const& epi)
 {
   const bool weighted = use_weights && L.w.data() != nullptr;
   auto* const sweep_kernel = weighted ? k_sweep<T, true> : k_sweep<T, false>;
-  auto* const tail_kernel  = weighted ? k_sweep_tail<T, true> : k_sweep_tail<T, false>;
+  auto* const tail_kernel  = epi.x_next ? (weighted ? k_sweep_tail<T, true, true> : k_sweep_tail<T, false, true>)
+                                        : (weighted ? k_sweep_tail<T, true, false> : k_sweep_tail<T, false, false>);
   // the attribute is per device and cheap to set: no process-wide "done" flag (a second device would miss it)
   CUDA_TRY(cudaFuncSetAttribute(sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
   sweep_args_t<T> a;
@@ -838,7 +938,7 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
   const int32_t finish_rows = covered_rows_only ? L.n_cov : c.n_rows;
   const bool tail           = L.n_str < L.n_cov;  // rows of small in-degree left the stream (sweep_layout.cuh)
   // band by band: the band's rows are finished while its accumulators are in the L2, before the next band's REDs evict them.
-  // y must not overlap x: a band's finish writes y while later bands (and the tail) still read x.
+  // y (and the epilogue's x_next) must not overlap x: a band's finish writes y while later bands (and the tail) still read x.
   for (int band = 0; band < L.n_bands; ++band) {
     // the last band also writes the empty rows, unless the tail launch does
     const int row_hi = band < L.n_bands - 1 ? L.band_row[band + 1] : (tail ? L.n_str : finish_rows);
@@ -851,7 +951,7 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
     const int n_ph = a.ph_hi - a.ph_lo + (band == L.n_bands - 1 && tail ? 1 : 0);
     const int n    = std::max((row_hi - row_lo + 2 * kFinishSteps - 1) / (2 * kFinishSteps), n_ph);  // threads: 16 rows each
     B200_LAUNCH(h, (k_sweep_finish<T, kFinishSteps>), (std::max(n, 1) + 255) / 256, 256, 0, acc, row_lo, L.n_str, row_hi, y,
-                c.row_vertex.as<int32_t>(), alpha, L.cursor.as<int>() + a.ph_lo, n_ph, st);
+                c.row_vertex.as<int32_t>(), alpha, L.cursor.as<int>() + a.ph_lo, n_ph, st, epi);
   }
   if (tail) {  // the rows [n_str, n_cov) and (unless covered_rows_only) the empty rows, by k_sweep_tail
     tail_args_t<T> t;
@@ -867,6 +967,7 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
     t.empty_hi   = finish_rows;
     t.W          = L.W;
     t.alpha      = alpha;
+    t.epi        = epi;
     const int units  = L.tail_runs.back().first_unit;
     const int blocks = std::max(1, std::min(h.sm_count, (units + kTailThreads / 32 - 1) / (kTailThreads / 32)));
     CUDA_TRY(cudaFuncSetAttribute(tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
