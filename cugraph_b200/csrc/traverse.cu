@@ -651,6 +651,7 @@ k_select_window(O const* __restrict__ off, DA dist, int n, sssp_window_t<T> cons
 // which could only consist of same-distance edges — would need one that points at a later one.  (An id-ordered acceptance
 // inside a plateau in pass 1 looked like a shortcut and is wrong: x takes the smaller-id v in pass 1, the orphan v then finds
 // the "attached" x.)  The reference records the predecessor at the relaxation that set the distance, sssp_impl.cuh:43-73.
+// An unreached vertex holds max(), which a sum that rounds to exactly max() would match: it never takes a parent.
 template <typename O, typename T>
 __global__ void k_sssp_pred(O const* __restrict__ off, int32_t const* __restrict__ idx, T const* __restrict__ w,
                             T const* __restrict__ dist, int32_t n_vertices, int32_t source, T unreached,
@@ -664,7 +665,7 @@ __global__ void k_sssp_pred(O const* __restrict__ off, int32_t const* __restrict
     for (long long e = (long long)off[u] + lane; e < (long long)off[u + 1]; e += 32) {
       const int v = idx[e];
       const T dv  = dist[v];
-      if (v != source && v != (int)u && du < dv && du + w[e] == dv) pred[v] = (int32_t)u;
+      if (v != source && v != (int)u && du < dv && dv != unreached && du + w[e] == dv) pred[v] = (int32_t)u;
     }
   }
 }
@@ -679,7 +680,7 @@ struct sssp_pred_op {
   __device__ __forceinline__ void edge(int src, long long e, int nbr) const
   {
     const T du = dist[src], dv = dist[nbr];
-    if (du != unreached && nbr != source && nbr != src && du < dv && du + w[e] == dv) pred[nbr] = src;
+    if (du != unreached && dv != unreached && nbr != source && nbr != src && du < dv && du + w[e] == dv) pred[nbr] = src;
   }
 };
 

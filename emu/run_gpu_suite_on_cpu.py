@@ -21,6 +21,9 @@ with emulated_python_surface():
                           *[a for t in ("rmat", "rmat_scrambled_int64_and_renumber_false", "random_both_orientations", "offs64",
                                         "loops_multi_edges_and_wcc", "inputs", "phase_shapes") for a in ("--deselect", f"tests/test_scc_gpu.py::test_scc_{t}_gpu")],
                           "--deselect", "tests/test_scc_gpu.py::test_reference_scc_c_test_gpu",
+                          # SSSP on every shape, weight family, cutoff and knob set (hundreds of traversals);
+                          # tests/test_traversal_shapes_cpu.py runs the same checks on fewer cases
+                          "--deselect", "tests/test_traversal_shapes_gpu.py::test_sssp_shapes",
                           # multi-GPU SCC at GPU sizes (RMAT-14/16 on four grids); tests/test_mg_scc_cpu.py runs the same checks smaller
                           *[a for t in ("simulated", "phases", "edge_cases", "offs64", "weighted_blocks")
                             for a in ("--deselect", f"tests/test_mg_scc_gpu.py::test_mg_scc_{t}_on_one_gpu")],

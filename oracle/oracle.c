@@ -284,6 +284,10 @@ int oracle_sssp(const int64_t* offsets,
   const double inf = use_float ? (double)FLT_MAX : DBL_MAX;
   if (source < 0 || source >= V) return -1;
   if (cutoff > inf) cutoff = inf;
+  /* the cutoff is compared in weight_t: the reference rounds it first (cpp/src/c_api/sssp.cpp:109,
+   * static_cast<weight_t>(cutoff_)).  A double cutoff above a float distance d that rounds down to d must
+   * leave the vertex at d unreached.  (Clamped first: the conversion is only defined within float's range.) */
+  if (use_float) cutoff = (double)(float)cutoff;
   for (int32_t i = 0; i < V; ++i) {
     distances[i]    = inf;
     predecessors[i] = -1;

@@ -94,10 +94,10 @@ def _assert_predecessor_tree(dist, pred, source, unreached):
 
 
 # ------------------------------------------------------------------------------------------------------------ BFS
-def _bfs(h, g, sources, do, depth_limit=0):
+def _bfs(h, g, sources, do, depth_limit=0, vertex_dtype=np.int32):
     import torch
     from cugraph_b200 import pylibcugraph as plc
-    dist, pred, verts = plc.bfs(h, g, torch.as_tensor(np.asarray(sources, np.int32)).cuda(), do, depth_limit, True, False)
+    dist, pred, verts = plc.bfs(h, g, torch.as_tensor(np.asarray(sources, vertex_dtype)).cuda(), do, depth_limit, True, False)
     return verts, dist, pred
 
 
@@ -301,16 +301,24 @@ def check_structure(monkeypatch, knobs, scale):
     dist = by_vertex(verts, dist, V)
     ref_d, _ = oracle.bfs(s, d, V, [source])
     assert np.array_equal(dist, ref_d)
+    _assert_bfs_paths(s, d, V, source, dests, dist, paths)
+
+
+def _assert_bfs_paths(s, d, V, source, dests, dist, paths):
+    """extract_paths rows against the BFS distances: the row length is 1 + the largest reached distance of a destination;
+    a reached destination's row is a chain of graph edges from the source, one hop per BFS level, padded with -1; an
+    unreached destination's row is all -1"""
     assert paths.shape[1] == 1 + int(dist[dests][dist[dests] < INT_MAX].max())
     keys = np.unique(s.astype(np.int64) * V + d)
-    for row, t in zip(paths, dests.tolist()):
+    for row, t in zip(paths, np.asarray(dests).tolist()):
         if dist[t] == INT_MAX:
             assert (row == -1).all()
             continue
         n = int(dist[t]) + 1
         assert row[0] == source and row[n - 1] == t and (row[n:] == -1).all()
         hop = row[:n - 1].astype(np.int64) * V + row[1:n]
-        assert np.isin(hop, keys).all() and np.array_equal(dist[row[:n]], np.arange(n))
+        pos = np.minimum(np.searchsorted(keys, hop), keys.size - 1)   # keys are sorted: a lookup, not np.isin's sort
+        assert (keys[pos] == hop).all() and np.array_equal(dist[row[:n]], np.arange(n))
 
 
 def check_csr_input(monkeypatch, knobs):
