@@ -136,6 +136,8 @@ def lib():
     _sig(L.cugraph_b200_generate_rmat_edgelist, i32, [vp, sz, sz, dbl, dbl, dbl, C.c_uint64, i32, i32, vp, vp, pvp])
     _sig(L.cugraph_b200_generate_uniform, i32, [vp, C.c_uint64, dbl, dbl, vp, pvp])
     _sig(L.cugraph_b200_block_bfs_pull, i32, [vp, vp, vp, vp, sz, i32, i32, vp, pvp])
+    _sig(L.cugraph_b200_block_bfs_push, i32, [vp, vp, vp, vp, sz, i32, i32, vp, pvp])
+    _sig(L.cugraph_b200_bfs_bottom_up, i32, [vp, i32, sz, sz, sz, sz, sz])
     _sig(L.cugraph_b200_block_sssp_relax, i32, [vp, vp, vp, dbl, sz, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_block_sssp_pred, i32, [vp, vp, vp, vp, sz, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_block_wcc_min, i32, [vp, vp, vp, vp, pvp])

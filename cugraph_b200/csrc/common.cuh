@@ -156,6 +156,19 @@ inline handle_impl const& H(const cugraph_resource_handle_t* h)
   return *reinterpret_cast<handle_impl const*>(h);
 }
 
+// Beamer's direction switch of a direction-optimising BFS level (the reference: bfs_impl.cuh:291-297), with the handle's
+// CUGRAPH_B200_BFS_ALPHA / _BETA.  n_f, m_f: vertices and out-edges of the current frontier; prev_n_f: vertices of the
+// previous one (0 at the first level); m_u: edges into the unvisited vertices; n_unvisited: vertices not visited yet.
+// Returns the direction of this level (true = bottom-up), given that of the last one.  Single-GPU BFS (run_bfs) and
+// multi-GPU BFS (cugraph_b200_bfs_bottom_up) both decide with it.
+inline bool bfs_bottom_up(handle_impl const& h, bool bottom_up, long long n_f, long long prev_n_f, unsigned long long m_f,
+                          unsigned long long m_u, long long n_unvisited)
+{
+  if (!bottom_up && (double)m_f * h.tune.bfs_alpha > (double)m_u && n_f >= prev_n_f) return true;
+  if (bottom_up && (double)n_f * h.tune.bfs_beta < (double)n_unvisited && n_f < prev_n_f) return false;
+  return bottom_up;
+}
+
 // streams of live handles: buffers that outlive their handle (graphs, results) are freed
 // synchronously instead of on a destroyed stream (capi_basic.cu)
 bool stream_is_live(cudaStream_t s);

@@ -7,8 +7,8 @@
 // the C ABI (the resource handle bound to the caller's CUDA stream is made in capi_basic.cu): rectangular edge blocks with the
 // same binned / column-blocked layout as the single-GPU graph, the block pull sweep and the fused
 // per-iteration vertex step, the transposed block sweep, the owner steps of Katz, eigenvector centrality and HITS, the BFS
-// pull step, the SSSP push relaxation, the WCC min-label round and the two sides of an extract_paths round.  All calls only ENQUEUE work on the handle's stream (the
-// SSSP and WCC calls read back one queue size; the first transposed sweep of a block builds its column-major copy).
+// pull and push steps, the SSSP push relaxation, the WCC min-label round and the two sides of an extract_paths round.  All calls only ENQUEUE work on the handle's stream (the
+// push calls of BFS, SSSP, WCC and SCC read back one queue size; the first transposed sweep of a block builds its column-major copy).
 #include "advance.cuh"
 #include "centrality_ops.cuh"
 
@@ -20,7 +20,7 @@
 
 namespace b200 {
 
-// the column-major copy of a block (built by the first SSSP, WCC or transposed sweep call on the block): physical rows are
+// the column-major copy of a block (built by the first BFS push, SSSP, WCC, SCC or transposed sweep call on the block): physical rows are
 // the block's column slots in descending out-degree (row_vertex = column slot), neighbours are row slots
 struct block_push_t {
   std::unique_ptr<csx_t> csx;
@@ -42,7 +42,7 @@ struct block_rows_queue_t {
 
 struct block_impl {
   std::unique_ptr<csx_t> csx;
-  std::unique_ptr<block_push_t> push;  // lazily built (multi-GPU SSSP, WCC and transposed sweeps)
+  std::unique_ptr<block_push_t> push;  // lazily built (multi-GPU BFS push steps, SSSP, WCC, SCC and transposed sweeps)
   std::unique_ptr<block_rows_queue_t> rows_queue;  // lazily built (multi-GPU SCC's backward push)
   int32_t n_rows{0}, n_cols{0}, n_span{0};
   bool weighted{false};
@@ -191,6 +191,7 @@ struct block_queue_counts_t {
 __device__ __forceinline__ bool column_active(float v) { return v < INFINITY; }
 __device__ __forceinline__ bool column_active(double v) { return v < INFINITY; }
 __device__ __forceinline__ bool column_active(long long v) { return v != LLONG_MAX; }
+__device__ __forceinline__ bool column_active(uint8_t f) { return f != 0; }  // a BFS frontier flag
 
 // physical rows r < n_ne of the push copy whose column slot row_vertex[r] is active, with their degrees
 template <typename O, typename T>
@@ -260,6 +261,35 @@ struct block_pred_op {
     if (k < code[nbr]) atomicMin(code + nbr, k);
   }
 };
+
+// ---- one level of multi-GPU BFS on this GPU's edge block, push direction (the MG form of bfs_topdown_op, traverse.cu;
+// reference: the top-down step of bfs_impl.cuh on an edge partition).  The frontier columns (byte flags, gathered as for
+// the pull step) are queued through the push copy, and every edge into an unvisited row offers the global code of its
+// source; the row keeps the largest, so a level's candidate does not depend on the order of the atomics.
+struct block_bfs_push_op {
+  int32_t const* col_of;   // column slot of a physical row of the push copy
+  uint8_t const* visited;  // over row slots
+  long long maxpart;
+  int grid_cols, grid_c;
+  long long* cand;         // over row slots, -1 = no frontier source
+  __device__ __forceinline__ void edge(int src, long long, int nbr) const
+  {
+    if (visited[nbr]) return;
+    const long long code = column_code(col_of[src], maxpart, grid_cols, grid_c);
+    if (code > cand[nbr]) atomicMax(cand + nbr, code);  // a stale read is smaller than the current value: never skips a win
+  }
+};
+
+// argument checks shared by the two BFS block calls
+void check_bfs_block_args(block_impl const& b, device_array_view_impl const* fv, device_array_view_impl const* vv,
+                          device_array_view_impl const* cv, size_t maxpart, int grid_cols, int grid_c)
+{
+  B200_EXPECTS(dtype_size(fv->type) == 1 && dtype_size(vv->type) == 1, CUGRAPH_INVALID_INPUT, "frontier / visited are byte flags");
+  B200_EXPECTS(cv->type == INT64, CUGRAPH_INVALID_INPUT, "cand must be INT64");
+  B200_EXPECTS(fv->size >= (size_t)b.n_cols && vv->size >= (size_t)b.n_rows && cv->size >= (size_t)b.n_rows,
+               CUGRAPH_INVALID_INPUT, "flag / candidate arrays shorter than the block's slots");
+  B200_EXPECTS(maxpart > 0 && grid_cols > 0 && grid_c >= 0 && grid_c < grid_cols, CUGRAPH_INVALID_INPUT, "bad grid position");
+}
 
 // the column-major copy of the block, built on first use (the mirror image of pull_view / out_sweep_view, graph_build.cu)
 block_push_t& push_copy(handle_impl const& h, block_impl& b)
@@ -881,11 +911,7 @@ cugraph_error_code_t cugraph_b200_block_bfs_pull(const cugraph_resource_handle_t
     auto const* fv = V(frontier_cols);
     auto const* vv = V(visited_rows);
     auto const* cv = V(cand);
-    B200_EXPECTS(dtype_size(fv->type) == 1 && dtype_size(vv->type) == 1, CUGRAPH_INVALID_INPUT, "frontier / visited are byte flags");
-    B200_EXPECTS(cv->type == INT64, CUGRAPH_INVALID_INPUT, "cand must be INT64");
-    B200_EXPECTS(fv->size >= (size_t)b->n_cols && vv->size >= (size_t)b->n_rows && cv->size >= (size_t)b->n_rows,
-                 CUGRAPH_INVALID_INPUT, "flag / candidate arrays shorter than the block's slots");
-    B200_EXPECTS(maxpart > 0 && grid_cols > 0 && grid_c >= 0 && grid_c < grid_cols, CUGRAPH_INVALID_INPUT, "bad grid position");
+    check_bfs_block_args(*b, fv, vv, cv, maxpart, grid_cols, grid_c);
     csx_t const& c = *b->csx;
     if (c.offs64)
       block_bfs_pull<int64_t>(h, c, (uint8_t const*)fv->data, (uint8_t const*)vv->data, (long long)maxpart, grid_cols, grid_c,
@@ -895,6 +921,45 @@ cugraph_error_code_t cugraph_b200_block_bfs_pull(const cugraph_resource_handle_t
                               (long long*)cv->data, b->n_rows);
     check_last("block_bfs_pull");
   });
+}
+
+// cand[row slot] = largest global code of a frontier source of that (unvisited) row, or -1.  Asynchronous, apart from the
+// read-back of the queue size (and the first call's push copy).
+cugraph_error_code_t cugraph_b200_block_bfs_push(const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+                                                 const cugraph_type_erased_device_array_view_t* frontier_cols,
+                                                 const cugraph_type_erased_device_array_view_t* visited_rows, size_t maxpart,
+                                                 int grid_cols, int grid_c, cugraph_type_erased_device_array_view_t* cand,
+                                                 cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(block && frontier_cols && visited_rows && cand, CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto* b        = reinterpret_cast<block_impl*>(block);
+    auto const* fv = V(frontier_cols);
+    auto const* vv = V(visited_rows);
+    auto const* cv = V(cand);
+    check_bfs_block_args(*b, fv, vv, cv, maxpart, grid_cols, grid_c);
+    auto* out = (long long*)cv->data;
+    B200_LAUNCH(h, k_fill<long long>, grid_for(b->n_rows, 1, h.sm_count * 8), kBlock, 0, out, (int64_t)b->n_rows, -1ll);
+    block_push_t& p     = push_copy(h, *b);
+    auto const* front   = (uint8_t const*)fv->data;
+    const block_bfs_push_op op{p.csx->row_vertex.as<int32_t>(), (uint8_t const*)vv->data, (long long)maxpart, grid_cols, grid_c,
+                               out};
+    if (p.csx->offs64) block_push_round<int64_t>(h, p, front, op);
+    else block_push_round<int32_t>(h, p, front, op);
+    check_last("block_bfs_push");
+  });
+}
+
+// whether a direction-optimising BFS level runs bottom-up (bfs_bottom_up, common.cuh, with the handle's knobs)
+bool_t cugraph_b200_bfs_bottom_up(const cugraph_resource_handle_t* handle, bool_t bottom_up_now, size_t n_f, size_t prev_n_f,
+                                  size_t m_f, size_t m_u, size_t n_unvisited)
+{
+  if (!handle) return bottom_up_now;
+  return bfs_bottom_up(H(handle), bottom_up_now == TRUE, (long long)n_f, (long long)prev_n_f, (unsigned long long)m_f,
+                       (unsigned long long)m_u, (long long)n_unvisited)
+           ? TRUE
+           : FALSE;
 }
 
 // cand_rows[row slot] = min key over the proposals dist_cols[col] + w < cutoff of the active columns, else INT64_MAX

@@ -255,17 +255,13 @@ void run_bfs(handle_impl const& h, csx_t const& c, int32_t nv, int32_t const* so
   bool bottom_up = false, frontier_is_bitmap = false;
   bool deg_ready = false;  // cur_l holds the degrees of the entries of cur (written by the top-down level that built it)
   int level = 0, prev_n_f = 0;
-  // Beamer's switch points (the reference: bfs_impl.cuh:291-297, alpha ~ E/V*0.267, beta = 24)
-  const double alpha = h.tune.bfs_alpha, beta = h.tune.bfs_beta;  // only the schedule depends on them, never the result
-  const bool trace   = h.tune.bfs_trace;
+  // Beamer's switch points (bfs_bottom_up, common.cuh): only the schedule depends on them, never the result
+  const bool trace = h.tune.bfs_trace;
   advance_scratch_t adv;
   adv.init(h, nv, (int64_t)c.nnz);
   while (n_f > 0 && level < depth_limit) {
-    if (direction_optimizing) {
-      unsigned long long m_u = m_total - std::min(m_vis, m_total);
-      if (!bottom_up && (double)m_f * alpha > (double)m_u && n_f >= prev_n_f) bottom_up = true;
-      else if (bottom_up && (double)n_f * beta < (double)(nv - n_vis) && n_f < prev_n_f) bottom_up = false;
-    }
+    if (direction_optimizing)
+      bottom_up = bfs_bottom_up(h, bottom_up, n_f, prev_n_f, m_f, m_total - std::min(m_vis, m_total), nv - n_vis);
     CUDA_TRY(cudaMemsetAsync(cnt.data(), 0, sizeof(frontier_counters_t), h.stream));
     if (!bottom_up) {
       if (frontier_is_bitmap) {

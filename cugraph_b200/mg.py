@@ -346,6 +346,7 @@ class MGGraph:
         self._w_sum_local = float(ones.sum().item()) if self.weighted else 0.0   # SSSP's initial window width
         self._sssp_avg = None                                                       # (average weight, average degree)
         self._id_order = None                                  # (local ids by external id, sorted external ids)
+        self.last_bfs_stats = None
         self.last_sssp_stats = None
         self.last_wcc_stats = None
         self.last_scc_stats = None
@@ -552,12 +553,15 @@ class MGGraph:
     # fill_edge_dst_property broadcasts (fill_edge_src_dst_property.cuh:1368) and an all-to-all-v of the discovered
     # (vertex, predecessor) pairs over the row communicator (transform_reduce_if_v_frontier_outgoing_e_by_dst.cuh:981-1074).
     # Here one level is: all-gather of the owners' frontier flags inside the column group (-> flags over the block's
-    # source slots), all-gather of the visited flags inside the row group (-> flags over its destination slots), the
-    # block's pull step on the device (cugraph_b200_block_bfs_pull: every unvisited destination looks for a source in the
-    # frontier), ONE max-reduce-scatter of the candidate predecessors inside the row group, and the owners' update.
+    # source slots), all-gather of the visited flags inside the row group (-> flags over its destination slots), ONE step
+    # on the block, ONE max-reduce-scatter of the candidate predecessors inside the row group, the owners' update and one
+    # all-reduce of the new frontier's size (with its degree sums when the direction is chosen per level).  The step is
+    # top-down (cugraph_b200_block_bfs_push: the frontier columns push their edges into the unvisited rows) or bottom-up
+    # (cugraph_b200_block_bfs_pull: every unvisited row looks for a source in the frontier); both take and give the same
+    # arrays, so the collectives of a level never depend on its direction.
     # Distances are the BFS levels (bit-exact vs single-GPU); a predecessor is any frontier neighbour, as in the reference.
     # ------------------------------------------------------------------------------------------
-    def bfs(self, source, depth_limit=-1, compute_predecessors=True):
+    def bfs(self, source, depth_limit=-1, compute_predecessors=True, *, direction_optimizing=False):
         """BFS from one source or from a set of sources.  Returns (vertices, distances, predecessors) of the vertices this
         rank owns: int32 distances (INT32_MAX = unreachable), predecessors as external ids (-1 = none), or None when not
         requested.
@@ -568,7 +572,16 @@ class MGGraph:
             as cugraph_bfs does with several sources; with no id on any rank every vertex is unreached.  Every rank raises
             the same error (one all-reduce): TypeError for ids in a dtype other than the edge ids' on some rank,
             CugraphValueError for an id that is not a vertex.
-        Every rank must pass the same form, a scalar or an array (not checked: the collectives would not match)."""
+          direction_optimizing: False runs every level top-down, as cugraph_bfs does.  True picks each level's direction
+            by single GPU's rule and knobs (cugraph_b200_bfs_bottom_up, CUGRAPH_B200_BFS_ALPHA / _BETA) over global counts:
+            the frontier's size and out-degree sum, the unvisited vertices and the sum of their in-degrees (the first call
+            counts the degrees, see degrees()).  Unlike cugraph_bfs, True is accepted on every graph, directed ones
+            included: the block stores its edges by destination, so its bottom-up step reads true in-edges, and whether
+            an edge list is symmetric is not known here anyway.  Only the schedule depends on the flag: the distances are
+            the same, the predecessors may differ (any frontier neighbour).
+        Every rank must pass the same form, a scalar or an array, and the same direction_optimizing (not checked: the
+        collectives would not match).  Sets last_bfs_stats = dict(levels, top_down, bottom_up): the levels run and how
+        many ran in each direction."""
         p, g = self.part, self.part.groups
         dev, mp = self.device, p.maxpart
         imax = torch.iinfo(torch.int32).max
@@ -588,25 +601,52 @@ class MGGraph:
             dist_own[lids] = 0
             visited[lids] = 1
             frontier[lids] = 1
+        do = bool(direction_optimizing)
+        if do:
+            # (out, in)-degrees over the owned slots, 0 in the padding; the frontier's counts and the edge total
+            self.degrees()
+            deg = torch.zeros((2, mp), dtype=torch.int64, device=dev)
+            deg[0, :p.n_local] = self._degrees[1]
+            deg[1, :p.n_local] = self._degrees[0]
+            head = torch.cat([frontier.sum().to(torch.int64).reshape(1), (deg * frontier).sum(1), deg[1].sum().reshape(1)])
+            dist.all_reduce(head)
+            n_f, m_f, m_vis_in, m_total = head.tolist()          # m_vis_in: the in-degree sum of the visited vertices
+            n_vis, prev_n_f = n_f, 0
         f_cols = torch.zeros(self.n_cols, dtype=torch.uint8, device=dev)
         v_rows = torch.zeros(self.n_rows, dtype=torch.uint8, device=dev)
         cand = torch.full((self.n_rows,), -1, dtype=torch.int64, device=dev)
         cand_own = torch.full((mp,), -1, dtype=torch.int64, device=dev)
-        level = 0
+        level = n_bottom_up = 0
+        bottom_up = False
         with _views(f_cols, v_rows, cand) as (vf, vv, vc):
             while depth_limit < 0 or level < depth_limit:
+                if do:
+                    bottom_up = bool(self.lib.cugraph_b200_bfs_bottom_up(self.handle.ptr, 1 if bottom_up else 0, n_f, prev_n_f,
+                                                                         m_f, m_total - m_vis_in, p.n_global - n_vis))
                 all_gather_into(f_cols, frontier, g.col_group)
                 all_gather_into(v_rows, visited, g.row_group)
-                self._call("cugraph_b200_block_bfs_pull", self.block, vf.ptr, vv.ptr, mp, g.C, g.c, vc.ptr)
+                step = "cugraph_b200_block_bfs_pull" if bottom_up else "cugraph_b200_block_bfs_push"
+                self._call(step, self.block, vf.ptr, vv.ptr, mp, g.C, g.c, vc.ptr)
                 reduce_scatter_into(cand_own, cand, g.row_group, op=dist.ReduceOp.MAX)
                 new = (visited == 0) & (cand_own >= 0)
                 level += 1
+                n_bottom_up += int(bottom_up)
                 dist_own[new] = level
                 pred_code[new] = cand_own[new]
                 visited |= new.to(torch.uint8)
                 frontier = new.to(torch.uint8)
-                if _global_count(new) == 0:
+                if do:
+                    counts = torch.cat([new.sum().to(torch.int64).reshape(1), (deg * new).sum(1)])
+                    dist.all_reduce(counts)
+                    n_new, m_new, in_new = counts.tolist()
+                    prev_n_f, n_f, m_f = n_f, n_new, m_new
+                    n_vis += n_new
+                    m_vis_in += in_new
+                else:
+                    n_new = _global_count(new)
+                if n_new == 0:
                     break
+        self.last_bfs_stats = dict(levels=level, top_down=level - n_bottom_up, bottom_up=n_bottom_up)
         verts = p.vertices
         d_out = dist_own[:p.n_local].clone()
         if not compute_predecessors:
@@ -1367,10 +1407,11 @@ class _SccRun:
         return label
 
 
-def bfs(graph: MGGraph, sources, depth_limit=-1, compute_predecessors=True):
+def bfs(graph: MGGraph, sources, depth_limit=-1, compute_predecessors=True, *, direction_optimizing=False):
     """(vertices, distances, predecessors) of the vertices owned by this rank (the MG contract of pylibcugraph.bfs).
-    sources: one external id, the same on every rank, or a 1-D tensor / array of this rank's source ids (see MGGraph.bfs)."""
-    return graph.bfs(sources, depth_limit, compute_predecessors)
+    sources: one external id, the same on every rank, or a 1-D tensor / array of this rank's source ids;
+    direction_optimizing: top-down on every level (False) or single GPU's per-level switch (True) (see MGGraph.bfs)."""
+    return graph.bfs(sources, depth_limit, compute_predecessors, direction_optimizing=direction_optimizing)
 
 
 def extract_paths(graph: MGGraph, distances, predecessors, destinations):

@@ -4,7 +4,7 @@
  *  - multi-GPU: the reference receives NCCL communicators inside a raft::handle_t built by raft-dask / MPI
  *    (python/pylibcugraph/pylibcugraph/comms/comms_wrapper.pyx:10-32, cpp/tests/utilities/mg_utilities.cpp:37-55) and keeps
  *    the 2D-partitioned blocks inside graph_t.  raft is not part of this build: cugraph_graph_create_mg and the multi-GPU
- *    algorithm entry points return CUGRAPH_NOT_IMPLEMENTED; multi-GPU PageRank, BFS, extract_paths, SSSP, WCC, Katz,
+ *    algorithm entry points return CUGRAPH_NOT_IMPLEMENTED; multi-GPU PageRank, BFS, extract_paths, SSSP, WCC, SCC, Katz,
  *    eigenvector centrality and HITS are driven by the launcher (cugraph_b200/mg.py, one process per GPU over torch.distributed / NCCL) on top of
  *    the cugraph_b200_block_* and owner-step device pieces declared below.
  *  - profiling hooks used by bench.py to time the dominant kernel on the handle's stream.
@@ -183,6 +183,29 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_bfs_pull(
   const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
   const cugraph_type_erased_device_array_view_t* frontier_cols, const cugraph_type_erased_device_array_view_t* visited_rows,
   size_t maxpart, int grid_cols, int grid_c, cugraph_type_erased_device_array_view_t* cand, cugraph_error_t** error);
+
+/* The same level in the push direction (the role of the top-down step of cpp/src/traversal/bfs_impl.cuh on one edge
+ * partition).  Same arguments and the same checks as cugraph_b200_block_bfs_pull.  cand is first filled with -1; then the
+ * frontier columns are queued through the block's column-major copy (shared with cugraph_b200_block_sssp_relax / _wcc_min /
+ * _scc_push / the transposed sweep, built by the first of these calls on the block and kept), and every edge (row, col) of a
+ * frontier column into an unvisited row raises cand[row] to col's global code (atomic max).  cand[row] is therefore the
+ * LARGEST code among the row's frontier sources, whatever order the edges are visited in.  Asynchronous, apart from one
+ * read-back of the number of frontier columns and their edge count. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_bfs_push(
+  const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+  const cugraph_type_erased_device_array_view_t* frontier_cols, const cugraph_type_erased_device_array_view_t* visited_rows,
+  size_t maxpart, int grid_cols, int grid_c, cugraph_type_erased_device_array_view_t* cand, cugraph_error_t** error);
+
+/* The direction of one level of a direction-optimising BFS (Beamer's rule, as single-GPU cugraph_bfs decides it, with the
+ * handle's CUGRAPH_B200_BFS_ALPHA / _BETA), given the direction of the last level (bottom_up_now):
+ *   top-down -> bottom-up when m_f * alpha > m_u and n_f >= prev_n_f;
+ *   bottom-up -> top-down when n_f * beta < n_unvisited and n_f < prev_n_f;
+ *   otherwise the direction stays.
+ * n_f, m_f: vertices and out-edges of the current frontier; prev_n_f: vertices of the previous frontier (0 at the first
+ * level); m_u: edges into the unvisited vertices; n_unvisited: vertices not visited yet.  Returns TRUE for bottom-up.  A NULL
+ * handle returns bottom_up_now.  Host only, no device work. */
+CUGRAPH_EXPORT bool_t cugraph_b200_bfs_bottom_up(const cugraph_resource_handle_t* handle, bool_t bottom_up_now, size_t n_f,
+                                                 size_t prev_n_f, size_t m_f, size_t m_u, size_t n_unvisited);
 
 /* One relaxation round of multi-GPU SSSP on this GPU's edge block (push direction; the role of the MG relaxation of
  * cpp/src/traversal/sssp_impl.cuh:301-375 on one edge partition).  The block must have been created with weights.

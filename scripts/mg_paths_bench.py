@@ -5,12 +5,15 @@
 
 Input: BASELINE's BFS configuration, as bench.py builds it for one GPU: RMAT-`scale` ef-16 (seed 0) symmetrised, unweighted.
 Every rank generates the edge list and keeps its share.
-Cases: MG BFS from 1 and from 64 sources (random vertices with edges, seed 1; the 64 dealt round-robin to the ranks), then
+Cases: MG BFS from 1 and from 64 sources (random vertices with edges, seed 1; the 64 dealt round-robin to the ranks) in
+three schedules: top-down on every level (bfs_<k>_sources, MGGraph.bfs's default), direction-optimising
+(bfs_<k>_sources_optimizing) and every level bottom-up (bfs_<k>_sources_all_bottom_up: direction_optimizing=True on a
+second MGGraph built under CUGRAPH_B200_BFS_ALPHA = CUGRAPH_B200_BFS_BETA = 1e30), each with its last_bfs_stats; then
 extract_paths of 2^16 random vertices (dealt the same way) and of every vertex (each rank its own vertices) on the
-64-source result.  Single GPU (world size 1 only: the whole graph on one GPU): cugraph_bfs from the same sources and
+64-source top-down result.  Single GPU (world size 1 only: the whole graph on one GPU): cugraph_bfs from the same sources and
 cugraph_extract_paths of the same destinations, the same way.
-Parity first: on RMAT-16 from 64 sources, the MG distances must equal single-GPU cugraph_bfs's and the MG max_path_length
-cugraph_extract_paths' on rank 0; a mismatch ends the run.
+Parity first: on RMAT-16 from 64 sources, the MG distances of the top-down and the direction-optimising schedule must equal
+single-GPU cugraph_bfs's and the MG max_path_length cugraph_extract_paths' on rank 0; a mismatch ends the run.
 Timing: one warm-up call, then `calls` timed calls, each with a host clock that ends in a device synchronise, the max over
 ranks.  Prints one JSON line on rank 0 (ms per call, position rounds of each extract_paths case), with the card name and
 power limit read in the same run.  --backend gloo runs the same steps over gloo (a functional check of the script)."""
@@ -115,8 +118,9 @@ def parity(groups, scale=16):
     G = mg.MGGraph(s, d, None, groups)
     v, dd, pred = G.bfs(_deal(srcs, rank, world))
     _, length = G.extract_paths(dd, pred, _deal(dests, rank, world))
+    _, dd_opt, _ = G.bfs(_deal(srcs, rank, world), direction_optimizing=True)
     parts = [None] * world
-    dist.all_gather_object(parts, (v.cpu(), dd.cpu()))
+    dist.all_gather_object(parts, (v.cpu(), dd.cpu(), dd_opt.cpu()))
     del G
     if rank != 0:
         return None
@@ -125,7 +129,7 @@ def parity(groups, scale=16):
     ref = sg.distances()
     sg_len = sg.extract_paths(dests.to("cuda"))
     sg.free()
-    same = all(torch.equal(ref[pv.long()], pd.long()) for pv, pd in parts)
+    same = all(torch.equal(ref[pv.long()], pd.long()) and torch.equal(pd, po) for pv, pd, po in parts)
     return {"ok": bool(same and sg_len == length), "scale": scale, "max_path_length": length}
 
 
@@ -196,12 +200,32 @@ def main(argv=None):
     mg_res = {}
     for k, src in srcs.items():
         mine = _deal(src, rank, world)
+        mg_res[f"bfs_{k}_sources_optimizing"], _ = _series(lambda: G.bfs(mine, direction_optimizing=True), args.calls)
+        mg_res[f"bfs_{k}_sources_optimizing"].update(G.last_bfs_stats)
         mg_res[f"bfs_{k}_sources"], last = _series(lambda: G.bfs(mine), args.calls)
+        mg_res[f"bfs_{k}_sources"].update(G.last_bfs_stats)
     _, dd, pred = last
     for name, dests in (("paths_2^16", _deal(dests16, rank, world)), ("paths_all", G.part.vertices)):
         mg_res[name], (_, length) = _series(lambda: G.extract_paths(dd, pred, dests), args.calls)
         mg_res[name].update(rounds=G.last_paths_stats["rounds"], max_path_length=length)
     del G, dd, pred, last
+    torch.cuda.empty_cache()
+    # every level bottom-up: the knobs are read when the graph's handle is made
+    knobs = {k: os.environ.get(k) for k in ("CUGRAPH_B200_BFS_ALPHA", "CUGRAPH_B200_BFS_BETA")}
+    os.environ.update({k: "1e30" for k in knobs})
+    s, d, _ = _graph(args.scale, rank, world)
+    G = mg.MGGraph(s, d, None, groups)
+    del s, d
+    for k, v in knobs.items():
+        if v is None:
+            os.environ.pop(k)
+        else:
+            os.environ[k] = v
+    for k, src in srcs.items():
+        mine = _deal(src, rank, world)
+        mg_res[f"bfs_{k}_sources_all_bottom_up"], _ = _series(lambda: G.bfs(mine, direction_optimizing=True), args.calls)
+        mg_res[f"bfs_{k}_sources_all_bottom_up"].update(G.last_bfs_stats)
+    del G
     torch.cuda.empty_cache()
     sg_res = None
     if world == 1:
