@@ -3,8 +3,9 @@ for step against fp64 references: the harness of tests/test_sweep_drivers_gpu.py
 tests/test_sweep_drivers_cpu.py (the emulation build of the library, tests/emu_py.py).
 
 Each check calls the C entry point, reads the iteration count k the driver reports, and runs its fp64 reference for exactly
-k steps.  k itself must be the step at which the reference converges under the driver's own test (Katz: diff < epsilon;
-eigenvector, HITS: diff < V epsilon, the threshold formed in T as the driver forms it).  The two may differ by one step only
+k steps (check_*: the call; verify_*: the check of a result by internal id, which the multi-GPU harness shares).  k itself
+must be the step at which the reference converges under the driver's own test (Katz: diff < epsilon; eigenvector, HITS:
+diff < V epsilon, the threshold formed in T as the driver forms it).  The two may differ by one step only
 where the reference's difference at the earlier of the two steps lies within the bound below of the threshold; in float64
 that bound is ~1e-12 of the threshold, so there the counts must agree.  HITS' hub_score_differences must match the
 reference's last difference within the same bound.
@@ -39,6 +40,21 @@ The bound.  Every driver iterates a non-negative map (weights and values are non
   covered by the factor SECOND_ORDER.
 - Exact zeros: where the reference is 0 (the hubs of a vertex without out-edges, the authorities of one without in-edges,
   personalized scores of vertices nothing reaches) the driver must give exactly 0.
+
+The multi-GPU drivers (cugraph_b200/mg.py, checked by tests/mg_sweep_drivers.py) run the same steps with the sweep spread
+over an R x C grid: x is all-gathered, every block sweeps its rows, and the partial y are reduce-scattered over a group of
+G members (the row group, G = C, for the pull sweep; the column group, G = R, for HITS' transposed sweep).
+- The all-gather copies: x is exact.
+- A block's row holds a subset of the graph row's entries, at most d_max of them, and every term is non-negative, so the
+  block's partial y is within sweep_delta(T, d_max) of its own exact value, relatively (the bound above, rounded to T).
+- The reduce-scatter adds G non-negative values in T: G - 1 roundings, each relative to a partial sum no larger than the
+  total, whatever the order (NCCL's ring and the in-process stand-in alike).  So one sweep adds at most
+      delta_G = sweep_delta(T, d_max) + (G - 1) u,
+  which the verifiers take as extra = (G - 1) u on top of delta; HITS takes one for each of its two sweeps.
+- Out-weight sums: fp64 sums over the blocks, reduce-scattered in fp64 and rounded once to T: one summation tree of the
+  vertex's out-weights, at most d_max_out - 1 fp64 additions, as on one GPU.  The owner steps' partials (norms,
+  differences, the dangling sum) are fp64 sums of non-negative terms all-reduced in fp64: within n e.  Maxima are exact.
+So every bound above holds with delta_G in place of delta, and nothing else changes.
 
 The worst |got - ref| / (rtol |ref|) of each check is returned, recorded in WORST, printed with -s, and quoted with the
 bound in any failure message.
@@ -328,13 +344,20 @@ def katz_alpha(graph, share=0.5):
 
 
 def check_katz(h, g, graph, alpha, beta, epsilon, betas=False, key=None, max_iterations=1000):
-    """Katz from x = 0, x <- alpha A x + beta until sum |x - x_prev| < epsilon, then x / ||x||_2"""
-    T, V, A = graph.T, graph.V, graph.A
-    label = f"Katz {graph.label} alpha={alpha:.4g} beta={beta} epsilon={epsilon}{' betas' if betas else ''}"
-    bv = _view(_dev(np.full(V, 7.0), T) if betas else None)       # the C API ignores betas
+    """cugraph_katz_centrality on the graph, checked by verify_katz"""
+    bv = _view(_dev(np.full(graph.V, 7.0), graph.T) if betas else None)       # the C API ignores betas
     verts, vals, k = centrality_call("katz_centrality", h, g, bv.ptr, float(alpha), float(beta), float(epsilon),
                                      int(max_iterations), 0)
     bv.free()
+    return verify_katz(graph, graph.dense(verts, vals), k, alpha, beta, epsilon, key=key, max_iterations=max_iterations,
+                       tag=" betas" if betas else "")
+
+
+def verify_katz(graph, got, k, alpha, beta, epsilon, extra=0.0, key=None, max_iterations=1000, tag=""):
+    """Katz from x = 0, x <- alpha A x + beta until sum |x - x_prev| < epsilon, then x / ||x||_2: `got` (by internal id)
+    after the k steps the driver reports; `extra` is the relative rounding a sweep adds past one GPU's"""
+    T, V, A = graph.T, graph.V, graph.A
+    label = f"Katz {graph.label} alpha={alpha:.4g} beta={beta} epsilon={epsilon}{tag}"
     thr = float(T(epsilon))
 
     def step(x):
@@ -344,7 +367,7 @@ def check_katz(h, g, graph, alpha, beta, epsilon, betas=False, key=None, max_ite
     u = unit(T)
     rho = alpha * float(abs(A).sum(axis=1).max())
     assert rho < 1.0, rho
-    delta = sweep_delta(T, int(graph.indeg.max()))
+    delta = sweep_delta(T, int(graph.indeg.max())) + extra
     err = [delta * min(j, 1.0 / (1.0 - rho)) for j in range(len(xs))]
     l1 = [float(x.sum()) for x in xs]
     tol_diff = [SECOND_ORDER * (err[j + 1] * l1[j + 1] + err[j] * l1[j] + V * E * (l1[j + 1] + l1[j]))
@@ -353,17 +376,23 @@ def check_katz(h, g, graph, alpha, beta, epsilon, betas=False, key=None, max_ite
     x = xs[k]
     ref = x / math.sqrt(float((x * x).sum()))
     rtol = SECOND_ORDER * (2.0 * err[k] + V * E + u + 2.0 * E)
-    return compare(graph.dense(verts, vals), ref, rtol, f"{label}, {k} steps", key or f"katz {np.dtype(T).name}")
+    return compare(got, ref, rtol, f"{label}, {k} steps", key or f"katz {np.dtype(T).name}")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # eigenvector centrality
 # ---------------------------------------------------------------------------------------------------------------------
 def check_eigenvector(h, g, graph, epsilon, key=None, max_iterations=1000):
-    """x <- (A x + x) / ||A x + x||_2 from x = 1/V until sum |x - x_prev| < V epsilon"""
-    T, V, A = graph.T, graph.V, graph.A
-    label = f"eigenvector {graph.label} epsilon={epsilon}"
+    """cugraph_eigenvector_centrality on the graph, checked by verify_eigenvector"""
     verts, vals, k = centrality_call("eigenvector_centrality", h, g, float(epsilon), int(max_iterations), 0)
+    return verify_eigenvector(graph, graph.dense(verts, vals), k, epsilon, key=key, max_iterations=max_iterations)
+
+
+def verify_eigenvector(graph, got, k, epsilon, extra=0.0, key=None, max_iterations=1000, tag=""):
+    """x <- (A x + x) / ||A x + x||_2 from x = 1/V until sum |x - x_prev| < V epsilon: `got` (by internal id) after the
+    k steps the driver reports; `extra` is the relative rounding a sweep adds past one GPU's"""
+    T, V, A = graph.T, graph.V, graph.A
+    label = f"eigenvector {graph.label} epsilon={epsilon}{tag}"
     thr = float(T(V) * T(epsilon))
 
     def step(x):
@@ -373,29 +402,38 @@ def check_eigenvector(h, g, graph, epsilon, key=None, max_iterations=1000):
     xs, diffs, k_ref = run_until(step, np.full(V, 1.0 / V), k, thr, max_iterations)
     u = unit(T)
     theta = V * E + u + 2.0 * E
-    D = [2.0 * j * (sweep_delta(T, int(graph.indeg.max())) + 2.0 * u + 2.0 * E) for j in range(len(xs))]
+    D = [2.0 * j * (sweep_delta(T, int(graph.indeg.max())) + extra + 2.0 * u + 2.0 * E) for j in range(len(xs))]
     rt = [SECOND_ORDER * (math.expm1(Dj) + theta) for Dj in D]
     l1 = [float(x.sum()) for x in xs]
     tol_diff = [rt[j + 1] * l1[j + 1] + rt[j] * l1[j] + V * E * (l1[j + 1] + l1[j]) for j in range(len(diffs))]
     check_count(k, k_ref, diffs, thr, tol_diff, T, label)
-    return compare(graph.dense(verts, vals), xs[k], rt[k], f"{label}, {k} steps", key or f"eigenvector {np.dtype(T).name}")
+    return compare(got, xs[k], rt[k], f"{label}, {k} steps", key or f"eigenvector {np.dtype(T).name}")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # HITS
 # ---------------------------------------------------------------------------------------------------------------------
 def check_hits(h, g, graph, epsilon, guess=None, normalize=True, key=None, max_iterations=1000):
-    """authorities = N hubs, hubs = N^T authorities (N: the unweighted multigraph), both divided by their maximum, until
-    sum |hubs - hubs_prev| < V epsilon; divided by their sums with `normalize`.  guess = (internal ids, values): the
-    initial hubs, 0 for the vertices it leaves out, divided by their sum"""
-    T, V, N, Nt = graph.T, graph.V, graph.N, graph.Nt
-    label = (f"HITS {graph.label} epsilon={epsilon} normalize={normalize}"
-             f"{f' guess on {len(guess[0])} vertices' if guess is not None else ''}")
+    """cugraph_hits on the graph, checked by verify_hits"""
     gd = None
     if guess is not None:
         vt = np.int32 if graph.ids is None else np.int64
-        gd = (_dev(graph.ext(np.asarray(guess[0])), vt), _dev(guess[1], T))
+        gd = (_dev(graph.ext(np.asarray(guess[0])), vt), _dev(guess[1], graph.T))
     verts, hubs, auth, hdiff, k = hits_call(h, g, epsilon, max_iterations, gd, normalize)
+    return verify_hits(graph, graph.dense(verts, hubs), graph.dense(verts, auth), hdiff, k, epsilon, guess, normalize,
+                       key=key, max_iterations=max_iterations)
+
+
+def verify_hits(graph, hubs, auth, hdiff, k, epsilon, guess=None, normalize=True, extra=(0.0, 0.0), key=None,
+                max_iterations=1000, tag=""):
+    """authorities = N hubs, hubs = N^T authorities (N: the unweighted multigraph), both divided by their maximum, until
+    sum |hubs - hubs_prev| < V epsilon; divided by their sums with `normalize`.  guess = (internal ids, values): the
+    initial hubs, 0 for the vertices it leaves out, divided by their sum.  hubs, auth (by internal id), hdiff
+    (hub_score_differences) and k as the driver reports them; extra = (pull, transposed): the relative rounding each of the
+    two sweeps adds past one GPU's"""
+    T, V, N, Nt = graph.T, graph.V, graph.N, graph.Nt
+    label = (f"HITS {graph.label} epsilon={epsilon} normalize={normalize}"
+             f"{f' guess on {len(guess[0])} vertices' if guess is not None else ''}{tag}")
     thr = float(T(V) * T(epsilon))
     if guess is None:
         h0 = np.full(V, 1.0 / V)
@@ -413,7 +451,8 @@ def check_hits(h, g, graph, epsilon, guess=None, normalize=True, key=None, max_i
         return c, float(np.abs(c - hv).sum())
     xs, diffs, k_ref = run_until(step, h0, k, thr, max_iterations)
     u = unit(T)
-    d_in, d_out = sweep_delta(T, int(graph.indeg.max())), sweep_delta(T, int(graph.outdeg.max()))
+    d_in = sweep_delta(T, int(graph.indeg.max())) + extra[0]
+    d_out = sweep_delta(T, int(graph.outdeg.max())) + extra[1]
     D0 = 2.0 * (u + 2.0 * E) if guess is not None else 0.0
     Dh = [D0 + 2.0 * j * (d_in + d_out + u + 2.0 * E) for j in range(len(xs))]
     rt = [SECOND_ORDER * math.expm1(Dj) for Dj in Dh]
@@ -430,8 +469,8 @@ def check_hits(h, g, graph, epsilon, guess=None, normalize=True, key=None, max_i
         ref_h, ref_a = ref_h / ref_h.sum(), ref_a / ref_a.sum()
         rt_h, rt_a = rt_h + V * E + u + 2.0 * E, rt_a + V * E + u + 2.0 * E
     key = key or f"hits {np.dtype(T).name}"
-    w1 = compare(graph.dense(verts, hubs), ref_h, SECOND_ORDER * rt_h, f"{label}, hubs after {k} steps", key)
-    w2 = compare(graph.dense(verts, auth), ref_a, SECOND_ORDER * rt_a, f"{label}, authorities after {k} steps", key)
+    w1 = compare(hubs, ref_h, SECOND_ORDER * rt_h, f"{label}, hubs after {k} steps", key)
+    w2 = compare(auth, ref_a, SECOND_ORDER * rt_a, f"{label}, authorities after {k} steps", key)
     return max(w1, w2)
 
 
@@ -439,12 +478,18 @@ def check_hits(h, g, graph, epsilon, guess=None, normalize=True, key=None, max_i
 # PageRank
 # ---------------------------------------------------------------------------------------------------------------------
 def check_pagerank(h, g, graph, steps=30, alpha=0.85, pers=None, guess=None, out_w=None, key=None):
-    """`steps` steps at epsilon = 0 against oracle.pagerank; pers / guess / out_w: (internal ids, values in T)"""
+    """`steps` steps of cugraph_[personalized_]pagerank at epsilon = 0, checked by verify_pagerank"""
+    verts, vals, k = pagerank_call(h, g, graph, alpha, 0.0, steps, pers, guess, out_w)
+    return verify_pagerank(graph, graph.dense(verts, vals), k, steps, alpha, pers, guess, out_w, key=key)
+
+
+def verify_pagerank(graph, got, k, steps=30, alpha=0.85, pers=None, guess=None, out_w=None, extra=0.0, key=None, tag=""):
+    """`got` (by internal id) after `steps` steps at epsilon = 0 (k: the count the driver reports) against oracle.pagerank;
+    pers / guess / out_w: (internal ids, values in T); `extra` is the relative rounding a sweep adds past one GPU's"""
     import oracle
     T, V = graph.T, graph.V
     parts = [n for n, p in (("personalized", pers), ("initial guess", guess), ("out-weights", out_w)) if p is not None]
-    label = f"PageRank {graph.label}{' ' + ', '.join(parts) if parts else ''}"
-    verts, vals, k = pagerank_call(h, g, graph, alpha, 0.0, steps, pers, guess, out_w)
+    label = f"PageRank {graph.label}{' ' + ', '.join(parts) if parts else ''}{tag}"
     assert k == steps, f"{label}: {k} steps at epsilon 0, expected {steps}"
 
     def dense(p):
@@ -459,9 +504,10 @@ def check_pagerank(h, g, graph, steps=30, alpha=0.85, pers=None, guess=None, out
                                 precomputed_out_w=None if out_w is None else dense(out_w))
     u = unit(T)
     n_pers = 0 if pers is None else len(pers[0])
-    per_step = sweep_delta(T, int(graph.indeg.max())) + 3.0 * u + (int(graph.outdeg.max()) + V + n_pers) * E + 8.0 * E
+    per_step = (sweep_delta(T, int(graph.indeg.max())) + extra + 3.0 * u + (int(graph.outdeg.max()) + V + n_pers) * E
+                + 8.0 * E)
     rtol = SECOND_ORDER * (u + steps * per_step)
-    return compare(graph.dense(verts, vals), ref, rtol, f"{label}, {steps} steps",
+    return compare(got, ref, rtol, f"{label}, {steps} steps",
                    key or f"{'personalized ' if pers is not None else ''}pagerank {np.dtype(T).name}")
 
 
