@@ -135,12 +135,16 @@ def lib():
     _sig(L.cugraph_b200_block_pull_sweep, i32, [vp, vp, vp, vp, dbl, pvp])
     _sig(L.cugraph_b200_generate_rmat_edgelist, i32, [vp, sz, sz, dbl, dbl, dbl, C.c_uint64, i32, i32, vp, vp, pvp])
     _sig(L.cugraph_b200_generate_uniform, i32, [vp, C.c_uint64, dbl, dbl, vp, pvp])
+    _sig(L.cugraph_b200_generate_rmat_edgelist_at, i32,
+         [vp, sz, C.c_uint64, sz, dbl, dbl, dbl, C.c_uint64, i32, i32, vp, vp, pvp])
+    _sig(L.cugraph_b200_generate_uniform_at, i32, [vp, C.c_uint64, C.c_uint64, dbl, dbl, vp, pvp])
     _sig(L.cugraph_b200_block_bfs_pull, i32, [vp, vp, vp, vp, sz, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_block_bfs_push, i32, [vp, vp, vp, vp, sz, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_bfs_bottom_up, i32, [vp, i32, sz, sz, sz, sz, sz])
     _sig(L.cugraph_b200_block_sssp_relax, i32, [vp, vp, vp, dbl, sz, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_block_sssp_pred, i32, [vp, vp, vp, vp, sz, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_block_wcc_min, i32, [vp, vp, vp, vp, pvp])
+    _sig(L.cugraph_b200_block_check_paths, i32, [vp, vp, vp, vp, vp, dbl, sz, i32, i32, vp, vp, C.POINTER(C.c_uint64), pvp])
     _sig(L.cugraph_b200_block_scc_push, i32, [vp, vp, i32, i32, vp, vp, vp, sz, i32, i32, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_paths_answer, i32, [vp, vp, vp, vp, sz, vp, pvp])
     _sig(L.cugraph_b200_paths_advance, i32, [vp, vp, vp, vp, vp, sz, sz, i32, vp, vp, vp, vp, pvp])

@@ -11,9 +11,12 @@
 namespace b200 {
 namespace {
 std::mutex g_stream_mutex;
-std::unordered_set<cudaStream_t>& live_streams()
+// stream -> the number of live handles on it.  Counted: several handles may borrow one stream (every handle made on torch's
+// current stream), and the stream stays live until the last of them is freed; a buffer of a stream that is no longer live
+// is freed with a synchronous cudaFree, which must never happen while another handle still queues work that uses it.
+std::unordered_map<cudaStream_t, int>& live_streams()
 {
-  static auto* s = new std::unordered_set<cudaStream_t>();  // leaked on purpose: used during exit
+  static auto* s = new std::unordered_map<cudaStream_t, int>();  // leaked on purpose: used during exit
   return *s;
 }
 // Freed blocks per stream (see block_alloc in common.cuh).  Leaked on purpose like the stream set.
@@ -97,11 +100,13 @@ bool stream_is_live(cudaStream_t s)
 void register_stream(cudaStream_t s)
 {
   std::lock_guard<std::mutex> lk(g_stream_mutex);
-  live_streams().insert(s);
+  ++live_streams()[s];
 }
 void unregister_stream(cudaStream_t s)
 {
   std::lock_guard<std::mutex> lk(g_stream_mutex);
+  auto live = live_streams().find(s);
+  if (live != live_streams().end() && --live->second > 0) return;  // another handle still works on this stream
   auto it = block_caches().find(s);
   if (it != block_caches().end()) {  // the caller synchronised the stream: the cached blocks are idle
     flush_cache_locked(s, it->second, true);

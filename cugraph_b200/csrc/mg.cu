@@ -17,6 +17,7 @@
 #include <cmath>
 #include <initializer_list>
 #include <limits>
+#include <type_traits>
 
 namespace b200 {
 
@@ -192,6 +193,7 @@ __device__ __forceinline__ bool column_active(float v) { return v < INFINITY; }
 __device__ __forceinline__ bool column_active(double v) { return v < INFINITY; }
 __device__ __forceinline__ bool column_active(long long v) { return v != LLONG_MAX; }
 __device__ __forceinline__ bool column_active(uint8_t f) { return f != 0; }  // a BFS frontier flag
+__device__ __forceinline__ bool column_active(int32_t d) { return d != INT_MAX; }  // a reached BFS distance
 
 // physical rows r < n_ne of the push copy whose column slot row_vertex[r] is active, with their degrees
 template <typename O, typename T>
@@ -259,6 +261,42 @@ struct block_pred_op {
     if (dist[col] + w[e] != want) return;
     const long long k = column_code(col, maxpart, grid_cols, grid_c);
     if (k < code[nbr]) atomicMin(code + nbr, k);
+  }
+};
+
+// ---- the edge part of the BFS / SSSP certificate (MGGraph.validate_bfs / validate_sssp) on this GPU's edge block.  The
+// launcher gathers the given distances over the column slots (unreached: INT32_MAX for BFS, +inf for SSSP, so that only
+// the reached columns are queued) and over the row slots (as given), and the predecessor codes over the row slots.  For
+// every stored edge u -> v of a reached column whose step is allowed (nd = d[u] + w, or d[u] + 1 with unit steps, below the
+// cutoff, in the arithmetic of block_relax_op) the op counts an `edge` violation when d[v] > nd (or is NaN), and marks
+// the row when the row's predecessor is this column at exactly d[v] = nd: 1, or 2 for a flat step (d[u] = d[v]).
+// Unit steps (T = int32_t) add in 64 bits, so the cutoff d[u] < depth_limit reads nd < depth_limit + 1.
+template <typename T>
+struct block_check_op {
+  using A = std::conditional_t<std::is_same<T, int32_t>::value, long long, T>;
+  int32_t const* col_of;     // column slot of a physical row of the push copy
+  T const* w;                // nullptr: unit steps
+  T const* dist_cols;        // over column slots, unreached = inactive
+  T const* dist_rows;        // over row slots
+  long long const* pred_rows;  // over row slots: predecessor code, -1 = none
+  A cutoff;
+  long long maxpart;
+  int grid_cols, grid_c;
+  uint8_t* flag_rows;        // over row slots
+  unsigned long long* violations;
+  __device__ __forceinline__ void edge(int src, long long e, int nbr) const
+  {
+    const int col = col_of[src];
+    const A du    = (A)dist_cols[col];
+    const A nd    = w ? (A)(dist_cols[col] + w[e]) : du + (A)1;
+    const bool allowed = nd < cutoff;
+    const A dv         = (A)dist_rows[nbr];
+    const bool bad     = allowed && !(dv <= nd);
+    if (allowed && dv == nd && pred_rows[nbr] == column_code(col, maxpart, grid_cols, grid_c))
+      flag_rows[nbr] = du == dv ? 2 : 1;  // every match of a row writes the same value: d[u] is the predecessor's
+    const unsigned mask = __activemask();
+    const unsigned n    = (unsigned)__popc(__ballot_sync(mask, bad));
+    if (n && (threadIdx.x & 31) == __ffs(mask) - 1) atomicAdd(violations, (unsigned long long)n);
   }
 };
 
@@ -380,9 +418,9 @@ cugraph_error_code_t owner_step(cugraph_error_t** error, const char* what, const
   });
 }
 
-// active rows -> queue (one read-back of its size and edge count) -> advance with `op`
+// active rows -> queue (one read-back of its size and edge count) -> advance with `op`; returns the queue's counts
 template <typename O, typename T, typename Op>
-void block_push_round(handle_impl const& h, block_push_t& p, T const* dist_cols, Op op)
+block_queue_counts_t block_push_round(handle_impl const& h, block_push_t& p, T const* dist_cols, Op op)
 {
   csx_t const& pc = *p.csx;
   auto* cnt       = p.counts.as<block_queue_counts_t>();
@@ -394,6 +432,7 @@ void block_push_round(handle_impl const& h, block_push_t& p, T const* dist_cols,
   const block_queue_counts_t hc = read_back(h, cnt);
   advance<O>(h, p.adv, pc.offsets.as<O>(), pc.indices.as<int32_t>(), p.queue.as<int32_t>(), hc.n, hc.edges, op,
              p.q_deg.as<int32_t>());
+  return hc;
 }
 
 // out[row slot] = INT64_MAX (no proposal), then one push round of `op` over the columns active in `active_cols`
@@ -1093,6 +1132,67 @@ cugraph_error_code_t cugraph_b200_block_scc_push(const cugraph_resource_handle_t
       else block_push_round<int32_t>(h, p, vals, op);
     }
     check_last("block_scc_push");
+  });
+}
+
+// the edge rules of the BFS / SSSP certificate over the block (see block_check_op): flag_rows (zeroed first) and
+// violations[0] (zeroed first); *edges_from_reached = the edges of the reached columns
+cugraph_error_code_t cugraph_b200_block_check_paths(const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+                                                    const cugraph_type_erased_device_array_view_t* dist_cols,
+                                                    const cugraph_type_erased_device_array_view_t* dist_rows,
+                                                    const cugraph_type_erased_device_array_view_t* pred_rows, double cutoff,
+                                                    size_t maxpart, int grid_cols, int grid_c,
+                                                    cugraph_type_erased_device_array_view_t* flag_rows,
+                                                    cugraph_type_erased_device_array_view_t* violations,
+                                                    uint64_t* edges_from_reached, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(block && dist_cols && dist_rows && pred_rows && flag_rows && violations && edges_from_reached,
+                 CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto* b        = reinterpret_cast<block_impl*>(block);
+    auto const* dc = V(dist_cols);
+    auto const* dr = V(dist_rows);
+    auto const* pr = V(pred_rows);
+    auto const* fv = V(flag_rows);
+    auto const* vv = V(violations);
+    const bool unit = dc->type == INT32;
+    B200_EXPECTS(dr->type == dc->type, CUGRAPH_INVALID_INPUT, "dist_cols / dist_rows dtypes differ");
+    B200_EXPECTS(unit || (b->weighted && dc->type == b->wtype), CUGRAPH_INVALID_INPUT,
+                 "distances must be INT32 (unit steps) or the weight type of a weighted block");
+    B200_EXPECTS(pr->type == INT64 && dtype_size(fv->type) == 1 && vv->type == INT64 && vv->size >= 1, CUGRAPH_INVALID_INPUT,
+                 "pred_rows must be INT64, flag_rows byte flags, violations INT64");
+    B200_EXPECTS(dc->size >= (size_t)b->n_cols && dr->size >= (size_t)b->n_rows && pr->size >= (size_t)b->n_rows &&
+                   fv->size >= (size_t)b->n_rows,
+                 CUGRAPH_INVALID_INPUT, "distance / predecessor / flag arrays shorter than the block's slots");
+    B200_EXPECTS(maxpart > 0 && grid_cols > 0 && grid_c >= 0 && grid_c < grid_cols, CUGRAPH_INVALID_INPUT, "bad grid position");
+    CUDA_TRY(cudaMemsetAsync(fv->data, 0, (size_t)b->n_rows, h.stream));
+    CUDA_TRY(cudaMemsetAsync(vv->data, 0, sizeof(long long), h.stream));
+    block_push_t& p = push_copy(h, *b);
+    auto* flags     = (uint8_t*)fv->data;
+    auto* viol      = (unsigned long long*)vv->data;
+    auto run        = [&](auto op, auto const* cols) {
+      const block_queue_counts_t hc =
+        p.csx->offs64 ? block_push_round<int64_t>(h, p, cols, op) : block_push_round<int32_t>(h, p, cols, op);
+      *edges_from_reached = (uint64_t)hc.edges;
+    };
+    if (unit) {
+      auto const* d = (int32_t const*)dc->data;
+      const long long lim = cutoff >= 9.2e18 ? LLONG_MAX : (long long)cutoff;
+      run(block_check_op<int32_t>{p.csx->row_vertex.as<int32_t>(), nullptr, d, (int32_t const*)dr->data,
+                                  (long long const*)pr->data, lim, (long long)maxpart, grid_cols, grid_c, flags, viol},
+          d);
+    } else {
+      by_float_type(b->wtype, [&](auto z) {
+        using T       = decltype(z);
+        auto const* d = (T const*)dc->data;
+        run(block_check_op<T>{p.csx->row_vertex.as<int32_t>(), p.csx->weights.as<T>(), d, (T const*)dr->data,
+                              (long long const*)pr->data, rounded_cutoff<T>(cutoff), (long long)maxpart, grid_cols, grid_c,
+                              flags, viol},
+            d);
+      });
+    }
+    check_last("block_check_paths");
   });
 }
 

@@ -670,7 +670,7 @@ class MGGraph:
             raise ValueError(f"{what} source {source} is not a vertex of the graph")
         return lid
 
-    def _sources_to_owners(self, sources):
+    def _sources_to_owners(self, sources, where="MGGraph.bfs"):
         """the local ids of the sources, from every rank, that this rank owns (duplicates kept): each rank's ids travel to
         their owners in one all-to-all-v; one all-reduce of the error counts, and every rank raises the same error"""
         from cugraph_b200 import _capi as capi
@@ -684,9 +684,9 @@ class MGGraph:
         dist.all_reduce(errs)
         bad_type, invalid = errs.tolist()
         if bad_type:
-            raise TypeError("MGGraph.bfs: sources must have the dtype of the edge ids on every rank")
+            raise TypeError(f"{where}: sources must have the dtype of the edge ids on every rank")
         if invalid:
-            raise capi.CugraphValueError(capi.INVALID_INPUT, "Found invalid vertex in the input sources", "MGGraph.bfs")
+            raise capi.CugraphValueError(capi.INVALID_INPUT, "Found invalid vertex in the input sources", where)
         return lid
 
     def _codes_to_external(self, codes):
@@ -904,6 +904,171 @@ class MGGraph:
         if not compute_predecessors:
             return verts, d_out, None
         return verts, d_out, self._codes_to_external(pred_code[:p.n_local])
+
+    # ------------------------------------------------------------------------------------------
+    # BFS / SSSP certificate (validate_bfs, validate_sssp): the checks of a Graph500 validation, distributed over the same
+    # edge block the traversals use, so that a result of any size on any grid is checked without gathering it.  Each rank
+    # gives any set of (external id, distance, predecessor id) triples.  One all-to-all-v brings them to their owners, one
+    # all-to-all-v there and back turns the predecessor ids into codes (owner rank * maxpart + local id, the inverse of
+    # _codes_to_external).  The owners' distances are all-gathered over the block's column slots (column group) and its
+    # row slots (row group), the predecessor codes over its row slots; ONE push round over the block's column-major copy
+    # (cugraph_b200_block_check_paths) counts the edges that could still shorten a distance and marks every row whose
+    # predecessor edge attains its distance (2 for a flat edge, d[p] = d[v]); ONE MAX reduce-scatter brings the marks to
+    # the owners, whose per-vertex rules are torch passes.  SSSP predecessors can close a cycle only over flat edges: when
+    # some exist, pointer jumping over them (an all-to-all-v there and back per round, as extract_paths walks) finds the
+    # vertices whose chain never leaves them.  One all-reduce of the counters gives every rank the same verdict.
+    # ------------------------------------------------------------------------------------------
+    def validate_bfs(self, vertices, distances, predecessors, sources, depth_limit=-1):
+        """Check a BFS result on this graph: returns a dict, the same on every rank, with `ok` and one count per rule
+        (see _validate): not_vertex, missing, duplicate, bad_value, root, unreached, edge, tree_edge, cycle (always 0 for
+        BFS), and edges_from_reached (stored edges whose source is reached; for a graph that stores both directions of
+        every input edge, twice the input edges of the sources' component).  vertices, distances (int32, INT32_MAX =
+        unreached) and predecessors (external ids, -1 = none) are this rank's triples, any of them, in any order: what
+        MGGraph.bfs returned, or on a 1x1 grid a whole single-GPU cugraph_bfs result.  sources takes both forms bfs
+        accepts; depth_limit as in bfs.  Every rank raises the same error: ValueError for arrays of unequal length or
+        predecessors=None, TypeError for ids in another dtype than the edge ids' or distances that are not int32, and the
+        errors of bfs for the sources.  No input is modified."""
+        return self._validate(True, vertices, distances, predecessors, sources, depth_limit=depth_limit)
+
+    def validate_sssp(self, vertices, distances, predecessors, source, cutoff=math.inf):
+        """Check an SSSP result on this graph, as validate_bfs checks a BFS result: distances in the graph's weight dtype
+        (finfo.max = unreached), `source` one external id (the same on every rank), cutoff as in sssp.  Predecessors must
+        form no cycle (`cycle` counts the vertices whose predecessor chain runs into one).  ValueError on an unweighted
+        graph."""
+        if not self.weighted:
+            raise ValueError("SSSP requires a weighted graph")
+        return self._validate(False, vertices, distances, predecessors, source, cutoff=cutoff)
+
+    def _validate(self, bfs, vertices, distances, predecessors, sources, depth_limit=-1, cutoff=math.inf):
+        """The rules (d = distance, p = predecessor, unreached = the sentinel):
+          not_vertex, missing, duplicate: every given id is a vertex; every vertex is given exactly once over all ranks.
+          bad_value: d lies in [0, sentinel] and is not NaN (a bad value then counts as unreached).
+          root: BFS, v is a source <=> d = 0 and p = -1; SSSP, the source has d = 0 and p = -1.
+          unreached: a vertex other than a source is unreached <=> p = -1.
+          edge: every stored edge u -> v with u reached and the step allowed has d[v] <= d[u] + 1 (BFS) or d[v] <= d[u] + w
+            (SSSP, added in the weight dtype).  Allowed: BFS, depth_limit < 0 or d[u] < depth_limit; SSSP, d[u] + w below
+            the cutoff rounded to the weight dtype (the arithmetic of the relaxation).
+          tree_edge: every v with p != -1 has a stored edge p -> v with p reached, the step allowed and d[v] = d[p] + 1
+            (BFS) or d[p] + w exactly (SSSP).
+          cycle (SSSP): the predecessors form no cycle."""
+        p, g, dev, mp = self.part, self.part.groups, self.device, self.part.maxpart
+        P, n = g.world, p.n_local
+        i64 = torch.int64
+        ddt = torch.int32 if bfs else self.dtype
+        vdt = p.vertices.dtype
+        unreached = torch.iinfo(torch.int32).max if bfs else torch.finfo(ddt).max
+        flat_t = lambda a: None if a is None else torch.as_tensor(a).to(dev).reshape(-1)  # noqa: E731
+        v_in, d_in, p_in = flat_t(vertices), flat_t(distances), flat_t(predecessors)
+        bad_size = int(v_in is None or d_in is None or p_in is None or not v_in.numel() == d_in.numel() == p_in.numel())
+        bad_ids = int(not bad_size and (v_in.dtype != vdt or p_in.dtype != vdt))
+        bad_dist = int(not bad_size and d_in.dtype != ddt)
+        errs = torch.tensor([bad_size, bad_ids, bad_dist], dtype=i64, device=dev)
+        dist.all_reduce(errs)
+        bad_size, bad_ids, bad_dist = errs.tolist()
+        where = "MGGraph.validate_bfs" if bfs else "MGGraph.validate_sssp"
+        if bad_size:
+            raise ValueError(f"{where}: vertices, distances and predecessors must be given, with equal lengths, on every rank")
+        if bad_ids:
+            raise TypeError(f"{where}: vertices and predecessors must have the dtype of the edge ids on every rank")
+        if bad_dist:
+            raise TypeError(f"{where}: distances must be {str(ddt)[6:]} on every rank")
+        is_src = torch.zeros(mp, dtype=torch.bool, device=dev)
+        if bfs and not _is_scalar(sources):
+            is_src[self._sources_to_owners(sources, where)] = True
+        else:
+            lid = self._source_lid(sources, "validate_bfs" if bfs else "validate_sssp")
+            if lid >= 0:
+                is_src[lid] = True
+        # the triples -> their owners
+        vid = v_in.to(i64)
+        (rv, rd, rp), _, _, _ = exchange([vid, d_in, p_in.to(i64)], vertex_owner(vid, P), P)
+        lid, hit = self._owned_lids(rv)
+        n_not_vertex = (~hit).sum()
+        lid, rd, rp = lid[hit], rd[hit], rp[hit]
+        cnt = torch.bincount(lid, minlength=mp)
+        n_dup = (cnt - 1).clamp(min=0).sum()
+        given = cnt > 0
+        n_missing = (~given[:n]).sum()
+        bad = rd < 0 if bfs else torch.isnan(rd) | (rd < 0) | (rd > unreached)
+        d_own = torch.full((mp,), unreached, dtype=ddt, device=dev)
+        d_own[lid] = torch.where(bad, torch.full_like(rd, unreached), rd)
+        pext = torch.full((mp,), -1, dtype=i64, device=dev)
+        pext[lid] = rp
+        # predecessor ids -> codes, answered by their owners (-2: not a vertex)
+        has = pext != -1
+        ask = pext[has]
+        (req,), order, sc, rc = exchange([ask], vertex_owner(ask, P), P)
+        l2, h2 = self._owned_lids(req)
+        ans = torch.where(h2, g.rank * mp + l2, -2)
+        back = torch.empty(sum(sc), dtype=i64, device=dev)
+        dist.all_to_all_single(back, ans, output_split_sizes=sc, input_split_sizes=rc)
+        code = torch.full((mp,), -1, dtype=i64, device=dev)
+        code[has] = _unpermute(back, order)
+        # the edge rules on the block
+        reached = given & (d_own != unreached)
+        d_act = d_own if bfs else torch.where(reached, d_own, torch.tensor(math.inf, dtype=ddt, device=dev))
+        d_cols = torch.empty(self.n_cols, dtype=ddt, device=dev)
+        d_rows = torch.empty(self.n_rows, dtype=ddt, device=dev)
+        c_rows = torch.empty(self.n_rows, dtype=i64, device=dev)
+        all_gather_into(d_cols, d_act, g.col_group)
+        all_gather_into(d_rows, d_own, g.row_group)
+        all_gather_into(c_rows, code, g.row_group)
+        flags = torch.empty(self.n_rows, dtype=torch.uint8, device=dev)
+        viol = torch.zeros(1, dtype=i64, device=dev)
+        edges = C.c_uint64(0)
+        lim = (float(depth_limit) + 1.0 if depth_limit >= 0 else math.inf) if bfs else float(cutoff)
+        with _views(d_cols, d_rows, c_rows, flags, viol) as (vc, vr, vp, vf, vv):
+            self._call("cugraph_b200_block_check_paths", self.block, vc.ptr, vr.ptr, vp.ptr, lim, mp, g.C, g.c, vf.ptr, vv.ptr,
+                       C.byref(edges))
+        flag = torch.empty(mp, dtype=torch.uint8, device=dev)
+        reduce_scatter_into(flag, flags, g.row_group, op=dist.ReduceOp.MAX)
+        # the per-vertex rules at the owners
+        gv, dv, cv, sv, fv = given[:n], d_own[:n], code[:n], is_src[:n], flag[:n]
+        zero_root = (dv == 0) & (cv == -1)
+        root = gv & (sv != zero_root) if bfs else gv & sv & ~zero_root
+        unreach = gv & ~sv & ((dv == unreached) != (cv == -1))
+        tree = gv & (cv != -1) & (fv == 0)
+        n_cycle = torch.zeros((), dtype=i64, device=dev)
+        if not bfs:
+            flat = torch.zeros(mp, dtype=torch.bool, device=dev)
+            flat[:n] = gv & (cv >= 0) & (fv == 2)
+            n_flat = _global_count(flat)
+            if n_flat:
+                n_cycle = self._flat_cycles(flat, code, n_flat)
+        counts = torch.stack([n_not_vertex, n_missing, n_dup, bad.sum(), root.sum(), unreach.sum(), viol[0], tree.sum(),
+                              n_cycle, torch.tensor(edges.value, device=dev)]).to(i64)
+        dist.all_reduce(counts)
+        names = ("not_vertex", "missing", "duplicate", "bad_value", "root", "unreached", "edge", "tree_edge", "cycle",
+                 "edges_from_reached")
+        out = dict(zip(names, counts.tolist()))
+        out["ok"] = not any(out[k] for k in names[:-1])
+        return out
+
+    def _flat_cycles(self, flat, code, n_flat):
+        """the vertices, over all ranks, whose predecessor chain through flat tree edges never ends: pointer jumping (each
+        round: every unfinished vertex asks the owner of its pointer for that vertex's pointer and whether it is finished,
+        an all-to-all-v there and back, then one all-reduce of the unfinished count).  A chain of k flat edges ends within
+        log2(k) + 1 rounds; what is left after log2(n_flat) + 2 rounds lies on a cycle or leads into one."""
+        g, dev, mp = self.part.groups, self.device, self.part.maxpart
+        own = g.rank * mp + torch.arange(mp, dtype=torch.int64, device=dev)
+        ptr = torch.where(flat, code, own)
+        done = ~flat
+        for _ in range(n_flat.bit_length() + 2):
+            open_ = ~done
+            ask = ptr[open_]
+            (req,), order, sc, rc = exchange([ask], torch.div(ask, mp, rounding_mode="floor"), g.world)
+            loc = req % mp
+            ans = torch.stack([ptr[loc], done[loc].to(torch.int64)], 1).reshape(-1)
+            back = torch.empty(2 * sum(sc), dtype=torch.int64, device=dev)
+            dist.all_to_all_single(back, ans, output_split_sizes=[2 * k for k in sc], input_split_sizes=[2 * k for k in rc])
+            got = _unpermute(back.view(-1, 2), order)
+            fin = got[:, 1] != 0
+            ptr[open_] = torch.where(fin, ask, got[:, 0])
+            done[open_] = fin
+            left = _global_count(~done)
+            if left == 0:
+                break
+        return torch.tensor(left, dtype=torch.int64, device=dev)
 
     # ------------------------------------------------------------------------------------------
     # multi-GPU weakly connected components: min-label propagation.  Every owned vertex starts with its own code (owner
@@ -1203,6 +1368,13 @@ class MGGraph:
         return p.vertices, prev[:p.n_local].clone(), auth[:p.n_local].clone()
 
 
+def _unpermute(x, order):
+    """the answers of an exchange() in the order of the requests: x[k] answers request order[k]"""
+    out = torch.empty_like(x)
+    out[order] = x
+    return out
+
+
 def _is_scalar(x):
     """a Python / NumPy integer or a 0-d tensor / array: MGGraph.bfs's one-source form"""
     if isinstance(x, (torch.Tensor, np.ndarray)):
@@ -1412,6 +1584,34 @@ def bfs(graph: MGGraph, sources, depth_limit=-1, compute_predecessors=True, *, d
     sources: one external id, the same on every rank, or a 1-D tensor / array of this rank's source ids;
     direction_optimizing: top-down on every level (False) or single GPU's per-level switch (True) (see MGGraph.bfs)."""
     return graph.bfs(sources, depth_limit, compute_predecessors, direction_optimizing=direction_optimizing)
+
+
+def validate_bfs(graph: MGGraph, vertices, distances, predecessors, sources, depth_limit=-1):
+    """the certificate of a BFS result given as this rank's (vertices, distances, predecessors): a dict, the same on every
+    rank (see MGGraph.validate_bfs)"""
+    return graph.validate_bfs(vertices, distances, predecessors, sources, depth_limit)
+
+
+def validate_sssp(graph: MGGraph, vertices, distances, predecessors, source, cutoff=math.inf):
+    """the certificate of an SSSP result given as this rank's (vertices, distances, predecessors): a dict, the same on
+    every rank (see MGGraph.validate_sssp)"""
+    return graph.validate_sssp(vertices, distances, predecessors, source, cutoff)
+
+
+def rmat_edgelist_share(scale, num_edges, a=0.57, b=0.19, c=0.19, seed=0, clip_and_flip=False, scramble_ids=True,
+                        groups: Groups | None = None, device="cuda"):
+    """This rank's slice [r * E // P, (r + 1) * E // P) of the global RMAT stream of `seed` (E = num_edges, P ranks, r this
+    rank), generated on its own: returns (src, dst, first), first = the slice's first edge index.  The stream is counter-based
+    (cugraph_b200_generate_rmat_edgelist_at), so the ranks' slices in rank order are the single-call output
+    generators.rmat_edgelist(scale, E, ...) bit for bit, whatever P is; values drawn per edge at the same global indices
+    (generators.uniform_values(..., first=first)) stay attached to the same edges.  groups: the grid's Groups (default:
+    the default process group)."""
+    from cugraph_b200.generators import rmat_edgelist
+    rank, world = (groups.rank, groups.world) if groups is not None else (dist.get_rank(), dist.get_world_size())
+    first = rank * int(num_edges) // world
+    count = (rank + 1) * int(num_edges) // world - first
+    src, dst = rmat_edgelist(scale, count, a, b, c, seed, scramble_ids, clip_and_flip, device=device, first_edge=first)
+    return src, dst, first
 
 
 def extract_paths(graph: MGGraph, distances, predecessors, destinations):

@@ -238,30 +238,42 @@ def generate_rmat_edgelist(resource_handle, random_state, scale, num_edges, a, b
                            min_edge_type_value, max_edge_type_value, multi_gpu):
     """generate_rmat_edgelist.pyx: returns (sources, destinations, weights | None, edge ids | None, edge types | None).
     The edges come from the library's device generator (the reference's sampling rule over a counter-based stream seeded with
-    `random_state`), weights / types from its uniform generator; ids are 0 .. num_edges-1 (as the reference numbers them)."""
+    `random_state`), weights / types from its uniform generator; ids are 0 .. num_edges-1 (as the reference numbers them).
+    multi_gpu=True (on the default torch.distributed group): num_edges is this rank's count, and the rank generates edges
+    [start, start + num_edges) of the same stream, start = the sum of the counts of the lower ranks (one all-gather, as the
+    reference numbers multi-GPU edge ids); weights and types are drawn at the same global indices and ids are start + k.
+    The ranks' outputs in rank order are then one single-GPU call over the total count, bit for bit."""
     import numpy as np
     import torch
-    if multi_gpu:
-        raise NotImplementedError("generate_rmat_edgelist: multi_gpu=True is not part of this build")
     L = _capi.lib()
     dev = "cuda" if torch.cuda.is_available() else "cpu"
     seed = int(random_state) if random_state is not None else 0
+    start, total = 0, int(num_edges)
+    if multi_gpu:
+        from cugraph_b200 import mg
+        mine = torch.tensor([int(num_edges)], dtype=torch.int64, device=dev)
+        counts = torch.empty(mg.dist.get_world_size(), dtype=torch.int64, device=dev)
+        mg.all_gather_into(counts, mine, None)
+        counts = counts.tolist()
+        start, total = sum(counts[:mg.dist.get_rank()]), sum(counts)
     src = torch.empty(num_edges, dtype=torch.int32, device=dev)
     dst = torch.empty(num_edges, dtype=torch.int32, device=dev)
     vs, vd, err = View(src), View(dst), C.c_void_p()
     resource_handle.order_after_caller()
-    code = L.cugraph_b200_generate_rmat_edgelist(resource_handle.ptr, int(scale), int(num_edges), float(a), float(b), float(c), seed,
-                                                 int(bool(clip_and_flip)), int(bool(scramble_vertex_ids)), vs.ptr, vd.ptr, C.byref(err))
+    code = L.cugraph_b200_generate_rmat_edgelist_at(resource_handle.ptr, int(scale), start, int(num_edges), float(a), float(b),
+                                                    float(c), seed, int(bool(clip_and_flip)), int(bool(scramble_vertex_ids)),
+                                                    vs.ptr, vd.ptr, C.byref(err))
     vs.free()
     vd.free()
-    _capi.check(code, err, "cugraph_b200_generate_rmat_edgelist")
+    _capi.check(code, err, "cugraph_b200_generate_rmat_edgelist_at")
 
     def uniform(tdtype, lo, hi, salt):
         out = torch.empty(num_edges, dtype=tdtype, device=dev)
         vo, e2 = View(out), C.c_void_p()
-        c2 = L.cugraph_b200_generate_uniform(resource_handle.ptr, seed + salt, float(lo), float(hi), vo.ptr, C.byref(e2))
+        c2 = L.cugraph_b200_generate_uniform_at(resource_handle.ptr, seed + salt, start, float(lo), float(hi), vo.ptr,
+                                                C.byref(e2))
         vo.free()
-        _capi.check(c2, e2, "cugraph_b200_generate_uniform")
+        _capi.check(c2, e2, "cugraph_b200_generate_uniform_at")
         return out
 
     weights = ids = types = None
@@ -269,7 +281,8 @@ def generate_rmat_edgelist(resource_handle, random_state, scale, num_edges, a, b
         tdt = torch.float64 if np.dtype(dtype) == np.float64 else torch.float32
         weights = uniform(tdt, minimum_weight, maximum_weight, 0x9E37)
     if include_edge_ids:
-        ids = torch.arange(num_edges, dtype=torch.int32, device=dev)
+        ids = torch.arange(start, start + int(num_edges), dtype=torch.int64 if multi_gpu and total > 2**31 else torch.int32,
+                           device=dev)
     if include_edge_types:
         types = uniform(torch.int32, min_edge_type_value, max_edge_type_value + 1, 0x79B9)
     import torch as _t

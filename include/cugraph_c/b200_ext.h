@@ -174,6 +174,20 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_generate_uniform(const cugraph_
                                                                   double hi, cugraph_type_erased_device_array_view_t* out,
                                                                   cugraph_error_t** error);
 
+/* Slices of the same two streams.  Both are counter-based (edge e draws from mix64(seed ^ (64 e + bit)), value i from
+ * mix64(seed ^ i)), so edges [first_edge, first_edge + num_edges) of the RMAT stream, and values [first, first + size(out))
+ * of the uniform stream, are written to elements 0, 1, ... of the arrays: the concatenation of consecutive slices is the
+ * output of one call over their union, bit for bit.  cugraph_b200_generate_rmat_edgelist / _uniform are the slices at 0;
+ * arguments and checks are theirs. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_generate_rmat_edgelist_at(
+  const cugraph_resource_handle_t* handle, size_t scale, uint64_t first_edge, size_t num_edges, double a, double b, double c,
+  uint64_t seed, bool_t clip_and_flip, bool_t scramble_vertex_ids, cugraph_type_erased_device_array_view_t* src,
+  cugraph_type_erased_device_array_view_t* dst, cugraph_error_t** error);
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_generate_uniform_at(const cugraph_resource_handle_t* handle, uint64_t seed,
+                                                                     uint64_t first, double lo, double hi,
+                                                                     cugraph_type_erased_device_array_view_t* out,
+                                                                     cugraph_error_t** error);
+
 /* One level of multi-GPU BFS on this GPU's edge block (pull direction; the role of the bottom-up step of
  * cpp/src/traversal/bfs_impl.cuh:593-869 on one edge partition).  frontier_cols / visited_rows: byte flags over the block's
  * column (source) / row (destination) slots, gathered by the launcher inside the column / row group.  cand (INT64, one per row
@@ -232,6 +246,28 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_sssp_pred(
   const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
   const cugraph_type_erased_device_array_view_t* dist_cols, const cugraph_type_erased_device_array_view_t* win_rows,
   size_t maxpart, int grid_cols, int grid_c, cugraph_type_erased_device_array_view_t* code_rows, cugraph_error_t** error);
+
+/* The edge rules of a BFS / SSSP certificate on this GPU's edge block (MGGraph.validate_bfs / validate_sssp).  One push
+ * round over the block's column-major copy (shared with cugraph_b200_block_sssp_relax and the others).
+ *   dist_cols (one per column slot, gathered by the launcher inside the column group) and dist_rows (one per row slot,
+ *     gathered inside the row group) are INT32 BFS levels with unit steps (weights ignored; INT32_MAX = unreached), or the
+ *     weight type of a weighted block (SSSP; the unreached columns must hold +inf so that they are not queued).
+ *   pred_rows (INT64, one per row slot): the predecessor code of every row slot (owner rank * maxpart + local id, as
+ *     cugraph_b200_block_bfs_pull gives them), -1 = none.
+ * For every edge (row, col) of a reached column with nd < cutoff, where nd = dist_cols[col] + w in the weight type (the
+ * sum of cugraph_b200_block_sssp_relax, cutoff rounded as there) or dist_cols[col] + 1 in 64-bit integers (unit steps;
+ * pass depth_limit + 1, or +inf for none):
+ *   violations[0] (INT64, zeroed first) counts the edges with dist_rows[row] > nd or NaN;
+ *   flag_rows[row] (byte flags, zeroed first) = 1 when pred_rows[row] is the column's code and dist_rows[row] == nd, 2
+ *     when besides dist_cols[col] == dist_rows[row] (a flat step).
+ * *edges_from_reached (host) = the number of edges of the reached columns, self-loops and multi-edges included.  NULL
+ * arguments, other dtypes, short arrays and a bad grid position return CUGRAPH_INVALID_INPUT.  Asynchronous, apart from
+ * one read-back of the number of reached columns and their edge count. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_check_paths(
+  const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block, const cugraph_type_erased_device_array_view_t* dist_cols,
+  const cugraph_type_erased_device_array_view_t* dist_rows, const cugraph_type_erased_device_array_view_t* pred_rows,
+  double cutoff, size_t maxpart, int grid_cols, int grid_c, cugraph_type_erased_device_array_view_t* flag_rows,
+  cugraph_type_erased_device_array_view_t* violations, uint64_t* edges_from_reached, cugraph_error_t** error);
 
 /* One round of multi-GPU weakly connected components on this GPU's edge block (min-label propagation).  The block may be
  * unweighted or weighted; weights are ignored.  label_cols (INT64, at least one per column slot, gathered by the launcher
