@@ -121,6 +121,9 @@ struct handle_deleter {
   void operator()(handle_impl* h) const
   {
     if (h->pinned) cudaFreeHost(h->pinned);
+    if (h->fork) cudaEventDestroy(h->fork);
+    if (h->join) cudaEventDestroy(h->join);
+    if (h->side) cudaStreamDestroy(h->side);
     if (h->stream && !h->borrowed_stream) cudaStreamDestroy(h->stream);
     delete h;
   }
@@ -137,6 +140,9 @@ cugraph_resource_handle_t* create_handle(const char* entry, cudaStream_t stream,
     h->borrowed_stream = borrowed;
     CUDA_TRY(cudaGetDevice(&h->device));
     if (!borrowed) CUDA_TRY(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
+    CUDA_TRY(cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking));
+    CUDA_TRY(cudaEventCreateWithFlags(&h->fork, cudaEventDisableTiming));
+    CUDA_TRY(cudaEventCreateWithFlags(&h->join, cudaEventDisableTiming));
     cudaDeviceProp prop{};
     CUDA_TRY(cudaGetDeviceProperties(&prop, h->device));
     h->sm_count = prop.multiProcessorCount;

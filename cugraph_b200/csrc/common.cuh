@@ -99,6 +99,8 @@ struct tuning_t {
   int sweep_bands{0};                    // CUGRAPH_B200_SWEEP_BANDS: row bands of the piece stream (0: sized to the L2)
   int sweep_tail_degree{0};              // CUGRAPH_B200_SWEEP_TAIL_DEGREE: rows below this in-degree leave the piece stream
                                          // (0: the default rule, 1: no tail, 2/4/8/16/32: that bound on any graph)
+  int sweep_tail_sms{-1};                // CUGRAPH_B200_SWEEP_TAIL_SMS: SMs the tail sweep gets beside the piece stream (< 0: chosen
+                                         // from the layout, 0: no split, the tail after the bands on every SM)
   double bfs_alpha{40.0}, bfs_beta{24.0};  // CUGRAPH_B200_BFS_ALPHA / _BETA (Beamer switch points; alpha 14 -> 40: -7 % per source on RMAT-24, r02_notes)
   bool sssp_adaptive{true};                // CUGRAPH_B200_SSSP_ADAPTIVE
   double sssp_delta_scale{1.0};            // CUGRAPH_B200_SSSP_DELTA_SCALE
@@ -118,6 +120,7 @@ struct tuning_t {
     if (auto e = get("CUGRAPH_B200_SWEEP_BANK_ORDER")) t.sweep_bank_order = std::atoi(e) != 0;
     if (auto e = get("CUGRAPH_B200_SWEEP_BANDS")) t.sweep_bands = std::max(0, std::atoi(e));
     if (auto e = get("CUGRAPH_B200_SWEEP_TAIL_DEGREE")) t.sweep_tail_degree = std::max(0, std::atoi(e));
+    if (auto e = get("CUGRAPH_B200_SWEEP_TAIL_SMS")) t.sweep_tail_sms = std::atoi(e);
     if (auto e = get("CUGRAPH_B200_BFS_ALPHA")) t.bfs_alpha = std::atof(e);
     if (auto e = get("CUGRAPH_B200_BFS_BETA")) t.bfs_beta = std::atof(e);
     if (auto e = get("CUGRAPH_B200_SSSP_ADAPTIVE")) t.sssp_adaptive = std::atoi(e) != 0;
@@ -137,13 +140,17 @@ struct tuning_t {
 };
 
 // ---------------------------------------------------------------------------------------------
-// resource handle: one device, one stream, the device's default stream-ordered pool.
+// resource handle: one device, one stream, the device's default stream-ordered pool.  A side stream and two events let one
+// kernel run beside the work of `stream` (the pull sweep's tail, sweep.cuh): forked from `stream` by `fork`, joined back
+// into it by `join` before anything after it is enqueued, so everything outside that fork is ordered on `stream` alone.
 // ---------------------------------------------------------------------------------------------
 struct handle_impl {
   tuning_t tune{};
   int device{0};
   cudaStream_t stream{nullptr};
   bool borrowed_stream{false};  // stream belongs to the caller (torch): never destroyed here
+  cudaStream_t side{nullptr};   // the handle's own, borrowed stream or not
+  cudaEvent_t fork{nullptr}, join{nullptr};
   int sm_count{132};
   size_t l2_bytes{0};
   mutable size_t launches{0};
@@ -314,11 +321,12 @@ inline int grid_for(int64_t n, int per_thread = 1, int max_grid = 1 << 20)
   return (int)std::min<int64_t>(std::max<int64_t>(b, 1), std::min(max_grid, 1 << 20));
 }
 
+// B200_LAUNCH_ON: on stream s of handle h (its stream or its side stream), counted like every launch
 #ifndef B200_HOST_EMU
-#define B200_LAUNCH(h, kernel, grid, block, smem, ...)                           \
+#define B200_LAUNCH_ON(h, s, kernel, grid, block, smem, ...)                     \
   do {                                                                           \
     if ((grid) > 0) {                                                            \
-      kernel<<<(grid), (block), (smem), (h).stream>>>(__VA_ARGS__);              \
+      kernel<<<(grid), (block), (smem), (s)>>>(__VA_ARGS__);                     \
       (h).launches++;                                                            \
     }                                                                            \
   } while (0)
@@ -326,16 +334,19 @@ inline int grid_for(int64_t n, int per_thread = 1, int max_grid = 1 << 20)
 __device__ __forceinline__ bool is_commit_lane() { return (threadIdx.x & 31) == 0; }
 #else
 // host emulation of the staging kernels (emu/cuda_runtime.h, tests/test_emu_staging_cpu.py): every thread of the
-// launch runs to completion, one after the other; warp shuffles are identities, so every thread commits for itself
-#define B200_LAUNCH(h, kernel, grid, block, smem, ...)                           \
+// launch runs to completion, one after the other; warp shuffles are identities, so every thread commits for itself.  Streams
+// are in order here: a launch on the side stream runs where it is enqueued
+#define B200_LAUNCH_ON(h, s, kernel, grid, block, smem, ...)                     \
   do {                                                                           \
     if ((grid) > 0) {                                                            \
+      (void)(s);                                                                 \
       emu_launch((grid), (block), (size_t)(smem), [&] { kernel(__VA_ARGS__); }); \
       (h).launches++;                                                            \
     }                                                                            \
   } while (0)
 inline bool is_commit_lane() { return true; }
 #endif
+#define B200_LAUNCH(h, kernel, grid, block, smem, ...) B200_LAUNCH_ON(h, (h).stream, kernel, grid, block, smem, __VA_ARGS__)
 
 __device__ __forceinline__ double warp_sum(double v)
 {

@@ -22,9 +22,10 @@
 //     first.  k_sweep_finish turns acc into y, clears it and resets the cursors.
 //   * the rows are split into bands whose accumulators fit in the L2 (sweep_layout.cuh); the sweep runs band by band, k_sweep over
 //     the band's phases, then k_sweep_finish over its rows while their accumulators are still in the L2.
-//   * on large graphs the rows of small in-degree (the tail, sweep_layout.cuh) are not in the stream: one k_sweep_tail launch after
-//     the bands gathers their few edges directly from a layout of their own (runs of equal in-degree, lane-interleaved: no
-//     RED, and fewer stream rows need fewer bands), the hubs' x from a shared-memory copy of the first column block.
+//   * on large graphs the rows of small in-degree (the tail, sweep_layout.cuh) are not in the stream: one k_sweep_tail launch
+//     gathers their few edges directly from a layout of their own (runs of equal in-degree, lane-interleaved: no RED, and
+//     fewer stream rows need fewer bands), the hubs' x from a shared-memory copy of the first column block.  It runs on a
+//     share of the SMs beside the bands, from the handle's side stream (launch_sweep), or after them on every SM.
 #pragma once
 #include "spmv.cuh"
 #include "sweep_layout.cuh"
@@ -722,7 +723,8 @@ struct tail_args_t {
   T const* __restrict__ x;
   T* __restrict__ y;
   int32_t const* __restrict__ row_vertex;
-  int* __restrict__ cursor;
+  int* __restrict__ cursor;  // this launch's slot of the tail cursor
+  int* __restrict__ spent;   // the other slot, left behind by the launch before: cleared for the next one
   pr_state_t const* __restrict__ st;
   int n_runs, empty_hi, W;
   double alpha;
@@ -822,6 +824,7 @@ __global__ void __launch_bounds__(kTailThreads, 1) k_sweep_tail(tail_args_t<T> a
   T const* sx = reinterpret_cast<T const*>(smem_raw);
   __shared__ uint64_t bar;
   __shared__ tail_run_t s_run[kTailMaxDegree + 1];
+  if (blockIdx.x == 0 && threadIdx.x == 0) *a.spent = 0;  // also once the loop is done: a later sweep may start a new one
   if (a.st->done) return;
   const unsigned long long pol = make_l2_policy_evict_first(), keep = make_l2_policy_evict_last();
   const int lane = threadIdx.x & 31;
@@ -907,7 +910,11 @@ __global__ void __launch_bounds__(kTailThreads, 1) k_sweep_tail(tail_args_t<T> a
   if constexpr (EPI) epi_flush(a.epi, sums);
 }
 
-// x must hold padded_x_elems() elements, zero behind n_vertices (slices are copied whole)
+// x must hold padded_x_elems() elements, zero behind n_vertices (slices are copied whole).
+// With a tail and L.tail_sms > 0 the tail runs on the handle's side stream, forked from h.stream before the bands and
+// joined back into it after them: k_sweep_tail on tail_sms SMs beside the bands' k_sweep on the other L.n_cta.  They share
+// nothing but x (read by both), the fp64 sums of the row epilogue in *st (atomics) and the tail's cursor, which the tail
+// launches alternate (sweep_layout_t::cursor).  Whatever the caller enqueues on h.stream afterwards runs after both.
 template <typename T>
 void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L, T const* x, T* y, double* acc, double alpha,
                   pr_state_t const* st, bool use_weights, bool covered_rows_only, row_epi_t<T> const& epi)
@@ -918,6 +925,39 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
                                         : (weighted ? k_sweep_tail<T, true, false> : k_sweep_tail<T, false, false>);
   // the attribute is per device and cheap to set: no process-wide "done" flag (a second device would miss it)
   CUDA_TRY(cudaFuncSetAttribute(sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
+  // covered_rows_only: y of the rows without edges already holds their (unvarying) value — multi-GPU blocks, where more than
+  // half of the row slots are empty and the unvarying term is 0 (mg.cu)
+  const int32_t finish_rows = covered_rows_only ? L.n_cov : c.n_rows;
+  const bool tail           = L.n_str < L.n_cov;  // rows of small in-degree left the stream (sweep_layout.cuh)
+  const bool split          = tail && L.tail_sms > 0;
+  // the rows [n_str, n_cov) and (unless covered_rows_only) the empty rows, by k_sweep_tail
+  auto launch_tail = [&](cudaStream_t s, int sms) {
+    tail_args_t<T> t;
+    const unsigned slot = L.tail_sweeps++ & 1u;
+    t.runs       = L.tail_run.as<tail_run_t>();
+    t.ids        = L.tail_ids.as<int32_t>();
+    t.w          = weighted ? L.tail_w.as<T>() : nullptr;
+    t.x          = x;
+    t.y          = y;
+    t.row_vertex = c.row_vertex.as<int32_t>();
+    t.cursor     = L.cursor.as<int>() + L.n_phases + slot;
+    t.spent      = L.cursor.as<int>() + L.n_phases + (slot ^ 1u);
+    t.st         = st;
+    t.n_runs     = L.n_tail_runs;
+    t.empty_hi   = finish_rows;
+    t.W          = L.W;
+    t.alpha      = alpha;
+    t.epi        = epi;
+    const int units  = L.tail_runs.back().first_unit;
+    const int blocks = std::max(1, std::min(sms, (units + kTailThreads / 32 - 1) / (kTailThreads / 32)));
+    CUDA_TRY(cudaFuncSetAttribute(tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
+    B200_LAUNCH_ON(h, s, tail_kernel, blocks, kTailThreads, kSweepDynSmem, t);
+  };
+  if (split) {
+    CUDA_TRY(cudaEventRecord(h.fork, h.stream));
+    CUDA_TRY(cudaStreamWaitEvent(h.side, h.fork, 0));
+    launch_tail(h.side, L.tail_sms);
+  }
   sweep_args_t<T> a;
   a.p.ids     = L.ids.as<uint4>();
   a.p.rows    = L.rows.as<int32_t>();
@@ -933,10 +973,6 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
   a.p.acc_pol = 0;
   // 8 steps of 64 rows per warp: faster than 4 or 2 steps
   constexpr int kFinishSteps = 8;
-  // covered_rows_only: y of the rows without edges already holds their (unvarying) value — multi-GPU blocks, where more than
-  // half of the row slots are empty and the unvarying term is 0 (mg.cu)
-  const int32_t finish_rows = covered_rows_only ? L.n_cov : c.n_rows;
-  const bool tail           = L.n_str < L.n_cov;  // rows of small in-degree left the stream (sweep_layout.cuh)
   // band by band: the band's rows are finished while its accumulators are in the L2, before the next band's REDs evict them.
   // y (and the epilogue's x_next) must not overlap x: a band's finish writes y while later bands (and the tail) still read x.
   for (int band = 0; band < L.n_bands; ++band) {
@@ -947,31 +983,16 @@ void launch_sweep(handle_impl const& h, csx_t const& c, sweep_layout_t const& L,
     a.ph_lo          = L.band_phase[band];
     a.ph_hi          = L.band_phase[band + 1];
     B200_LAUNCH(h, sweep_kernel, L.n_cta, kSweepThreads, kSweepDynSmem, a);
-    // the cursors to reset: the band's phases', and on the last band the tail's behind them (its previous sweep is done)
-    const int n_ph = a.ph_hi - a.ph_lo + (band == L.n_bands - 1 && tail ? 1 : 0);
+    const int n_ph = a.ph_hi - a.ph_lo;  // the cursors to reset: the band's phases'
     const int n    = std::max((row_hi - row_lo + 2 * kFinishSteps - 1) / (2 * kFinishSteps), n_ph);  // threads: 16 rows each
     B200_LAUNCH(h, (k_sweep_finish<T, kFinishSteps>), (std::max(n, 1) + 255) / 256, 256, 0, acc, row_lo, L.n_str, row_hi, y,
                 c.row_vertex.as<int32_t>(), alpha, L.cursor.as<int>() + a.ph_lo, n_ph, st, epi);
   }
-  if (tail) {  // the rows [n_str, n_cov) and (unless covered_rows_only) the empty rows, by k_sweep_tail
-    tail_args_t<T> t;
-    t.runs       = L.tail_run.as<tail_run_t>();
-    t.ids        = L.tail_ids.as<int32_t>();
-    t.w          = weighted ? L.tail_w.as<T>() : nullptr;
-    t.x          = x;
-    t.y          = y;
-    t.row_vertex = c.row_vertex.as<int32_t>();
-    t.cursor     = L.cursor.as<int>() + L.n_phases;
-    t.st         = st;
-    t.n_runs     = L.n_tail_runs;
-    t.empty_hi   = finish_rows;
-    t.W          = L.W;
-    t.alpha      = alpha;
-    t.epi        = epi;
-    const int units  = L.tail_runs.back().first_unit;
-    const int blocks = std::max(1, std::min(h.sm_count, (units + kTailThreads / 32 - 1) / (kTailThreads / 32)));
-    CUDA_TRY(cudaFuncSetAttribute(tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSweepDynSmem));
-    B200_LAUNCH(h, tail_kernel, blocks, kTailThreads, kSweepDynSmem, t);
+  if (split) {
+    CUDA_TRY(cudaEventRecord(h.join, h.side));
+    CUDA_TRY(cudaStreamWaitEvent(h.stream, h.join, 0));
+  } else if (tail) {
+    launch_tail(h.stream, h.sm_count);
   }
 }
 

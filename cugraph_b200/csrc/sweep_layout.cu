@@ -439,6 +439,35 @@ int sweep_bands(handle_impl const& h, int32_t n_str)
   return std::min(std::max(P, 1), most);
 }
 
+// The tail's share of the SMs.  k_sweep_tail runs on k SMs from the handle's side stream while the bands' k_sweep runs on the
+// other sm_count - k (k_sweep is bound by the L2's sector rate more than by its SMs, the tail by the latency of its gathers:
+// side by side the two take less than one after the other, DESIGN.md §3.2).  By default k splits the SMs in proportion to
+// the two kernels' work: the stream's in the planner's cost unit (sweep_group_cost, summed over the chunks plan_sweep will
+// cut), the tail's in entries (an empty row counts a quarter of an entry, a tail row one more), converted by
+// kTailEntryCost.  CUGRAPH_B200_SWEEP_TAIL_SMS forces k (tests, A/B runs); 0 = no split: the tail after the bands on every SM.
+// Measured on an H100 80GB HBM3 at 700 W, RMAT-24 PageRank (DESIGN.md §8.1): k_sweep takes 0.45-0.50 ms per sweep on 132,
+// 116, 100 or 84 CTAs when it runs alone, so it is not bound by its SMs; side by side with the tail the iteration took 0.644
+// / 0.730 / 0.647 / 0.611 / 0.658 ms at k = 0 / 40 / 48 / 56 / 64.  The ratio puts RMAT-24 at k = 56.
+constexpr double kTailEntryCost = 1.4;  // sweep_group_cost units per tail entry
+constexpr double kTailRowEntries = 1.0, kTailEmptyEntries = 0.25;
+
+int sweep_tail_sms(handle_impl const& h, std::vector<int32_t> const& cstart, int n_bands, int B, int64_t tail_entries,
+                   int64_t tail_rows, int64_t empty_rows, double* stream_cost, double* tail_cost)
+{
+  double stream = 0.0;
+  for (int key = 0; key < n_bands * B * kNumKinds; ++key) {
+    const int kind = key % kNumKinds, ppg = kind_pieces(kind);
+    stream += (double)(((int64_t)cstart[key + 1] - cstart[key] + ppg - 1) / ppg) * sweep_group_cost(kind);
+  }
+  const double tail = kTailEntryCost * ((double)tail_entries + kTailRowEntries * (double)tail_rows + kTailEmptyEntries * (double)empty_rows);
+  *stream_cost = stream;
+  *tail_cost   = tail;
+  if (tail_rows <= 0 || h.sm_count < 2) return 0;
+  int k = h.tune.sweep_tail_sms;
+  if (k < 0) k = (int)std::lround(h.sm_count * tail / std::max(stream + tail, 1.0));
+  return std::min(std::max(k, 0), h.sm_count - 1);
+}
+
 // The piece stream holds the rows [0, seg[k]) for the bin k this returns: rows of in-degree >= kSegThreshold[k].
 // By default the rows of in-degree < kSweepTailDegree leave it on graphs of at least kSweepTailMinEdges edges, and it holds
 // every non-empty row on smaller ones.  CUGRAPH_B200_SWEEP_TAIL_DEGREE forces a bound on any graph (tests, A/B runs):
@@ -537,9 +566,11 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
     }
   }
 
-  // 4. chunks, CTA ranges, phases
+  // 4. chunks, CTA ranges, phases, on the SMs the tail leaves to the stream
+  double stream_cost = 0.0, tail_cost = 0.0;
+  L->tail_sms = sweep_tail_sms(h, cstart, n_bands, B, c.nnz - nnz, n_cov - n_str, c.n_rows - n_cov, &stream_cost, &tail_cost);
   sweep_plan_t plan;
-  if (!plan_sweep(cstart, n_bands, B, h.sm_count, plan)) return nullptr;  // step-row numbers overflow 31 bits
+  if (!plan_sweep(cstart, n_bands, B, h.sm_count - L->tail_sms, plan)) return nullptr;  // step-row numbers overflow 31 bits
   L->band_phase = plan.band_phase;
   L->n_steprows = plan.n_steprows;
   L->n_rowslots = plan.n_rowslots;
@@ -557,8 +588,8 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
   }
   CUDA_TRY(cudaMemcpyAsync(L->cta_phase.data(), plan.cta_phase.data(), sizeof(int32_t) * plan.cta_phase.size(), cudaMemcpyHostToDevice, h.stream));
   sync(h);  // the host vectors are pageable
-  L->cursor = make_dbuf<int>(L->n_phases + 1, h.stream);  // the last one: the tail's
-  CUDA_TRY(cudaMemsetAsync(L->cursor.data(), 0, sizeof(int) * (L->n_phases + 1), h.stream));
+  L->cursor = make_dbuf<int>(L->n_phases + 2, h.stream);  // the last two: the tail's
+  CUDA_TRY(cudaMemsetAsync(L->cursor.data(), 0, sizeof(int) * (L->n_phases + 2), h.stream));
 
   // 5. step-rows and row slots
   L->ids  = make_dbuf<uint4>((size_t)std::max<int64_t>(L->n_steprows, 1) * 32, h.stream);
@@ -596,6 +627,9 @@ std::unique_ptr<sweep_layout_t> build_sweep_layout(handle_impl const& h, csx_t c
     std::fprintf(stderr, "[sweep] %lld step-rows = %.1f MB of ids, %lld row slots = %.1f MB, %d chunks, %d phases, %d CTAs\n",
                  (long long)L->n_steprows, (double)L->n_steprows * 512 / 1e6, (long long)L->n_rowslots,
                  (double)L->n_rowslots * 4 / 1e6, L->n_chunks, L->n_phases, L->n_cta);
+    std::fprintf(stderr, "[sweep] split: tail on %d of %d SMs%s (cost: stream %.4g, tail %.4g = %.1f %%)\n", L->tail_sms,
+                 h.sm_count, h.tune.sweep_tail_sms >= 0 ? ", forced" : "", stream_cost, tail_cost,
+                 100.0 * tail_cost / std::max(stream_cost + tail_cost, 1.0));
     for (int band = 0; band < n_bands; ++band) {  // slice loads: a CTA loads a block's slice once per phase
       const int p0 = plan.band_phase[band], p1 = plan.band_phase[band + 1];
       const int c0 = p1 > p0 ? plan.phases[p0].chunk_begin : 0, c1 = p1 > p0 ? plan.phases[p1 - 1].chunk_end : 0;

@@ -99,11 +99,14 @@ struct sweep_layout_t {
   dbuf phases;     // n_phases x sweep_phase_t
   dbuf cta_phase;  // (n_bands * n_cta + 1) x int32: in band b, CTA c owns phases [cta_phase[b * n_cta + c], the next entry)
                    // (cost-balanced, contiguous chunks)
-  dbuf cursor;     // n_phases + 1 x int: next chunk of the phase (relative), then the tail's next work unit; reset by the
-                   // finish kernel (the tail's by the last band's, which runs after the previous sweep's tail)
+  dbuf cursor;     // n_phases + 2 x int: next chunk of the phase (relative), reset by the band's finish kernel; then the tail's
+                   // next work unit, in two slots that alternate from sweep to sweep (tail_sweeps): each tail launch uses
+                   // one and clears the other, which the tail launch before it used and left behind
   int32_t n_chunks{0};
   int32_t n_phases{0};
-  int n_cta{0};
+  int n_cta{0};     // persistent CTAs of the stream: the SMs the tail does not take
+  int tail_sms{0};  // SMs the tail sweeps on beside the stream, from a side stream; 0: after the bands, on every SM
+  mutable unsigned tail_sweeps{0};  // tail launches so far: the cursor slot of the next one is tail_sweeps & 1
   int n_bands{1};
   std::vector<int32_t> band_row;    // n_bands + 1: band b holds rows [band_row[b], band_row[b+1]); band_row[n_bands] = n_str
   std::vector<int32_t> band_phase;  // n_bands + 1: the phases of band b are [band_phase[b], band_phase[b+1])
