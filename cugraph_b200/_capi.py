@@ -97,6 +97,7 @@ def lib():
     _sig(L.cugraph_paths_result_get_predecessors, vp, [vp])
     _sig(L.cugraph_paths_result_free, None, [vp])
     _sig(L.cugraph_bfs, i32, [vp, vp, vp, i32, sz, i32, i32, pvp, pvp])
+    _sig(L.cugraph_b200_multi_source_bfs, i32, [vp, vp, vp, sz, i32, pvp, pvp])
     _sig(L.cugraph_sssp, i32, [vp, vp, sz, dbl, i32, i32, pvp, pvp])
     _sig(L.cugraph_extract_paths, i32, [vp, vp, vp, vp, vp, pvp, pvp])
     _sig(L.cugraph_extract_paths_result_get_max_path_length, sz, [vp])

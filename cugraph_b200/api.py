@@ -127,6 +127,32 @@ def bfs(G: Graph, start=None, depth_limit=None, i_start=None, directed=None, ret
     return _frame(**cols)
 
 
+def multi_source_bfs(G: Graph, sources, components=None, depth_limit=None, offload=False):
+    """cugraph.multi_source_bfs (traversal/ms_bfs.py): a BFS from each source; data frame 'vertex', then 'distance_<s>' and
+    'predecessor_<s>' for each source s in the order given.  The edge-list forms the reference documents for `components`
+    and `offload=True` are not built.  At least one source, no duplicates, no more sources than vertices."""
+    from cugraph_b200.traversal import multi_source_bfs as ms_bfs
+    if components is not None:
+        raise NotImplementedError("multi_source_bfs with components (BFS edge lists per source) is not implemented")
+    if offload:
+        raise NotImplementedError("multi_source_bfs with offload=True (results written to disk) is not implemented")
+    starts = np.atleast_1d(np.asarray(sources, dtype=G._edges[0].dtype))
+    if starts.size == 0:
+        raise ValueError("multi_source_bfs needs at least one source")
+    if np.unique(starts).size != starts.size:
+        raise ValueError("multi_source_bfs sources must be distinct: each names a column pair")
+    if starts.size > G.number_of_vertices():
+        raise ValueError("multi_source_bfs takes at most as many sources as the graph has vertices")
+    h, g = G._plc_graph(False)
+    dist, pred, verts = ms_bfs(h, g, _dev(starts), -1 if depth_limit is None else int(depth_limit), True)
+    dist, pred = _host(dist), _host(pred)
+    cols = dict(vertex=_host(verts))
+    for k, s in enumerate(starts.tolist()):
+        cols[f"distance_{s}"] = dist[k]
+        cols[f"predecessor_{s}"] = pred[k]
+    return _frame(**cols)
+
+
 def sssp(G: Graph, source=None, method=None, directed=None, return_predecessors=None, unweighted=None, overwrite=None,
          indices=None, cutoff=None):
     """cugraph.sssp (traversal/sssp.py:108-330): 'vertex', 'distance', 'predecessor'; the graph must be weighted"""

@@ -147,6 +147,8 @@ void int_to_ext(handle_impl const& h, graph_impl const& g, int32_t const* in, si
 dbuf reported_vertices(handle_impl const& h, graph_impl const& g);
 // permute a per-vertex result from internal order into reported order (no-op copy when renumbered)
 dbuf to_reported_order(handle_impl const& h, graph_impl const& g, void const* internal_vals, size_t elem_size);
+// the same into out (V elements, not overlapping internal_vals)
+void to_reported_order_into(handle_impl const& h, graph_impl const& g, void const* internal_vals, size_t elem_size, void* out);
 
 // (vertex, value) pairs with external ids -> dense internal-order vector, missing = fill
 template <typename T>

@@ -1088,19 +1088,24 @@ dbuf reported_vertices(handle_impl const& h, graph_impl const& g)
   return out;
 }
 
+void to_reported_order_into(handle_impl const& h, graph_impl const& g, void const* vals, size_t es, void* out)
+{
+  if (g.n_vertices == 0) return;
+  if (g.renumbered) {
+    CUDA_TRY(cudaMemcpyAsync(out, vals, (size_t)g.n_vertices * es, cudaMemcpyDeviceToDevice, h.stream));
+  } else if (es == 4) {
+    B200_LAUNCH(h, (k_permute<uint32_t>), grid_for(g.n_vertices), kBlock, 0, (uint32_t const*)vals,
+                g.int_of_rank.as<int32_t>(), g.n_vertices, (uint32_t*)out);
+  } else {
+    B200_LAUNCH(h, (k_permute<uint64_t>), grid_for(g.n_vertices), kBlock, 0, (uint64_t const*)vals,
+                g.int_of_rank.as<int32_t>(), g.n_vertices, (uint64_t*)out);
+  }
+}
+
 dbuf to_reported_order(handle_impl const& h, graph_impl const& g, void const* vals, size_t es)
 {
   dbuf out((size_t)g.n_vertices * es, h.stream);
-  if (g.n_vertices == 0) return out;
-  if (g.renumbered) {
-    CUDA_TRY(cudaMemcpyAsync(out.data(), vals, (size_t)g.n_vertices * es, cudaMemcpyDeviceToDevice, h.stream));
-  } else if (es == 4) {
-    B200_LAUNCH(h, (k_permute<uint32_t>), grid_for(g.n_vertices), kBlock, 0, (uint32_t const*)vals,
-                g.int_of_rank.as<int32_t>(), g.n_vertices, out.as<uint32_t>());
-  } else {
-    B200_LAUNCH(h, (k_permute<uint64_t>), grid_for(g.n_vertices), kBlock, 0, (uint64_t const*)vals,
-                g.int_of_rank.as<int32_t>(), g.n_vertices, out.as<uint64_t>());
-  }
+  to_reported_order_into(h, g, vals, es, out.data());
   return out;
 }
 

@@ -20,6 +20,7 @@
 
 #include <algorithm>
 #include <cfloat>
+#include <chrono>
 #include <climits>
 #include <cstdlib>
 #include <cmath>
@@ -298,6 +299,316 @@ void run_bfs(handle_impl const& h, csx_t const& c, int32_t nv, int32_t const* so
     ++level;
   }
   check_last("bfs");
+}
+
+// ------------------------------------------------------------------------------------------
+// Multi-source BFS: one BFS per source, a batch of up to 64 sources per pass over the graph (bit-parallel BFS: Then et al.,
+// "The More the Merrier", VLDB 2015).  Bit j of a vertex's 64-bit words stands for source j of the batch:
+//   seen : the sources that have reached the vertex;   cur : those that reached it at this level;   next : at the next one.
+// A top-down level advances the vertices with a non-zero cur word (a queue, as in run_bfs) and ORs cur[u] into next[v] for
+// every edge u -> v; a bottom-up level ORs the cur words of v's in-edges into the bits v still wants.  One edge read
+// advances every BFS of the batch.  dist / pred hold one int32 row of V entries per source of the batch, row j at j * V.
+// ------------------------------------------------------------------------------------------
+struct ms_counters_t {
+  frontier_counters_t f;        // next frontier: vertices with a non-zero word (n_small, n_conv) and their out-degree sum (m_f)
+  unsigned long long n_full;    // vertices whose seen word became the whole batch ...
+  unsigned long long m_full;    // ... and their out-degree sum (Beamer's rule counts them as visited)
+};
+
+// write distance d (and predecessor u) of vertex v into the rows of the bits set in `bits`
+__device__ __forceinline__ void ms_write_rows(unsigned long long bits, int v, long long nv, int32_t d, int32_t* dist, int32_t* pred,
+                                              int u)
+{
+  while (bits) {
+    const long long j = __ffsll((long long)bits) - 1;
+    dist[j * nv + v] = d;
+    if (pred) pred[j * nv + v] = u;
+    bits &= bits - 1;
+  }
+}
+
+__device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v)
+{
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// the four level counters of a thread, summed over the warp and added with one atomic each (every lane must call it)
+__device__ __forceinline__ void ms_commit(ms_counters_t* cnt, unsigned long long n, unsigned long long m, unsigned long long n_full,
+                                          unsigned long long m_full)
+{
+  n = warp_sum_u64(n), m = warp_sum_u64(m), n_full = warp_sum_u64(n_full), m_full = warp_sum_u64(m_full);
+  if ((threadIdx.x & 31) == 0) {
+    if (n) atomicAdd(&cnt->f.n_small, (int)n);
+    if (m) atomicAdd(&cnt->f.m_f, m);
+    if (n_full) atomicAdd(&cnt->n_full, n_full);
+    if (m_full) atomicAdd(&cnt->m_full, m_full);
+  }
+}
+
+template <typename O>
+__device__ __forceinline__ unsigned long long out_degree(O const* off, int v)
+{
+  return (unsigned long long)((long long)off[v + 1] - (long long)off[v]);
+}
+
+// bit j for source j of the batch; every distinct source vertex is queued once, with its degree
+template <typename O>
+__global__ void k_ms_seed(int32_t const* __restrict__ src, int n, O const* __restrict__ off, unsigned long long* seen,
+                          unsigned long long* cur, int32_t* dist, long long nv, unsigned long long mask, int32_t* q, int32_t* q_deg,
+                          ms_counters_t* cnt)
+{
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const int v                   = src[i];
+    const unsigned long long bit  = 1ull << i;
+    const unsigned long long old  = atomicOr(seen + v, bit);
+    atomicOr(cur + v, bit);
+    dist[i * nv + v] = 0;
+    if (old == 0) {
+      const unsigned d = enqueue_with_degree(off, v, q, q_deg, &cnt->f);
+      atomicAdd(&cnt->f.m_f, (unsigned long long)d);
+    }
+    if ((old | bit) == mask) {
+      atomicAdd(&cnt->n_full, 1ull);
+      atomicAdd(&cnt->m_full, out_degree(off, v));
+    }
+  }
+}
+
+// top-down edge u -> v: the sources that reached u at this level and have not reached v.  seen is read-only during the
+// level (k_ms_fold folds next into it afterwards); the thread whose atomicOr set a bit first writes that source's row.
+template <typename O>
+struct ms_topdown_op {
+  O const* off;
+  unsigned long long const* cur;
+  unsigned long long const* seen;
+  unsigned long long* next;
+  int32_t* dist;
+  int32_t* pred;  // may be null
+  long long nv;
+  int32_t* next_q;
+  int32_t* next_q_deg;
+  frontier_counters_t* cnt;
+  int level;
+  __device__ __forceinline__ void edge(int src, long long, int nbr) const
+  {
+    const unsigned long long bits = cur[src] & ~seen[nbr];
+    if (!(bits & ~next[nbr])) return;  // next only gains bits during the level: a stale read costs an atomic, never a bit
+    const unsigned long long old = atomicOr(next + nbr, bits);
+    ms_write_rows(bits & ~old, nbr, nv, level + 1, dist, pred, src);
+    if (old == 0) {
+      const unsigned d = enqueue_with_degree(off, nbr, next_q, next_q_deg, cnt);
+      warp_add_u64(&cnt->m_f, d);
+    }
+  }
+};
+
+// after a top-down level: seen |= next for the vertices of the new queue (*n_new entries, written by the level), and the
+// cur words of the old queue are cleared, so that cur serves as the next level's all-zero `next`
+template <typename O>
+__global__ void __launch_bounds__(kBlock)
+k_ms_fold(int32_t const* __restrict__ old_q, int n_old, int32_t const* __restrict__ new_q, int const* __restrict__ n_new,
+          unsigned long long* __restrict__ cur, unsigned long long const* __restrict__ next, unsigned long long* __restrict__ seen,
+          unsigned long long mask, O const* __restrict__ off, ms_counters_t* cnt)
+{
+  const long long n = (long long)n_old + *n_new;
+  unsigned long long n_full = 0, m_full = 0;
+  for (long long i0 = blockIdx.x * (long long)blockDim.x; i0 < n; i0 += (long long)gridDim.x * blockDim.x) {
+    const long long i = i0 + threadIdx.x;
+    if (i < n_old) {
+      cur[old_q[i]] = 0ull;
+    } else if (i < n) {
+      const int v                    = new_q[i - n_old];
+      const unsigned long long s     = seen[v] | next[v];
+      seen[v]                        = s;
+      if (s == mask) {  // next[v] holds bits seen[v] lacked: the word became whole now
+        n_full += 1;
+        m_full += out_degree(off, v);
+      }
+    }
+  }
+  ms_commit(cnt, 0, 0, n_full, m_full);
+}
+
+// Bottom-up level over the physical rows of the in-edge view: v ORs cur[u] & want over its in-edges u, want = the batch
+// bits v has not seen, and stops once every wanted bit is found.  The predecessor of a bit is the in-neighbour that first
+// supplied it.  The kernel owns v's words: it writes next[v], seen[v] and v's entries of the rows itself.  Rows are sorted
+// by descending in-degree: the first n_hub (degree >= 32) are read by a warp each, 32 in-edges per step with a prefix OR
+// over the lanes to find which lane supplied a bit first; the rest by a thread each.
+template <typename OI, typename O>
+__global__ void __launch_bounds__(kBlock)
+k_ms_bottomup(OI const* __restrict__ in_off, int32_t const* __restrict__ in_idx, int32_t const* __restrict__ row_vertex,
+              int n_rows, int n_hub, O const* __restrict__ off, unsigned long long const* __restrict__ cur,
+              unsigned long long* __restrict__ next, unsigned long long* __restrict__ seen, int32_t* __restrict__ dist,
+              int32_t* __restrict__ pred, long long nv, unsigned long long mask, int level, ms_counters_t* cnt)
+{
+  const int lane         = threadIdx.x & 31;
+  const long long tid    = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  unsigned long long c_n = 0, c_m = 0, c_full = 0, c_mfull = 0;
+  for (long long r = tid >> 5; r < n_hub; r += stride >> 5) {
+    const int v                     = row_vertex ? row_vertex[r] : (int)r;
+    const unsigned long long s      = seen[v];
+    const unsigned long long want   = ~s & mask;
+    if (!want) continue;  // warp-uniform
+    unsigned long long found = 0;
+    const long long end      = (long long)in_off[r + 1];
+    for (long long e0 = (long long)in_off[r]; e0 < end; e0 += 32) {
+      const long long e             = e0 + lane;
+      const int u                   = e < end ? in_idx[e] : 0;
+      const unsigned long long mine = e < end ? cur[u] & want & ~found : 0ull;
+      unsigned long long incl       = mine;  // inclusive prefix OR over the lanes
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl |= t;
+      }
+      const unsigned long long before = __shfl_up_sync(0xffffffffu, incl, 1);
+      ms_write_rows(lane ? mine & ~before : mine, v, nv, level + 1, dist, pred, u);
+      found |= __shfl_sync(0xffffffffu, incl, 31);
+      if (found == want) break;
+    }
+    if (lane == 0 && found) {
+      next[v] = found;
+      seen[v] = s | found;
+      c_n += 1;
+      c_m += out_degree(off, v);
+      if ((s | found) == mask) {
+        c_full += 1;
+        c_mfull += out_degree(off, v);
+      }
+    }
+  }
+  for (long long r = n_hub + tid; r < n_rows; r += stride) {
+    const int v                   = row_vertex ? row_vertex[r] : (int)r;
+    const unsigned long long s    = seen[v];
+    const unsigned long long want = ~s & mask;
+    if (!want) continue;
+    unsigned long long found = 0;
+    const long long end      = (long long)in_off[r + 1];
+    for (long long e = (long long)in_off[r]; e < end; ++e) {
+      const int u                   = in_idx[e];
+      const unsigned long long bits = cur[u] & want & ~found;
+      if (!bits) continue;
+      ms_write_rows(bits, v, nv, level + 1, dist, pred, u);
+      found |= bits;
+      if (found == want) break;
+    }
+    if (found) {
+      next[v] = found;
+      seen[v] = s | found;
+      c_n += 1;
+      c_m += out_degree(off, v);
+      if ((s | found) == mask) {
+        c_full += 1;
+        c_mfull += out_degree(off, v);
+      }
+    }
+  }
+  ms_commit(cnt, c_n, c_m, c_full, c_mfull);
+}
+
+// queue of the vertices with a non-zero word (a switch from bottom-up back to top-down); the whole CTA takes each step
+__global__ void k_ms_words_to_queue(unsigned long long const* __restrict__ words, int n, int32_t* __restrict__ q, int* counter)
+{
+  for (long long v0 = blockIdx.x * (long long)blockDim.x; v0 < n; v0 += (long long)gridDim.x * blockDim.x) {
+    const long long v   = v0 + threadIdx.x;
+    const bool on       = v < n && words[v] != 0ull;
+    const unsigned ball = __ballot_sync(0xffffffffu, on);
+    const int lane      = threadIdx.x & 31;
+    int base            = 0;
+    if (lane == 0 && ball) base = atomicAdd(counter, __popc(ball));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (on) q[base + __popc(ball & ((1u << lane) - 1u))] = (int32_t)v;
+  }
+}
+
+// One batch of nb <= 64 sources (internal ids).  dist and pred (may be null) hold nb rows of nv entries, filled here.
+// Direction per level: Beamer's rule (bfs_bottom_up), with a vertex counted as visited once every source of the batch has
+// reached it.  Only the schedule depends on it, never the result.
+template <typename O>
+void run_multi_source_bfs_batch(handle_impl const& h, graph_impl& g, csx_t const& c, int32_t nv, int32_t const* sources, int nb,
+                                int depth_limit, int32_t* dist, int32_t* pred, int batch)
+{
+  using u64          = unsigned long long;
+  O const* off       = c.offsets.as<O>();
+  int32_t const* idx = c.indices.as<int32_t>();
+  const u64 mask     = nb == 64 ? ~0ull : (1ull << nb) - 1ull;
+  const long long cells = (long long)nb * nv;
+  dbuf seen = make_dbuf<u64>(nv, h.stream), wa = make_dbuf<u64>(nv, h.stream), wb = make_dbuf<u64>(nv, h.stream);
+  for (dbuf* w : {&seen, &wa, &wb}) CUDA_TRY(cudaMemsetAsync(w->data(), 0, sizeof(u64) * nv, h.stream));
+  dbuf qa = make_dbuf<int32_t>(nv, h.stream), qb = make_dbuf<int32_t>(nv, h.stream);
+  dbuf la = make_dbuf<int32_t>((size_t)nv + 1, h.stream), lb = make_dbuf<int32_t>((size_t)nv + 1, h.stream);  // queue degrees
+  dbuf cnt = make_dbuf<ms_counters_t>(1, h.stream);
+  ms_counters_t* dc = cnt.as<ms_counters_t>();
+  CUDA_TRY(cudaMemsetAsync(cnt.data(), 0, sizeof(ms_counters_t), h.stream));
+  B200_LAUNCH(h, (k_fill<int32_t>), grid_for(cells, 1, h.sm_count * 32), kBlock, 0, dist, (int64_t)cells, INT_MAX);
+  if (pred) B200_LAUNCH(h, (k_fill<int32_t>), grid_for(cells, 1, h.sm_count * 32), kBlock, 0, pred, (int64_t)cells, -1);
+  u64 *cur = wa.as<u64>(), *nxt = wb.as<u64>();
+  int32_t *cur_q = qa.as<int32_t>(), *nxt_q = qb.as<int32_t>();
+  int32_t *cur_l = la.as<int32_t>(), *nxt_l = lb.as<int32_t>();
+  B200_LAUNCH(h, (k_ms_seed<O>), 1, 64, 0, sources, nb, off, seen.as<u64>(), cur, dist, (long long)nv, mask, cur_q, cur_l, dc);
+  auto* hc = reinterpret_cast<ms_counters_t*>(h.pinned);
+  CUDA_TRY(cudaMemcpyAsync(hc, cnt.data(), sizeof(ms_counters_t), cudaMemcpyDeviceToHost, h.stream));
+  sync(h);
+  int n_f = hc->f.n_small, prev_n_f = 0;
+  u64 m_f = hc->f.m_f, m_full = hc->m_full;
+  long long n_full = (long long)hc->n_full;
+  const u64 m_total = (u64)c.nnz;
+  // the frontier is the cur words, and also a queue (cur_q; degrees in cur_l once a top-down level or the seed wrote them)
+  // except after a bottom-up level
+  bool bottom_up = false, have_queue = true, deg_ready = true;
+  csx_t const* in = nullptr;  // the in-edge view, fetched at the first bottom-up level (a non-symmetric CSR graph builds it then)
+  advance_scratch_t adv;
+  adv.init(h, nv, (int64_t)c.nnz);
+  const bool trace = h.tune.bfs_trace;
+  for (int level = 0; n_f > 0 && level < depth_limit; ++level) {
+    const auto t0 = std::chrono::steady_clock::now();
+    bottom_up     = bfs_bottom_up(h, bottom_up, n_f, prev_n_f, m_f, m_total - std::min(m_full, m_total), nv - n_full);
+    CUDA_TRY(cudaMemsetAsync(cnt.data(), 0, sizeof(ms_counters_t), h.stream));
+    if (!bottom_up) {
+      if (!have_queue) {
+        B200_LAUNCH(h, k_ms_words_to_queue, grid_for(nv, 1, h.sm_count * 16), kBlock, 0, cur, nv, cur_q, &dc->f.n_conv);
+        have_queue = true;
+        deg_ready  = false;
+      }
+      ms_topdown_op<O> op{off, cur, seen.as<u64>(), nxt, dist, pred, (long long)nv, nxt_q, nxt_l, &dc->f, level};
+      advance<O>(h, adv, off, idx, cur_q, n_f, m_f, op, deg_ready ? cur_l : (int32_t const*)nullptr);
+      B200_LAUNCH(h, (k_ms_fold<O>), grid_for((int64_t)n_f + nv, 1, h.sm_count * 8), kBlock, 0, cur_q, n_f, nxt_q,
+                  &dc->f.n_small, cur, nxt, seen.as<u64>(), mask, off, dc);
+      std::swap(cur_q, nxt_q);
+      std::swap(cur_l, nxt_l);
+      deg_ready = true;
+    } else {
+      if (!in) in = &pull_view(h, g);  // rows = destinations: the primary itself on a symmetric or transposed graph
+      const int n_hub = in->seg[0];    // rows of in-degree >= 32
+      const int grid  = grid_for(std::max<int64_t>((int64_t)n_hub * 32, (int64_t)nv - n_hub), 1, h.sm_count * 16);
+      if (in->offs64)
+        B200_LAUNCH(h, (k_ms_bottomup<int64_t, O>), grid, kBlock, 0, in->offsets.as<int64_t>(), in->indices.as<int32_t>(),
+                    in->row_vertex.as<int32_t>(), in->n_rows, n_hub, off, cur, nxt, seen.as<u64>(), dist, pred, (long long)nv,
+                    mask, level, dc);
+      else
+        B200_LAUNCH(h, (k_ms_bottomup<int32_t, O>), grid, kBlock, 0, in->offsets.as<int32_t>(), in->indices.as<int32_t>(),
+                    in->row_vertex.as<int32_t>(), in->n_rows, n_hub, off, cur, nxt, seen.as<u64>(), dist, pred, (long long)nv,
+                    mask, level, dc);
+      CUDA_TRY(cudaMemsetAsync(cur, 0, sizeof(u64) * nv, h.stream));
+      have_queue = false;
+    }
+    std::swap(cur, nxt);
+    CUDA_TRY(cudaMemcpyAsync(hc, cnt.data(), sizeof(ms_counters_t), cudaMemcpyDeviceToHost, h.stream));
+    sync(h);
+    if (trace)
+      std::fprintf(stderr, "ms-bfs batch %d level %d %s n_f=%d m_f=%llu full=%lld -> next n_f=%d m_f=%llu, %.3f ms\n", batch, level,
+                   bottom_up ? "bottom-up" : "top-down", n_f, m_f, n_full, hc->f.n_small, hc->f.m_f,
+                   std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count());
+    prev_n_f = n_f;
+    n_f      = hc->f.n_small;
+    m_f      = hc->f.m_f;
+    n_full += (long long)hc->n_full;
+    m_full += hc->m_full;
+  }
+  check_last("multi_source_bfs");
 }
 
 // ------------------------------------------------------------------------------------------
@@ -960,12 +1271,17 @@ void run_sssp(handle_impl const& h, csx_t const& c, int32_t nv, int32_t source, 
 
 device_array_impl* make_array(dbuf&& b, size_t n, cugraph_data_type_id_t t) { return new device_array_impl{std::move(b), n, t}; }
 
-// internal predecessors (int32, internal ids) -> reported order, external ids, graph's vertex dtype
-device_array_impl* finish_predecessors(handle_impl const& h, graph_impl const& g, int32_t const* pred_int)
+// internal predecessors (int32, internal ids) -> reported order, external ids, graph's vertex dtype, into ext_out (V elements)
+void predecessors_to_ext(handle_impl const& h, graph_impl const& g, int32_t const* pred_int, void* ext_out)
 {
   dbuf ordered = to_reported_order(h, g, pred_int, sizeof(int32_t));
+  int_to_ext(h, g, ordered.as<int32_t>(), (size_t)g.n_vertices, ext_out);
+}
+
+device_array_impl* finish_predecessors(handle_impl const& h, graph_impl const& g, int32_t const* pred_int)
+{
   dbuf ext((size_t)g.n_vertices * dtype_size(g.vertex_type), h.stream);
-  int_to_ext(h, g, ordered.as<int32_t>(), (size_t)g.n_vertices, ext.data());
+  predecessors_to_ext(h, g, pred_int, ext.data());
   return make_array(std::move(ext), (size_t)g.n_vertices, g.vertex_type);
 }
 
@@ -1098,6 +1414,74 @@ cugraph_error_code_t cugraph_bfs(const cugraph_resource_handle_t* handle, cugrap
     }
     if (compute_predecessors) res->predecessors = finish_predecessors(h, *g, pred.as<int32_t>());
     else res->predecessors = make_array(dbuf(0, h.stream), 0, g->vertex_type);
+    sync(h);
+    *result = reinterpret_cast<cugraph_paths_result_t*>(res.release());
+  });
+}
+
+cugraph_error_code_t cugraph_b200_multi_source_bfs(const cugraph_resource_handle_t* handle, cugraph_graph_t* graph,
+                                                   const cugraph_type_erased_device_array_view_t* sources, size_t depth_limit,
+                                                   bool_t compute_predecessors, cugraph_paths_result_t** result,
+                                                   cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    auto* g       = G(graph);
+    B200_EXPECTS(result != nullptr, CUGRAPH_INVALID_INPUT, "result out-pointer is NULL");
+    *result = nullptr;
+    B200_EXPECTS(sources != nullptr, CUGRAPH_INVALID_INPUT, "sources is NULL");
+    auto const* s = V(sources);
+    B200_EXPECTS(s->type == g->vertex_type, CUGRAPH_INVALID_INPUT, "vertex type of graph and sources must match");
+    const int32_t nv = g->n_vertices;
+    const size_t n   = s->size;
+    dbuf src_int     = make_dbuf<int32_t>(std::max<size_t>(n, 1), h.stream);
+    ext_to_int(h, *g, s->data, n, src_int.as<int32_t>());
+    if (n > 0) {
+      std::vector<int32_t> hs(n);
+      CUDA_TRY(cudaMemcpyAsync(hs.data(), src_int.data(), sizeof(int32_t) * n, cudaMemcpyDeviceToHost, h.stream));
+      sync(h);
+      for (auto v : hs) B200_EXPECTS(v >= 0, CUGRAPH_INVALID_INPUT, "Found invalid vertex in the input sources");
+    }
+    // source-major results: row k (source k) starts at entry k * nv, 64-bit offsets (n * nv passes 2^31 early)
+    const size_t es    = dtype_size(g->vertex_type);
+    const size_t cells = n * (size_t)nv;
+    dbuf dist_out(cells * es, h.stream), pred_out(compute_predecessors ? cells * es : 0, h.stream);
+    const int dl = (int)std::min<size_t>(depth_limit, (size_t)INT_MAX);
+    if (cells > 0) {
+      csx_t const& c  = push_view(h, *g);
+      const int nb_max = (int)std::min<size_t>(n, 64);
+      // one batch's internal rows; each row goes to reported order and external ids straight into the result
+      dbuf dist_b = make_dbuf<int32_t>((size_t)nb_max * nv, h.stream), pred_b;
+      if (compute_predecessors) pred_b = make_dbuf<int32_t>((size_t)nb_max * nv, h.stream);
+      dbuf wide_tmp;
+      if (g->vertex_type == INT64) wide_tmp = make_dbuf<int32_t>(nv, h.stream);
+      for (size_t b0 = 0; b0 < n; b0 += 64) {
+        const int nb = (int)std::min<size_t>(n - b0, 64);
+        if (c.offs64)
+          run_multi_source_bfs_batch<int64_t>(h, *g, c, nv, src_int.as<int32_t>() + b0, nb, dl, dist_b.as<int32_t>(),
+                                              pred_b.as<int32_t>(), (int)(b0 / 64));
+        else
+          run_multi_source_bfs_batch<int32_t>(h, *g, c, nv, src_int.as<int32_t>() + b0, nb, dl, dist_b.as<int32_t>(),
+                                              pred_b.as<int32_t>(), (int)(b0 / 64));
+        for (int j = 0; j < nb; ++j) {
+          int32_t const* row = dist_b.as<int32_t>() + (size_t)j * nv;
+          char* out          = dist_out.as<char>() + (b0 + j) * (size_t)nv * es;
+          if (g->vertex_type == INT64) {
+            to_reported_order_into(h, *g, row, sizeof(int32_t), wide_tmp.data());
+            B200_LAUNCH(h, k_widen_dist, grid_for(nv), kBlock, 0, wide_tmp.as<int32_t>(), nv, (int64_t*)out);
+          } else {
+            to_reported_order_into(h, *g, row, sizeof(int32_t), out);
+          }
+          if (compute_predecessors)
+            predecessors_to_ext(h, *g, pred_b.as<int32_t>() + (size_t)j * nv, pred_out.as<char>() + (b0 + j) * (size_t)nv * es);
+        }
+      }
+      check_last("multi_source_bfs");
+    }
+    auto res          = std::make_unique<paths_result_impl>();
+    res->vertices     = make_array(reported_vertices(h, *g), (size_t)nv, g->vertex_type);
+    res->distances    = make_array(std::move(dist_out), cells, g->vertex_type);
+    res->predecessors = make_array(std::move(pred_out), compute_predecessors ? cells : 0, g->vertex_type);
     sync(h);
     *result = reinterpret_cast<cugraph_paths_result_t*>(res.release());
   });

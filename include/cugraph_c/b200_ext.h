@@ -188,6 +188,21 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_generate_uniform_at(const cugra
                                                                      cugraph_type_erased_device_array_view_t* out,
                                                                      cugraph_error_t** error);
 
+/* Breadth-first search from each of the n sources separately (not from their union, as cugraph_bfs does).  The result's
+   distances and predecessors hold n x V entries, source-major: entry s*V + i belongs to sources[s] and to vertices[i].
+   Row s equals what cugraph_bfs returns for the single source sources[s] with the same depth_limit: the distances in the
+   graph's vertex type (INT32_MAX / INT64_MAX unreached), predecessors in external ids (-1 for the source and unreached
+   vertices), a parent being any in-neighbour one level closer.  Out-edges are followed on any graph, symmetric or not;
+   weights are ignored.  compute_predecessors = FALSE: predecessors has size 0.  Duplicate sources give identical rows.
+   The sources run in batches of 64, each one pass over the graph per level, in either direction (Beamer's rule with
+   CUGRAPH_B200_BFS_ALPHA / _BETA; the result does not depend on it).  cugraph_extract_paths accepts a result of one row
+   only.  Errors as cugraph_bfs: NULL result or sources, a source type that is not the graph's, a source that is not a
+   vertex (CUGRAPH_INVALID_INPUT). */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_multi_source_bfs(
+  const cugraph_resource_handle_t* handle, cugraph_graph_t* graph,
+  const cugraph_type_erased_device_array_view_t* sources, size_t depth_limit, bool_t compute_predecessors,
+  cugraph_paths_result_t** result, cugraph_error_t** error);
+
 /* One level of multi-GPU BFS on this GPU's edge block (pull direction; the role of the bottom-up step of
  * cpp/src/traversal/bfs_impl.cuh:593-869 on one edge partition).  frontier_cols / visited_rows: byte flags over the block's
  * column (source) / row (destination) slots, gathered by the launcher inside the column / row group.  cand (INT64, one per row
