@@ -142,6 +142,11 @@ def lib():
     _sig(L.cugraph_b200_block_bfs_pull, i32, [vp, vp, vp, vp, sz, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_block_bfs_push, i32, [vp, vp, vp, vp, sz, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_bfs_bottom_up, i32, [vp, i32, sz, sz, sz, sz, sz])
+    _sig(L.cugraph_b200_block_ms_bfs_push, i32, [vp, vp, vp, vp, i32, vp, pvp])
+    _sig(L.cugraph_b200_block_ms_bfs_pull, i32, [vp, vp, vp, vp, i32, vp, pvp])
+    _sig(L.cugraph_b200_block_ms_bfs_pred, i32, [vp, vp, vp, vp, sz, i32, i32, sz, vp, pvp])
+    _sig(L.cugraph_b200_ms_bfs_owner_step, i32, [vp, vp, i32, sz, sz, i32, i32, vp, vp, vp, vp, vp, vp, pvp])
+    _sig(L.cugraph_b200_ms_bfs_owner_pred, i32, [vp, vp, vp, sz, i32, vp, pvp])
     _sig(L.cugraph_b200_block_sssp_relax, i32, [vp, vp, vp, dbl, sz, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_block_sssp_pred, i32, [vp, vp, vp, vp, sz, i32, i32, vp, pvp])
     _sig(L.cugraph_b200_block_wcc_min, i32, [vp, vp, vp, vp, pvp])

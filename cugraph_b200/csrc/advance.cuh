@@ -35,6 +35,14 @@ __device__ __forceinline__ void warp_add_u64(unsigned long long* target, unsigne
   if ((threadIdx.x & 31) == __ffs(mask) - 1) atomicAdd(target, (unsigned long long)sum);
 }
 
+// the sum of v over a whole warp, in every lane (every lane must call it)
+__device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v)
+{
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
 // ------------------------------------------------------------------------------------------
 // generic load-balanced advance over a queue of frontier vertices (merge-path style):
 //   1. degrees of the queue entries -> exclusive scan (CUB, library code for the tiny per-level scan)

@@ -7,7 +7,7 @@
 // the C ABI (the resource handle bound to the caller's CUDA stream is made in capi_basic.cu): rectangular edge blocks with the
 // same binned / column-blocked layout as the single-GPU graph, the block pull sweep and the fused
 // per-iteration vertex step, the transposed block sweep, the owner steps of Katz, eigenvector centrality and HITS, the BFS
-// pull and push steps, the SSSP push relaxation, the WCC min-label round and the two sides of an extract_paths round.  All calls only ENQUEUE work on the handle's stream (the
+// pull and push steps, the multi-source BFS level, predecessor and owner steps, the SSSP push relaxation, the WCC min-label round and the two sides of an extract_paths round.  All calls only ENQUEUE work on the handle's stream (the
 // push calls of BFS, SSSP, WCC and SCC read back one queue size; the first transposed sweep of a block builds its column-major copy).
 #include "advance.cuh"
 #include "centrality_ops.cuh"
@@ -194,6 +194,7 @@ __device__ __forceinline__ bool column_active(double v) { return v < INFINITY; }
 __device__ __forceinline__ bool column_active(long long v) { return v != LLONG_MAX; }
 __device__ __forceinline__ bool column_active(uint8_t f) { return f != 0; }  // a BFS frontier flag
 __device__ __forceinline__ bool column_active(int32_t d) { return d != INT_MAX; }  // a reached BFS distance
+__device__ __forceinline__ bool column_active(unsigned long long w) { return w != 0ull; }  // a multi-source BFS frontier word
 
 // physical rows r < n_ne of the push copy whose column slot row_vertex[r] is active, with their degrees
 template <typename O, typename T>
@@ -442,6 +443,271 @@ void block_push_min(handle_impl const& h, block_impl const& b, block_push_t& p, 
   B200_LAUNCH(h, k_fill<long long>, grid_for(b.n_rows, 1, h.sm_count * 8), kBlock, 0, out, (int64_t)b.n_rows, LLONG_MAX);
   if (p.csx->offs64) block_push_round<int64_t>(h, p, active_cols, op);
   else block_push_round<int32_t>(h, p, active_cols, op);
+}
+
+// ---- multi-GPU multi-source BFS (MGGraph.multi_source_bfs): one BFS per source of a batch of up to 64, bit j of a 64-bit
+// word standing for source j (the words of single GPU's multi-source BFS, traverse.cu).  The launcher gathers the owners'
+// `cur` words (the sources that reached a vertex at this level) over the block's column slots and their `seen` words over
+// its row slots.  A level step, push or pull (the same arrays in and out), writes a partial `next` word per row slot; the
+// launcher ORs the row group's partials at the owners (one all-to-all) and the owner step keeps the new bits and writes the
+// distances.  The predecessor step is separate, so that push and pull share it and a run without predecessors skips it.
+using u64 = unsigned long long;
+
+inline u64 batch_mask(int n_sources) { return n_sources >= 64 ? ~0ull : (1ull << n_sources) - 1ull; }
+
+// push: for every edge col -> row of a frontier column, the sources that reached col at this level and have not reached row
+// (the MG form of ms_topdown_op, traverse.cu)
+struct block_ms_push_op {
+  int32_t const* col_of;  // column slot of a physical row of the push copy
+  u64 const* cur;         // over column slots
+  u64 const* seen;        // over row slots
+  u64 mask;
+  u64* next;              // over row slots, zeroed first
+  __device__ __forceinline__ void edge(int src, long long, int nbr) const
+  {
+    const u64 bits = cur[col_of[src]] & ~seen[nbr] & mask;
+    if (bits & ~next[nbr]) atomicOr(next + nbr, bits);  // next only gains bits during the step: a stale read costs an atomic
+  }
+};
+
+__device__ __forceinline__ u64 warp_or_u64(u64 v)
+{
+  const unsigned lo = __reduce_or_sync(0xffffffffu, (unsigned)v);
+  const unsigned hi = __reduce_or_sync(0xffffffffu, (unsigned)(v >> 32));
+  return ((u64)hi << 32) | lo;
+}
+
+// pull: every row slot ORs cur over its columns into the bits it still wants (want = ~seen & mask) and stops once it has
+// them all.  Rows of degree >= 32 (the prefix of the degree-ordered physical rows) take a warp each, 32 edges per step.
+template <typename O>
+__global__ void __launch_bounds__(256)
+k_block_ms_pull_hi(O const* __restrict__ off, int32_t const* __restrict__ idx, int32_t const* __restrict__ row_vertex, int32_t n_hi,
+                   u64 const* __restrict__ cur, u64 const* __restrict__ seen, u64 mask, u64* __restrict__ next)
+{
+  const int lane = threadIdx.x & 31;
+  for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < n_hi; r += ((long long)gridDim.x * blockDim.x) >> 5) {
+    const int slot = row_vertex ? row_vertex[r] : (int)r;
+    const u64 want = ~seen[slot] & mask;
+    if (!want) continue;  // warp-uniform
+    const long long e1 = (long long)off[r + 1];
+    u64 found          = 0;
+    for (long long e0 = (long long)off[r]; e0 < e1; e0 += 32) {
+      const long long e = e0 + lane;
+      found |= warp_or_u64(e < e1 ? cur[idx[e]] & want : 0ull);
+      if (found == want) break;
+    }
+    if (lane == 0 && found) next[slot] = found;
+  }
+}
+
+template <typename O>
+__global__ void __launch_bounds__(256)
+k_block_ms_pull_low(O const* __restrict__ off, int32_t const* __restrict__ idx, int32_t const* __restrict__ row_vertex, int32_t r0,
+                    int32_t r1, u64 const* __restrict__ cur, u64 const* __restrict__ seen, u64 mask, u64* __restrict__ next)
+{
+  for (long long r = r0 + blockIdx.x * (long long)blockDim.x + threadIdx.x; r < r1; r += (long long)gridDim.x * blockDim.x) {
+    const int slot = row_vertex ? row_vertex[r] : (int)r;
+    const u64 want = ~seen[slot] & mask;
+    if (!want) continue;
+    u64 found          = 0;
+    const long long e1 = (long long)off[r + 1];
+    for (long long e = (long long)off[r]; e < e1 && found != want; ++e) found |= cur[idx[e]] & want;
+    if (found) next[slot] = found;
+  }
+}
+
+template <typename O>
+void block_ms_pull(handle_impl const& h, csx_t const& c, u64 const* cur, u64 const* seen, u64 mask, u64* next, int32_t n_row_slots)
+{
+  CUDA_TRY(cudaMemsetAsync(next, 0, sizeof(u64) * (size_t)n_row_slots, h.stream));
+  const int32_t n_hi = c.degree_sorted ? c.seg[0] : 0;
+  const int32_t n_ne = c.degree_sorted ? c.seg[kNumSeg - 2] : c.n_rows;  // rows with at least one edge
+  if (n_hi > 0)
+    B200_LAUNCH(h, (k_block_ms_pull_hi<O>), grid_for((int64_t)n_hi * 32, 1, h.sm_count * 16), kBlock, 0, c.offsets.as<O>(),
+                c.indices.as<int32_t>(), c.row_vertex.as<int32_t>(), n_hi, cur, seen, mask, next);
+  if (n_ne > n_hi)
+    B200_LAUNCH(h, (k_block_ms_pull_low<O>), grid_for(n_ne - n_hi, 1, h.sm_count * 16), kBlock, 0, c.offsets.as<O>(),
+                c.indices.as<int32_t>(), c.row_vertex.as<int32_t>(), n_hi, n_ne, cur, seen, mask, next);
+}
+
+// out[i] = popc(words[i])
+__global__ void __launch_bounds__(kBlock) k_ms_popc(u64 const* __restrict__ words, long long n, long long* __restrict__ out)
+{
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    out[i] = __popcll(words[i]);
+}
+
+// scan[i] = the set bits of words[0, i): where the bits of word i start in a list of (word, bit) pairs
+dbuf popc_scan(handle_impl const& h, u64 const* words, int64_t n)
+{
+  dbuf cnt = make_dbuf<long long>((size_t)std::max<int64_t>(n, 1), h.stream);
+  dbuf scan = make_dbuf<long long>((size_t)std::max<int64_t>(n, 1), h.stream);
+  if (n == 0) return scan;
+  B200_LAUNCH(h, k_ms_popc, grid_for(n, 1, h.sm_count * 8), kBlock, 0, words, (long long)n, cnt.as<long long>());
+  size_t bytes = 0;
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, bytes, cnt.as<long long>(), scan.as<long long>(), n, h.stream));
+  dbuf tmp(bytes, h.stream);
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp.data(), bytes, cnt.as<long long>(), scan.as<long long>(), n, h.stream));
+  h.launches += 2;
+  return scan;
+}
+
+// write `code` for every bit j of `win` at base + (the bits of b below j)
+__device__ __forceinline__ void ms_write_pairs(u64 win, u64 b, long long base, long long lim, long long code, long long* pairs)
+{
+  while (win) {
+    const int j         = __ffsll((long long)win) - 1;
+    const long long pos = base + __popcll(b & ((1ull << j) - 1ull));
+    if (pos < lim) pairs[pos] = code;
+    win &= win - 1;
+  }
+}
+
+// predecessors: for every row slot with new bits b and every bit j of b, the largest code of a column with bit j in cur.
+// A row lists its columns in ascending slot order (build_binned_rows sorts by (row, column)) and the code grows with the slot,
+// so a scan from the row's end that stops once every bit of b is found gives the maxima without atomics.  The pair of (row
+// slot, bit j) goes to k * seg + (scan[slot] - scan[k * maxpart]) + popc(b below j), k = slot / maxpart: owner segment k,
+// padded to seg entries; entries past seg are dropped.
+struct ms_pairs_at {
+  long long const* scan;
+  long long maxpart, seg;
+  __device__ __forceinline__ long long base(int slot) const
+  {
+    const long long k = slot / maxpart;
+    return k * seg + scan[slot] - scan[k * maxpart];
+  }
+  __device__ __forceinline__ long long lim(int slot) const { return (slot / maxpart + 1) * seg; }
+};
+
+template <typename O>
+__global__ void __launch_bounds__(256)
+k_block_ms_pred_hi(O const* __restrict__ off, int32_t const* __restrict__ idx, int32_t const* __restrict__ row_vertex, int32_t n_hi,
+                   u64 const* __restrict__ cur, u64 const* __restrict__ new_rows, ms_pairs_at at, int grid_cols, int grid_c,
+                   long long* __restrict__ pairs)
+{
+  const int lane = threadIdx.x & 31;
+  for (long long r = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5; r < n_hi; r += ((long long)gridDim.x * blockDim.x) >> 5) {
+    const int slot = row_vertex ? row_vertex[r] : (int)r;
+    const u64 b    = new_rows[slot];
+    if (!b) continue;  // warp-uniform
+    const long long base = at.base(slot), lim = at.lim(slot), e0 = (long long)off[r];
+    u64 left             = b;
+    // 32 edges per step from the row's end: lane 0 holds the largest column, so bit j goes to the lowest lane that has it
+    for (long long e1 = (long long)off[r + 1]; e1 > e0 && left; e1 -= 32) {
+      const long long e = e1 - 1 - lane;
+      const int col     = e >= e0 ? idx[e] : 0;
+      const u64 mine    = e >= e0 ? cur[col] & left : 0ull;
+      u64 incl          = mine;  // inclusive prefix OR over the lanes
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const u64 t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl |= t;
+      }
+      const u64 before = __shfl_up_sync(0xffffffffu, incl, 1);
+      const u64 win    = lane ? mine & ~before : mine;
+      if (win) ms_write_pairs(win, b, base, lim, column_code(col, at.maxpart, grid_cols, grid_c), pairs);
+      left &= ~__shfl_sync(0xffffffffu, incl, 31);
+    }
+  }
+}
+
+template <typename O>
+__global__ void __launch_bounds__(256)
+k_block_ms_pred_low(O const* __restrict__ off, int32_t const* __restrict__ idx, int32_t const* __restrict__ row_vertex, int32_t r0,
+                    int32_t r1, u64 const* __restrict__ cur, u64 const* __restrict__ new_rows, ms_pairs_at at, int grid_cols,
+                    int grid_c, long long* __restrict__ pairs)
+{
+  for (long long r = r0 + blockIdx.x * (long long)blockDim.x + threadIdx.x; r < r1; r += (long long)gridDim.x * blockDim.x) {
+    const int slot = row_vertex ? row_vertex[r] : (int)r;
+    const u64 b    = new_rows[slot];
+    if (!b) continue;
+    const long long base = at.base(slot), lim = at.lim(slot), e0 = (long long)off[r];
+    u64 left             = b;
+    for (long long e = (long long)off[r + 1] - 1; e >= e0 && left; --e) {
+      const int col = idx[e];
+      const u64 win = cur[col] & left;
+      if (!win) continue;
+      ms_write_pairs(win, b, base, lim, column_code(col, at.maxpart, grid_cols, grid_c), pairs);
+      left &= ~win;
+    }
+  }
+}
+
+template <typename O>
+void block_ms_pred(handle_impl const& h, csx_t const& c, u64 const* cur, u64 const* new_rows, int32_t n_row_slots, long long maxpart,
+                   int grid_cols, int grid_c, long long seg, long long* pairs)
+{
+  B200_LAUNCH(h, k_fill<long long>, grid_for(std::max<long long>(grid_cols * seg, 1), 1, h.sm_count * 8), kBlock, 0, pairs,
+              (int64_t)grid_cols * seg, -1ll);
+  if (n_row_slots == 0 || seg == 0) return;
+  dbuf scan = popc_scan(h, new_rows, n_row_slots);
+  const ms_pairs_at at{scan.as<long long>(), maxpart, seg};
+  const int32_t n_hi = c.degree_sorted ? c.seg[0] : 0;
+  const int32_t n_ne = c.degree_sorted ? c.seg[kNumSeg - 2] : c.n_rows;
+  if (n_hi > 0)
+    B200_LAUNCH(h, (k_block_ms_pred_hi<O>), grid_for((int64_t)n_hi * 32, 1, h.sm_count * 16), kBlock, 0, c.offsets.as<O>(),
+                c.indices.as<int32_t>(), c.row_vertex.as<int32_t>(), n_hi, cur, new_rows, at, grid_cols, grid_c, pairs);
+  if (n_ne > n_hi)
+    B200_LAUNCH(h, (k_block_ms_pred_low<O>), grid_for(n_ne - n_hi, 1, h.sm_count * 16), kBlock, 0, c.offsets.as<O>(),
+                c.indices.as<int32_t>(), c.row_vertex.as<int32_t>(), n_hi, n_ne, cur, new_rows, at, grid_cols, grid_c, pairs);
+}
+
+// owner step over the owned slots: next = OR of the `parts` received partials, new = next & ~seen, seen |= new, cur = new,
+// dist[j][v] = level for every bit j of new; counts += (vertices with new bits, their out-degree sum, vertices whose seen
+// became the whole batch, their in-degree sum, the new bits)
+__global__ void __launch_bounds__(kBlock)
+k_ms_owner_step(u64 const* __restrict__ recv, int parts, long long maxpart, int32_t n_local, u64 mask, int32_t level, u64* __restrict__ seen,
+                u64* __restrict__ cur, int32_t* __restrict__ dist, long long const* __restrict__ deg_out,
+                long long const* __restrict__ deg_in, unsigned long long* __restrict__ counts)
+{
+  u64 c_n = 0, c_m = 0, c_full = 0, c_in = 0, c_bits = 0;
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < n_local; v += gridDim.x * blockDim.x) {
+    u64 nxt = 0;
+    for (int k = 0; k < parts; ++k) nxt |= recv[k * maxpart + v];
+    const u64 s  = seen[v];
+    const u64 nw = nxt & ~s & mask;
+    cur[v]       = nw;
+    if (!nw) continue;
+    seen[v] = s | nw;
+    for (u64 w = nw; w; w &= w - 1) dist[(long long)(__ffsll((long long)w) - 1) * n_local + v] = level;
+    c_n += 1;
+    c_bits += (u64)__popcll(nw);
+    if (deg_out) c_m += (u64)deg_out[v];
+    if ((s | nw) == mask) {
+      c_full += 1;
+      if (deg_in) c_in += (u64)deg_in[v];
+    }
+  }
+  const u64 c[5] = {warp_sum_u64(c_n), warp_sum_u64(c_m), warp_sum_u64(c_full), warp_sum_u64(c_in), warp_sum_u64(c_bits)};
+  if ((threadIdx.x & 31) == 0)
+    for (int i = 0; i < 5; ++i)
+      if (c[i]) atomicAdd(counts + i, c[i]);
+}
+
+// pred[j][v] = pairs[scan[v] + popc(new[v] below j)] for every bit j of new[v] (the owner's segment of the pair buffer)
+__global__ void __launch_bounds__(kBlock)
+k_ms_owner_pred(u64 const* __restrict__ nw, long long const* __restrict__ scan, int32_t n_local, long long const* __restrict__ pairs,
+                long long n_pairs, long long* __restrict__ pred)
+{
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < n_local; v += gridDim.x * blockDim.x) {
+    const u64 b = nw[v];
+    for (u64 w = b; w; w &= w - 1) {
+      const int j         = __ffsll((long long)w) - 1;
+      const long long pos = scan[v] + __popcll(b & ((1ull << j) - 1ull));
+      if (pos < n_pairs) pred[(long long)j * n_local + v] = pairs[pos];
+    }
+  }
+}
+
+// argument checks shared by the multi-source push and pull steps
+void check_ms_bfs_block_args(block_impl const& b, device_array_view_impl const* cv, device_array_view_impl const* sv,
+                             device_array_view_impl const* nv, int n_sources)
+{
+  B200_EXPECTS(cv->type == INT64 && sv->type == INT64 && nv->type == INT64, CUGRAPH_INVALID_INPUT,
+               "cur_cols / seen_rows / next_rows must be INT64");
+  B200_EXPECTS(cv->size >= (size_t)b.n_cols && sv->size >= (size_t)b.n_rows && nv->size >= (size_t)b.n_rows,
+               CUGRAPH_INVALID_INPUT, "word arrays shorter than the block's slots");
+  B200_EXPECTS(n_sources >= 1 && n_sources <= 64, CUGRAPH_INVALID_INPUT, "n_sources must be in [1, 64]");
 }
 
 template <typename T>
@@ -999,6 +1265,165 @@ bool_t cugraph_b200_bfs_bottom_up(const cugraph_resource_handle_t* handle, bool_
                        (unsigned long long)m_u, (long long)n_unvisited)
            ? TRUE
            : FALSE;
+}
+
+// next_rows[row slot] = the batch bits of the frontier columns of that row which the row has not seen.  Asynchronous, apart
+// from the read-back of the queue size (and the first call's push copy).
+cugraph_error_code_t cugraph_b200_block_ms_bfs_push(const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+                                                    const cugraph_type_erased_device_array_view_t* cur_cols,
+                                                    const cugraph_type_erased_device_array_view_t* seen_rows, int n_sources,
+                                                    cugraph_type_erased_device_array_view_t* next_rows, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(block && cur_cols && seen_rows && next_rows, CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto* b        = reinterpret_cast<block_impl*>(block);
+    auto const* cv = V(cur_cols);
+    auto const* sv = V(seen_rows);
+    auto const* nv = V(next_rows);
+    check_ms_bfs_block_args(*b, cv, sv, nv, n_sources);
+    auto* next = (u64*)nv->data;
+    CUDA_TRY(cudaMemsetAsync(next, 0, sizeof(u64) * (size_t)b->n_rows, h.stream));
+    block_push_t& p = push_copy(h, *b);
+    auto const* cur = (u64 const*)cv->data;
+    const block_ms_push_op op{p.csx->row_vertex.as<int32_t>(), cur, (u64 const*)sv->data, batch_mask(n_sources), next};
+    if (p.csx->offs64) block_push_round<int64_t>(h, p, cur, op);
+    else block_push_round<int32_t>(h, p, cur, op);
+    check_last("block_ms_bfs_push");
+  });
+}
+
+// the same words by the block's own rows (pull direction).  Asynchronous.
+cugraph_error_code_t cugraph_b200_block_ms_bfs_pull(const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+                                                    const cugraph_type_erased_device_array_view_t* cur_cols,
+                                                    const cugraph_type_erased_device_array_view_t* seen_rows, int n_sources,
+                                                    cugraph_type_erased_device_array_view_t* next_rows, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(block && cur_cols && seen_rows && next_rows, CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto* b        = reinterpret_cast<block_impl*>(block);
+    auto const* cv = V(cur_cols);
+    auto const* sv = V(seen_rows);
+    auto const* nv = V(next_rows);
+    check_ms_bfs_block_args(*b, cv, sv, nv, n_sources);
+    csx_t const& c = *b->csx;
+    auto const* cur  = (u64 const*)cv->data;
+    auto const* seen = (u64 const*)sv->data;
+    if (c.offs64) block_ms_pull<int64_t>(h, c, cur, seen, batch_mask(n_sources), (u64*)nv->data, b->n_rows);
+    else block_ms_pull<int32_t>(h, c, cur, seen, batch_mask(n_sources), (u64*)nv->data, b->n_rows);
+    check_last("block_ms_bfs_pull");
+  });
+}
+
+// pairs[k * seg + ...] = for every row slot with new bits and every such bit, the largest code of a column of that row with
+// the bit in cur_cols, else -1.  Asynchronous.
+cugraph_error_code_t cugraph_b200_block_ms_bfs_pred(const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block,
+                                                    const cugraph_type_erased_device_array_view_t* cur_cols,
+                                                    const cugraph_type_erased_device_array_view_t* new_rows, size_t maxpart,
+                                                    int grid_cols, int grid_c, size_t seg,
+                                                    cugraph_type_erased_device_array_view_t* pairs, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(block && cur_cols && new_rows && pairs, CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto* b        = reinterpret_cast<block_impl*>(block);
+    auto const* cv = V(cur_cols);
+    auto const* nv = V(new_rows);
+    auto const* pv = V(pairs);
+    B200_EXPECTS(cv->type == INT64 && nv->type == INT64 && pv->type == INT64, CUGRAPH_INVALID_INPUT,
+                 "cur_cols / new_rows / pairs must be INT64");
+    B200_EXPECTS(maxpart > 0 && grid_cols > 0 && grid_c >= 0 && grid_c < grid_cols, CUGRAPH_INVALID_INPUT, "bad grid position");
+    B200_EXPECTS((size_t)b->n_rows <= (size_t)grid_cols * maxpart, CUGRAPH_INVALID_INPUT,
+                 "the block has more row slots than grid_cols * maxpart");
+    B200_EXPECTS(cv->size >= (size_t)b->n_cols && nv->size >= (size_t)b->n_rows, CUGRAPH_INVALID_INPUT,
+                 "word arrays shorter than the block's slots");
+    B200_EXPECTS(pv->size >= (size_t)grid_cols * seg, CUGRAPH_INVALID_INPUT, "pairs must hold grid_cols * seg entries");
+    csx_t const& c = *b->csx;
+    auto const* cur = (u64 const*)cv->data;
+    auto const* nw  = (u64 const*)nv->data;
+    if (c.offs64)
+      block_ms_pred<int64_t>(h, c, cur, nw, b->n_rows, (long long)maxpart, grid_cols, grid_c, (long long)seg, (long long*)pv->data);
+    else
+      block_ms_pred<int32_t>(h, c, cur, nw, b->n_rows, (long long)maxpart, grid_cols, grid_c, (long long)seg, (long long*)pv->data);
+    check_last("block_ms_bfs_pred");
+  });
+}
+
+// the owners' level update of a multi-source BFS batch (see k_ms_owner_step); counts[0..5) are overwritten.  Asynchronous.
+cugraph_error_code_t cugraph_b200_ms_bfs_owner_step(const cugraph_resource_handle_t* handle,
+                                                    const cugraph_type_erased_device_array_view_t* recv, int parts, size_t maxpart,
+                                                    size_t n_local, int n_sources, int level,
+                                                    cugraph_type_erased_device_array_view_t* seen,
+                                                    cugraph_type_erased_device_array_view_t* cur,
+                                                    cugraph_type_erased_device_array_view_t* distances,
+                                                    const cugraph_type_erased_device_array_view_t* deg_out,
+                                                    const cugraph_type_erased_device_array_view_t* deg_in,
+                                                    cugraph_type_erased_device_array_view_t* counts, cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(recv && seen && cur && distances && counts, CUGRAPH_INVALID_INPUT, "NULL argument");
+    B200_EXPECTS((deg_out == nullptr) == (deg_in == nullptr), CUGRAPH_INVALID_INPUT, "give both degree arrays or neither");
+    auto const* rv = V(recv);
+    auto const* sv = V(seen);
+    auto const* cv = V(cur);
+    auto const* dv = V(distances);
+    auto const* kv = V(counts);
+    B200_EXPECTS(rv->type == INT64 && sv->type == INT64 && cv->type == INT64 && kv->type == INT64, CUGRAPH_INVALID_INPUT,
+                 "recv / seen / cur / counts must be INT64");
+    B200_EXPECTS(dv->type == INT32, CUGRAPH_INVALID_INPUT, "distances must be INT32");
+    B200_EXPECTS(n_sources >= 1 && n_sources <= 64, CUGRAPH_INVALID_INPUT, "n_sources must be in [1, 64]");
+    B200_EXPECTS(parts > 0 && maxpart > 0 && n_local <= maxpart && n_local < (1u << 31) && level > 0, CUGRAPH_INVALID_INPUT,
+                 "bad parts / maxpart / n_local / level");
+    B200_EXPECTS(rv->size >= (size_t)parts * maxpart, CUGRAPH_INVALID_INPUT, "recv must hold parts * maxpart words");
+    B200_EXPECTS(sv->size >= n_local && cv->size >= n_local, CUGRAPH_INVALID_INPUT, "seen / cur shorter than n_local");
+    B200_EXPECTS(dv->size >= (size_t)n_sources * n_local, CUGRAPH_INVALID_INPUT, "distances must hold n_sources * n_local");
+    B200_EXPECTS(kv->size >= 5, CUGRAPH_INVALID_INPUT, "counts must hold 5 entries");
+    long long const *dout = nullptr, *din = nullptr;
+    if (deg_out) {
+      auto const* ov = V(deg_out);
+      auto const* iv = V(deg_in);
+      B200_EXPECTS(ov->type == INT64 && iv->type == INT64 && ov->size >= n_local && iv->size >= n_local, CUGRAPH_INVALID_INPUT,
+                   "degrees must be INT64 arrays of n_local entries");
+      dout = (long long const*)ov->data;
+      din  = (long long const*)iv->data;
+    }
+    auto* cnt = (unsigned long long*)kv->data;
+    CUDA_TRY(cudaMemsetAsync(cnt, 0, 5 * sizeof(long long), h.stream));
+    if (n_local == 0) return;
+    B200_LAUNCH(h, k_ms_owner_step, grid_for((int64_t)n_local, 1, h.sm_count * 8), kBlock, 0, (u64 const*)rv->data, parts,
+                (long long)maxpart, (int32_t)n_local, batch_mask(n_sources), level, (u64*)sv->data, (u64*)cv->data,
+                (int32_t*)dv->data, dout, din, cnt);
+    check_last("ms_bfs_owner_step");
+  });
+}
+
+// pred[j * n_local + v] = the owner's pair of (v, bit j) for every bit j of new_words[v].  Asynchronous.
+cugraph_error_code_t cugraph_b200_ms_bfs_owner_pred(const cugraph_resource_handle_t* handle,
+                                                    const cugraph_type_erased_device_array_view_t* new_words,
+                                                    const cugraph_type_erased_device_array_view_t* pairs, size_t n_local,
+                                                    int n_sources, cugraph_type_erased_device_array_view_t* predecessors,
+                                                    cugraph_error_t** error)
+{
+  return guarded(error, [&] {
+    auto const& h = H(handle);
+    B200_EXPECTS(new_words && pairs && predecessors, CUGRAPH_INVALID_INPUT, "NULL argument");
+    auto const* nv = V(new_words);
+    auto const* av = V(pairs);
+    auto const* pv = V(predecessors);
+    B200_EXPECTS(nv->type == INT64 && av->type == INT64 && pv->type == INT64, CUGRAPH_INVALID_INPUT,
+                 "new_words / pairs / predecessors must be INT64");
+    B200_EXPECTS(n_sources >= 1 && n_sources <= 64, CUGRAPH_INVALID_INPUT, "n_sources must be in [1, 64]");
+    B200_EXPECTS(n_local < (1u << 31) && nv->size >= n_local, CUGRAPH_INVALID_INPUT, "new_words shorter than n_local");
+    B200_EXPECTS(pv->size >= (size_t)n_sources * n_local, CUGRAPH_INVALID_INPUT, "predecessors must hold n_sources * n_local");
+    if (n_local == 0) return;
+    auto const* nw = (u64 const*)nv->data;
+    dbuf scan      = popc_scan(h, nw, (int64_t)n_local);
+    B200_LAUNCH(h, k_ms_owner_pred, grid_for((int64_t)n_local, 1, h.sm_count * 8), kBlock, 0, nw, scan.as<long long>(),
+                (int32_t)n_local, (long long const*)av->data, (long long)av->size, (long long*)pv->data);
+    check_last("ms_bfs_owner_pred");
+  });
 }
 
 // cand_rows[row slot] = min key over the proposals dist_cols[col] + w < cutoff of the active columns, else INT64_MAX

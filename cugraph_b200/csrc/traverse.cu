@@ -327,13 +327,6 @@ __device__ __forceinline__ void ms_write_rows(unsigned long long bits, int v, lo
   }
 }
 
-__device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v)
-{
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // the four level counters of a thread, summed over the warp and added with one atomic each (every lane must call it)
 __device__ __forceinline__ void ms_commit(ms_counters_t* cnt, unsigned long long n, unsigned long long m, unsigned long long n_full,
                                           unsigned long long m_full)

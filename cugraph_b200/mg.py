@@ -13,7 +13,8 @@ one 2-element all_reduce and never touch the host unless epsilon > 0, and the lo
 same column-blocked shared-memory kernel as on one GPU (C-ABI: cugraph_b200_block_*).
 
 BFS moves byte flags per level (one max-reduce-scatter of candidate predecessors), from one source or a set of sources
-given by every rank; extract_paths walks the BFS predecessors one path position per round, each an all-to-all-v of local
+given by every rank (multi_source_bfs: one BFS per source, 64-bit words per vertex for a batch of 64, see
+MGGraph.multi_source_bfs); extract_paths walks the BFS predecessors one path position per round, each an all-to-all-v of local
 ids to their owners and one of (external id, predecessor code) answers back (see MGGraph.extract_paths); SSSP runs
 Δ-windows of rounds, each an all-gather of the frontier's distances, the block's push relaxation on the device and one
 min-reduce-scatter of INT64 (distance, predecessor) keys (see MGGraph.sssp); WCC propagates the smallest vertex code per round, with one
@@ -347,6 +348,7 @@ class MGGraph:
         self._sssp_avg = None                                                       # (average weight, average degree)
         self._id_order = None                                  # (local ids by external id, sorted external ids)
         self.last_bfs_stats = None
+        self.last_ms_bfs_stats = None
         self.last_sssp_stats = None
         self.last_wcc_stats = None
         self.last_scc_stats = None
@@ -688,6 +690,165 @@ class MGGraph:
         if invalid:
             raise capi.CugraphValueError(capi.INVALID_INPUT, "Found invalid vertex in the input sources", where)
         return lid
+
+    # ------------------------------------------------------------------------------------------
+    # multi-GPU multi-source BFS: one BFS per source, a batch of up to 64 sources per level (single GPU's bit-parallel BFS,
+    # cugraph_b200_multi_source_bfs, on the partition).  The owners keep three INT64 words per owned slot, bit j for source j
+    # of the batch: seen (reached), cur (reached at this level) and the received partials of next.  One level: all-gather of
+    # cur inside the column group (-> the block's column slots) and of seen inside the row group (-> its row slots), ONE block
+    # step (cugraph_b200_block_ms_bfs_push or _pull: the same arrays in and out) writing a partial next word per row slot, ONE
+    # all-to-all of the partials inside the row group (NCCL has no bitwise reduce-scatter: each member receives the C slices
+    # of its own slots and the owner step ORs them, the bytes of a reduce-scatter), the owner step
+    # (cugraph_b200_ms_bfs_owner_step: new bits, distances, counts) and ONE all-reduce of the counts, which is also the
+    # termination test.  With predecessors a level adds an all-gather of the new words inside the row group, the block's
+    # predecessor step (cugraph_b200_block_ms_bfs_pred) into a pair buffer sized from the counts already read, ONE MAX
+    # reduce-scatter of it, and the owners' scatter into the predecessor rows (cugraph_b200_ms_bfs_owner_pred).  The
+    # predecessor of v in row k is the largest code among v's in-neighbours that source k reached one level earlier: what
+    # the top-down MGGraph.bfs(sources[k]) keeps, whichever direction the batch's levels run.
+    # ------------------------------------------------------------------------------------------
+    def multi_source_bfs(self, sources, depth_limit=-1, compute_predecessors=True, *, direction_optimizing=False):
+        """BFS from each of the sources separately.  sources: a 1-D tensor or array of external ids in the edge ids' dtype,
+        the SAME list in the same order on every rank (source k names row k of the result); duplicates each get their own
+        row.  Returns (vertices, distances, predecessors) of the vertices this rank owns: distances int32 [n, n_local]
+        (INT32_MAX = unreached), predecessors [n, n_local] external ids in the vertices' dtype (-1 = none), or None when not
+        requested.  Row k equals MGGraph.bfs(sources[k], depth_limit) on the same graph and grid: the same distances, and the
+        predecessors of its default top-down schedule.  The sources run in batches of 64.
+          direction_optimizing: False runs every level top-down; True picks each level's direction by Beamer's rule
+            (cugraph_b200_bfs_bottom_up) over global counts, a vertex counting as visited once every source of the batch
+            has reached it, with its in-degree for the unvisited edges (as MGGraph.bfs counts them).  Only the schedule
+            depends on it.
+        Every rank raises the same error: TypeError for sources in a dtype other than the edge ids' on some rank,
+        ValueError when the lists differ between ranks, CugraphValueError for a source that is not a vertex.  Sets
+        last_ms_bfs_stats = dict(batches, levels, top_down, bottom_up), the levels summed over the batches."""
+        p = self.part
+        lids = self._ms_sources(sources)
+        n, n_loc = lids.numel(), p.n_local
+        dist_out = torch.full((n, n_loc), torch.iinfo(torch.int32).max, dtype=torch.int32, device=self.device)
+        pred_out = torch.full((n, n_loc), -1, dtype=p.vertices.dtype, device=self.device) if compute_predecessors else None
+        deg = None
+        if direction_optimizing:
+            self.degrees()
+            deg = (self._degrees[1].to(torch.int64), self._degrees[0].to(torch.int64))   # (out, in)
+        stats = dict(batches=0, levels=0, top_down=0, bottom_up=0)
+        for b0 in range(0, n, 64):
+            nb = min(64, n - b0)
+            codes = self._ms_bfs_batch(lids[b0:b0 + nb], dist_out[b0:b0 + nb], depth_limit, compute_predecessors, deg, stats)
+            if compute_predecessors:   # one batch of int64 codes alive at a time, its exchange in pieces of <= 2^27 codes
+                step = max(1, (1 << 27) // p.maxpart)          # the same on every rank: each piece is a collective
+                for k0 in range(0, nb, step):
+                    k1 = min(k0 + step, nb)
+                    pred_out[b0 + k0:b0 + k1] = self._codes_to_external(codes[k0 * n_loc:k1 * n_loc]).reshape(k1 - k0, n_loc)
+        self.last_ms_bfs_stats = stats
+        return p.vertices, dist_out, pred_out
+
+    def _ms_sources(self, sources):
+        """multi_source_bfs's source list -> the local id of every source on this rank, -1 where another rank owns it.  Two
+        MAX all-reduces check that every rank has the same list: [n, -n, dtype error], then [ids, -ids, invalid]; a list
+        that differs at some position shows there as max != -max(-x) on every rank."""
+        from cugraph_b200 import _capi as capi
+        p, g, dev = self.part, self.part.groups, self.device
+        where = "MGGraph.multi_source_bfs"
+        s = torch.as_tensor(sources)
+        bad_type = int(s.dtype != p.vertices.dtype)
+        s = s.to(dev).reshape(-1).to(torch.int64)
+        n = s.numel()
+        head = torch.tensor([n, -n, bad_type], dtype=torch.int64, device=dev)
+        dist.all_reduce(head, op=dist.ReduceOp.MAX)
+        n_max, n_min_neg, bad_type = head.tolist()
+        if bad_type:
+            raise TypeError(f"{where}: sources must have the dtype of the edge ids on every rank")
+        if n_max != -n_min_neg:
+            raise ValueError(f"{where}: sources must be the same list, in the same order, on every rank")
+        if n == 0:
+            return torch.zeros(0, dtype=torch.int64, device=dev)
+        lid, hit = self._owned_lids(s)
+        invalid = ((vertex_owner(s, g.world) == g.rank) & ~hit).sum().reshape(1)   # every id has one owner to check it
+        chk = torch.cat([s, -s, invalid])
+        dist.all_reduce(chk, op=dist.ReduceOp.MAX)
+        if bool(((chk[:n] != s) | (chk[n:2 * n] != -s)).any()):
+            raise ValueError(f"{where}: sources must be the same list, in the same order, on every rank")
+        if int(chk[2 * n].item()):
+            raise capi.CugraphValueError(capi.INVALID_INPUT, "Found invalid vertex in the input sources", where)
+        return torch.where(hit, lid, -1)
+
+    def _ms_bfs_batch(self, lids, dist_rows, depth_limit, want_pred, deg, stats):
+        """one batch of nb <= 64 sources (their local ids here, -1 elsewhere): fills dist_rows [nb, n_local] and returns the
+        predecessor codes (nb * n_local, -1 = none) or None"""
+        p, g, dev, mp = self.part, self.part.groups, self.device, self.part.maxpart
+        n_loc, nb, i64 = p.n_local, lids.numel(), torch.int64
+        mask = -1 if nb == 64 else (1 << nb) - 1
+        seen = torch.zeros(mp, dtype=i64, device=dev)
+        seen[n_loc:] = mask                                   # padding slots never take part
+        mine = (lids >= 0).nonzero().reshape(-1)              # the batch positions whose source this rank owns
+        ml = lids[mine]
+        seen.index_put_((ml,), torch.bitwise_left_shift(torch.ones_like(mine), mine), accumulate=True)  # distinct bits: sum = OR
+        cur = torch.zeros(mp, dtype=i64, device=dev)
+        cur[:n_loc] = seen[:n_loc]
+        dist_rows[mine, ml] = 0
+        do = deg is not None
+        if do:
+            u = torch.unique(ml)
+            full = seen[u] == mask
+            head = torch.stack([torch.tensor(u.numel(), device=dev), deg[0][u].sum(), full.sum(), deg[1][u[full]].sum(),
+                                deg[1].sum()]).to(i64)
+            dist.all_reduce(head)
+            n_f, m_f, n_full, in_full, m_total = head.tolist()
+            prev_n_f = 0
+        cur_cols = torch.empty(self.n_cols, dtype=i64, device=dev)
+        seen_rows = torch.empty(self.n_rows, dtype=i64, device=dev)
+        next_rows = torch.empty(self.n_rows, dtype=i64, device=dev)
+        recv = next_rows if g.C == 1 else torch.empty(self.n_rows, dtype=i64, device=dev)   # C slices of maxpart
+        counts = torch.zeros(5, dtype=i64, device=dev)
+        tot = torch.zeros(4 + g.world, dtype=i64, device=dev)   # the four counts, then every rank's new bits
+        codes = torch.full((nb * n_loc,), -1, dtype=i64, device=dev) if want_pred else None
+        new_rows = torch.empty(self.n_rows, dtype=i64, device=dev) if want_pred else None
+        d_out, d_in = deg if do else (None, None)
+        level = n_bottom_up = 0
+        bottom_up = False
+        with _views(cur_cols, seen_rows, next_rows, recv, seen, cur, dist_rows.reshape(-1), d_out, d_in, counts, new_rows,
+                    codes) as (vcc, vsr, vnr, vrc, vs, vc, vd, vdo, vdi, vk, vnw, vcode):
+            while depth_limit < 0 or level < depth_limit:
+                if do:
+                    bottom_up = bool(self.lib.cugraph_b200_bfs_bottom_up(self.handle.ptr, 1 if bottom_up else 0, n_f, prev_n_f,
+                                                                         m_f, m_total - in_full, p.n_global - n_full))
+                all_gather_into(cur_cols, cur, g.col_group)
+                all_gather_into(seen_rows, seen, g.row_group)
+                step = "cugraph_b200_block_ms_bfs_pull" if bottom_up else "cugraph_b200_block_ms_bfs_push"
+                self._call(step, self.block, vcc.ptr, vsr.ptr, nb, vnr.ptr)
+                if g.C > 1:
+                    dist.all_to_all_single(recv, next_rows, group=g.row_group)
+                level += 1
+                n_bottom_up += int(bottom_up)
+                self._call("cugraph_b200_ms_bfs_owner_step", vrc.ptr, g.C, mp, n_loc, nb, level, vs.ptr, vc.ptr, vd.ptr, vdo.ptr,
+                           vdi.ptr, vk.ptr)
+                tot.zero_()
+                tot[:4] = counts[:4]
+                tot[4 + g.rank] = counts[4]
+                dist.all_reduce(tot)
+                t = tot.tolist()
+                n_new = t[0]
+                # the row group's pair buffer: C segments, each as long as the most new bits one member owns
+                seg = max(t[4 + g.r * g.C + k] for k in range(g.C)) if want_pred else 0
+                if seg:
+                    all_gather_into(new_rows, cur, g.row_group)
+                    pairs = torch.empty(g.C * seg, dtype=i64, device=dev)
+                    pairs_own = torch.empty(seg, dtype=i64, device=dev)
+                    with _views(pairs) as (vp,):
+                        self._call("cugraph_b200_block_ms_bfs_pred", self.block, vcc.ptr, vnw.ptr, mp, g.C, g.c, seg, vp.ptr)
+                    reduce_scatter_into(pairs_own, pairs, g.row_group, op=dist.ReduceOp.MAX)
+                    with _views(pairs_own) as (vpo,):
+                        self._call("cugraph_b200_ms_bfs_owner_pred", vc.ptr, vpo.ptr, n_loc, nb, vcode.ptr)
+                if do:
+                    prev_n_f, n_f, m_f = n_f, n_new, t[1]
+                    n_full += t[2]
+                    in_full += t[3]
+                if n_new == 0:
+                    break
+        stats["batches"] += 1
+        stats["levels"] += level
+        stats["top_down"] += level - n_bottom_up
+        stats["bottom_up"] += n_bottom_up
+        return codes
 
     def _codes_to_external(self, codes):
         """predecessor codes (owner rank * maxpart + local id, -1 = none) -> external ids, answered by the owners (one
@@ -1584,6 +1745,12 @@ def bfs(graph: MGGraph, sources, depth_limit=-1, compute_predecessors=True, *, d
     sources: one external id, the same on every rank, or a 1-D tensor / array of this rank's source ids;
     direction_optimizing: top-down on every level (False) or single GPU's per-level switch (True) (see MGGraph.bfs)."""
     return graph.bfs(sources, depth_limit, compute_predecessors, direction_optimizing=direction_optimizing)
+
+
+def multi_source_bfs(graph: MGGraph, sources, depth_limit=-1, compute_predecessors=True, *, direction_optimizing=False):
+    """(vertices, distances [n, n_local], predecessors [n, n_local]) of the vertices owned by this rank: one BFS per source,
+    row k from sources[k]; sources is the same list on every rank (see MGGraph.multi_source_bfs)."""
+    return graph.multi_source_bfs(sources, depth_limit, compute_predecessors, direction_optimizing=direction_optimizing)
 
 
 def validate_bfs(graph: MGGraph, vertices, distances, predecessors, sources, depth_limit=-1):

@@ -236,6 +236,63 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_bfs_push(
 CUGRAPH_EXPORT bool_t cugraph_b200_bfs_bottom_up(const cugraph_resource_handle_t* handle, bool_t bottom_up_now, size_t n_f,
                                                  size_t prev_n_f, size_t m_f, size_t m_u, size_t n_unvisited);
 
+/* One level of a multi-GPU multi-source BFS batch on this GPU's edge block (MGGraph.multi_source_bfs).  Bit j of a 64-bit word
+ * stands for source j of a batch of n_sources (1 to 64).  cur_cols (INT64, one word per column slot, gathered by the launcher
+ * inside the column group): the sources that reached each column at this level.  seen_rows (INT64, one per row slot,
+ * gathered inside the row group): the sources that have reached each row.  next_rows (INT64, one per row slot) is first
+ * zeroed, then receives for every row slot the OR of cur_cols[col] & ~seen_rows[row] over the row's columns, limited to the
+ * batch's bits; the launcher ORs the row group's words at the owners.  No distance is written here.
+ *   _push queues the columns with a non-zero word through the block's column-major copy (shared with
+ *     cugraph_b200_block_bfs_push and the others, built by the first of these calls and kept) and ORs each edge's bits with
+ *     an atomic.  Asynchronous, apart from one read-back of the number of such columns and their edge count.
+ *   _pull scans every row slot that still wants a bit over its own columns, and stops once it has them all (a warp per row of
+ *     degree >= 32, a thread per other row).  Asynchronous.
+ * Both take the same arguments, with the same checks: INT64 arrays no shorter than the block's slots, n_sources in [1, 64]. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_ms_bfs_push(
+  const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block, const cugraph_type_erased_device_array_view_t* cur_cols,
+  const cugraph_type_erased_device_array_view_t* seen_rows, int n_sources, cugraph_type_erased_device_array_view_t* next_rows,
+  cugraph_error_t** error);
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_ms_bfs_pull(
+  const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block, const cugraph_type_erased_device_array_view_t* cur_cols,
+  const cugraph_type_erased_device_array_view_t* seen_rows, int n_sources, cugraph_type_erased_device_array_view_t* next_rows,
+  cugraph_error_t** error);
+
+/* The predecessors of a level of a multi-source BFS batch on this GPU's edge block.  cur_cols: the level's frontier words, as
+ * given to the level step; new_rows (INT64, one per row slot, gathered inside the row group): the bits the owners accepted at
+ * this level.  For every row slot with new bits b and every bit j of b, the entry of (row, j) receives the largest code
+ * ((col / maxpart) * grid_cols + grid_c) * maxpart + col % maxpart over the row's columns with bit j in cur_cols[col], or -1
+ * when this block has none.  The entries are laid out as grid_cols owner segments of seg entries (pairs: INT64, at least
+ * grid_cols * seg, filled with -1 first): row slot r lies in segment k = r / maxpart, and (r, j) sits at
+ * k * seg + (the new bits of the row slots k * maxpart .. r - 1) + (the bits of b below j).  seg must be at least the new
+ * bits of every segment; entries past it are dropped.  A MAX reduce-scatter of pairs in the row group then gives every owner
+ * its own segment.  The block must have at most grid_cols * maxpart row slots.  Asynchronous. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_block_ms_bfs_pred(
+  const cugraph_resource_handle_t* handle, cugraph_b200_block_t* block, const cugraph_type_erased_device_array_view_t* cur_cols,
+  const cugraph_type_erased_device_array_view_t* new_rows, size_t maxpart, int grid_cols, int grid_c, size_t seg,
+  cugraph_type_erased_device_array_view_t* pairs, cugraph_error_t** error);
+
+/* The owners' update of one level of a multi-source BFS batch, over the n_local owned slots.  recv (INT64, parts * maxpart
+ * words): the row group's partial next words for the owned slots, one slice of maxpart per member.  For every owned slot v:
+ * new = (OR of the parts slices at v) & ~seen[v] (batch bits only), seen[v] |= new, cur[v] = new, and
+ * distances[j * n_local + v] = level (INT32) for every bit j of new.  counts (INT64, 5 entries, overwritten) = the slots with
+ * new bits, their deg_out sum, the slots whose seen word became the whole batch, their deg_in sum, and the new bits in all.
+ * deg_out / deg_in (INT64, n_local entries) may both be NULL: their sums are then 0.  Asynchronous. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_ms_bfs_owner_step(
+  const cugraph_resource_handle_t* handle, const cugraph_type_erased_device_array_view_t* recv, int parts, size_t maxpart,
+  size_t n_local, int n_sources, int level, cugraph_type_erased_device_array_view_t* seen,
+  cugraph_type_erased_device_array_view_t* cur, cugraph_type_erased_device_array_view_t* distances,
+  const cugraph_type_erased_device_array_view_t* deg_out, const cugraph_type_erased_device_array_view_t* deg_in,
+  cugraph_type_erased_device_array_view_t* counts, cugraph_error_t** error);
+
+/* The owners' side of the predecessor step: new_words (INT64, n_local) are the level's new bits, pairs (INT64) the owner's
+ * segment of cugraph_b200_block_ms_bfs_pred's buffer after the MAX reduce-scatter.  predecessors[j * n_local + v] (INT64)
+ * = the entry of (v, j) for every bit j of new_words[v], at (the new bits of the slots before v) + (the bits below j);
+ * entries past the end of pairs are skipped.  Asynchronous. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_b200_ms_bfs_owner_pred(
+  const cugraph_resource_handle_t* handle, const cugraph_type_erased_device_array_view_t* new_words,
+  const cugraph_type_erased_device_array_view_t* pairs, size_t n_local, int n_sources,
+  cugraph_type_erased_device_array_view_t* predecessors, cugraph_error_t** error);
+
 /* One relaxation round of multi-GPU SSSP on this GPU's edge block (push direction; the role of the MG relaxation of
  * cpp/src/traversal/sssp_impl.cuh:301-375 on one edge partition).  The block must have been created with weights.
  * dist_cols (the block's weight type, one value per column slot, gathered by the launcher inside the column group) holds the
