@@ -116,6 +116,14 @@ def lib():
     _sig(L.cugraph_hits_result_get_hub_score_differences, dbl, [vp])
     _sig(L.cugraph_hits_result_get_number_of_iterations, sz, [vp])
     _sig(L.cugraph_hits_result_free, None, [vp])
+    _sig(L.cugraph_betweenness_centrality, i32, [vp, vp, vp, i32, i32, i32, pvp, pvp])
+    _sig(L.cugraph_edge_betweenness_centrality, i32, [vp, vp, vp, i32, i32, pvp, pvp])
+    for f in ("src_vertices", "dst_vertices", "edge_ids", "values"):
+        _sig(getattr(L, f"cugraph_edge_centrality_result_get_{f}"), vp, [vp])
+    _sig(L.cugraph_edge_centrality_result_free, None, [vp])
+    _sig(L.cugraph_rng_state_create, i32, [vp, C.c_uint64, pvp, pvp])
+    _sig(L.cugraph_rng_state_free, None, [vp])
+    _sig(L.cugraph_select_random_vertices, i32, [vp, vp, vp, sz, pvp, pvp])
     _sig(L.cugraph_weakly_connected_components, i32, [vp, vp, i32, pvp, pvp])
     _sig(L.cugraph_strongly_connected_components, i32, [vp, vp, i32, pvp, pvp])
     _sig(L.cugraph_labeling_result_get_vertices, vp, [vp])

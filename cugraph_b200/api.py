@@ -198,6 +198,46 @@ def hits(G: Graph, max_iter=100, tol=1.0e-5, nstart=None, normalized=True):
     return _frame(vertex=_host(verts), hubs=_host(hubs), authorities=_host(auth))
 
 
+def _bc_k(G: Graph, k):
+    """k as the pylibcugraph layer takes it: None, an int, or the listed vertices on the device"""
+    if k is None or isinstance(k, (int, np.integer)):
+        return None if k is None else int(k)
+    return _dev(np.atleast_1d(np.asarray(k, dtype=G._edges[0].dtype)))
+
+
+def betweenness_centrality(G: Graph, k=None, normalized=True, weight=None, endpoints=False, seed=None, random_state=None,
+                           result_dtype=np.float64):
+    """cugraph.betweenness_centrality (centrality/betweenness_centrality.py): 'vertex', 'betweenness_centrality'.  k: None
+    (every vertex a source), an int (that many sources drawn with random_state) or a list of vertices.  Edge weights are
+    not used; `weight` raises NotImplementedError, as in the reference."""
+    if weight is not None:
+        raise NotImplementedError("weighted implementation of betweenness centrality not currently supported")
+    if result_dtype not in (np.float32, np.float64):
+        raise TypeError("result type can only be np.float32 or np.float64")
+    plc = _plc()
+    h, g = G._plc_graph(False)
+    verts, vals = plc.betweenness_centrality(h, g, _bc_k(G, k), random_state, normalized, endpoints, False)
+    return _frame(vertex=_host(verts), betweenness_centrality=_host(vals).astype(result_dtype))
+
+
+def edge_betweenness_centrality(G: Graph, k=None, normalized=True, weight=None, seed=None, result_dtype=np.float64):
+    """cugraph.edge_betweenness_centrality: 'src', 'dst', 'betweenness_centrality'.  On an undirected graph the two
+    directions of an edge are folded into one row (src < dst) holding their sum, as the reference does."""
+    if weight is not None:
+        raise NotImplementedError("weighted implementation of edge betweenness centrality not currently supported")
+    if result_dtype not in (np.float32, np.float64):
+        raise TypeError("result type can only be np.float32 or np.float64")
+    plc = _plc()
+    h, g = G._plc_graph(False)
+    src, dst, vals, _ = plc.edge_betweenness_centrality(h, g, _bc_k(G, k), seed, normalized, False)
+    df = _frame(src=_host(src), dst=_host(dst), betweenness_centrality=_host(vals).astype(result_dtype))
+    if not G.directed:
+        lower = df["src"] >= df["dst"]
+        df.loc[lower, ["src", "dst"]] = df.loc[lower, ["dst", "src"]].to_numpy()
+        df = df.groupby(by=["src", "dst"]).sum().reset_index()
+    return df
+
+
 def weakly_connected_components(G: Graph, directed=None, connection=None, return_labels=None):
     """cugraph.weakly_connected_components (components/connectivity.py): 'vertex', 'labels'.  The graph must be undirected."""
     plc = _plc()

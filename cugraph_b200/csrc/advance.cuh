@@ -43,6 +43,22 @@ __device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v)
   return v;
 }
 
+// queue of the vertices with a non-zero word (multi-source BFS after a bottom-up level: traverse.cu, betweenness.cu); the
+// whole CTA takes each step
+__global__ void k_ms_words_to_queue(unsigned long long const* __restrict__ words, int n, int32_t* __restrict__ q, int* counter)
+{
+  for (long long v0 = blockIdx.x * (long long)blockDim.x; v0 < n; v0 += (long long)gridDim.x * blockDim.x) {
+    const long long v   = v0 + threadIdx.x;
+    const bool on       = v < n && words[v] != 0ull;
+    const unsigned ball = __ballot_sync(0xffffffffu, on);
+    const int lane      = threadIdx.x & 31;
+    int base            = 0;
+    if (lane == 0 && ball) base = atomicAdd(counter, __popc(ball));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (on) q[base + __popc(ball & ((1u << lane) - 1u))] = (int32_t)v;
+  }
+}
+
 // ------------------------------------------------------------------------------------------
 // generic load-balanced advance over a queue of frontier vertices (merge-path style):
 //   1. degrees of the queue entries -> exclusive scan (CUB, library code for the tiny per-level scan)

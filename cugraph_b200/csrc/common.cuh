@@ -112,6 +112,7 @@ struct tuning_t {
   long long offs64_min_edges{1ll << 31};  // CUGRAPH_B200_OFFS64_MIN_EDGES: a csx with this many edges stores 64-bit offsets, in [0, 2^31]
                                           // (tests: 0; lazily built views follow the handle passed to the algorithm)
   bool bfs_trace{false}, sssp_trace{false}, build_trace{false}, scc_trace{false};  // CUGRAPH_B200_{BFS,SSSP,BUILD,SCC}_TRACE
+  bool bc_trace{false};  // CUGRAPH_B200_BC_TRACE: betweenness prints each batch's BFS, sigma and backward times (CUDA events)
   static tuning_t from_env()
   {
     tuning_t t;
@@ -135,6 +136,7 @@ struct tuning_t {
     t.sssp_trace  = get("CUGRAPH_B200_SSSP_TRACE") != nullptr;
     t.build_trace = get("CUGRAPH_B200_BUILD_TRACE") != nullptr;
     t.scc_trace   = get("CUGRAPH_B200_SCC_TRACE") != nullptr;
+    t.bc_trace    = get("CUGRAPH_B200_BC_TRACE") != nullptr;
     return t;
   }
 };

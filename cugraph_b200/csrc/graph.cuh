@@ -138,6 +138,19 @@ void pull_sweep(handle_impl const& h, csx_t const& c, int32_t n_vertices, T cons
 // build now what pull_sweep would build on its first call for elements of `elem_size` bytes (the piece stream, if c gets one)
 void prepare_pull_sweep(handle_impl const& h, csx_t const& c, int32_t n_vertices, size_t elem_size);
 
+// ---- multi-source BFS (traverse.cu): one batch of nb <= 64 sources (internal ids), bit j of a vertex's 64-bit word for
+// sources[j].  dist / pred (each may be null) get nb rows of V entries.  After the seed (level 0) and after every level d
+// that reached something, sink->level(d, words, queue, n) sees the frontier: the n vertices that gained bits at level d and,
+// in words[v] (V entries), exactly those bits.  queue lists the n vertices, or is null after a bottom-up level (then the
+// vertices are those with a non-zero word).  Both are only valid during the call; the sink may enqueue work on h.stream.
+struct ms_level_sink {
+  virtual void level(int d, unsigned long long const* words, int32_t const* queue, int n) = 0;
+ protected:
+  ~ms_level_sink() = default;
+};
+void multi_source_bfs_batch(handle_impl const& h, graph_impl& g, int32_t const* sources, int nb, int depth_limit, int32_t* dist,
+                            int32_t* pred, int batch, ms_level_sink* sink);
+
 // external <-> internal id helpers (graph_build.cu)
 // out[i] = internal id of ext[i], or -1 if ext[i] is not a vertex.
 void ext_to_int(handle_impl const& h, graph_impl const& g, void const* ext, size_t n, int32_t* out);

@@ -319,6 +319,7 @@ struct ms_counters_t {
 __device__ __forceinline__ void ms_write_rows(unsigned long long bits, int v, long long nv, int32_t d, int32_t* dist, int32_t* pred,
                                               int u)
 {
+  if (!dist) return;  // betweenness: the levels are kept as queues instead (ms_level_sink)
   while (bits) {
     const long long j = __ffsll((long long)bits) - 1;
     dist[j * nv + v] = d;
@@ -357,7 +358,7 @@ __global__ void k_ms_seed(int32_t const* __restrict__ src, int n, O const* __res
     const unsigned long long bit  = 1ull << i;
     const unsigned long long old  = atomicOr(seen + v, bit);
     atomicOr(cur + v, bit);
-    dist[i * nv + v] = 0;
+    if (dist) dist[i * nv + v] = 0;
     if (old == 0) {
       const unsigned d = enqueue_with_degree(off, v, q, q_deg, &cnt->f);
       atomicAdd(&cnt->f.m_f, (unsigned long long)d);
@@ -502,27 +503,12 @@ k_ms_bottomup(OI const* __restrict__ in_off, int32_t const* __restrict__ in_idx,
   ms_commit(cnt, c_n, c_m, c_full, c_mfull);
 }
 
-// queue of the vertices with a non-zero word (a switch from bottom-up back to top-down); the whole CTA takes each step
-__global__ void k_ms_words_to_queue(unsigned long long const* __restrict__ words, int n, int32_t* __restrict__ q, int* counter)
-{
-  for (long long v0 = blockIdx.x * (long long)blockDim.x; v0 < n; v0 += (long long)gridDim.x * blockDim.x) {
-    const long long v   = v0 + threadIdx.x;
-    const bool on       = v < n && words[v] != 0ull;
-    const unsigned ball = __ballot_sync(0xffffffffu, on);
-    const int lane      = threadIdx.x & 31;
-    int base            = 0;
-    if (lane == 0 && ball) base = atomicAdd(counter, __popc(ball));
-    base = __shfl_sync(0xffffffffu, base, 0);
-    if (on) q[base + __popc(ball & ((1u << lane) - 1u))] = (int32_t)v;
-  }
-}
-
-// One batch of nb <= 64 sources (internal ids).  dist and pred (may be null) hold nb rows of nv entries, filled here.
+// One batch of nb <= 64 sources (internal ids).  dist and pred (each may be null) hold nb rows of nv entries, filled here.
 // Direction per level: Beamer's rule (bfs_bottom_up), with a vertex counted as visited once every source of the batch has
-// reached it.  Only the schedule depends on it, never the result.
+// reached it.  Only the schedule depends on it, never the result.  sink (may be null) is handed every level's frontier.
 template <typename O>
 void run_multi_source_bfs_batch(handle_impl const& h, graph_impl& g, csx_t const& c, int32_t nv, int32_t const* sources, int nb,
-                                int depth_limit, int32_t* dist, int32_t* pred, int batch)
+                                int depth_limit, int32_t* dist, int32_t* pred, int batch, ms_level_sink* sink)
 {
   using u64          = unsigned long long;
   O const* off       = c.offsets.as<O>();
@@ -536,7 +522,7 @@ void run_multi_source_bfs_batch(handle_impl const& h, graph_impl& g, csx_t const
   dbuf cnt = make_dbuf<ms_counters_t>(1, h.stream);
   ms_counters_t* dc = cnt.as<ms_counters_t>();
   CUDA_TRY(cudaMemsetAsync(cnt.data(), 0, sizeof(ms_counters_t), h.stream));
-  B200_LAUNCH(h, (k_fill<int32_t>), grid_for(cells, 1, h.sm_count * 32), kBlock, 0, dist, (int64_t)cells, INT_MAX);
+  if (dist) B200_LAUNCH(h, (k_fill<int32_t>), grid_for(cells, 1, h.sm_count * 32), kBlock, 0, dist, (int64_t)cells, INT_MAX);
   if (pred) B200_LAUNCH(h, (k_fill<int32_t>), grid_for(cells, 1, h.sm_count * 32), kBlock, 0, pred, (int64_t)cells, -1);
   u64 *cur = wa.as<u64>(), *nxt = wb.as<u64>();
   int32_t *cur_q = qa.as<int32_t>(), *nxt_q = qb.as<int32_t>();
@@ -556,6 +542,7 @@ void run_multi_source_bfs_batch(handle_impl const& h, graph_impl& g, csx_t const
   advance_scratch_t adv;
   adv.init(h, nv, (int64_t)c.nnz);
   const bool trace = h.tune.bfs_trace;
+  if (sink && n_f > 0) sink->level(0, cur, cur_q, n_f);
   for (int level = 0; n_f > 0 && level < depth_limit; ++level) {
     const auto t0 = std::chrono::steady_clock::now();
     bottom_up     = bfs_bottom_up(h, bottom_up, n_f, prev_n_f, m_f, m_total - std::min(m_full, m_total), nv - n_full);
@@ -600,9 +587,24 @@ void run_multi_source_bfs_batch(handle_impl const& h, graph_impl& g, csx_t const
     m_f      = hc->f.m_f;
     n_full += (long long)hc->n_full;
     m_full += hc->m_full;
+    if (sink && n_f > 0) sink->level(level + 1, cur, have_queue ? cur_q : nullptr, n_f);
   }
   check_last("multi_source_bfs");
 }
+
+}  // namespace
+
+void multi_source_bfs_batch(handle_impl const& h, graph_impl& g, int32_t const* sources, int nb, int depth_limit, int32_t* dist,
+                            int32_t* pred, int batch, ms_level_sink* sink)
+{
+  csx_t const& c = push_view(h, g);
+  if (c.offs64)
+    run_multi_source_bfs_batch<int64_t>(h, g, c, g.n_vertices, sources, nb, depth_limit, dist, pred, batch, sink);
+  else
+    run_multi_source_bfs_batch<int32_t>(h, g, c, g.n_vertices, sources, nb, depth_limit, dist, pred, batch, sink);
+}
+
+namespace {
 
 // ------------------------------------------------------------------------------------------
 // SSSP: near/far piles with threshold stepping (sssp_impl.cuh:246-265, 373-566)
@@ -1441,7 +1443,6 @@ cugraph_error_code_t cugraph_b200_multi_source_bfs(const cugraph_resource_handle
     dbuf dist_out(cells * es, h.stream), pred_out(compute_predecessors ? cells * es : 0, h.stream);
     const int dl = (int)std::min<size_t>(depth_limit, (size_t)INT_MAX);
     if (cells > 0) {
-      csx_t const& c  = push_view(h, *g);
       const int nb_max = (int)std::min<size_t>(n, 64);
       // one batch's internal rows; each row goes to reported order and external ids straight into the result
       dbuf dist_b = make_dbuf<int32_t>((size_t)nb_max * nv, h.stream), pred_b;
@@ -1450,12 +1451,8 @@ cugraph_error_code_t cugraph_b200_multi_source_bfs(const cugraph_resource_handle
       if (g->vertex_type == INT64) wide_tmp = make_dbuf<int32_t>(nv, h.stream);
       for (size_t b0 = 0; b0 < n; b0 += 64) {
         const int nb = (int)std::min<size_t>(n - b0, 64);
-        if (c.offs64)
-          run_multi_source_bfs_batch<int64_t>(h, *g, c, nv, src_int.as<int32_t>() + b0, nb, dl, dist_b.as<int32_t>(),
-                                              pred_b.as<int32_t>(), (int)(b0 / 64));
-        else
-          run_multi_source_bfs_batch<int32_t>(h, *g, c, nv, src_int.as<int32_t>() + b0, nb, dl, dist_b.as<int32_t>(),
-                                              pred_b.as<int32_t>(), (int)(b0 / 64));
+        multi_source_bfs_batch(h, *g, src_int.as<int32_t>() + b0, nb, dl, dist_b.as<int32_t>(), pred_b.as<int32_t>(),
+                               (int)(b0 / 64), nullptr);
         for (int j = 0; j < nb; ++j) {
           int32_t const* row = dist_b.as<int32_t>() + (size_t)j * nv;
           char* out          = dist_out.as<char>() + (b0 + j) * (size_t)nv * es;

@@ -7,6 +7,7 @@ from cugraph_b200.pylibcugraph.resource_handle import ResourceHandle
 from cugraph_b200.pylibcugraph.graph_properties import GraphProperties
 from cugraph_b200.pylibcugraph.graphs import SGGraph
 from cugraph_b200.pylibcugraph.algorithms import (pagerank, personalized_pagerank, bfs, sssp, katz_centrality, eigenvector_centrality, hits,
+                                                  betweenness_centrality, edge_betweenness_centrality, select_random_vertices,
                                                   weakly_connected_components, strongly_connected_components,
                                                   generate_rmat_edgelist, in_degrees, out_degrees, degrees)
 
@@ -16,4 +17,4 @@ __version__ = "26.10.00+b200"   # the reference version this surface mirrors (ra
 __git_commit__ = ""             # only non-empty in a built distribution, as in the reference
 
 __all__ = ["FailedToConvergeError", "ResourceHandle", "GraphProperties", "SGGraph",
-           "pagerank", "personalized_pagerank", "bfs", "sssp", "katz_centrality", "eigenvector_centrality", "hits", "weakly_connected_components", "strongly_connected_components", "generate_rmat_edgelist", "in_degrees", "out_degrees", "degrees"]
+           "pagerank", "personalized_pagerank", "bfs", "sssp", "katz_centrality", "eigenvector_centrality", "hits", "betweenness_centrality", "edge_betweenness_centrality", "select_random_vertices", "weakly_connected_components", "strongly_connected_components", "generate_rmat_edgelist", "in_degrees", "out_degrees", "degrees"]

@@ -129,6 +129,64 @@ def katz_centrality(resource_handle, graph, betas, alpha, beta, epsilon, max_ite
     return (verts, vals)
 
 
+def select_random_vertices(resource_handle, graph, random_state, num_vertices):
+    """num_vertices distinct vertices of the graph drawn with cugraph_select_random_vertices from a state seeded with
+    random_state (None: seed 0) — select_random_vertices.pyx.  The draw is not the reference's (INTEGRATION.md)."""
+    L = _capi.lib()
+    st, err = C.c_void_p(), C.c_void_p()
+    code = L.cugraph_rng_state_create(resource_handle.ptr, int(random_state or 0) & (2**64 - 1), C.byref(st), C.byref(err))
+    _capi.check(code, err, "cugraph_rng_state_create")
+    arr, err = C.c_void_p(), C.c_void_p()
+    resource_handle.order_after_caller()
+    code = L.cugraph_select_random_vertices(resource_handle.ptr, graph.ptr, st, int(num_vertices), C.byref(arr), C.byref(err))
+    L.cugraph_rng_state_free(st)
+    _capi.check(code, err, "select_random_vertices")
+    view = L.cugraph_type_erased_device_array_view(arr)
+    out = copy_to_torch(resource_handle, view)
+    L.cugraph_type_erased_device_array_free(arr)
+    return out
+
+
+def _betweenness_sources(resource_handle, graph, k, random_state):
+    """k: an int (that many sources drawn with select_random_vertices), a vertex array or None (every vertex)"""
+    if isinstance(k, int):
+        return select_random_vertices(resource_handle, graph, random_state, k)
+    assert_CAI_type(k, "k", allow_none=True)
+    return k
+
+
+def betweenness_centrality(resource_handle, graph, k, random_state, normalized, include_endpoints, do_expensive_check):
+    """Returns (vertices, values) — betweenness_centrality.pyx."""
+    vl = View(_betweenness_sources(resource_handle, graph, k, random_state))
+    res, err = C.c_void_p(), C.c_void_p()
+    resource_handle.order_after_caller()
+    code = _capi.lib().cugraph_betweenness_centrality(resource_handle.ptr, graph.ptr, vl.ptr, int(bool(normalized)),
+                                                      int(bool(include_endpoints)), int(bool(do_expensive_check)), C.byref(res),
+                                                      C.byref(err))
+    vl.free()
+    _capi.check(code, err, "cugraph_betweenness_centrality")
+    verts, vals, _, _ = _centrality_result(resource_handle, res)
+    return (verts, vals)
+
+
+def edge_betweenness_centrality(resource_handle, graph, k, random_state, normalized, do_expensive_check):
+    """Returns (src_vertices, dst_vertices, values, edge_ids) — edge_betweenness_centrality.pyx; edge_ids is None (graphs
+    here hold no edge ids)."""
+    L = _capi.lib()
+    vl = View(_betweenness_sources(resource_handle, graph, k, random_state))
+    res, err = C.c_void_p(), C.c_void_p()
+    resource_handle.order_after_caller()
+    code = L.cugraph_edge_betweenness_centrality(resource_handle.ptr, graph.ptr, vl.ptr, int(bool(normalized)),
+                                                 int(bool(do_expensive_check)), C.byref(res), C.byref(err))
+    vl.free()
+    _capi.check(code, err, "cugraph_edge_betweenness_centrality")
+    src = copy_to_torch(resource_handle, L.cugraph_edge_centrality_result_get_src_vertices(res))
+    dst = copy_to_torch(resource_handle, L.cugraph_edge_centrality_result_get_dst_vertices(res))
+    vals = copy_to_torch(resource_handle, L.cugraph_edge_centrality_result_get_values(res))
+    L.cugraph_edge_centrality_result_free(res)
+    return (src, dst, vals, None)
+
+
 def eigenvector_centrality(resource_handle, graph, epsilon, max_iterations, do_expensive_check):
     """Returns (vertices, values) — eigenvector_centrality.pyx."""
     res, err = C.c_void_p(), C.c_void_p()

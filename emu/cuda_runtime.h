@@ -254,6 +254,7 @@ inline cudaError_t cudaFreeAsync(void* p, cudaStream_t) { std::free(p); return c
 inline cudaError_t cudaFreeHost(void* p) { std::free(p); return cudaSuccess; }
 inline cudaError_t cudaMemcpy(void* d, const void* s, size_t n, cudaMemcpyKind) { if (n) std::memmove(d, s, n); return cudaSuccess; }
 inline cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind k, cudaStream_t = nullptr) { return cudaMemcpy(d, s, n, k); }
+inline cudaError_t cudaMemGetInfo(size_t* free_b, size_t* total_b) { *free_b = *total_b = 1ull << 34; return cudaSuccess; }
 inline cudaError_t cudaMemset(void* d, int v, size_t n) { if (n) std::memset(d, v, n); return cudaSuccess; }
 inline cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t = nullptr) { return cudaMemset(d, v, n); }
 inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) { *s = (cudaStream_t)std::malloc(8); return cudaSuccess; }

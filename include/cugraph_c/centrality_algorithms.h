@@ -98,6 +98,34 @@ CUGRAPH_EXPORT cugraph_error_code_t cugraph_hits(
   const cugraph_type_erased_device_array_view_t* initial_hubs_guess_values, bool_t normalize, bool_t do_expensive_check,
   cugraph_hits_result_t** result, cugraph_error_t** error);
 
+/* Betweenness centrality: centrality_algorithms.h:366-486, cpp/src/c_api/betweenness_centrality.cpp,
+ * cpp/src/centrality/betweenness_centrality_impl.cuh.  Brandes' algorithm over batches of up to 64 sources on the multi-source
+ * BFS levels (betweenness.cu); shortest paths are counted by hops and edge weights are not used.  vertex_list == NULL: every
+ * vertex is a source; else its vertices are the sources (cugraph_select_random_vertices draws such a list).  Values have the
+ * graph's weight type (FLOAT32 on an unweighted graph), scaled as the reference scales them.  A source that is not a vertex
+ * gives CUGRAPH_INVALID_INPUT. */
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_betweenness_centrality(
+  const cugraph_resource_handle_t* handle, cugraph_graph_t* graph, const cugraph_type_erased_device_array_view_t* vertex_list,
+  bool_t normalized, bool_t include_endpoints, bool_t do_expensive_check, cugraph_centrality_result_t** result,
+  cugraph_error_t** error);
+
+/* Edge betweenness: one value per edge of the graph, multi-edges each with their own.  Edge ids are not stored by this
+ * library (graph creation validates and drops them), so get_edge_ids returns NULL, as the reference's result of a graph
+ * created without edge ids holds none. */
+typedef struct { int32_t align_; } cugraph_edge_centrality_result_t;
+CUGRAPH_EXPORT cugraph_type_erased_device_array_view_t* cugraph_edge_centrality_result_get_src_vertices(
+  cugraph_edge_centrality_result_t* result);
+CUGRAPH_EXPORT cugraph_type_erased_device_array_view_t* cugraph_edge_centrality_result_get_dst_vertices(
+  cugraph_edge_centrality_result_t* result);
+CUGRAPH_EXPORT cugraph_type_erased_device_array_view_t* cugraph_edge_centrality_result_get_edge_ids(
+  cugraph_edge_centrality_result_t* result);
+CUGRAPH_EXPORT cugraph_type_erased_device_array_view_t* cugraph_edge_centrality_result_get_values(
+  cugraph_edge_centrality_result_t* result);
+CUGRAPH_EXPORT void cugraph_edge_centrality_result_free(cugraph_edge_centrality_result_t* result);
+CUGRAPH_EXPORT cugraph_error_code_t cugraph_edge_betweenness_centrality(
+  const cugraph_resource_handle_t* handle, cugraph_graph_t* graph, const cugraph_type_erased_device_array_view_t* vertex_list,
+  bool_t normalized, bool_t do_expensive_check, cugraph_edge_centrality_result_t** result, cugraph_error_t** error);
+
 #ifdef __cplusplus
 }
 #endif
